@@ -1,9 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — events/sec of the segmented event fold (BASELINE.json metric) on N B200s of one node.
+"""bench.py — events/sec of the segmented event fold (BASELINE.json metric) on N H100s of one node.
 
 A "step" is one full pass of the hot path over one batch of synthetic input: rebuilding every aggregate's state from its
 CSR event log (configs[1]: 1,048,576 aggregates x 32 fixed 64-byte events = 2 GiB of events per GPU; the log is far larger
-than the 126 MB L2, so no flush is needed between timed iterations).
+than the 50 MB L2, so no flush is needed between timed iterations).
+
+`--dump-outputs DIR` writes the state table of the last timed step (what sgr_export_states hands a caller) to DIR/states.npy
+as float64 (every int32 word exact), so that two builds can be compared output for output on identical seeded inputs.
 
   value   whole-job events/s with the log resident in HBM, K pipelined folds, CUDA events on the engine's stream, max over
           ranks (weak scaling of the fold itself: every rank folds its own shard of aggregates)
@@ -21,8 +24,8 @@ than the 126 MB L2, so no flush is needed between timed iterations).
           whole state table (sum over ranks; identical at N = 1, 2, 4, 8 by construction of the log), the same hash from an
           independent vectorised torch restatement of the Counter fold over the full table, and a 4096-aggregate sample
           checked against the CPU oracle.
-  configs every other BASELINE.json config (N = 1 only): configs[0] BankAccount, configs[3] Zipf / variable records at full
-          size, configs[4] streaming micro-batches — each with its own parity check.
+  configs every other BASELINE.json config (N = 1 only): configs[0] BankAccount, configs[3] Zipf / variable records (sized for
+          80 GB), configs[4] streaming micro-batches — each with its own parity check.
 
 `--impl reference` times the reference's CPU implementation of the path instead (the oracle port: the reference is Scala/JVM
 and cannot be built in this image), rank 0 only.
@@ -45,11 +48,11 @@ N_AGG = 1 << 20
 EVENTS_PER_AGG = 32
 STATE_BYTES = 16
 METRIC = "events/sec replayed (segmented per-aggregate event fold)"
-WORKLOAD = "configs[1]: 1,048,576 aggregates x 32 fixed-width 64-B events, single B200 segmented fold (per GPU)"
+WORKLOAD = "configs[1]: 1,048,576 aggregates x 32 fixed-width 64-B events, single H100 segmented fold (per GPU)"
 ROUTED_N_GLOBAL = 10_000_000     # configs[2]: 10 M aggregates x 100 events, hash-partitioned, one exchange
 ROUTED_EPA = 100
 ROUTED_SEED = 3
-NVLINK_PEAK_GBS = 770.0          # measured peer copy per direction per GPU on this pool (B200_PROFILING.md)
+NVLINK_PEAK_GBS = 450.0          # H100 SXM data sheet: NVLink 4 at 900 GB/s both directions together (not measured here)
 M64 = (1 << 64) - 1
 
 
@@ -65,7 +68,7 @@ def measured_peak_gbs() -> tuple[float, str]:
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not a measured peak"
 
 
 class ClockSampler:
@@ -87,6 +90,23 @@ class ClockSampler:
             self.max_mhz = int(pynvml.nvmlDeviceGetMaxClockInfo(self.h, pynvml.NVML_CLOCK_SM))
         except Exception:  # noqa: BLE001
             self.nv = None
+        self.power_limit_w = self._power_limit_w()
+
+    def _power_limit_w(self):
+        """The card's power limit: absolute numbers are only comparable at the same limit (a capped card clocks down)."""
+        try:
+            if self.nv is not None:
+                return self.nv.nvmlDeviceGetPowerManagementLimit(self.h) / 1000.0
+        except Exception:  # noqa: BLE001
+            pass
+        try:
+            import subprocess
+
+            r = subprocess.run(["nvidia-smi", f"--id={self.index}", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                               capture_output=True, text=True, timeout=20)
+            return float(r.stdout.strip().splitlines()[0])
+        except Exception:  # noqa: BLE001
+            return None
 
     def _run(self):
         nv = self.nv
@@ -119,10 +139,10 @@ class ClockSampler:
         if self._t is not None:
             self._t.join(timeout=2)
         if not self.samples:
-            return {"sm_mhz": None, "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons), "samples": 0}
+            return {"sm_mhz": None, "sm_max_mhz": self.max_mhz, "power_limit_w": self.power_limit_w, "reasons": sorted(self.reasons), "samples": 0}
         mhz = [m for m, _ in self.samples]
-        return {"sm_mhz": int(statistics.median(mhz)), "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons),
-                "samples": len(mhz)}
+        return {"sm_mhz": int(statistics.median(mhz)), "sm_max_mhz": self.max_mhz, "power_limit_w": self.power_limit_w,
+                "reasons": sorted(self.reasons), "samples": len(mhz)}
 
 
 # ---------------------------------------------------------------------------------------------------- CPU legs
@@ -422,7 +442,8 @@ def config0_bank(dev, peak):
 
 
 def config3_zipf(dev, peak, scale: float):
-    """configs[3]: Zipf(1.1) keys, 10 M aggregates, 3.2e8 events, payloads 32-512 B (variable records, ~95 GB) on one B200."""
+    """configs[3]: Zipf(1.1) keys, 10 M aggregates, 1.6e8 events, payloads 32-512 B (variable records, ~47 GB) on one H100.
+    (3.2e8 events would make a ~95 GB log, more than an 80 GB H100 holds; the aggregate count and key skew stay.)"""
     import numpy as np
     import torch
 
@@ -431,12 +452,14 @@ def config3_zipf(dev, peak, scale: float):
     from surge_b200 import native as N
     from surge_b200 import programs as P
 
-    n_keys, n_events = int(10_000_000 * scale), int(320_000_000 * scale)
+    n_keys, n_events = int(10_000_000 * scale), int(160_000_000 * scale)
     gen = torch.Generator(device=dev)
     gen.manual_seed(4)
-    w = 1.0 / torch.pow(torch.arange(1, n_keys + 1, device=dev, dtype=torch.float64), 1.1)
+    # the CDF is summed on the host: a float64 cumsum on the device is not bitwise reproducible, and a last-bit change moves
+    # keys between aggregates, i.e. changes the log from run to run
+    w = 1.0 / torch.pow(torch.arange(1, n_keys + 1, dtype=torch.float64), 1.1)
     cdf = torch.cumsum(w, 0)
-    cdf /= cdf[-1].clone()
+    cdf = (cdf / cdf[-1]).to(dev)
     counts = torch.zeros(n_keys, dtype=torch.int64, device=dev)
     step = 40_000_000
     for lo in range(0, n_events, step):   # inverse-CDF sampling, in slices (temporaries stay small)
@@ -472,7 +495,7 @@ def config3_zipf(dev, peak, scale: float):
     torch.cuda.synchronize()
     hot = int(counts.max())
     b_alg = total + 8 * (n_keys + 1) + 16 * n_keys + 8 * (n_events + 1)
-    out = {"workload": f"configs[3]{'' if scale == 1.0 else f' x {scale}'}: Zipf(1.1) keys, {n_keys} aggregates, {n_events} events, payloads 32-512 B, {total / 1e9:.1f} GB log, one B200",
+    out = {"workload": f"configs[3]{'' if scale == 1.0 else f' x {scale}'}: Zipf(1.1) keys, {n_keys} aggregates, {n_events} events, payloads 32-512 B, {total / 1e9:.1f} GB log, one H100",
            "hottest_key_share": hot / n_events, "algorithmic_bytes": b_alg}
     with ReplayEngine(0) as e:
         e.register_program(P.counter_program(N.REC_VAR16))
@@ -568,6 +591,8 @@ def main() -> None:
     ap.add_argument("--no-configs", action="store_true", help="skip configs[0], [3], [4] (N = 1)")
     ap.add_argument("--scale", type=float, default=1.0, help="shrink configs[2] and configs[3] (debugging on a busy box); 1.0 = the BASELINE sizes")
     ap.add_argument("--routed-iters", type=int, default=3)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the state table of the last timed step to DIR/states.npy (float64)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)
@@ -640,6 +665,11 @@ def main() -> None:
     launches = K * int(eng.stats().fold_launches)
     folded_events = int(eng.stats().n_events)
     assert folded_events == n_events, (folded_events, n_events)
+    if args.dump_outputs and rank == 0:
+        # the table the last timed step left (N_AGG x 4 int32 words; float64 holds every int32 exactly): 32 MiB
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        states = eng.states_tensor().view(torch.int32).cpu().numpy().astype(np.float64)
+        np.save(os.path.join(args.dump_outputs, "states.npy"), states)
 
     # ---- timed region 2 (e2e): host buffers through the C ABI, H2D + fold + D2H every step
     ke = args.e2e_steps or min(K, 20)
@@ -819,28 +849,19 @@ def main() -> None:
 
     if rank == 0:
         achieved = b_alg / (kernel_ms * 1e-3) / 1e9
-        traffic, traffic_src = None, None
-        for name in ("r02_fold_runs_traffic.json", "r01_fold_runs_traffic.json"):
-            tp = os.path.join(ROOT, "profiles", name)
-            if os.path.exists(tp):
-                try:
-                    traffic = json.load(open(tp))["dram_bytes_per_launch"]
-                    traffic_src = f"profiles/{name} (ncu --set full capture of the same kernel and shape; not re-measured in this run)"
-                    break
-                except Exception:  # noqa: BLE001
-                    traffic = None
         out = {
             "metric": METRIC, "value": value, "unit": "events/s", "n_gpus": world, "steps": K, "warmup": W,
             "ms_per_step": ms_total / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "i32", "data": "synthetic",
             "config": {"workload": WORKLOAD, "aggregates_per_gpu": N_AGG, "events_per_aggregate": EVENTS_PER_AGG,
                        "record_bytes": 64, "state_bytes": STATE_BYTES, "model": "Counter (scaladsl TestBoundedContext)",
-                       "l2": "inputs (2 GiB log per GPU) are 16x the 126 MB L2; no flush between iterations",
+                       "gpu": torch.cuda.get_device_name(dev), "power_limit_w": clocks["power_limit_w"],
+                       "l2": "inputs (2 GiB log per GPU) are 40x the 50 MB L2; no flush between iterations",
                        "sharding": "value: aggregates sharded across ranks, no data-path collective; the hash-partitioned configuration with "
                                    "its exchange (configs[2]) is the `routed` block (see DESIGN.md multi-GPU)"},
             "gpu_launches": launches,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "traffic_source": traffic_src, "algorithmic_bytes_per_launch": b_alg, "kernel": "fold_runs_kernel",
+                         "algorithmic_bytes_per_launch": b_alg, "kernel": "fold_runs_kernel",
                          "kernel_ms": kernel_ms, "peak_source": peak_src,
                          "pipelined_frac": (b_alg / (ms_total / K * 1e-3) / 1e9) / peak},
             # e2e: the events of the step enter as HOST bytes in the format the reference's topic holds (lz4 RecordBatch v2, what its

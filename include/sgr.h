@@ -1,5 +1,5 @@
 /*
- * sgr.h — C ABI of the B200 batched event-replay engine ("surge gpu replay").
+ * sgr.h — C ABI of the H100 batched event-replay engine ("surge gpu replay").
  *
  * This is the drop-in boundary for ONE path of UltimateSoftware/surge: rebuilding
  * aggregate state by folding each aggregate's ordered event log through the model's

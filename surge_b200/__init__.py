@@ -1,7 +1,7 @@
-"""surge_b200 — B200-native batched event-replay engine behind Surge's state-store boundary.
+"""surge_b200 — H100-native batched event-replay engine behind Surge's state-store boundary.
 
 Only what the hot path needs lives here:
-  csrc/        hand-written sm_100a CUDA kernels + the C ABI (include/sgr.h) -> lib/libsgr.so
+  csrc/        hand-written sm_90a CUDA kernels + the C ABI (include/sgr.h) -> lib/libsgr.so
   native.py    ctypes binding of the C ABI (fails loudly when the CUDA library is missing)
   formats.py   packed record / state layouts (the binary SurgeAggregateFormatting)
   programs.py  declarative fold programs for the reference's sample models

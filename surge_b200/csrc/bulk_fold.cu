@@ -1,4 +1,4 @@
-// bulk_fold.cu — sort-free fold of a LARGE arrival-order log (sm_100a): the K6 formulation of incremental.cu as two
+// bulk_fold.cu — sort-free fold of a LARGE arrival-order log (sm_90a): the K6 formulation of incremental.cu as two
 // plain launches, for logs much larger than the state table (a whole Kafka partition log, or what arrives from the
 // other ranks after routing).
 //
@@ -47,14 +47,12 @@ __device__ __forceinline__ uint4 ldg_stream(const void* p, uint64_t pol) {
   else asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
   return v;
 }
-// one 32-byte sector in one request (LDG.256): the two halves of a record's first sector never travel twice — matters when
-// the records are read from a peer over NVLink
+// one 32-byte sector as two adjacent 16-byte loads (128 bits is the widest global load sm_90 has); both are issued
+// back to back, so a warp's requests for the sector coalesce into the same L2 transaction
 template <bool HINTS>
 __device__ __forceinline__ void ldg_stream32(const void* p, uint64_t pol, uint4& a, uint4& b) {
-  if (HINTS) asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8], %9;"
-                          : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(p), "l"(pol));
-  else asm volatile("ld.global.nc.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                    : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(p));
+  a = ldg_stream<HINTS>(p, pol);
+  b = ldg_stream<HINTS>(static_cast<const uint8_t*>(p) + 16, pol);
 }
 template <bool HINTS>
 __device__ __forceinline__ void red_add_u32(uint32_t* p, uint32_t v, uint64_t pol) {

@@ -22,7 +22,7 @@ struct BulkLayout {
                              // that would mark the slot as touched)
 };
 
-// measurement knobs (sgr_set_option "bulk_unroll" / "bulk_hints" / "bulk_blocks_per_sm"); the defaults are the measured best
+// measurement knobs (sgr_set_option "bulk_unroll" / "bulk_hints" / "bulk_blocks_per_sm"; scripts/bulk_ab.py sweeps them)
 struct BulkTuning { int unroll = 4; int hints = 1; int blocks_per_sm = 8; };
 BulkTuning& bulk_tuning();
 cudaError_t bulk_preload_kernels();   // force the (lazy) load of every kernel of this file

@@ -1,4 +1,4 @@
-// dingest_kernels.cu — Kafka RecordBatch v2 decode ON THE DEVICE (sm_100a): the step right before the fold (SURVEY §8 f1).
+// dingest_kernels.cu — Kafka RecordBatch v2 decode ON THE DEVICE (sm_90a): the step right before the fold (SURVEY §8 f1).
 //
 // What feeds the store today is a read_committed consumer of a topic whose producer compresses with lz4
 // (modules/common/src/main/scala/surge/kafka/streams/SurgeStateStoreConsumer.scala:38; modules/common/src/main/resources/
@@ -23,7 +23,7 @@
 // byte work — no tensor cores anywhere.
 //
 // Two generations live here. The first (dg_crc_size_kernel, dg_decode_walk_kernel; SGR_DINGEST_V1=1 selects it) walks the bytes
-// through global memory and spends ~10 ms on the decode of ANY number of batches: ~10 dependent memory round trips per lz4
+// through global memory and spends the same time on the decode of ANY number of batches: ~10 dependent memory round trips per lz4
 // sequence, and in a warp of 32 independent batches some lane misses at every step. The second (the *_fast kernels, default)
 // reads its input through a per-thread cp.async ring in shared memory and keeps memory current behind an 8-byte output
 // accumulator (lz4_fast.h) — one dependent access per sequence — and claims each batch's arena slot with an atomicAdd in the size pass, so that CRC -> decode -> parse of a group of batches is one chain of launches with
@@ -62,9 +62,8 @@ cudaError_t ensure_crc_tables() {
   return e;
 }
 
-// A lone thread walking a byte stream pays one global access (hundreds of ns) per byte it looks at: the profile of the first
-// version (profiles/r02_dingest_launches.csv) shows the decode kernel taking ~10 ms whatever the number of batches — it is the
-// serial latency of ONE batch. ByteWin keeps the aligned 16-byte chunk around the cursor in registers: one load per 16 bytes of
+// A lone thread walking a byte stream pays one global access (hundreds of ns) per byte it looks at: a decode kernel that does
+// so takes the same time whatever the number of batches — it is the serial latency of ONE batch. ByteWin keeps the aligned 16-byte chunk around the cursor in registers: one load per 16 bytes of
 // tokens, lengths, offsets and varints instead of one per byte. (Buffers are padded so the chunk load never leaves them.)
 struct ByteWin {
   const uint8_t* chunk;
@@ -301,7 +300,7 @@ template <int WARP>
 __global__ void __launch_bounds__(kThreads) dg_decode_walk_kernel(const uint8_t* __restrict__ wire, uint8_t* __restrict__ arena, DgBatch* __restrict__ batches,
                                                                   uint32_t n, uint32_t index_base, uint32_t* __restrict__ rec_off, uint32_t* __restrict__ rec_batch) {
   // WARP == 1: one warp per batch (cooperative copies); 0: one thread per batch (word-wise copies, 32x more batches in flight —
-  // measured faster on 16 KiB producer batches, where the token chain, not the copy width, is the latency)
+  // for 16 KiB producer batches, where the token chain, not the copy width, is the latency)
   const uint32_t i = WARP ? (blockIdx.x * kThreads + threadIdx.x) >> 5 : blockIdx.x * kThreads + threadIdx.x;
   const uint32_t lane = WARP ? threadIdx.x & 31 : 0;
   if (i >= n) return;
@@ -697,7 +696,7 @@ __global__ void dg_copy16_kernel(const uint4* __restrict__ src, uint4* __restric
 cudaError_t dg_copy_from_mapped_host(const void* host_mapped, void* dst, uint64_t nbytes, cudaStream_t st) {
   if (!nbytes) return cudaSuccess;
   const uint64_t n16 = (nbytes + 15) / 16;
-  const uint32_t blocks = (uint32_t)((n16 + 255) / 256 < 592 ? (n16 + 255) / 256 : 592);
+  const uint32_t blocks = (uint32_t)((n16 + 255) / 256 < 528 ? (n16 + 255) / 256 : 528);   // 4 CTAs on each of H100's 132 SMs
   dg_copy16_kernel<<<blocks, 256, 0, st>>>((const uint4*)host_mapped, (uint4*)dst, n16);
   return cudaGetLastError();
 }

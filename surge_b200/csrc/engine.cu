@@ -99,10 +99,10 @@ struct sgr_engine {
                                   // 2 force runs (fold_runs.cu), 3 record-per-lane rows (fold_rows.cu)
   int64_t opt_variant = -1;
   int64_t opt_long_threshold = 0;
-  int64_t opt_var_stages = 1;     // measured: 1 stage x 16 warps/SM (5.0 TB/s) beats 2 x 9 (4.4) and 3 x 6 (3.2) on configs[3]
+  int64_t opt_var_stages = 1;     // 1 stage leaves shared memory for the most resident warps per SM (2 or 3 trade warps for depth)
   int64_t opt_var_stage_bytes = 12288;  // smem bytes staged per 32-record step of the variable-record kernel
   int64_t opt_replay_budget = 1ll << 24;  // K6: in-kernel replay of throwing slots only while n_err * n stays below this
-                                          // (measured ~15 ps per slot-record; beyond it one group-by of the batch is cheaper)
+                                          // (beyond it one group-by of the batch is cheaper)
   int64_t opt_force_route = 0;    // profiling aid: run K4 even on a single rank
   int64_t opt_incremental = 0;    // 0 auto (sort-free K6 when the program allows), 1 force the sort-based path
   int64_t opt_max_record_bytes = 528;
@@ -254,7 +254,7 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
                      uint64_t n_seg, bool use_prior, uint64_t event_bytes, bool aligned64, uint64_t log_begin, uint64_t log_end) {
   const uint8_t* states_in = use_prior ? (const uint8_t*)e->states.p : nullptr;
   // 64-byte states: the transformer scan moves 16 registers per lane per step and the lane-per-aggregate TMA kernel is
-  // faster on balanced logs (measured 2.47 vs 1.76 TB/s on BankAccount); the record-parallel kernel is taken when a
+  // faster on balanced logs (BankAccount); the record-parallel kernel is taken when a
   // long segment would otherwise serialise one lane
   const bool wide_balanced = e->row_prog.user_words == 14 && e->opt_kernel == 0 && d_offsets == e->d_offsets && e->max_seg_bytes <= (256u << 10);
   bool use_rows = e->row_ok && !wide_balanced && e->program.record_kind == SGR_REC_FIXED64 && aligned64 && e->opt_kernel != 1 && n_seg < (1ull << 32) && n_seg > 0;
@@ -467,8 +467,8 @@ int32_t sgr_create(const sgr_config* cfg, sgr_engine** out) {
   cudaDeviceProp prop;
   if ((ce = cudaGetDeviceProperties(&prop, dev)) != cudaSuccess)
     return fail(nullptr, SGR_ERR_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(ce));
-  if (prop.major != 10)
-    return fail(nullptr, SGR_ERR_NO_DEVICE, "device %d is sm_%d%d; kernels are built for sm_100a only", dev, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(nullptr, SGR_ERR_NO_DEVICE, "device %d is sm_%d%d; kernels are built for sm_90a only", dev, prop.major, prop.minor);
   std::unique_ptr<sgr_engine> e(new sgr_engine());
   e->device = dev;
   e->num_sms = prop.multiProcessorCount;

@@ -1,4 +1,4 @@
-// fold_kernels.cu — K1/K2: CSR segmented left fold of packed event records (sm_100a).
+// fold_kernels.cu — K1/K2: CSR segmented left fold of packed event records (sm_90a).
 //
 // Replaces, for every aggregate at once, the per-actor
 //   events.foldLeft(state)((stateAccum, evt) => handleEvent(stateAccum, evt))
@@ -439,8 +439,8 @@ cudaError_t launch_fold_stream(const FoldArgs& args, const DevProgram& prog, int
     return launch_variant(variant, args, prog, num_sms, stream, info);
   }
   if (explicit_variant) return launch_variant(variant, args, prog, num_sms, stream, info);
-  // fixed records: more warps per SM win (measured on configs[1]: 256 thr 3.0 TB/s, 192 thr 2.3, 128 thr 2.1); take the
-  // widest configuration whose rings + state tables fit in shared memory
+  // fixed records: more warps per SM hide more of the memory latency; take the widest configuration whose rings + state
+  // tables fit in shared memory
   const int order[] = {1, 2, 0, 3};
   cudaError_t e = cudaErrorInvalidConfiguration;
   for (int v : order) {

@@ -1,4 +1,4 @@
-// fold_rows.cu — K1/K3: record-parallel segmented fold of fixed 64-byte records (sm_100a).
+// fold_rows.cu — K1/K3: record-parallel segmented fold of fixed 64-byte records (sm_90a).
 //
 // Same contract as fold_kernels.cu (events.foldLeft(state)(handleEvent) per aggregate,
 // modules/command-engine/scaladsl/src/main/scala/surge/scaladsl/command/CommandModels.scala:25-28),
@@ -140,6 +140,14 @@ __global__ void __launch_bounds__(kRowThreads, 3) fold_rows_kernel(const __grid_
   const uint64_t base = a.log_begin;
   const uint64_t total_bytes = a.log_end - base;
   const uint64_t total_steps = (total_bytes + 2047) / 2048;
+  if (total_steps == 0) {  // every segment is empty: no warp has a span, so the grid writes each state (prior or None) itself
+    Xf<W> none; none.m = 0;
+#pragma unroll
+    for (int w = 0; w < W; ++w) none.v[w] = 0;
+    for (uint64_t s = (uint64_t)blockIdx.x * kRowThreads + threadIdx.x; s < n_seg; s += (uint64_t)gridDim.x * kRowThreads)
+      finish_segment<W>(a, s, false, none, 0u);
+    return;
+  }
   const uint64_t spw = (total_steps + n_warps - 1) / n_warps;  // steps per warp
   uint64_t step = gw * spw;
   const uint64_t step_end = step + spw < total_steps ? step + spw : total_steps;

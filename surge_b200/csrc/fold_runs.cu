@@ -1,4 +1,4 @@
-// fold_runs.cu — K1/K3 (primary): segmented fold of fixed 64-byte records, lane-runs + warp scan (sm_100a).
+// fold_runs.cu — K1/K3 (primary): segmented fold of fixed 64-byte records, lane-runs + warp scan (sm_90a).
 //
 // Contract: for every aggregate, events.foldLeft(state)(handleEvent)
 // (modules/command-engine/scaladsl/src/main/scala/surge/scaladsl/command/CommandModels.scala:25-28) with the

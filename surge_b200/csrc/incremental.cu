@@ -1,4 +1,4 @@
-// incremental.cu — K6: append a micro-batch (arrival order) to the live state table without sorting (sm_100a).
+// incremental.cu — K6: append a micro-batch (arrival order) to the live state table without sorting (sm_90a).
 //
 // Contract: for every aggregate touched by the batch, ApplyEvents(id, its events in arrival order) on the live
 // actor state — PersistentActor.doApplyEvent, modules/command-engine/core/src/main/scala/surge/internal/persistence/

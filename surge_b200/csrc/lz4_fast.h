@@ -4,8 +4,7 @@
 // topics): a serial chain, so a batch is a thread and the parallelism is the tens of thousands of batches of a poll. In a warp
 // of 32 independent batches every memory access of the chain costs the WHOLE warp a round trip: some lane always misses, and the
 // scoreboard that guards a load's destination register is per warp, not per lane — a register "prefetch" by one lane stalls the
-// next instruction of any other lane that touches the same register name (measured: profiles/r02b_dingest_fast_v1_ncu.txt, 65 %
-// of all stall samples on three window-shift MOVs). So:
+// next instruction of any other lane that touches the same register name. So:
 //   * input   comes through a policy object. On the device it is a per-thread ring of eight 16-byte chunks in SHARED memory
 //             filled by cp.async six chunks ahead (RingIn, dingest_kernels.cu): asynchronous copies have no destination register,
 //             and tokens, lengths, offsets and literals are cut out of two shared-memory words. On the host (HostIn) it reads

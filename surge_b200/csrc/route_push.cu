@@ -1,4 +1,4 @@
-// route_push.cu — pipelined route + exchange + fold over peer memory (sm_100a, NVLink 5 / NVSwitch).
+// route_push.cu — pipelined route + exchange + fold over peer memory (sm_90a, NVLink 4 / NVSwitch).
 //
 // The reference shards by key and lets the BROKER shuffle: aggregateId -> partitionForKey
 // (modules/common/src/main/scala/surge/kafka/KafkaPartitioner.scala:7-9) -> owner node
@@ -266,20 +266,22 @@ __global__ void __launch_bounds__(kPushThreads) route_push_kernel(const __grid_c
 }
 
 // The same partition WITHOUT staging the records in shared memory: every thread keeps ITS records in registers.
-//   load    2 x LDG.256 per record, all issued up front (each 32-byte sector requested exactly once)
+//   load    4 x LDG.128 per record, all issued up front (each 32-byte sector as two adjacent halves)
 //   place   owner | local index from the record's aggregate index, stable rank by ballots, per-owner counts, look-back
-//   store   2 x STG.256 per record at its position in the owner's region (agg rewritten to the owner's local index)
+//   store   4 x STG.128 per record at its position in the owner's region (agg rewritten to the owner's local index)
 // One read of every byte, one write, 3 barriers, a few hundred bytes of shared memory: eight CTAs per SM, and the DRAM latency
 // of the records overlaps the latency chain of the placement (route lookup -> counts -> look-back). Consecutive records of one
 // owner land on consecutive positions, so L2 merges the 64-byte writes into full lines. This is the kernel of the PULL mode,
 // where every region is in this rank's own HBM; contiguous per-owner runs (route_push_kernel) only pay for stores over NVLink.
+// 32 bytes as two 16-byte accesses: 128 bits is the widest global load / store sm_90 has
 __device__ __forceinline__ void ldg256(const void* p, uint4& a, uint4& b) {
-  asm volatile("ld.global.nc.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(p));
+  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w) : "l"(p));
+  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(static_cast<const uint8_t*>(p) + 16));
 }
 __device__ __forceinline__ void stg256(void* p, const uint4& a, const uint4& b) {
-  asm volatile("st.global.v8.u32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b.x), "r"(b.y),
-               "r"(b.z), "r"(b.w) : "memory");
+  asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w) : "memory");
+  asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(static_cast<uint8_t*>(p) + 16), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w) : "memory");
 }
 __device__ __forceinline__ uint32_t word_of(const uint4& a, const uint4& b, const uint4& c, const uint4& d, uint32_t w) {
   // value selects only: taking a reference to one of the four would push the records to local memory

@@ -18,7 +18,7 @@ namespace sgr {
 //                the regions are written over NVLink (pull == 0)
 // "push_fold_blocks_per_sm": grid cap of the fold launches beside the partition kernel; 0 = one tile per CTA (the low-priority fold
 //                            then fills what the high-priority partition leaves free)
-struct PushTuning { int tile = 512; int pull = 1; int fold_blocks_per_sm = 2; int staged = -1; };   // measured best at N = 2, 4 (scripts/push_ab.py)
+struct PushTuning { int tile = 512; int pull = 1; int fold_blocks_per_sm = 2; int staged = -1; };   // scripts/push_ab.py sweeps them
 PushTuning& push_tuning();
 
 struct PushFoldArgs {

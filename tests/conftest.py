@@ -13,7 +13,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run by the driver with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); select with -m gpu")
 
 
 def _has_gpu() -> bool:
