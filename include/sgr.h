@@ -494,8 +494,7 @@ int32_t sgr_dingest_reset(sgr_dingest* g);
 /* host-clock milliseconds of the last sgr_dingest_fold: [0] wait for the copies and for every group's chain (CRC, lz4 decode +
  * record walk, record parse + id interning — launched by the submits behind the copies), [1] a repeat from an exact arena
  * layout when the 3x estimate was too small (normally 0), [2] unused, [3] launch of the new ids' gather and download,
- * [4] table growth + fold, with the ids handed to the key table by a helper thread meanwhile, [5] the whole call.
- * (SGR_DINGEST_V1=1, the first generation: [0] copies + CRC / size pass, [1] decode + walk, [2] parse + intern.) */
+ * [4] table growth + fold, with the ids handed to the key table by a helper thread meanwhile, [5] the whole call. */
 int32_t sgr_dingest_last_timing(sgr_dingest* g, float* ms8);
 int32_t sgr_dingest_get_stats(sgr_dingest* g, sgr_ingest_stats* out);
 

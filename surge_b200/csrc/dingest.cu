@@ -17,8 +17,6 @@
 //          then do the partitions' positions advance. All or nothing.
 // The arena the batches decompress into is sized from the wire bytes (3x); if a poll compresses better than that the claims
 // overflow, the flag comes back with the verdicts and the poll is decoded again from an exact host-side layout.
-// SGR_DINGEST_V1=1 selects the first generation (memory-walking kernels, arena laid out on the host between two
-// synchronisations) for A/B runs.
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -112,12 +110,10 @@ struct sgr_dingest {
   cudaStream_t copy_stream = nullptr;       // H2D copies of the wire bytes: they overlap the decode of earlier submissions
   // device scratch
   KeepBuf arena, d_batches;
-  uint64_t d_batches_used = 0;              // descriptors uploaded by the submissions of this poll
-  uint64_t crc_launched = 0;                // ... of which the CRC + size pass (v1) / the whole chain (default) has been launched
   KeepBuf rec_off, rec_batch, out;          // per record slot; they keep their content when a later group needs them larger
   DevBuf key_offs_dev, key_bytes_dev;
   // chains of launches per group of batches
-  bool v1 = false;                          // SGR_DINGEST_V1
+  uint64_t launched_batches = 0;            // batches of this poll whose chain has been launched
   uint32_t group_batches = 8192;            // SGR_DINGEST_GROUP
   static constexpr int kGroupStreams = 8;
   cudaStream_t gstream[kGroupStreams] = {};
@@ -137,9 +133,9 @@ struct sgr_dingest {
   cudaEvent_t keys_landed = nullptr;
   uint64_t generation = 0;                  // bumped by sgr_dingest_reset: a new dictionary is a new owner of the engine's key table
   void* h_ctl = nullptr;                    // page-locked landing area
-  bool timing_syncs = false;                // SGR_DINGEST_TIMING=1: an extra synchronisation separates decode from parse in ms[]
-  float ms[8] = {};                         // last fold: [0] wait for H2D + crc/size [1] decode + walk [2] parse + intern [3] keys to host
-                                            //            [4] table growth + fold [5] total
+  bool timing_syncs = false;                // SGR_DINGEST_TIMING=1: record the per-group device timeline (tl_events)
+  float ms[8] = {};                         // last fold: [0] wait for the copies and every chain [1] exact-layout repeat [2] unused
+                                            //            [3] keys to host [4] table growth + fold [5] total
 };
 
 namespace {
@@ -193,8 +189,8 @@ cudaError_t reset_poll_counters(sgr_dingest* g) {
 }
 
 void clear_poll(sgr_dingest* g) {
-  g->wire.used = 0; g->batches.clear(); g->n_record_slots = 0; g->poll = sgr_ingest_stats{}; g->subs.clear(); g->d_batches_used = 0; g->crc_launched = 0;
-  g->n_groups = 0; g->launched_records = 0;
+  g->wire.used = 0; g->batches.clear(); g->n_record_slots = 0; g->poll = sgr_ingest_stats{}; g->subs.clear();
+  g->launched_batches = 0; g->n_groups = 0; g->launched_records = 0;
 }
 
 void discard_poll(sgr_dingest* g) {
@@ -229,10 +225,10 @@ cudaError_t set_arena_capacity(sgr_dingest* g) {
   return cudaMemcpy((unsigned long long*)g->ctl.p + 9, &cap, 8, cudaMemcpyHostToDevice);
 }
 
-// Enqueue descriptors-up -> crc_size (+ arena claim) -> decode_walk -> parse for the batches [crc_launched, batch_end) — record
-// slots [launched_records, rec_end) — behind `landed` (the copy of the last fetch that contributes to the group).
+// Enqueue descriptors-up -> crc_size (+ arena claim) -> decode_walk -> parse for the batches [launched_batches, batch_end) —
+// record slots [launched_records, rec_end) — behind `landed` (the copy of the last fetch that contributes to the group).
 int32_t launch_group(sgr_dingest* g, uint64_t batch_end, uint64_t rec_end, cudaEvent_t landed) {
-  const uint64_t b0 = g->crc_launched, nb = batch_end - b0;
+  const uint64_t b0 = g->launched_batches, nb = batch_end - b0;
   if (!nb) return SGR_OK;
   const uint64_t r0 = g->launched_records;
   DG_TRY(g, grow_keeping(g, g->d_batches, b0 * sizeof(DgBatch), batch_end * sizeof(DgBatch) + 64));
@@ -274,7 +270,7 @@ int32_t launch_group(sgr_dingest* g, uint64_t batch_end, uint64_t rec_end, cudaE
   if (tl) DG_TRY(g, cudaEventRecord(tl[3], s));
   DG_TRY(g, cudaEventRecord(g->group_events[g->n_groups], s));
   ++g->n_groups;
-  g->crc_launched = batch_end; g->launched_records = rec_end;
+  g->launched_batches = batch_end; g->launched_records = rec_end;
   return SGR_OK;
 }
 }  // namespace
@@ -289,7 +285,6 @@ int32_t sgr_dingest_create(sgr_engine* e, uint64_t max_keys, uint64_t max_id_byt
   sgr_dingest* g = new sgr_dingest();
   g->eng = e; g->stream = (cudaStream_t)st;
   g->timing_syncs = getenv("SGR_DINGEST_TIMING") != nullptr;
-  g->v1 = getenv("SGR_DINGEST_V1") != nullptr;
   if (const char* gb = getenv("SGR_DINGEST_GROUP")) { const long v = atol(gb); if (v >= 64 && v <= (1l << 24)) g->group_batches = (uint32_t)v; }
   if (dg_prepare() != cudaSuccess) { delete g; return SGR_ERR_CUDA; }
   if (cudaStreamCreateWithFlags(&g->copy_stream, cudaStreamNonBlocking) != cudaSuccess) { delete g; return SGR_ERR_CUDA; }
@@ -458,30 +453,10 @@ int32_t sgr_dingest_submit(sgr_dingest* g, int32_t partition, const void* data, 
       if (!g->batches.reserve(g->batches.n + add.size())) return dfail(g, SGR_ERR_OOM, "page-locked descriptor array");
     }
     memcpy(g->batches.p + g->batches.n, add.data(), add.size() * sizeof(DgBatch));
-    const DgBatch* src_desc = g->batches.p + g->batches.n;   // (the first generation uploads them from here right away)
-    (void)src_desc;
     g->batches.n += add.size();
-    if (!g->v1) {
-      g->d_batches_used += add.size();
-      if (g->d_batches_used - g->crc_launched >= g->group_batches) {
-        const int32_t rc = launch_group(g, g->d_batches_used, g->n_record_slots + slots, sub.copied);
-        if (rc) { discard_poll(g); return rc; }
-      }
-    } else {
-      // descriptors go up right away; the CRC + lz4 size pass is launched once >= 32 k batches are waiting (one thread per batch:
-      // a small launch takes as long as a large one, it is the serial walk of ONE batch) — it then runs while the host walks
-      // the next fetches and the copy engine brings them in; sgr_dingest_fold launches the remainder
-      if ((g->d_batches_used + add.size()) * sizeof(DgBatch) > g->d_batches.b.cap) DG_TRY(g, cudaStreamSynchronize(g->stream));
-      g->d_batches.used = g->d_batches_used * sizeof(DgBatch);
-      DG_TRY(g, g->d_batches.ensure(add.size() * sizeof(DgBatch) + 64, g->stream));
-      DgBatch* db = (DgBatch*)g->d_batches.b.p + g->d_batches_used;
-      DG_TRY(g, cudaMemcpyAsync(db, src_desc, add.size() * sizeof(DgBatch), cudaMemcpyHostToDevice, g->stream));
-      g->d_batches_used += add.size();
-      if (g->d_batches_used - g->crc_launched >= 32768) {
-        DG_TRY(g, cudaStreamWaitEvent(g->stream, sub.copied, 0));
-        DG_TRY(g, dg_launch_crc_size((const uint8_t*)g->wire.b.p, (DgBatch*)g->d_batches.b.p + g->crc_launched, (uint32_t)(g->d_batches_used - g->crc_launched), g->stream));
-        g->crc_launched = g->d_batches_used;
-      }
+    if (g->batches.n - g->launched_batches >= g->group_batches) {
+      const int32_t rc = launch_group(g, g->batches.n, g->n_record_slots + slots, sub.copied);
+      if (rc) { discard_poll(g); return rc; }
     }
   }
   g->n_record_slots += slots;
@@ -508,89 +483,54 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
   memset(g->ms, 0, sizeof g->ms);
   if (nb) {
     DgParse p = parse_args(g);
-    if (!g->v1) {
-      // ---- chains: launch the remainder, wait for every group, bring the verdicts back
-      { const int32_t rc = launch_group(g, nb, nrec, g->subs.back().copied); if (rc) { discard_poll(g); return rc; } }
-      for (uint32_t k = 0; k < g->n_groups; ++k) DG_TRY(g, cudaStreamWaitEvent(g->stream, g->group_events[k], 0));
-      DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.b.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
-      DG_TRY(g, cudaMemcpyAsync(h, g->ctl.p, 128, cudaMemcpyDeviceToHost, g->stream));
-      DG_TRY(g, cudaStreamSynchronize(g->stream));
-      lap(0);
-      if (g->timing_syncs && g->tl_origin) {
-        for (uint32_t k = 0; k < g->n_groups; ++k) {
-          float t[4] = {0, 0, 0, 0};
-          for (int j = 0; j < 4; ++j) cudaEventElapsedTime(&t[j], g->tl_origin, g->tl_events[4 * (size_t)k + j]);
-          fprintf(stderr, "[dingest] group %u: landed %.2f  crc+size %.2f  decode+walk %.2f  parse %.2f ms\n", k, t[0], t[1], t[2], t[3]);
-        }
+    // ---- chains: launch the remainder, wait for every group, bring the verdicts back
+    { const int32_t rc = launch_group(g, nb, nrec, g->subs.back().copied); if (rc) { discard_poll(g); return rc; } }
+    for (uint32_t k = 0; k < g->n_groups; ++k) DG_TRY(g, cudaStreamWaitEvent(g->stream, g->group_events[k], 0));
+    DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.b.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
+    DG_TRY(g, cudaMemcpyAsync(h, g->ctl.p, 128, cudaMemcpyDeviceToHost, g->stream));
+    DG_TRY(g, cudaStreamSynchronize(g->stream));
+    lap(0);
+    if (g->timing_syncs && g->tl_origin) {
+      for (uint32_t k = 0; k < g->n_groups; ++k) {
+        float t[4] = {0, 0, 0, 0};
+        for (int j = 0; j < 4; ++j) cudaEventElapsedTime(&t[j], g->tl_origin, g->tl_events[4 * (size_t)k + j]);
+        fprintf(stderr, "[dingest] group %u: landed %.2f  crc+size %.2f  decode+walk %.2f  parse %.2f ms\n", k, t[0], t[1], t[2], t[3]);
       }
-      if (h[10]) {
-        // the arena claims overflowed (the poll compresses better than 3x): lay the arena out exactly and decode + parse again.
-        // Ids the first attempt interned stay (an id is an id); its records are overwritten slot for slot.
-        // (exact sizes first: the claim mode never measured them)
-        DG_TRY(g, dg_launch_crc_size_fast((const uint8_t*)g->wire.b.p, (DgBatch*)g->d_batches.b.p, nb, nullptr, g->stream));
-        DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.b.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
-        DG_TRY(g, cudaStreamSynchronize(g->stream));
-        uint64_t need = 0;
-        for (uint32_t i = 0; i < nb; ++i) {
-          DgBatch& b = g->batches[i];
-          if (b.err == DG_ARENA_FULL) b.err = DG_OK;
-          if (b.err) { const int32_t rc = dfail(g, SGR_ERR_INVALID, "offset %lld: %s", (long long)b.base_offset, dg_err_text(b.err)); discard_poll(g); return rc; }
-          b.err_record = 0;
-          if (b.codec == 3) { b.arena_off = need; need += ((uint64_t)b.dsize + 15) & ~15ull; }
-        }
-        g->arena.used = 0;
-        DG_TRY(g, g->arena.ensure(need + 512, g->stream));
-        DG_TRY(g, set_arena_capacity(g));
-        p = parse_args(g);
-        h[2] = h[3] = h[4] = h[5] = h[6] = 0; h[8] = need; h[10] = 0;
-        DG_TRY(g, cudaMemcpyAsync((unsigned long long*)g->ctl.p + 2, h + 2, 5 * 8, cudaMemcpyHostToDevice, g->stream));
-        DG_TRY(g, cudaMemcpyAsync((unsigned long long*)g->ctl.p + 8, h + 8, 8, cudaMemcpyHostToDevice, g->stream));
-        DG_TRY(g, cudaMemcpyAsync((unsigned long long*)g->ctl.p + 10, h + 10, 8, cudaMemcpyHostToDevice, g->stream));
-        DG_TRY(g, cudaMemsetAsync(g->rec_batch.b.p, 0xff, (size_t)nrec * 4 + 4, g->stream));
-        DG_TRY(g, cudaMemcpyAsync(g->d_batches.b.p, g->batches.data(), (size_t)nb * sizeof(DgBatch), cudaMemcpyHostToDevice, g->stream));
-        DG_TRY(g, dg_launch_decode_walk_fast((const uint8_t*)g->wire.b.p, (uint8_t*)g->arena.b.p, (DgBatch*)g->d_batches.b.p, nb, 0, (uint32_t*)g->rec_off.b.p, (uint32_t*)g->rec_batch.b.p, nullptr, g->stream));
-        p.n_batches = nb; p.rec_begin = 0; p.n_records = nrec;
-        DG_TRY(g, dg_launch_parse(p, g->stream));
-        DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.b.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
-        DG_TRY(g, cudaMemcpyAsync(h, g->ctl.p, 128, cudaMemcpyDeviceToHost, g->stream));
-        DG_TRY(g, cudaStreamSynchronize(g->stream));
-        lap(1);
-      }
-      for (uint32_t i = 0; i < nb; ++i) if (g->batches[i].codec == 3 && !g->batches[i].err) st.n_decompressed_bytes += g->batches[i].dsize;
-    } else {
-      DG_TRY(g, g->rec_off.b.reserve((size_t)nrec * 4 + 64));
-      DG_TRY(g, g->rec_batch.b.reserve((size_t)nrec * 4 + 64));
-      DG_TRY(g, g->out.b.reserve((size_t)nrec * 64 + 64));
-      p = parse_args(g);
-      DG_TRY(g, cudaMemsetAsync(g->rec_batch.b.p, 0xff, (size_t)nrec * 4 + 4, g->stream));
-      p.n_batches = nb;
-      // ---- the CRC + lz4 size pass: most of it was launched by sgr_dingest_submit behind the copies; the rest now
-      if (g->crc_launched < nb) {
-        DG_TRY(g, cudaStreamWaitEvent(g->stream, g->subs.back().copied, 0));
-        DG_TRY(g, dg_launch_crc_size((const uint8_t*)g->wire.b.p, (DgBatch*)g->d_batches.b.p + g->crc_launched, (uint32_t)(nb - g->crc_launched), g->stream));
-        g->crc_launched = nb;
-      }
+    }
+    if (h[10]) {
+      // the arena claims overflowed (the poll compresses better than 3x): lay the arena out exactly and decode + parse again.
+      // Ids the first attempt interned stay (an id is an id); its records are overwritten slot for slot.
+      // (exact sizes first: the claim mode never measured them)
+      DG_TRY(g, dg_launch_crc_size_fast((const uint8_t*)g->wire.b.p, (DgBatch*)g->d_batches.b.p, nb, nullptr, g->stream));
       DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.b.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
       DG_TRY(g, cudaStreamSynchronize(g->stream));
-      lap(0);
-      uint64_t arena_need = 0;
+      uint64_t need = 0;
       for (uint32_t i = 0; i < nb; ++i) {
         DgBatch& b = g->batches[i];
+        if (b.err == DG_ARENA_FULL) b.err = DG_OK;
         if (b.err) { const int32_t rc = dfail(g, SGR_ERR_INVALID, "offset %lld: %s", (long long)b.base_offset, dg_err_text(b.err)); discard_poll(g); return rc; }
-        if (b.codec == 3) { b.arena_off = arena_need; arena_need += ((uint64_t)b.dsize + 15) & ~15ull; st.n_decompressed_bytes += b.dsize; }
+        b.err_record = 0;
+        if (b.codec == 3) { b.arena_off = need; need += ((uint64_t)b.dsize + 15) & ~15ull; }
       }
       g->arena.used = 0;
-      DG_TRY(g, g->arena.ensure(arena_need + 64, g->stream));
+      DG_TRY(g, g->arena.ensure(need + 512, g->stream));
+      DG_TRY(g, set_arena_capacity(g));
+      p = parse_args(g);
+      h[2] = h[3] = h[4] = h[5] = h[6] = 0; h[8] = need; h[10] = 0;
+      DG_TRY(g, cudaMemcpyAsync((unsigned long long*)g->ctl.p + 2, h + 2, 5 * 8, cudaMemcpyHostToDevice, g->stream));
+      DG_TRY(g, cudaMemcpyAsync((unsigned long long*)g->ctl.p + 8, h + 8, 8, cudaMemcpyHostToDevice, g->stream));
+      DG_TRY(g, cudaMemcpyAsync((unsigned long long*)g->ctl.p + 10, h + 10, 8, cudaMemcpyHostToDevice, g->stream));
+      DG_TRY(g, cudaMemsetAsync(g->rec_batch.b.p, 0xff, (size_t)nrec * 4 + 4, g->stream));
       DG_TRY(g, cudaMemcpyAsync(g->d_batches.b.p, g->batches.data(), (size_t)nb * sizeof(DgBatch), cudaMemcpyHostToDevice, g->stream));
-      DG_TRY(g, dg_launch_decode_walk((const uint8_t*)g->wire.b.p, (uint8_t*)g->arena.b.p, (DgBatch*)g->d_batches.b.p, nb, 0, (uint32_t*)g->rec_off.b.p, (uint32_t*)g->rec_batch.b.p, g->stream));
-      if (g->timing_syncs) { DG_TRY(g, cudaStreamSynchronize(g->stream)); lap(1); }
-      p.wire = (const uint8_t*)g->wire.b.p; p.arena = (const uint8_t*)g->arena.b.p; p.rec_begin = 0; p.n_records = nrec;
+      DG_TRY(g, dg_launch_decode_walk_fast((const uint8_t*)g->wire.b.p, (uint8_t*)g->arena.b.p, (DgBatch*)g->d_batches.b.p, nb, 0, (uint32_t*)g->rec_off.b.p, (uint32_t*)g->rec_batch.b.p, nullptr, g->stream));
+      p.n_batches = nb; p.rec_begin = 0; p.n_records = nrec;
       DG_TRY(g, dg_launch_parse(p, g->stream));
       DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.b.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
       DG_TRY(g, cudaMemcpyAsync(h, g->ctl.p, 128, cudaMemcpyDeviceToHost, g->stream));
       DG_TRY(g, cudaStreamSynchronize(g->stream));
-      lap(2);
+      lap(1);
     }
+    for (uint32_t i = 0; i < nb; ++i) if (g->batches[i].codec == 3 && !g->batches[i].err) st.n_decompressed_bytes += g->batches[i].dsize;
     for (uint32_t i = 0; i < nb; ++i)
       if (g->batches[i].err) {
         const int32_t rc = dfail(g, SGR_ERR_INVALID, "offset %lld, record %u: %s", (long long)g->batches[i].base_offset, g->batches[i].err_record, dg_err_text(g->batches[i].err));

@@ -7,11 +7,14 @@
 // per-batch and per-record happens on the GPU; the host keeps only the walk over the 61-byte batch headers and the
 // read_committed bookkeeping (csrc/dingest.cu). csrc/ingest.cpp stays as the byte-equal checker (tests/test_gpu_dingest.py).
 //
+// One chain of three launches per group of batches, with no host round trip in between (csrc/dingest.cu runs such chains on
+// several streams behind the H2D copies):
 //   crc_size    one THREAD per batch: CRC-32C of the batch (slicing-by-8, tables in shared memory) against the header's field;
-//               lz4 frames: header + block walk that only ADDS UP sequence lengths -> decompressed size (the arena is then laid
-//               out by an exclusive scan on the host: 4 bytes per batch come back)
-//   decode_walk one thread per batch: lz4 sequences copied into the batch's arena slot (byte-serial by nature: matches may
-//               overlap their own output), then the record-boundary walk — a chain of varints — writes every record's offset
+//               every lz4 batch claims an arena slot of 3x its compressed size with an atomicAdd. (When the claims overflow, the
+//               poll is repeated without them: this pass then walks each lz4 frame adding up sequence lengths -> the exact
+//               decompressed size, and the host lays the arena out.)
+//   decode_walk one thread per batch: lz4 sequences decoded into the batch's arena slot (lz4_fast.h), then the record-boundary
+//               walk — a chain of varints — writes every record's offset
 //   parse       one thread per RECORD: varint fields, key -> aggregate id (up to ':', KafkaPartitioner.scala:38-42), value ->
 //               packed 64-byte record at the record's own slot (arrival order kept), id -> dense index through a device hash
 //               table (64-bit hash tag claimed by CAS, id bytes compared, index from an atomic counter)
@@ -20,19 +23,12 @@
 //
 // Thread-per-batch is deliberate: a 16 KiB producer batch is ~2 k lz4 sequences and ~500 varint-delimited records, strictly
 // serial inside; the parallelism is the tens of thousands of batches of a restore poll. All of it is HBM/latency-bound
-// byte work — no tensor cores anywhere.
-//
-// Two generations live here. The first (dg_crc_size_kernel, dg_decode_walk_kernel; SGR_DINGEST_V1=1 selects it) walks the bytes
-// through global memory and spends the same time on the decode of ANY number of batches: ~10 dependent memory round trips per lz4
-// sequence, and in a warp of 32 independent batches some lane misses at every step. The second (the *_fast kernels, default)
-// reads its input through a per-thread cp.async ring in shared memory and keeps memory current behind an 8-byte output
-// accumulator (lz4_fast.h) — one dependent access per sequence — and claims each batch's arena slot with an atomicAdd in the size pass, so that CRC -> decode -> parse of a group of batches is one chain of launches with
-// no host round trip in between (csrc/dingest.cu runs such chains on several streams behind the H2D copies).
+// byte work — no tensor cores anywhere. The two thread-per-batch kernels read their input through a per-thread cp.async ring in
+// shared memory (RingIn) and keep memory current behind an 8-byte output accumulator (lz4_fast.h): one dependent memory access
+// per lz4 sequence, where bytes walked straight from global memory cost ~10, and in a warp of 32 independent batches some lane
+// misses at every step.
 #include "dingest_kernels.cuh"
 #include "lz4_fast.h"
-
-#include <stdlib.h>
-#include <string.h>
 
 namespace sgr {
 namespace {
@@ -80,188 +76,6 @@ struct ByteWin {
 
 __device__ __forceinline__ uint32_t rd32le(const uint8_t* p) { return p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
 
-__device__ uint32_t crc32c_dev(const uint32_t (*tab)[256], const uint8_t* p, uint64_t n) {
-  uint32_t crc = 0xffffffffu;
-  while (n && ((uintptr_t)p & 7)) { crc = (crc >> 8) ^ tab[0][(crc ^ *p++) & 0xff]; --n; }
-  while (n >= 8) {
-    const unsigned long long w = *reinterpret_cast<const unsigned long long*>(p);
-    const uint32_t lo = (uint32_t)w ^ crc, hi = (uint32_t)(w >> 32);
-    crc = tab[7][lo & 0xff] ^ tab[6][(lo >> 8) & 0xff] ^ tab[5][(lo >> 16) & 0xff] ^ tab[4][lo >> 24] ^
-          tab[3][hi & 0xff] ^ tab[2][(hi >> 8) & 0xff] ^ tab[1][(hi >> 16) & 0xff] ^ tab[0][hi >> 24];
-    p += 8; n -= 8;
-  }
-  while (n--) crc = (crc >> 8) ^ tab[0][(crc ^ *p++) & 0xff];
-  return ~crc;
-}
-
-__device__ __forceinline__ uint32_t rotl32(uint32_t x, int r) { return (x << r) | (x >> (32 - r)); }
-__device__ uint32_t xxh32_dev(const uint8_t* p, uint64_t len, uint32_t seed) {
-  const uint32_t P1 = 2654435761u, P2 = 2246822519u, P3 = 3266489917u, P4 = 668265263u, P5 = 374761393u;
-  const uint8_t* end = p + len;
-  uint32_t h;
-  if (len >= 16) {
-    const uint8_t* limit = end - 16;
-    uint32_t v1 = seed + P1 + P2, v2 = seed + P2, v3 = seed, v4 = seed - P1;
-    do {
-      v1 = rotl32(v1 + rd32le(p) * P2, 13) * P1; p += 4;
-      v2 = rotl32(v2 + rd32le(p) * P2, 13) * P1; p += 4;
-      v3 = rotl32(v3 + rd32le(p) * P2, 13) * P1; p += 4;
-      v4 = rotl32(v4 + rd32le(p) * P2, 13) * P1; p += 4;
-    } while (p <= limit);
-    h = rotl32(v1, 1) + rotl32(v2, 7) + rotl32(v3, 12) + rotl32(v4, 18);
-  } else {
-    h = seed + P5;
-  }
-  h += (uint32_t)len;
-  while (p + 4 <= end) { h = rotl32(h + rd32le(p) * P3, 17) * P4; p += 4; }
-  while (p < end) { h = rotl32(h + (*p++) * P5, 11) * P1; }
-  h ^= h >> 15; h *= P2; h ^= h >> 13; h *= P3; h ^= h >> 16;
-  return h;
-}
-
-// dst[0..n) = src[0..n) for one thread, 4 bytes per memory instruction: aligned word stores, aligned word loads funnel-shifted
-// to the source's misalignment (a GPU has no unaligned accesses). The regions must not overlap within 8 bytes (the caller sends
-// close overlapping matches down the byte path). Byte-wise copies were the bulk of the decode: every byte access of every thread
-// is an L1 wavefront of its own.
-__device__ __forceinline__ void copy_words(uint8_t* dst, const uint8_t* src, uint64_t n) {
-  uint64_t k = 0;
-  while (k < n && ((uintptr_t)(dst + k) & 3)) { dst[k] = src[k]; ++k; }
-  if (n - k >= 4) {
-    const uint8_t* s = src + k;
-    const uint32_t mis = (uint32_t)((uintptr_t)s & 3);
-    const uint32_t* sw = reinterpret_cast<const uint32_t*>(s - mis);
-    uint32_t* dw = reinterpret_cast<uint32_t*>(dst + k);
-    const uint64_t words = (n - k) >> 2;
-    if (mis == 0) {
-      for (uint64_t w = 0; w < words; ++w) dw[w] = sw[w];
-    } else {
-      uint32_t lo = sw[0];
-      for (uint64_t w = 0; w < words; ++w) { const uint32_t hi = sw[w + 1]; dw[w] = __funnelshift_r(lo, hi, mis * 8); lo = hi; }
-    }
-    k += words << 2;
-  }
-  while (k < n) { dst[k] = src[k]; ++k; }
-}
-
-// LZ4 frame walk. out == nullptr: only the decoded size is computed (and everything validated except the content checksum).
-// Mirrors lz4_frame_decode of csrc/ingest.cpp decision for decision (same accept / reject behaviour).
-// `lane`/`lanes`: every participating thread runs the SAME control flow over the same compressed bytes (broadcast loads) and copies
-// its share of every literal run and match (bytes lane, lane + lanes, ...): one thread (0, 1) for the size pass, a whole warp
-// (lane, 32) for the decode — 32 consecutive bytes per step, coalesced. An overlapping match (offset < length) repeats its last
-// `offset` bytes, so byte k of the match is byte (k mod offset) of that period: independent per byte, no serial dependency.
-__device__ uint32_t lz4_frame(const uint8_t* src, uint64_t n, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint32_t lane = 0, uint32_t lanes = 1) {
-  if (n < 7) return DG_LZ4_HEADER;
-  if (rd32le(src) != 0x184D2204u) return DG_LZ4_HEADER;
-  const uint8_t flg = src[4], bd = src[5];
-  if ((flg >> 6) != 1 || (flg & 0x02)) return DG_LZ4_HEADER;
-  const bool block_checksum = flg & 0x10, content_size = flg & 0x08, content_checksum = flg & 0x04, dict_id = flg & 0x01;
-  const uint32_t bs_code = (bd >> 4) & 7;
-  if (bs_code < 4 || (bd & 0x8F)) return DG_LZ4_HEADER;
-  const uint64_t max_block = 1ull << (8 + 2 * bs_code);
-  const uint64_t desc_len = 2 + (content_size ? 8 : 0) + (dict_id ? 4 : 0);
-  if (n < 4 + desc_len + 1) return DG_LZ4_HEADER;
-  uint64_t declared = 0;
-  if (content_size) for (int k = 7; k >= 0; --k) declared = (declared << 8) | src[6 + k];
-  if (((xxh32_dev(src + 4, desc_len, 0) >> 8) & 0xff) != src[4 + desc_len]) return DG_LZ4_HEADER;
-  uint64_t pos = 4 + desc_len + 1, op = 0;
-  for (;;) {
-    if (pos + 4 > n) return DG_LZ4_BLOCK;
-    const uint32_t word = rd32le(src + pos); pos += 4;
-    if (word == 0) break;
-    const bool stored = word & 0x80000000u;
-    const uint64_t bsz = word & 0x7FFFFFFFu;
-    if (bsz > max_block) return DG_LZ4_BLOCK;
-    if (pos + bsz + (block_checksum ? 4 : 0) > n) return DG_LZ4_BLOCK;
-    const uint8_t* b = src + pos;
-    if (block_checksum && xxh32_dev(b, bsz, 0) != rd32le(b + bsz)) return DG_LZ4_CHECKSUM;
-    if (stored) {
-      if (out) {
-        if (op + bsz > out_cap) return DG_LZ4_TOO_LARGE;
-        if (lanes == 1) copy_words(out + op, b, bsz);
-        else { for (uint64_t k = lane; k < bsz; k += lanes) out[op + k] = b[k]; __syncwarp(); }
-      }
-      op += bsz;
-    } else {
-      const uint64_t block_start = op;
-      uint64_t ip = 0;
-      ByteWin win;
-      for (;;) {
-        if (ip >= bsz) return DG_LZ4_SEQUENCE;
-        const uint8_t token = (uint8_t)win.at(b + ip++);
-        uint64_t lit = token >> 4;
-        if (lit == 15) {
-          uint8_t s;
-          do { if (ip >= bsz) return DG_LZ4_SEQUENCE; s = (uint8_t)win.at(b + ip++); lit += s; } while (s == 255);
-        }
-        if (lit > bsz - ip) return DG_LZ4_SEQUENCE;
-        if (op - block_start + lit > max_block) return DG_LZ4_TOO_LARGE;
-        if (out) {
-          if (op + lit > out_cap) return DG_LZ4_TOO_LARGE;
-          if (lanes == 1) copy_words(out + op, b + ip, lit);
-          else for (uint64_t k = lane; k < lit; k += lanes) out[op + k] = b[ip + k];
-        }
-        op += lit; ip += lit;
-        if (ip == bsz) break;   // the last sequence carries literals only
-        if (ip + 2 > bsz) return DG_LZ4_SEQUENCE;
-        const uint32_t off = win.at(b + ip) | (win.at(b + ip + 1) << 8); ip += 2;
-        uint64_t mlen = token & 15;
-        if (mlen == 15) {
-          uint8_t s;
-          do { if (ip >= bsz) return DG_LZ4_SEQUENCE; s = (uint8_t)win.at(b + ip++); mlen += s; } while (s == 255);
-        }
-        mlen += 4;
-        if (off == 0 || off > op) return DG_LZ4_SEQUENCE;   // matches may reach back across blocks, never before the frame
-        if (op - block_start + mlen > max_block) return DG_LZ4_TOO_LARGE;
-        if (out) {
-          if (op + mlen > out_cap) return DG_LZ4_TOO_LARGE;
-          if (lanes > 1) __syncwarp();                                  // the literals (and earlier matches) this match may read
-          const uint8_t* period = out + op - off;
-          if (lanes == 1 && off >= 8) {
-            // a far match never reads a word it has not finished writing when copied in pieces of at most `off` bytes
-            for (uint64_t done = 0; done < mlen; done += off) copy_words(out + op + done, period + done, mlen - done < off ? mlen - done : off);
-          } else {
-            for (uint64_t k = lane; k < mlen; k += lanes) out[op + k] = period[off >= mlen ? k : k % off];
-          }
-          if (lanes > 1) __syncwarp();
-        }
-        op += mlen;
-      }
-    }
-    pos += bsz + (block_checksum ? 4 : 0);
-  }
-  if (content_checksum) {
-    if (pos + 4 > n) return DG_LZ4_BLOCK;
-    if (out && lanes > 1) __syncwarp();
-    if (out && xxh32_dev(out, op, 0) != rd32le(src + pos)) return DG_LZ4_CHECKSUM;
-    pos += 4;
-  }
-  if (content_size && declared != op) return DG_LZ4_BLOCK;
-  *out_len = op;
-  return DG_OK;
-}
-
-__global__ void __launch_bounds__(kThreads) dg_crc_size_kernel(const uint8_t* __restrict__ wire, DgBatch* __restrict__ batches, uint32_t n) {
-  __shared__ uint32_t tab[8][256];
-  for (int i = threadIdx.x; i < 8 * 256; i += kThreads) (&tab[0][0])[i] = (&g_crc_tab[0][0])[i];
-  __syncthreads();
-  const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
-  if (i >= n) return;
-  DgBatch bt = batches[i];
-  const uint8_t* b = wire + bt.src_off;
-  uint32_t err = DG_OK, dsize = bt.total_len - 61u;
-  if (crc32c_dev(tab, b + 21, (uint64_t)bt.total_len - 21) != bt.stored_crc) err = DG_CRC;
-  else if (bt.codec == 3) {
-    uint64_t len = 0;
-    err = lz4_frame(b + 61, (uint64_t)bt.total_len - 61, nullptr, 0, &len);
-    if (!err && len > 0xffffffffull) err = DG_LZ4_TOO_LARGE;
-    dsize = (uint32_t)len;
-  }
-  if (!err && (uint64_t)bt.n_records > (uint64_t)dsize / 7 + 1) err = DG_RECORD_COUNT;   // every record is at least 7 bytes on the wire
-  batches[i].dsize = dsize;
-  batches[i].err = err;
-  batches[i].err_record = 0;
-}
-
 struct Cur {   // zig-zag varints of org.apache.kafka.common.utils.ByteUtils over a byte range
   const uint8_t* p; uint64_t n, pos; bool ok;
   ByteWin win;
@@ -294,39 +108,7 @@ struct Cur {   // zig-zag varints of org.apache.kafka.common.utils.ByteUtils ove
   }
 };
 
-// one WARP per batch: cooperative lz4 copies, then the (serial) record-boundary walk run redundantly by all lanes — same loads,
-// broadcast — with the writes spread over the lanes
-template <int WARP>
-__global__ void __launch_bounds__(kThreads) dg_decode_walk_kernel(const uint8_t* __restrict__ wire, uint8_t* __restrict__ arena, DgBatch* __restrict__ batches,
-                                                                  uint32_t n, uint32_t index_base, uint32_t* __restrict__ rec_off, uint32_t* __restrict__ rec_batch) {
-  // WARP == 1: one warp per batch (cooperative copies); 0: one thread per batch (word-wise copies, 32x more batches in flight —
-  // for 16 KiB producer batches, where the token chain, not the copy width, is the latency)
-  const uint32_t i = WARP ? (blockIdx.x * kThreads + threadIdx.x) >> 5 : blockIdx.x * kThreads + threadIdx.x;
-  const uint32_t lane = WARP ? threadIdx.x & 31 : 0;
-  if (i >= n) return;
-  DgBatch bt = batches[i];
-  if (bt.err) return;
-  const uint8_t* sect = wire + bt.src_off + 61;
-  uint64_t sect_len = (uint64_t)bt.total_len - 61;
-  if (bt.codec == 3) {
-    uint64_t len = 0;
-    const uint32_t e = lz4_frame(sect, sect_len, arena + bt.arena_off, bt.dsize, &len, lane, WARP ? 32 : 1);
-    if (WARP) __syncwarp();
-    if (e || len != bt.dsize) { if (lane == 0) batches[i].err = e ? e : DG_LZ4_BLOCK; return; }
-    sect = arena + bt.arena_off; sect_len = len;
-  }
-  Cur c(sect, sect_len);
-  for (uint32_t r = 0; r < bt.n_records; ++r) {
-    const uint64_t at = c.pos;
-    const int32_t len = c.varint();
-    if (!c.ok || len < 0 || (uint64_t)len > sect_len - c.pos) { if (lane == 0) { batches[i].err = DG_RECORD_LENGTH; batches[i].err_record = r; } return; }
-    if (!WARP || lane == (r & 31u)) { rec_off[bt.rec_base + r] = (uint32_t)at; rec_batch[bt.rec_base + r] = index_base + i; }
-    c.pos += (uint64_t)len;
-  }
-  if (c.pos != sect_len && lane == 0) { batches[i].err = DG_STRAY_BYTES; batches[i].err_record = bt.n_records; }
-}
-
-// ---------------------------------------------------------------------------------------------- second generation
+// ---------------------------------------------------------------------------------------------- CRC + size, decode + walk
 constexpr int kFastThreads = 64;   // thread-per-batch kernels: small CTAs spread a group of a few thousand batches over all SMs
 constexpr int kRingChunks = 8;     // 16-byte chunks per thread in the input ring
 
@@ -364,7 +146,8 @@ struct RingIn {
       // One chunk at a time, each followed by its wait: a request goes into the slot of the OLDEST chunk, and that slot's
       // previous request must have landed first — copies in flight complete in any order, and two of them aimed at one slot
       // would leave whichever arrives last. (Issuing k requests and waiting once was wrong for k >= 3: the third reuses a slot
-      // whose copy may still be among the six allowed to be pending. Found by the 40-byte records of scripts/dingest_race.py.)
+      // whose copy may still be among the six allowed to be pending. Found on records of about 40 bytes; pinned by
+      // test_forty_byte_records_walk_through_the_ring and modelled in tests/test_ring_protocol_model.py.)
       do {
         issue(base + 16 * kRingChunks); base += 16;
         asm volatile("cp.async.wait_group %0;" ::"n"(kRingChunks - 2) : "memory");
@@ -382,22 +165,8 @@ struct RingIn {
   }
 };
 
-// The same interface over plain global loads (two aligned 8-byte words per read): the A/B partner of the ring
-// (SGR_DINGEST_DEBUG bit 1: record walk, bit 2: CRC + lz4 input) — every read is a dependent round trip.
-struct DirectIn {
-  __device__ __forceinline__ void seek(const uint8_t*) {}
-  __device__ __forceinline__ void advance(const uint8_t*) {}
-  __device__ __forceinline__ uint64_t get64(const uint8_t* p) const {
-    const uint8_t* a = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(p) & ~(uintptr_t)7);
-    return lzf::funnel(__ldcg(reinterpret_cast<const unsigned long long*>(a)), __ldcg(reinterpret_cast<const unsigned long long*>(a + 8)), (uint32_t)reinterpret_cast<uintptr_t>(p) & 7u);
-  }
-};
-
-__device__ uint32_t g_dbg_flags = 0;   // SGR_DINGEST_DEBUG: 1 walk without the ring, 2 CRC + lz4 input without the ring, 4 match sources bypass L1, 8 fence before the walk
-
 // CRC-32C over a byte range read through the ring
-template <class IN>
-__device__ uint32_t crc32c_ring(const uint32_t (*tab)[256], IN& in, const uint8_t* p, uint64_t n) {
+__device__ uint32_t crc32c_ring(const uint32_t (*tab)[256], RingIn& in, const uint8_t* p, uint64_t n) {
   uint32_t crc = 0xffffffffu;
   if (!n) return ~crc;
   in.seek(p);
@@ -417,8 +186,7 @@ __device__ uint32_t crc32c_ring(const uint32_t (*tab)[256], IN& in, const uint8_
 // arena_ctl (optional): [0] bytes claimed so far, [1] capacity, [2] set when a claim (or, later, a batch in its slot) did not fit.
 // With it: CRC only, and every lz4 batch leaves the kernel with an arena slot of 3x its compressed size. Without it: CRC and the
 // exact decoded size (an lz4 walk that only adds up lengths); the host then lays the arena out.
-template <class IN>
-__device__ __forceinline__ void crc_size_one(const uint32_t (*tab)[256], IN& in, const uint8_t* __restrict__ wire, DgBatch* __restrict__ batches, uint32_t i,
+__device__ __forceinline__ void crc_size_one(const uint32_t (*tab)[256], RingIn& in, const uint8_t* __restrict__ wire, DgBatch* __restrict__ batches, uint32_t i,
                                              unsigned long long* __restrict__ arena_ctl) {
   const DgBatch bt = batches[i];
   const uint8_t* b = wire + bt.src_off;
@@ -458,15 +226,13 @@ __global__ void __launch_bounds__(kFastThreads) dg_crc_size_fast_kernel(const ui
   if (i >= n) return;
   RingIn in;
   in.init(&ring[0][0]);
-  if (g_dbg_flags & 2u) { DirectIn din; crc_size_one(tab, din, wire, batches, i, arena_ctl); }
-  else crc_size_one(tab, in, wire, batches, i, arena_ctl);
+  crc_size_one(tab, in, wire, batches, i, arena_ctl);
   asm volatile("cp.async.wait_all;" ::: "memory");   // chunks requested ahead of the last byte land before the CTA's memory goes
 }
 
 // one thread per batch: lz4 into the batch's arena slot, then the record-boundary walk (a chain of varints) over the decoded
 // bytes, read back through the same ring three records ahead
-template <class IN, class WIN>
-__device__ __forceinline__ void decode_walk_one(IN& lzin, WIN& in, const uint8_t* __restrict__ wire, uint8_t* arena, DgBatch* __restrict__ batches, uint32_t i, uint32_t index_base,
+__device__ __forceinline__ void decode_walk_one(RingIn& in, const uint8_t* __restrict__ wire, uint8_t* arena, DgBatch* __restrict__ batches, uint32_t i, uint32_t index_base,
                                                 uint32_t* __restrict__ rec_off, uint32_t* __restrict__ rec_batch, unsigned long long* __restrict__ arena_ctl) {
   const DgBatch bt = batches[i];
   if (bt.err) return;
@@ -474,8 +240,7 @@ __device__ __forceinline__ void decode_walk_one(IN& lzin, WIN& in, const uint8_t
   uint64_t sect_len = (uint64_t)bt.total_len - 61;
   if (bt.codec == 3) {
     uint64_t len = 0;
-    const uint32_t e = lzf::frame<true>(lzin, sect, sect_len, arena + bt.arena_off, bt.dsize, &len, (g_dbg_flags & 4u) != 0);
-    if (g_dbg_flags & 8u) __threadfence();
+    const uint32_t e = lzf::frame<true>(in, sect, sect_len, arena + bt.arena_off, bt.dsize, &len);
     if (arena_ctl) {   // bt.dsize was the capacity of a claimed slot
       if (e == DG_LZ4_TOO_LARGE) { arena_ctl[2] = 1ull; batches[i].err = DG_ARENA_FULL; return; }   // (or a block past its maximum: the exact pass tells)
       if (e) { batches[i].err = e; return; }
@@ -502,23 +267,7 @@ __device__ __forceinline__ void decode_walk_one(IN& lzin, WIN& in, const uint8_t
       ok = ok && pos + used <= sect_len;
     }
     const int32_t len = (int32_t)(raw >> 1) ^ -(int32_t)(raw & 1u);
-    if (!ok || len < 0 || (uint64_t)len > sect_len - (pos + used)) {
-      uint32_t diag = 0;
-      if (g_dbg_flags & 16u) {   // diagnosis: does the same walk over plain L2 loads succeed? (bit 31: yes -> the ring served stale bytes)
-        DirectIn d; uint64_t q = 0; bool fine = true;
-        for (uint32_t r2 = 0; r2 < bt.n_records && fine; ++r2) {
-          if (q >= sect_len) { fine = false; break; }
-          const unsigned long long v2 = d.get64(sect + q);
-          uint32_t raw2 = 0, used2 = 0; bool t = false;
-          for (int k = 0; k < 5; ++k) { const uint32_t byte = (uint32_t)(v2 >> (8 * k)) & 0xffu; raw2 |= (byte & 0x7fu) << (7 * k); if (!(byte & 0x80u)) { used2 = k + 1; t = true; break; } }
-          const int32_t l2 = (int32_t)(raw2 >> 1) ^ -(int32_t)(raw2 & 1u);
-          if (!t || l2 < 0 || q + used2 > sect_len || (uint64_t)l2 > sect_len - (q + used2)) fine = false; else q += used2 + (uint64_t)l2;
-        }
-        if (fine && q == sect_len) diag = 0x80000000u;
-        diag |= ((uint32_t)pos & 0xfffffu) << 8;
-      }
-      batches[i].err = DG_RECORD_LENGTH; batches[i].err_record = r | diag; return;
-    }
+    if (!ok || len < 0 || (uint64_t)len > sect_len - (pos + used)) { batches[i].err = DG_RECORD_LENGTH; batches[i].err_record = r; return; }
     rec_off[bt.rec_base + r] = (uint32_t)pos; rec_batch[bt.rec_base + r] = index_base + i;
     pos += used + (uint64_t)len;
   }
@@ -533,12 +282,7 @@ __global__ void __launch_bounds__(kFastThreads) dg_decode_walk_fast_kernel(const
   if (i >= n) return;
   RingIn in;
   in.init(&ring[0][0]);
-  const uint32_t dbg = g_dbg_flags;
-  DirectIn din;
-  if ((dbg & 3u) == 0u) decode_walk_one(in, in, wire, arena, batches, i, index_base, rec_off, rec_batch, arena_ctl);
-  else if ((dbg & 3u) == 1u) decode_walk_one(in, din, wire, arena, batches, i, index_base, rec_off, rec_batch, arena_ctl);
-  else if ((dbg & 3u) == 2u) decode_walk_one(din, in, wire, arena, batches, i, index_base, rec_off, rec_batch, arena_ctl);
-  else decode_walk_one(din, din, wire, arena, batches, i, index_base, rec_off, rec_batch, arena_ctl);
+  decode_walk_one(in, wire, arena, batches, i, index_base, rec_off, rec_batch, arena_ctl);
   asm volatile("cp.async.wait_all;" ::: "memory");
 }
 
@@ -678,15 +422,6 @@ __global__ void __launch_bounds__(kThreads) dg_parse_kernel(const __grid_constan
 
 }  // namespace
 
-uint32_t dg_crc32c_host_reference_polynomial() { return 0x82F63B78u; }
-
-cudaError_t dg_launch_crc_size(const uint8_t* wire, DgBatch* batches, uint32_t n, cudaStream_t st) {
-  cudaError_t e = ensure_crc_tables();
-  if (e != cudaSuccess || !n) return e;
-  dg_crc_size_kernel<<<(n + kThreads - 1) / kThreads, kThreads, 0, st>>>(wire, batches, n);
-  return cudaGetLastError();
-}
-
 // descriptors host -> device by the SMs (zero-copy read of page-locked memory): the copy engine's queue is full of the poll's
 // fetches, and a cudaMemcpyAsync for 512 KiB of descriptors would wait behind ALL of them
 __global__ void dg_copy16_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, uint64_t n16) {
@@ -701,13 +436,7 @@ cudaError_t dg_copy_from_mapped_host(const void* host_mapped, void* dst, uint64_
   return cudaGetLastError();
 }
 
-cudaError_t dg_prepare() {
-  cudaError_t e = ensure_crc_tables();
-  if (e != cudaSuccess) return e;
-  const char* d = getenv("SGR_DINGEST_DEBUG");
-  const uint32_t flags = d ? (uint32_t)atoi(d) : 0u;
-  return cudaMemcpyToSymbol(g_dbg_flags, &flags, sizeof flags);
-}
+cudaError_t dg_prepare() { return ensure_crc_tables(); }
 
 cudaError_t dg_launch_crc_size_fast(const uint8_t* wire, DgBatch* batches, uint32_t n, unsigned long long* arena_ctl, cudaStream_t st) {
   cudaError_t e = ensure_crc_tables();
@@ -720,18 +449,6 @@ cudaError_t dg_launch_decode_walk_fast(const uint8_t* wire, uint8_t* arena, DgBa
                                        unsigned long long* arena_ctl, cudaStream_t st) {
   if (!n) return cudaSuccess;
   dg_decode_walk_fast_kernel<<<(n + kFastThreads - 1) / kFastThreads, kFastThreads, 0, st>>>(wire, arena, batches, n, index_base, rec_off, rec_batch, arena_ctl);
-  return cudaGetLastError();
-}
-
-cudaError_t dg_launch_decode_walk(const uint8_t* wire, uint8_t* arena, DgBatch* batches, uint32_t n, uint32_t index_base, uint32_t* rec_off, uint32_t* rec_batch, cudaStream_t st) {
-  if (!n) return cudaSuccess;
-  static const bool warp_mode = getenv("SGR_DINGEST_WARP_DECODE") != nullptr;
-  if (warp_mode) {
-    const uint32_t warps_per_block = kThreads / 32;
-    dg_decode_walk_kernel<1><<<(n + warps_per_block - 1) / warps_per_block, kThreads, 0, st>>>(wire, arena, batches, n, index_base, rec_off, rec_batch);
-  } else {
-    dg_decode_walk_kernel<0><<<(n + kThreads - 1) / kThreads, kThreads, 0, st>>>(wire, arena, batches, n, index_base, rec_off, rec_batch);
-  }
   return cudaGetLastError();
 }
 

@@ -55,19 +55,17 @@ struct DgParse {
   DgDict dict;
 };
 
-cudaError_t dg_launch_crc_size(const uint8_t* wire, DgBatch* batches, uint32_t n, cudaStream_t st);
-// batches: the sub-array to process (n of them), whose first element has index `index_base` in the full array (what rec_batch records)
-cudaError_t dg_launch_decode_walk(const uint8_t* wire, uint8_t* arena, DgBatch* batches, uint32_t n, uint32_t index_base, uint32_t* rec_off, uint32_t* rec_batch, cudaStream_t st);
 cudaError_t dg_launch_parse(const DgParse& p, cudaStream_t st);
-// second generation (register-window decode, device-side arena claims); wire and arena need 64 readable bytes past their content
 // nbytes rounded up to 16: both buffers need that much room; host_mapped is the DEVICE address of page-locked, mapped host memory
 cudaError_t dg_copy_from_mapped_host(const void* host_mapped, void* dst, uint64_t nbytes, cudaStream_t st);
 cudaError_t dg_prepare();   // uploads the CRC tables (a synchronous copy: call it before anything runs on other streams)
+// The two thread-per-batch kernels read wire and arena through a ring that runs up to 256 bytes past a batch's last byte: both
+// buffers need that much room past their content.
 cudaError_t dg_launch_crc_size_fast(const uint8_t* wire, DgBatch* batches, uint32_t n, unsigned long long* arena_ctl, cudaStream_t st);
+// batches: the sub-array to process (n of them), whose first element has index `index_base` in the full array (what rec_batch records);
 // arena_ctl as given to dg_launch_crc_size_fast for the same batches (nullptr: dsize is exact, not a slot capacity)
 cudaError_t dg_launch_decode_walk_fast(const uint8_t* wire, uint8_t* arena, DgBatch* batches, uint32_t n, uint32_t index_base, uint32_t* rec_off, uint32_t* rec_batch,
                                        unsigned long long* arena_ctl, cudaStream_t st);
 cudaError_t dg_gather_keys(const DgDict& d, uint64_t from, uint32_t n, uint32_t* d_offs, uint8_t* d_bytes, uint32_t* d_tmp, cudaStream_t st);
-uint32_t dg_crc32c_host_reference_polynomial();   // 0x82F63B78: the tables of the device CRC are built from it at first use
 
 }  // namespace sgr

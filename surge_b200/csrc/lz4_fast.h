@@ -97,14 +97,7 @@ struct Out8 {
   uint8_t* out;
   uint64_t op;
   uint64_t acc;
-  bool src_bypass_l1;   // device: read match sources with ld.global.cg
-  LZF_HD void init(uint8_t* o) { out = o; op = 0; acc = 0; src_bypass_l1 = false; }
-  LZF_HD uint64_t src64(const uint8_t* p) const {
-#if defined(__CUDA_ARCH__)
-    if (src_bypass_l1) return __ldcg(reinterpret_cast<const unsigned long long*>(p));
-#endif
-    return ld64(p);
-  }
+  LZF_HD void init(uint8_t* o) { out = o; op = 0; acc = 0; }
   LZF_HD void put(uint64_t v, uint32_t k) {   // append k (1..8) bytes; v is zero above them
     const uint32_t q = (uint32_t)op & 7, sh = q * 8;
     uint8_t* word = out + (op & ~7ull);
@@ -122,8 +115,8 @@ struct Out8 {
       const uint64_t s = op - off;
       const uint8_t* a = out + (s & ~7ull);
       const uint32_t i = (uint32_t)s & 7;
-      const uint64_t w0 = src64(a), w1 = src64(a + 8);
-      const uint64_t w2 = (off >= 16 && len > 8) ? src64(a + 16) : 0;   // (a load nobody needs still costs the warp its wavefronts)
+      const uint64_t w0 = ld64(a), w1 = ld64(a + 8);
+      const uint64_t w2 = (off >= 16 && len > 8) ? ld64(a + 16) : 0;   // (a load nobody needs still costs the warp its wavefronts)
       uint64_t v = funnel(w0, w1, i);
       if (off < 8) v = replicate(low_bytes(v, off), off);
       uint32_t k = len < 8 ? (uint32_t)len : 8u;
@@ -149,7 +142,7 @@ struct Out8 {
 
 // DECODE = false: validate and measure only (no output is touched). Returns an error code (enum above); *out_len = decoded bytes.
 template <bool DECODE, class IN>
-LZF_HDN uint32_t frame(IN& in, const uint8_t* src, uint64_t n, uint8_t* out, uint64_t out_cap, uint64_t* out_len, bool src_bypass_l1 = false) {
+LZF_HDN uint32_t frame(IN& in, const uint8_t* src, uint64_t n, uint8_t* out, uint64_t out_cap, uint64_t* out_len) {
   if (n < 7) return HEADER;
   if (rd32(src) != 0x184D2204u) return HEADER;
   const uint8_t flg = src[4], bd = src[5];
@@ -166,7 +159,6 @@ LZF_HDN uint32_t frame(IN& in, const uint8_t* src, uint64_t n, uint8_t* out, uin
   uint64_t pos = 4 + desc_len + 1;
   Out8 w;
   w.init(out);
-  w.src_bypass_l1 = src_bypass_l1;
   uint64_t op = 0;   // decoded bytes so far (== w.op when DECODE)
   for (;;) {
     if (pos + 4 > n) return BLOCK;

@@ -79,8 +79,8 @@ class DeviceIngest:
     def last_timing(self) -> Dict[str, float]:
         ms = (C.c_float * 8)()
         self._check(self._lib.sgr_dingest_last_timing(self._h, ms))
-        # default (chained) mode: [0] is the wait for the copies and every group's CRC -> decode -> parse chain, [1] only the repeat
-        # from an exact arena layout (0 normally), [2] unused; SGR_DINGEST_V1: the three passes of the first generation
+        # [0] is the wait for the copies and every group's CRC -> decode -> parse chain, [1] only the repeat from an exact arena
+        # layout (0 normally), [2] unused (its key stays so that recorded results keep their shape)
         return dict(zip(("wait_copies_and_chains", "decode_walk", "parse_intern", "keys_gather", "grow_fold_append_keys", "total"), [float(x) for x in ms[:6]]))
 
     def reset(self) -> None:

@@ -226,13 +226,6 @@ def test_arena_overflow_falls_back_to_an_exact_layout():
     assert st["n_decompressed_bytes"] > 3.2 * len(one), (st["n_decompressed_bytes"], len(one))
 
 
-def test_first_generation_kernels_still_agree(monkeypatch):
-    monkeypatch.setenv("SGR_DINGEST_V1", "1")
-    rng = np.random.default_rng(32)
-    fetches = [(p, _stream(rng, 20, 500, "lz4", base=p * 5000)[0]) for p in range(3)]
-    _compare_with_host(fetches)
-
-
 def test_forty_byte_records_walk_through_the_ring():
     """Records of ~38 bytes make the record walk advance its input ring by three 16-byte chunks per record, every record, in every
     lane — the access pattern that exposed two asynchronous copies aimed at one ring slot (csrc/dingest_kernels.cu, RingIn::advance).

@@ -22,8 +22,7 @@ from surge_b200.ingest import Ingest, IngestError
 
 pytestmark = pytest.mark.gpu
 
-SETTINGS = {"default": {}, "plain_loads": {"SGR_DINGEST_DEBUG": "3"}, "first_generation": {"SGR_DINGEST_V1": "1"},
-            "groups_of_64": {"SGR_DINGEST_GROUP": "64"}}
+SETTINGS = {"default": {}, "groups_of_64": {"SGR_DINGEST_GROUP": "64"}}
 
 
 @contextlib.contextmanager
@@ -117,7 +116,7 @@ def test_hostile_lz4_on_the_device_matches_the_restatement():
         assert st["n_decompressed_bytes"] > 0 and st["n_records"] > 500
 
 
-# ----------------------------------------------------------------------------- 2. ring geometry under every load path
+# ----------------------------------------------------------------------------- 2. ring geometry, one chain per poll and many
 def _ring_polls():
     """Records of 7 bytes (null key, null value) up to ~400 bytes (long headers), so the walk advances its input ring by 0, 1,
     2, ... 8 and more 16-byte chunks per record (advance and seek); stored and literal runs past 128 bytes; batch starts at
