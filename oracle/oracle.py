@@ -24,7 +24,8 @@ def build(force: bool = False) -> str:
     src = os.path.join(_HERE, "sgr_oracle.c")
     hdr = os.path.join(_HERE, "sgr_oracle.h")
     enc = os.path.join(_HERE, "kafka_encode.c")
-    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(os.path.getmtime(src), os.path.getmtime(hdr), os.path.getmtime(enc)):
+    prg = os.path.join(_HERE, "program_oracle.c")
+    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(os.path.getmtime(f) for f in (src, hdr, enc, prg)):
         subprocess.check_call(["make", "-s", "-C", _HERE, "-B"])
     return _LIB_PATH
 
@@ -62,6 +63,13 @@ def lib():
         L.orc_partition_for_key.argtypes = [C.c_void_p, C.c_uint32, C.c_int32]
         L.orc_take_while_not_colon.restype = C.c_uint32
         L.orc_take_while_not_colon.argtypes = [C.c_void_p, C.c_uint32]
+        # fold programs (oracle/program_oracle.c, bound in oracle/program_interp.py)
+        L.orc_prog_fold.restype = C.c_int
+        L.orc_prog_fold.argtypes = [u8p, u8p, u64p, C.c_uint64, u8p, u8p, u64p, u64p]
+        L.orc_prog_fold_var.restype = C.c_int
+        L.orc_prog_fold_var.argtypes = [u8p, C.c_uint32, u8p, u64p, C.c_uint64, u8p, u8p, u64p, u64p]
+        L.orc_prog_fold_arrival.restype = C.c_int
+        L.orc_prog_fold_arrival.argtypes = [u8p, u8p, C.c_uint64, u8p, C.c_uint64, u64p, u64p]
         _lib = L
     return _lib
 

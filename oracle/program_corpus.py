@@ -1,0 +1,262 @@
+"""TEST INFRASTRUCTURE — random fold programs and logs for the program tests (tests/test_gpu_program_fuzz.py,
+tests/test_gpu_program_scale.py, tests/test_program_oracle_cpu.py).
+
+draw_program / draw_log / interleave / draw_var_program / draw_var_log are the small-case drawers of the fuzz test, moved
+here unchanged: the same seeds give byte-identical programs and logs. The scale drawers below build logs of millions of
+records whose shape (segment lengths, hot aggregate, empty runs, throws) is chosen by the caller, with numpy only.
+"""
+from __future__ import annotations
+
+import numpy as np
+
+from oracle import program_interp as I
+
+SPECIAL_F64 = [0.0, -0.0, float("nan"), 1.5, float("inf"), -2.25]
+
+
+def draw_program(rng):
+    state_bytes = int(rng.choice([16, 32, 64, 48, 128], p=[0.35, 0.25, 0.2, 0.1, 0.1]))
+    user = state_bytes - 8
+    family = rng.choice(["class0", "class1", "mixed"], p=[0.45, 0.35, 0.2])
+    pool = {"class0": [I.MATERIALISE, I.CREATE, I.TOMBSTONE, I.THROW], "class1": [I.IF_EXISTS, I.CREATE, I.TOMBSTONE, I.THROW],
+            "mixed": [I.IF_EXISTS, I.MATERIALISE, I.CREATE, I.TOMBSTONE, I.THROW]}[family]
+    weights = {4: [0.55, 0.25, 0.1, 0.1], 5: [0.3, 0.3, 0.2, 0.1, 0.1]}[len(pool)]
+    wide_ops = rng.random() < 0.15
+    n_types = int(rng.integers(1, 7))
+    rules = []
+    for t in range(n_types):
+        ex = int(rng.choice(pool, p=weights)) if t else int(pool[0] if rng.random() < 0.5 else pool[1])   # type 0 creates something
+        ops = []
+        for _ in range(int(rng.integers(0, 5))):
+            opc = int(rng.choice([I.OP_SET, I.OP_ADD_I32, I.OP_SUB_I32])) if not wide_ops else int(rng.integers(0, 5))
+            ln = 4 if opc in (I.OP_ADD_I32, I.OP_SUB_I32) else 8 if opc in (I.OP_ADD_I64, I.OP_SUB_I64) else int(rng.choice([4, 8, 12, 16]))
+            ln = min(ln, user)
+            if opc in (I.OP_ADD_I64, I.OP_SUB_I64) and user < 8:
+                continue
+            dst = 4 * int(rng.integers(0, (user - ln) // 4 + 1))
+            src = 4 if rng.random() < 0.2 and ln == 4 else 16 + 4 * int(rng.integers(0, (48 - ln) // 4 + 1))
+            ops.append((opc, dst, src, ln))
+        rules.append((ex, ops))
+    f64 = []
+    if user >= 16 and rng.random() < 0.4:
+        off = 8 * int(rng.integers(0, user // 8))
+        f64 = [off]
+        # make sure some rule copies a double into that field, from an 8-aligned payload offset
+        t = int(rng.integers(0, n_types))
+        if rules[t][0] not in (I.TOMBSTONE, I.THROW):
+            rules[t] = (rules[t][0], list(rules[t][1])[:3] + [(I.OP_SET, off, 24, 8)])
+    return state_bytes, rules, f64
+
+
+def draw_log(rng, n_types, n_agg, long_len, f64):
+    counts = rng.integers(0, 13, size=n_agg)
+    counts[rng.integers(0, n_agg)] = long_len
+    counts[rng.integers(0, n_agg, size=n_agg // 10)] = 0
+    n = int(counts.sum())
+    rec = rng.integers(0, 256, size=(n, 64), dtype=np.uint8)
+    types = rng.integers(0, n_types, size=n).astype(np.uint32)
+    types[rng.random(n) < 0.004] = n_types                       # scala.MatchError
+    rec[:, 0:4] = types.view(np.uint8).reshape(-1, 4)
+    rec[:, 4:8] = np.arange(1, n + 1, dtype=np.uint32).view(np.uint8).reshape(-1, 4)
+    aggs = np.repeat(np.arange(n_agg, dtype=np.uint64), counts)
+    rec[:, 8:16] = aggs.view(np.uint8).reshape(-1, 8)
+    if f64:
+        hit = rng.random(n) < 0.5
+        vals = np.asarray(SPECIAL_F64)[rng.integers(0, len(SPECIAL_F64), size=n)]
+        rec[hit, 24:32] = vals[hit].view(np.uint8).reshape(-1, 8)
+    off = np.zeros(n_agg + 1, dtype=np.uint64)
+    np.cumsum(counts * 64, out=off[1:])
+    return rec, off, aggs
+
+
+def interleave(rng, aggs):
+    """A permutation that shuffles aggregates against each other but keeps every aggregate's records in order
+    (what a Kafka partition log looks like). `aggs` is in CSR order (non-decreasing)."""
+    t = rng.random(len(aggs))
+    times = t[np.lexsort((t, aggs))]     # within each aggregate the arrival times ascend with the log position
+    return np.argsort(times, kind="stable")
+
+
+# ------------------------------------------------------------------ variable records (SGR_REC_VAR16)
+def draw_var_program(rng):
+    """Like draw_program, with payload reads up to 80 bytes into the record and 16/32-byte states more likely (the
+    record-parallel variable-record kernel takes 16-byte class-0 programs, everything else the lane-sequential kernel)."""
+    state_bytes = int(rng.choice([16, 32, 64], p=[0.6, 0.25, 0.15]))
+    user = state_bytes - 8
+    pool = [I.MATERIALISE, I.CREATE, I.TOMBSTONE, I.THROW] if rng.random() < 0.7 else [I.IF_EXISTS, I.CREATE, I.TOMBSTONE, I.THROW]
+    rules = []
+    for t in range(int(rng.integers(1, 6))):
+        ex = int(rng.choice(pool, p=[0.6, 0.2, 0.1, 0.1])) if t else int(I.CREATE if pool[0] == I.IF_EXISTS else pool[int(rng.integers(0, 2))])
+        ops = []
+        for _ in range(int(rng.integers(0, 4))):
+            opc = int(rng.choice([I.OP_SET, I.OP_ADD_I32, I.OP_SUB_I32]))
+            ln = 4 if opc != I.OP_SET else min(int(rng.choice([4, 8])), user)
+            dst = 4 * int(rng.integers(0, (user - ln) // 4 + 1))
+            src = 4 if rng.random() < 0.2 and ln == 4 else 16 + 4 * int(rng.integers(0, (80 - ln) // 4 + 1))
+            ops.append((opc, dst, src, ln))
+        rules.append((ex, ops))
+    return state_bytes, rules
+
+
+def draw_var_log(rng, n_types, n_agg, long_len):
+    counts = rng.integers(0, 10, size=n_agg)
+    counts[rng.integers(0, n_agg)] = long_len
+    counts[rng.integers(0, n_agg, size=n_agg // 10)] = 0
+    n = int(counts.sum())
+    plen = rng.integers(80, 513, size=n)
+    short = rng.random(n) < 0.03
+    plen[short] = rng.integers(0, 80, size=int(short.sum()))          # too short for some event classes: those throw
+    rlen = 16 + ((plen + 15) // 16) * 16
+    rec_off = np.zeros(n + 1, dtype=np.uint64)
+    np.cumsum(rlen, out=rec_off[1:])
+    buf = rng.integers(0, 256, size=int(rec_off[-1]), dtype=np.uint8)
+    types = rng.integers(0, n_types, size=n).astype(np.uint32)
+    types[rng.random(n) < 0.004] = n_types
+    aggs = np.repeat(np.arange(n_agg, dtype=np.uint32), counts)
+    hdr = np.zeros((n, 4), dtype=np.uint32)
+    hdr[:, 0], hdr[:, 1], hdr[:, 2], hdr[:, 3] = types, np.arange(1, n + 1, dtype=np.uint32), plen.astype(np.uint32), aggs
+    hb = hdr.view(np.uint8).reshape(n, 16)
+    starts = rec_off[:-1].astype(np.int64)
+    for j in range(16):
+        buf[starts + j] = hb[:, j]
+    first = np.zeros(n_agg + 1, dtype=np.int64)
+    np.cumsum(counts, out=first[1:])
+    seg = rec_off[first].astype(np.uint64)
+    # malformed records: a payload length that runs past the end of its segment (last record of a few segments), and one absurd one
+    for a in rng.integers(0, n_agg, size=4):
+        if counts[a]:
+            j = int(first[a + 1] - 1)
+            buf[int(rec_off[j]) + 8:int(rec_off[j]) + 12] = np.frombuffer(np.uint32(int(plen[j]) + 64).tobytes(), np.uint8)
+    big = int(rng.integers(0, n))
+    buf[int(rec_off[big]) + 8:int(rec_off[big]) + 12] = np.frombuffer(np.uint32(0x7FFFFFF0).tobytes(), np.uint8)
+    return buf, seg, rec_off
+
+
+# ------------------------------------------------------------------ scale: programs whose kernel instantiation is known
+# Record words a row program may read: word 1 (seq) and the payload words 4..15 (words 2, 3 hold the aggregate index).
+SOURCE_WORDS = [1] + list(range(4, 16))
+
+
+def row_program(rng, user_words, cls, n_src):
+    """A program inside the transformer algebra (fold_rows.cu build_row_program): 32-bit SET/ADD/SUB ops only, no rule
+    writes a state word twice, and the ops read exactly `n_src` distinct record words, so the kernel sees
+    n_slots = 1 + n_src (slot 0 is the event type). cls 0: MATERIALISE / CREATE / TOMBSTONE / THROW; cls 1: IF_EXISTS /
+    CREATE / TOMBSTONE / THROW. Type 0 builds a state (MATERIALISE, or CREATE for class 1), type 1 carries the class."""
+    pool = [int(w) for w in rng.choice(SOURCE_WORDS, size=n_src, replace=False)]
+    base = I.MATERIALISE if cls == 0 else I.IF_EXISTS
+    n_op_rules = -(-n_src // user_words) + 1
+    n_types = min(16, n_op_rules + int(rng.integers(2, 5)))
+    exists = [I.MATERIALISE if cls == 0 else I.CREATE, base]
+    exists += [int(rng.choice([base, I.CREATE])) for _ in range(2, n_op_rules)]
+    exists += [int(rng.choice([base, base, I.CREATE, I.TOMBSTONE, I.THROW])) for _ in range(n_op_rules, n_types)]
+    todo = list(pool)
+    rng.shuffle(todo)
+    rules = []
+    for t, ex in enumerate(exists):
+        ops = []
+        if ex not in (I.TOMBSTONE, I.THROW):
+            dst_words = [int(w) for w in rng.permutation(user_words)]
+            n_ops = min(user_words, 8, len(todo)) if t < n_op_rules else int(rng.integers(0, min(user_words, 4) + 1))
+            n_ops = max(n_ops, min(user_words, 8, int(rng.integers(0, 3))))
+            for w in dst_words[:n_ops]:
+                src = todo.pop() if todo else int(rng.choice(pool))
+                ops.append((int(rng.choice([I.OP_SET, I.OP_ADD_I32, I.OP_SUB_I32])), 4 * w, 4 * src, 4))
+        rules.append((ex, ops))
+    assert not todo
+    return rules
+
+
+def type_mix(rules, n, rng, p_throw=2e-4):
+    """Event types for n records: throwing types (THROW rules, MatchErrors at n_types .. 16, 255, 2^32 - 1) with
+    probability p_throw, every other rule uniformly."""
+    ok = np.array([t for t, (ex, _) in enumerate(rules) if ex != I.THROW], dtype=np.uint32)
+    bad = np.array([t for t, (ex, _) in enumerate(rules) if ex == I.THROW] + list(range(len(rules), 17)) + [255, 0xFFFFFFFF],
+                   dtype=np.uint32)
+    types = ok[rng.integers(0, len(ok), size=n)]
+    hit = rng.random(n) < p_throw
+    types[hit] = bad[rng.integers(0, len(bad), size=int(hit.sum()))]
+    return types
+
+
+def shaped_counts(rng, n_agg, n_records, hot_share=0.25, step_records=256, empty_run=3000):
+    """Segment lengths for a CSR of about n_records records: one hot aggregate holding hot_share of the log and a second
+    one with a fifth of that, runs of `empty_run` empty segments at the start, the middle and the end, segments of exactly
+    one step, and segments that start and end on step and span multiples (step_records: the longest run-kernel step,
+    32 * 8 records). Returns (counts, hot, hot2)."""
+    rest = n_records - int(n_records * hot_share)
+    mean = rest / (n_agg - 3 * empty_run)
+    counts = rng.geometric(1.0 / (mean + 1), size=n_agg) - 1
+    counts[:empty_run] = 0
+    mid = n_agg // 2
+    counts[mid:mid + empty_run] = 0
+    counts[-empty_run:] = 0
+    hot, hot2 = empty_run + 1, n_agg - empty_run - 2
+    counts[hot] = int(n_records * hot_share)
+    counts[hot2] = int(n_records * hot_share / 5)
+    # a few aligned segments: pad the prefix to a multiple of a step, then 1, 2, 8 and 64 steps
+    for j, k in enumerate([1, 2, 8, 64, 1]):
+        a = mid + empty_run + 10 + 40 * j
+        pre = int(counts[:a].sum())
+        counts[a] += (-pre) % step_records
+        counts[a + 1] = k * step_records
+    return counts.astype(np.int64), hot, hot2
+
+
+def fixed_log(rng, rules, counts, f64_offsets=(), f64_values=SPECIAL_F64, pad_records=0, p_throw=2e-4):
+    """Fixed 64-byte records in CSR order for per-aggregate `counts`: random payload, types from type_mix, seq = position,
+    agg at +8. f64_offsets: record byte offsets that get values drawn from f64_values. pad_records: records in front of
+    the first segment (the CSR starts at a non-zero offset). Returns (buffer [pad + n, 64] u8, seg_offsets u64, aggs)."""
+    n = int(counts.sum())
+    buf = rng.integers(0, 256, size=(pad_records + n, 64), dtype=np.uint8)
+    rec = buf[pad_records:]
+    rec[:, 0:4] = type_mix(rules, n, rng, p_throw).view(np.uint8).reshape(-1, 4)
+    rec[:, 4:8] = np.arange(1, n + 1, dtype=np.uint32).view(np.uint8).reshape(-1, 4)
+    aggs = np.repeat(np.arange(len(counts), dtype=np.uint64), counts)
+    rec[:, 8:16] = aggs.view(np.uint8).reshape(-1, 8)
+    vals = np.asarray(f64_values, dtype=np.float64)
+    for off in f64_offsets:
+        rec[:, off:off + 8] = vals[rng.integers(0, len(vals), size=n)].view(np.uint8).reshape(-1, 8)
+    seg = np.zeros(len(counts) + 1, dtype=np.uint64)
+    np.cumsum(counts * 64, out=seg[1:])
+    seg += pad_records * 64
+    return buf, seg, aggs
+
+
+def set_type(buf, seg, agg, k, etype):
+    """Event type of record k of aggregate agg (k < 0 counts from the segment's end)."""
+    rec = np.asarray(buf).reshape(-1, 64)
+    lo, hi = int(seg[agg]) // 64, int(seg[agg + 1]) // 64
+    rec[(lo if k >= 0 else hi) + k, 0:4] = np.frombuffer(np.uint32(etype).tobytes(), np.uint8)
+
+
+def var_log(rng, rules, counts, payload_max, p_short=0.02, p_throw=2e-4, n_malformed=8):
+    """Variable records (SGR_REC_VAR16) in CSR order: payload lengths uniform in [80, payload_max] (a few shorter than
+    the ops of some event class read, which throw), a few records whose length runs past the end of their segment, and
+    one absurd length. Returns (log u8, seg_offsets u64, rec_offsets u64) — rec_offsets is the record directory."""
+    n = int(counts.sum())
+    plen = rng.integers(80, payload_max + 1, size=n)
+    short = rng.random(n) < p_short
+    plen[short] = rng.integers(0, 80, size=int(short.sum()))
+    plen[rng.integers(0, n, size=64)] = payload_max                     # at the cap, not past it
+    rlen = 16 + ((plen + 15) // 16) * 16
+    rec_off = np.zeros(n + 1, dtype=np.uint64)
+    np.cumsum(rlen, out=rec_off[1:])
+    buf = rng.integers(0, 256, size=int(rec_off[-1]), dtype=np.uint8)
+    hdr = np.zeros((n, 4), dtype=np.uint32)
+    hdr[:, 0] = type_mix(rules, n, rng, p_throw)
+    hdr[:, 1] = np.arange(1, n + 1, dtype=np.uint32)
+    hdr[:, 2] = plen.astype(np.uint32)
+    hdr[:, 3] = np.repeat(np.arange(len(counts), dtype=np.uint32), counts)
+    hb = hdr.view(np.uint8).reshape(n, 16)
+    starts = rec_off[:-1].astype(np.int64)
+    for j in range(16):
+        buf[starts + j] = hb[:, j]
+    first = np.zeros(len(counts) + 1, dtype=np.int64)
+    np.cumsum(counts, out=first[1:])
+    seg = rec_off[first].astype(np.uint64)
+    for a in rng.choice(np.nonzero(counts)[0], size=n_malformed, replace=False):
+        j = int(first[a + 1] - 1)
+        buf[int(rec_off[j]) + 8:int(rec_off[j]) + 12] = np.frombuffer(np.uint32(int(plen[j]) + 64).tobytes(), np.uint8)
+    big = int(rng.integers(0, n))
+    buf[int(rec_off[big]) + 8:int(rec_off[big]) + 12] = np.frombuffer(np.uint32(0x7FFFFFF0).tobytes(), np.uint8)
+    return buf, seg, rec_off

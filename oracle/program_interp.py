@@ -7,7 +7,8 @@ What it takes from the reference are the rules around the fold, restated exactly
   events.foldLeft(state)(handleEvent)                      CommandModels.scala:25-28
   handler throws -> ACKError, the actor keeps its state    PersistentActor.scala:260-263,303-309
   publish iff newState != oldState (Double fields: ==)     PersistentActor.scala:252-257
-Only tests/ may import it. One Python loop per event: use it on thousands of events, not millions.
+Only tests/ may import it. One Python loop per event: use it on thousands of events, not millions. The c_* functions at
+the end run the same semantics compiled (oracle/program_oracle.c) for logs of millions of records.
 """
 from __future__ import annotations
 
@@ -137,11 +138,12 @@ MAX_VAR_RECORD = 16 + 512   # include/sgr.h: a variable record is capped at 16 +
 
 
 def fold_var(rules: Sequence[Rule], state_bytes: int, log: np.ndarray, seg_offsets: Sequence[int], initial: Optional[np.ndarray] = None,
-             f64_fields: Sequence[int] = ()) -> np.ndarray:
+             f64_fields: Sequence[int] = (), max_record_bytes: int = MAX_VAR_RECORD) -> np.ndarray:
     """Variable records (SGR_REC_VAR16): 16-byte header {type, seq, payload_len, agg} + payload padded to 16 bytes. A record
-    that does not fit its segment, or is longer than the format allows, or is too short for the ops of its event class, is a
-    malformed event: the handler throws at that record. (Do not feed records between MAX_VAR_RECORD and 64 KiB: how
-    far past the cap a kernel still parses is an implementation detail the tests stay away from.)"""
+    that does not fit its segment, or is longer than the format allows (max_record_bytes, header included, before padding),
+    or is too short for the ops of its event class, is a malformed event: the handler throws at that record. (Do not feed
+    records between the cap and 64 KiB: how far past the cap a kernel still parses is an implementation detail the tests
+    stay away from.)"""
     user = state_bytes - 8
     buf = np.ascontiguousarray(log).view(np.uint8).reshape(-1).tobytes()
     n_agg = len(seg_offsets) - 1
@@ -160,7 +162,7 @@ def fold_var(rules: Sequence[Rule], state_bytes: int, log: np.ndarray, seg_offse
                     raise _Throw()
                 plen = struct.unpack_from("<I", buf, pos + 8)[0]
                 rlen = 16 + ((plen + 15) // 16) * 16
-                if 16 + plen > MAX_VAR_RECORD or rlen > end - pos:
+                if 16 + plen > max_record_bytes or rlen > end - pos:
                     raise _Throw()
                 cur = _handle(rules, user, cur, buf[pos:pos + rlen], avail=16 + plen)
             except _Throw:
@@ -177,3 +179,91 @@ def fold_var(rules: Sequence[Rule], state_bytes: int, log: np.ndarray, seg_offse
             flags |= ST_EXISTS
         out[i, user:] = np.frombuffer(struct.pack("<II", flags, err), dtype=np.uint8)
     return out
+
+
+# ------------------------------------------------------------------ the same semantics, compiled (oracle/program_oracle.c)
+# Same argument shapes as the Python functions above; each also returns (n_events, n_errors): the events applied (those after
+# a throw are dropped) and the aggregates whose handler threw. Use these at scale; tests/test_program_oracle_cpu.py pins
+# them to the Python loops.
+
+def _packed_program(rules: Sequence[Rule], state_bytes: int, f64_fields: Sequence[int]) -> np.ndarray:
+    """orc_program of program_oracle.c: state_bytes, n_types, n_f64, f64_off[8], exists[16], n_ops[16], ops[16][8][4]."""
+    p = np.zeros(3 + 8 + 16 + 16 + 16 * 8 * 4, dtype=np.uint32)
+    p[0], p[1], p[2] = state_bytes, len(rules), len(f64_fields)
+    p[3:3 + len(f64_fields)] = list(f64_fields)
+    ops = p[43:].reshape(16, 8, 4)
+    for t, (ex, tops) in enumerate(rules):
+        p[11 + t] = ex
+        p[27 + t] = len(tops)
+        for i, op in enumerate(tops):
+            ops[t, i] = op
+    return p
+
+
+def _lib():
+    from oracle import oracle as O
+    return O.lib()
+
+
+def _ptr(a):
+    return None if a is None else a.ctypes.data
+
+
+def _prior(initial, n_agg, state_bytes):
+    if initial is None:
+        return None
+    return np.ascontiguousarray(np.ascontiguousarray(initial).view(np.uint8).reshape(-1, state_bytes)[:n_agg])
+
+
+def c_fold(rules: Sequence[Rule], state_bytes: int, records: np.ndarray, seg_offsets, initial: Optional[np.ndarray] = None,
+           f64_fields: Sequence[int] = ()) -> Tuple[np.ndarray, int, int]:
+    """fold(): `records` starts at byte seg_offsets[0]."""
+    import ctypes as C
+    prog = _packed_program(rules, state_bytes, f64_fields)
+    recs = np.ascontiguousarray(records).view(np.uint8).reshape(-1)
+    off = np.ascontiguousarray(seg_offsets, dtype=np.uint64)
+    n_agg = len(off) - 1
+    if int(off[-1]) - int(off[0]) > recs.size:
+        raise ValueError("program oracle: CSR runs past the records")
+    out = np.zeros((n_agg, state_bytes), dtype=np.uint8)
+    ini = _prior(initial, n_agg, state_bytes)
+    nev, nerr = C.c_uint64(0), C.c_uint64(0)
+    if _lib().orc_prog_fold(_ptr(prog), _ptr(recs), _ptr(off), n_agg, _ptr(ini), _ptr(out), C.addressof(nev), C.addressof(nerr)):
+        raise ValueError("program oracle: malformed program or CSR")
+    return out, int(nev.value), int(nerr.value)
+
+
+def c_fold_var(rules: Sequence[Rule], state_bytes: int, log: np.ndarray, seg_offsets, initial: Optional[np.ndarray] = None,
+               f64_fields: Sequence[int] = (), max_record_bytes: int = MAX_VAR_RECORD) -> Tuple[np.ndarray, int, int]:
+    """fold_var(): seg_offsets are byte offsets into the whole `log`."""
+    import ctypes as C
+    prog = _packed_program(rules, state_bytes, f64_fields)
+    buf = np.ascontiguousarray(log).view(np.uint8).reshape(-1)
+    off = np.ascontiguousarray(seg_offsets, dtype=np.uint64)
+    n_agg = len(off) - 1
+    if n_agg and int(off[-1]) > buf.size:
+        raise ValueError("program oracle: CSR runs past the log")
+    out = np.zeros((n_agg, state_bytes), dtype=np.uint8)
+    ini = _prior(initial, n_agg, state_bytes)
+    nev, nerr = C.c_uint64(0), C.c_uint64(0)
+    if _lib().orc_prog_fold_var(_ptr(prog), max_record_bytes, _ptr(buf), _ptr(off), n_agg, _ptr(ini), _ptr(out),
+                                C.addressof(nev), C.addressof(nerr)):
+        raise ValueError("program oracle: malformed program or CSR")
+    return out, int(nev.value), int(nerr.value)
+
+
+def c_fold_arrival_order(rules: Sequence[Rule], state_bytes: int, records: np.ndarray, states: Optional[np.ndarray],
+                         f64_fields: Sequence[int] = (), n_agg: Optional[int] = None) -> Tuple[np.ndarray, int, int]:
+    """fold_arrival_order(). states=None folds from None everywhere onto a table of n_agg slots (what fold_unsorted does)."""
+    import ctypes as C
+    prog = _packed_program(rules, state_bytes, f64_fields)
+    recs = np.ascontiguousarray(records).view(np.uint8).reshape(-1)
+    if states is None:
+        table = np.zeros((int(n_agg), state_bytes), dtype=np.uint8)
+    else:
+        table = np.ascontiguousarray(states).view(np.uint8).reshape(-1, state_bytes).copy()
+    nev, nerr = C.c_uint64(0), C.c_uint64(0)
+    rc = _lib().orc_prog_fold_arrival(_ptr(prog), _ptr(recs), recs.size // 64, _ptr(table), table.shape[0], C.addressof(nev), C.addressof(nerr))
+    if rc:
+        raise ValueError("program oracle: aggregate index out of range" if rc == -1 else "program oracle: out of memory")
+    return table, int(nev.value), int(nerr.value)

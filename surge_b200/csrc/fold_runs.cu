@@ -58,9 +58,11 @@ __device__ __forceinline__ Xf<W> identity() {
 template <int W, int CLS = 1>
 __device__ __forceinline__ Xf<W> compose(const Xf<W>& a, const Xf<W>& b) {
   // class 1: b.ex == 0 means b holds only IF_EXISTS events (or nothing); they apply iff the state exists after a — a
-  // tombstoned prefix absorbs them. (In class 0, b.ex == 0 only for the identity, where the plain rule gives a too.)
-  if (CLS == 1 && b.ex == 0u && a.ex == EX_NONE) return a;
+  // tombstoned prefix absorbs them — but not a throw among them: a throwing event sets no exists-op, and the segment must
+  // still be replayed. (In class 0, b.ex == 0 only for the identity or a range of throwing events, where the plain rule
+  // gives a with b's error bit too.)
   Xf<W> r;
+  if (CLS == 1 && b.ex == 0u && a.ex == EX_NONE) { r = a; r.m |= b.m & M_ERR; return r; }
   r.m = a.m | b.m;
   r.ex = b.ex ? b.ex : a.ex;
 #pragma unroll

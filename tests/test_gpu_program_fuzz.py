@@ -10,68 +10,12 @@ import numpy as np
 import pytest
 
 from oracle import program_interp as I
+from oracle.program_corpus import draw_log, draw_program, draw_var_log, draw_var_program, interleave
 from surge_b200 import ReplayEngine, SgrError
 from surge_b200 import native as N
 from surge_b200 import programs as P
 
 pytestmark = pytest.mark.gpu
-
-SPECIAL_F64 = [0.0, -0.0, float("nan"), 1.5, float("inf"), -2.25]
-
-
-def draw_program(rng):
-    state_bytes = int(rng.choice([16, 32, 64, 48, 128], p=[0.35, 0.25, 0.2, 0.1, 0.1]))
-    user = state_bytes - 8
-    family = rng.choice(["class0", "class1", "mixed"], p=[0.45, 0.35, 0.2])
-    pool = {"class0": [I.MATERIALISE, I.CREATE, I.TOMBSTONE, I.THROW], "class1": [I.IF_EXISTS, I.CREATE, I.TOMBSTONE, I.THROW],
-            "mixed": [I.IF_EXISTS, I.MATERIALISE, I.CREATE, I.TOMBSTONE, I.THROW]}[family]
-    weights = {4: [0.55, 0.25, 0.1, 0.1], 5: [0.3, 0.3, 0.2, 0.1, 0.1]}[len(pool)]
-    wide_ops = rng.random() < 0.15
-    n_types = int(rng.integers(1, 7))
-    rules = []
-    for t in range(n_types):
-        ex = int(rng.choice(pool, p=weights)) if t else int(pool[0] if rng.random() < 0.5 else pool[1])   # type 0 creates something
-        ops = []
-        for _ in range(int(rng.integers(0, 5))):
-            opc = int(rng.choice([I.OP_SET, I.OP_ADD_I32, I.OP_SUB_I32])) if not wide_ops else int(rng.integers(0, 5))
-            ln = 4 if opc in (I.OP_ADD_I32, I.OP_SUB_I32) else 8 if opc in (I.OP_ADD_I64, I.OP_SUB_I64) else int(rng.choice([4, 8, 12, 16]))
-            ln = min(ln, user)
-            if opc in (I.OP_ADD_I64, I.OP_SUB_I64) and user < 8:
-                continue
-            dst = 4 * int(rng.integers(0, (user - ln) // 4 + 1))
-            src = 4 if rng.random() < 0.2 and ln == 4 else 16 + 4 * int(rng.integers(0, (48 - ln) // 4 + 1))
-            ops.append((opc, dst, src, ln))
-        rules.append((ex, ops))
-    f64 = []
-    if user >= 16 and rng.random() < 0.4:
-        off = 8 * int(rng.integers(0, user // 8))
-        f64 = [off]
-        # make sure some rule copies a double into that field, from an 8-aligned payload offset
-        t = int(rng.integers(0, n_types))
-        if rules[t][0] not in (I.TOMBSTONE, I.THROW):
-            rules[t] = (rules[t][0], list(rules[t][1])[:3] + [(I.OP_SET, off, 24, 8)])
-    return state_bytes, rules, f64
-
-
-def draw_log(rng, n_types, n_agg, long_len, f64):
-    counts = rng.integers(0, 13, size=n_agg)
-    counts[rng.integers(0, n_agg)] = long_len
-    counts[rng.integers(0, n_agg, size=n_agg // 10)] = 0
-    n = int(counts.sum())
-    rec = rng.integers(0, 256, size=(n, 64), dtype=np.uint8)
-    types = rng.integers(0, n_types, size=n).astype(np.uint32)
-    types[rng.random(n) < 0.004] = n_types                       # scala.MatchError
-    rec[:, 0:4] = types.view(np.uint8).reshape(-1, 4)
-    rec[:, 4:8] = np.arange(1, n + 1, dtype=np.uint32).view(np.uint8).reshape(-1, 4)
-    aggs = np.repeat(np.arange(n_agg, dtype=np.uint64), counts)
-    rec[:, 8:16] = aggs.view(np.uint8).reshape(-1, 8)
-    if f64:
-        hit = rng.random(n) < 0.5
-        vals = np.asarray(SPECIAL_F64)[rng.integers(0, len(SPECIAL_F64), size=n)]
-        rec[hit, 24:32] = vals[hit].view(np.uint8).reshape(-1, 8)
-    off = np.zeros(n_agg + 1, dtype=np.uint64)
-    np.cumsum(counts * 64, out=off[1:])
-    return rec, off, aggs
 
 
 def same(got, want, what):
@@ -130,69 +74,7 @@ def test_random_program_all_paths(seed):
             same(e.export_states(), table, f"{what} micro-batch {b}")
 
 
-def interleave(rng, aggs):
-    """A permutation that shuffles aggregates against each other but keeps every aggregate's records in order
-    (what a Kafka partition log looks like). `aggs` is in CSR order (non-decreasing)."""
-    t = rng.random(len(aggs))
-    times = t[np.lexsort((t, aggs))]     # within each aggregate the arrival times ascend with the log position
-    return np.argsort(times, kind="stable")
-
-
 # ------------------------------------------------------------------ variable records (SGR_REC_VAR16)
-def draw_var_program(rng):
-    """Like draw_program, with payload reads up to 80 bytes into the record and 16/32-byte states more likely (the
-    record-parallel variable-record kernel takes 16-byte class-0 programs, everything else the lane-sequential kernel)."""
-    state_bytes = int(rng.choice([16, 32, 64], p=[0.6, 0.25, 0.15]))
-    user = state_bytes - 8
-    pool = [I.MATERIALISE, I.CREATE, I.TOMBSTONE, I.THROW] if rng.random() < 0.7 else [I.IF_EXISTS, I.CREATE, I.TOMBSTONE, I.THROW]
-    rules = []
-    for t in range(int(rng.integers(1, 6))):
-        ex = int(rng.choice(pool, p=[0.6, 0.2, 0.1, 0.1])) if t else int(I.CREATE if pool[0] == I.IF_EXISTS else pool[int(rng.integers(0, 2))])
-        ops = []
-        for _ in range(int(rng.integers(0, 4))):
-            opc = int(rng.choice([I.OP_SET, I.OP_ADD_I32, I.OP_SUB_I32]))
-            ln = 4 if opc != I.OP_SET else min(int(rng.choice([4, 8])), user)
-            dst = 4 * int(rng.integers(0, (user - ln) // 4 + 1))
-            src = 4 if rng.random() < 0.2 and ln == 4 else 16 + 4 * int(rng.integers(0, (80 - ln) // 4 + 1))
-            ops.append((opc, dst, src, ln))
-        rules.append((ex, ops))
-    return state_bytes, rules
-
-
-def draw_var_log(rng, n_types, n_agg, long_len):
-    counts = rng.integers(0, 10, size=n_agg)
-    counts[rng.integers(0, n_agg)] = long_len
-    counts[rng.integers(0, n_agg, size=n_agg // 10)] = 0
-    n = int(counts.sum())
-    plen = rng.integers(80, 513, size=n)
-    short = rng.random(n) < 0.03
-    plen[short] = rng.integers(0, 80, size=int(short.sum()))          # too short for some event classes: those throw
-    rlen = 16 + ((plen + 15) // 16) * 16
-    rec_off = np.zeros(n + 1, dtype=np.uint64)
-    np.cumsum(rlen, out=rec_off[1:])
-    buf = rng.integers(0, 256, size=int(rec_off[-1]), dtype=np.uint8)
-    types = rng.integers(0, n_types, size=n).astype(np.uint32)
-    types[rng.random(n) < 0.004] = n_types
-    aggs = np.repeat(np.arange(n_agg, dtype=np.uint32), counts)
-    hdr = np.zeros((n, 4), dtype=np.uint32)
-    hdr[:, 0], hdr[:, 1], hdr[:, 2], hdr[:, 3] = types, np.arange(1, n + 1, dtype=np.uint32), plen.astype(np.uint32), aggs
-    hb = hdr.view(np.uint8).reshape(n, 16)
-    starts = rec_off[:-1].astype(np.int64)
-    for j in range(16):
-        buf[starts + j] = hb[:, j]
-    first = np.zeros(n_agg + 1, dtype=np.int64)
-    np.cumsum(counts, out=first[1:])
-    seg = rec_off[first].astype(np.uint64)
-    # malformed records: a payload length that runs past the end of its segment (last record of a few segments), and one absurd one
-    for a in rng.integers(0, n_agg, size=4):
-        if counts[a]:
-            j = int(first[a + 1] - 1)
-            buf[int(rec_off[j]) + 8:int(rec_off[j]) + 12] = np.frombuffer(np.uint32(int(plen[j]) + 64).tobytes(), np.uint8)
-    big = int(rng.integers(0, n))
-    buf[int(rec_off[big]) + 8:int(rec_off[big]) + 12] = np.frombuffer(np.uint32(0x7FFFFFF0).tobytes(), np.uint8)
-    return buf, seg, rec_off
-
-
 @pytest.mark.parametrize("seed", range(16))
 def test_random_program_variable_records(seed):
     rng = np.random.default_rng(7000 + seed)

@@ -1,0 +1,160 @@
+"""No GPU: the compiled fold-program oracle (oracle/program_oracle.c) equals the Python interpreter
+(oracle/program_interp.py) and the sample-model oracle (oracle/sgr_oracle.c).
+
+tests/test_gpu_program_scale.py checks the kernels against the compiled oracle at millions of records; this file is what
+ties that oracle to the written semantics: the same random programs and logs through both restatements, byte for byte,
+and its statistics against what the interpreter's table implies.
+"""
+import numpy as np
+import pytest
+
+from oracle import oracle as O
+from oracle import program_corpus as PC
+from oracle import program_interp as I
+from surge_b200 import programs as P
+from surge_b200 import synth as S
+
+
+def same(got, want, what):
+    if not np.array_equal(got, want):
+        bad = np.nonzero((got != want).any(axis=1))[0]
+        raise AssertionError(f"{what}: {len(bad)} of {len(want)} states differ; first {bad[:6]}\n got {got[bad[0]].tolist()}\nwant {want[bad[0]].tolist()}")
+
+
+def implied_stats(table, state_bytes, counts):
+    """(n_events, n_errors) a fold table implies: a throwing aggregate applied err_idx events, any other all of them."""
+    t = np.ascontiguousarray(table).reshape(-1, state_bytes)
+    flags = t[:, state_bytes - 8:state_bytes - 4].copy().view(np.uint32).ravel()
+    err = t[:, state_bytes - 4:].copy().view(np.uint32).ravel().astype(np.int64)
+    threw = (flags & I.ST_ERROR) != 0
+    return int(np.where(threw, err, np.asarray(counts, dtype=np.int64)).sum()), int(threw.sum())
+
+
+def rules_of(prog):
+    return [(int(prog.rules[t].exists_rule), [(int(o.opcode), int(o.dst_off), int(o.src_off), int(o.len))
+                                               for o in list(prog.rules[t].ops)[:prog.rules[t].n_ops]]) for t in range(prog.n_types)]
+
+
+@pytest.mark.parametrize("seed", range(160))
+def test_fixed_records_match_the_interpreter(seed):
+    """Random programs (every state width, 64-bit ops, f64 fields, all exists rules) on a CSR log, from None and on top
+    of the first table, and a CSR that starts at a non-zero offset."""
+    rng = np.random.default_rng(31000 + seed)
+    state_bytes, rules, f64 = PC.draw_program(rng)
+    rec, off, _ = PC.draw_log(rng, len(rules), 90, 150, f64)
+    counts = np.diff(off.astype(np.int64)) // 64
+    want = I.fold(rules, state_bytes, rec, off, f64_fields=f64)
+    got, nev, nerr = I.c_fold(rules, state_bytes, rec, off, f64_fields=f64)
+    what = f"seed {seed} state_bytes {state_bytes} rules {rules} f64 {f64}"
+    same(got, want, what)
+    assert (nev, nerr) == implied_stats(want, state_bytes, counts), what
+    rec2, off2, _ = PC.draw_log(rng, len(rules), 90, 40, f64)
+    off2 = off2 + 64 * 5                               # the records start at the first segment's offset
+    want2 = I.fold(rules, state_bytes, rec2, off2, initial=want, f64_fields=f64)
+    got2, nev2, nerr2 = I.c_fold(rules, state_bytes, rec2, off2, initial=want, f64_fields=f64)
+    same(got2, want2, what + " with prior states")
+    assert (nev2, nerr2) == implied_stats(want2, state_bytes, np.diff(off2.astype(np.int64)) // 64), what
+
+
+@pytest.mark.parametrize("seed", range(60))
+def test_arrival_order_matches_the_interpreter(seed):
+    """Micro-batches onto a live table (per-batch flags cleared, untouched slots kept), and the from-None form."""
+    rng = np.random.default_rng(32000 + seed)
+    state_bytes, rules, f64 = PC.draw_program(rng)
+    n_agg = 80
+    rec, off, aggs = PC.draw_log(rng, len(rules), n_agg, 100, f64)
+    perm = PC.interleave(rng, aggs)
+    want = I.fold(rules, state_bytes, rec, off, f64_fields=f64)
+    got, _, _ = I.c_fold_arrival_order(rules, state_bytes, rec[perm], None, f64_fields=f64, n_agg=n_agg)
+    what = f"seed {seed} state_bytes {state_bytes} rules {rules} f64 {f64}"
+    same(got, want, what + " from None")
+    table = want
+    for b in range(3):
+        recb, _, aggb = PC.draw_log(rng, len(rules), n_agg, [30, 5, 200][b], f64)
+        keep = rng.random(len(recb)) < 0.6                    # not every aggregate is touched
+        batch = recb[PC.interleave(rng, aggb)][keep[: len(recb)]]
+        want_b = I.fold_arrival_order(rules, state_bytes, batch, table, f64_fields=f64)
+        got_b, nev, nerr = I.c_fold_arrival_order(rules, state_bytes, batch, table, f64_fields=f64)
+        same(got_b, want_b, f"{what} batch {b}")
+        touched = np.bincount(batch[:, 8:16].copy().view(np.uint64).ravel().astype(np.int64), minlength=n_agg)
+        assert (nev, nerr) == implied_stats(want_b, state_bytes, touched), what
+        table = want_b
+    bad = rec[:3].copy()
+    bad[1, 8:16] = np.frombuffer(np.uint64(n_agg).tobytes(), np.uint8)
+    with pytest.raises(ValueError):
+        I.c_fold_arrival_order(rules, state_bytes, bad, table, f64_fields=f64)
+
+
+@pytest.mark.parametrize("max_record_bytes", [528, 1040, 2064])
+@pytest.mark.parametrize("seed", range(30))
+def test_variable_records_match_the_interpreter(seed, max_record_bytes):
+    """SGR_REC_VAR16 logs with short, overlong and truncated records, from None and with prior states, under each cap."""
+    rng = np.random.default_rng(33000 + seed)
+    state_bytes, rules = PC.draw_var_program(rng)
+    counts = rng.integers(0, 8, size=70)
+    counts[int(rng.integers(0, 70))] = 120
+    buf, seg, _ = PC.var_log(rng, rules, counts, max_record_bytes - 16 + 32, p_short=0.05, p_throw=0.01, n_malformed=3)
+    what = f"seed {seed} cap {max_record_bytes} state_bytes {state_bytes} rules {rules}"
+    want = I.fold_var(rules, state_bytes, buf, seg, max_record_bytes=max_record_bytes)
+    got, nev, nerr = I.c_fold_var(rules, state_bytes, buf, seg, max_record_bytes=max_record_bytes)
+    same(got, want, what)
+    t = want.reshape(-1, state_bytes)
+    assert nerr == int(((t[:, state_bytes - 8] & I.ST_ERROR) != 0).sum()), what
+    want2 = I.fold_var(rules, state_bytes, buf, seg, initial=want, max_record_bytes=max_record_bytes)
+    got2, _, _ = I.c_fold_var(rules, state_bytes, buf, seg, initial=want, max_record_bytes=max_record_bytes)
+    same(got2, want2, what + " with prior states")
+
+
+def test_the_draws_cover_what_the_pin_claims():
+    """The random programs above reach every state width, the 64-bit ops, Double fields and every exists rule."""
+    widths, ops, f64s, rules_seen = set(), set(), 0, set()
+    for seed in range(160):
+        state_bytes, rules, f64 = PC.draw_program(np.random.default_rng(31000 + seed))
+        widths.add(state_bytes); f64s += bool(f64)
+        for ex, tops in rules:
+            rules_seen.add(ex); ops.update(o[0] for o in tops)
+    assert widths == {16, 32, 48, 64, 128}
+    assert ops == {I.OP_SET, I.OP_ADD_I32, I.OP_SUB_I32, I.OP_ADD_I64, I.OP_SUB_I64}
+    assert rules_seen == {I.IF_EXISTS, I.MATERIALISE, I.CREATE, I.TOMBSTONE, I.THROW}
+    assert f64s >= 20
+
+
+SAMPLE_MODELS = [("counter", O.MODEL_COUNTER, P.counter_program), ("ml_counter", O.MODEL_ML_COUNTER, P.ml_counter_program),
+                 ("int_balance", O.MODEL_INT_BALANCE, P.int_balance_program), ("bank_account", O.MODEL_BANK_ACCOUNT, P.bank_account_program)]
+
+
+@pytest.mark.parametrize("name,model,make", SAMPLE_MODELS, ids=[m[0] for m in SAMPLE_MODELS])
+def test_sample_programs_match_the_sample_model_oracle(name, model, make):
+    """The four sample programs through the program oracle equal the hand-written Scala restatement, over 10^6 events
+    with throws, MatchErrors and (BankAccount) special Doubles, from None and on top of the first table."""
+    rng = np.random.default_rng(34000 + model)
+    prog = make()
+    rules, sb = rules_of(prog), int(prog.state_bytes)
+    f64 = [int(prog.f64_field_off[i]) for i in range(prog.n_f64_fields)]
+    counts = rng.integers(1, 10, size=250_000)
+    counts[17] = 20_000
+    counts[rng.integers(0, len(counts), size=30_000)] = 0
+    if model == O.MODEL_BANK_ACCOUNT:
+        n = int(counts.sum())
+        rec = rng.integers(0, 256, size=(n, 64), dtype=np.uint8)
+        types = np.where(rng.random(n) < 0.3, 0, 1).astype(np.uint32)
+        types[rng.random(n) < 0.001] = 2                                       # scala.MatchError
+        rec[:, 0:4] = types.view(np.uint8).reshape(-1, 4)
+        rec[:, 8:16] = np.repeat(np.arange(len(counts), dtype=np.uint64), counts).view(np.uint8).reshape(-1, 8)
+        rec[:, 32:40] = np.asarray(PC.SPECIAL_F64)[rng.integers(0, len(PC.SPECIAL_F64), size=n)].view(np.uint8).reshape(-1, 8)
+        off = np.zeros(len(counts) + 1, np.uint64)
+        np.cumsum(counts * 64, out=off[1:])
+    else:
+        rec, off = S.counter_csr(len(counts), counts, seed=71 + model, p_throw=0.0005)
+        if model == O.MODEL_INT_BALANCE:
+            rec = rec.copy()
+            rec["type"] = np.where(rng.random(len(rec)) < 0.001, 1, 0)        # type 1 is a MatchError for IntBalance
+    assert int(off[-1]) // 64 >= 1_000_000
+    want, nev, nerr = O.fold_packed(model, O.REC_FIXED64, rec, off)
+    got, gev, gerr = I.c_fold(rules, sb, rec, off, f64_fields=f64)
+    same(got, want, name)
+    assert (gev, gerr) == (nev, nerr) and nerr > 0, name
+    want2, nev2, nerr2 = O.fold_packed(model, O.REC_FIXED64, rec, off, want)
+    got2, gev2, gerr2 = I.c_fold(rules, sb, rec, off, initial=want, f64_fields=f64)
+    same(got2, want2, name + " with prior states")
+    assert (gev2, gerr2) == (nev2, nerr2), name
