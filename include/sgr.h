@@ -252,6 +252,20 @@ int32_t sgr_get(sgr_engine* e, const uint8_t* key, uint32_t klen,
 int32_t sgr_get_index(sgr_engine* e, uint64_t agg, void* out, uint32_t cap,
                       uint32_t* outlen, int32_t* exists, uint32_t* flags, uint32_t* err_idx);
 
+/* Recovery reads of many aggregate ids in one call, served from the device table (getAggregateBytes for a batch).
+ * Key i = keys[key_offsets[i] .. key_offsets[i+1]). Row i of `out` (state_bytes-8 bytes) = program bytes of key i,
+ * all zero when the state is None or the id is unknown. flags (optional, n x u32): the state's SGR_ST_* flags, 0 for an
+ * unknown id. indices (optional, n x i64): dense index, or -1 for an unknown id.
+ * Answers what sgr_get / sgr_get_index answer for each id, from the same key table (sgr_load_keys, or the ids an ingest
+ * appended). The ids are looked up in an index on the device, extended by the first call after ids are appended (only the new
+ * ids are uploaded) and rebuilt after sgr_load_keys or a new ingest; the host snapshot of sgr_get is not used. The call holds
+ * the engine's operation lock throughout and waits for an sgr_fold_async first: every row of a batch comes from one table
+ * generation, and batch readers serialise (one call should carry many ids). SGR_ERR_STATE before any fold; SGR_ERR_INVALID on
+ * non-monotone key_offsets or a duplicate id in the key table; SGR_ERR_CAPACITY (nothing written) when
+ * cap < n * (state_bytes - 8). n == 0 is a no-op. */
+int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n,
+                      void* out, uint64_t cap, uint32_t* flags, int64_t* indices);
+
 /* Export the whole state table (n_agg * state_bytes) and, optionally, bitmaps
  * (bit i of byte i/8, LSB first). Any out pointer may be NULL. */
 int32_t sgr_export_states(sgr_engine* e, void* out, uint64_t cap,

@@ -84,6 +84,19 @@ JNIEXPORT jbyteArray JNICALL Java_surge_gpu_Native_00024_get(JNIEnv* env, jobjec
   (*env)->SetByteArrayRegion(env, r, 0, (jsize)outlen, (const jbyte*)out);
   return r;
 }
+/* out and flags are direct buffers of n rows of (state_bytes - 8) bytes and n u32; SGR_ERR_CAPACITY when out is too short */
+JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_getBatch(JNIEnv* env, jobject o, jlong h, jobject keys, jobject offs, jlong n, jobject out, jobject flags) {
+  int ok = 1;
+  const uint32_t* ko = n >= 0 ? (const uint32_t*)direct(env, offs, (n + 1) * 4, "keyOffsets: direct buffer of (n + 1) u32", &ok) : 0;
+  if (!ok || !ko) return n < 0 ? bad_arg(env, "n must be non-negative") : SGR_ERR_INVALID;
+  const uint8_t* k = ko[n] ? (const uint8_t*)direct(env, keys, (jlong)ko[n], "keys: direct buffer shorter than keyOffsets[n]", &ok) : 0;
+  uint32_t* fl = ok ? (uint32_t*)direct(env, flags, n * 4, "flags: direct buffer of n u32", &ok) : 0;
+  void* rows = ok ? direct(env, out, 0, "out: direct buffer", &ok) : 0;
+  if (!ok) return SGR_ERR_INVALID;
+  int32_t rc = sgr_get_batch(H(h), k, ko, (uint64_t)n, rows, (uint64_t)(*env)->GetDirectBufferCapacity(env, out), fl, 0);
+  if (rc != SGR_OK) throw_for(env, H(h), rc);
+  return rc;
+}
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_exportStates(JNIEnv* env, jobject o, jlong h, jobject out, jobject changed) {
   return sgr_export_states(H(h), (*env)->GetDirectBufferAddress(env, out), (uint64_t)(*env)->GetDirectBufferCapacity(env, out), 0,
                            changed ? (uint8_t*)(*env)->GetDirectBufferAddress(env, changed) : 0, 0);

@@ -225,6 +225,37 @@ class GpuReplayKeyValueStore(storeName: String) extends KeyValueStore[Bytes, Arr
     if (packed == null) null else reg.codec.fromPacked(id, packed)
   }
 
+  /** get() for many keys: unflushed puts answer first, the rest go to the device in one sgr_get_batch call. */
+  def getBatch(batch: Seq[Bytes]): Seq[Array[Byte]] = {
+    if (!open) throw new InvalidStateStoreException(s"store $storeName is not open")
+    val ids = batch.map(k => new String(k.get(), "UTF-8"))
+    val out = new Array[Array[Byte]](batch.size)
+    val rest = ids.indices.filter { i =>
+      val u = unflushed.get(ids(i))
+      if (u != null) out(i) = u.map(_.clone()).orNull
+      u == null
+    }
+    if (rest.nonEmpty && folded) {
+      val user = reg.program.duplicate().order(ByteOrder.LITTLE_ENDIAN).getInt(0) - 8 // state_bytes is the first field
+      val offs = ByteBuffer.allocateDirect(4 * (rest.size + 1)).order(ByteOrder.LITTLE_ENDIAN)
+      val blob = new java.io.ByteArrayOutputStream()
+      offs.putInt(0)
+      rest.foreach { i => blob.write(batch(i).get()); offs.putInt(blob.size()) }
+      val kb = ByteBuffer.allocateDirect(math.max(blob.size(), 1)); kb.put(blob.toByteArray); kb.flip(); offs.flip()
+      val rows = ByteBuffer.allocateDirect(user * rest.size)
+      val flags = ByteBuffer.allocateDirect(4 * rest.size).order(ByteOrder.LITTLE_ENDIAN)
+      check(Native.getBatch(handle, kb, offs, rest.size.toLong, rows, flags))
+      rest.zipWithIndex.foreach { case (i, r) =>
+        if ((flags.getInt(4 * r) & 1) != 0) { // SGR_ST_EXISTS
+          val packed = new Array[Byte](user)
+          rows.position(r * user); rows.get(packed)
+          out(i) = reg.codec.fromPacked(ids(i), packed)
+        }
+      }
+    }
+    out.toSeq
+  }
+
   /** Snapshot of the keys in Bytes order (unsigned lexicographic over the UTF-8 bytes), values resolved lazily through get(). */
   private def orderedIterator(from: Bytes, to: Bytes): KeyValueIterator[Bytes, Array[Byte]] = {
     if (!open) throw new InvalidStateStoreException(s"store $storeName is not open")
@@ -277,5 +308,28 @@ class GpuReplayKeyValueStore(storeName: String) extends KeyValueStore[Bytes, Arr
     try { open = false; if (handle != 0L) Native.destroy(handle); handle = 0L }
     finally lock.writeLock().unlock()
     log.info(s"GPU replay state store '$storeName' closed")
+  }
+}
+
+/** The coalescing reader of surge_b200/store.py AggregateStateStore(coalesce_reads_us > 0): getAggregateBytes calls that arrive
+ *  within `windowMicros` of the first one are answered by one getBatch (one device call); each promise gets its own row, or the
+ *  batch's exception. The one-id-per-call recovery reads of PersistentActor reach the batch path without a change on their side. */
+class CoalescingAggregateReader(store: GpuReplayKeyValueStore, windowMicros: Long)(implicit ec: scala.concurrent.ExecutionContext) {
+  private val lock = new Object
+  private var waiting: List[(String, scala.concurrent.Promise[Option[Array[Byte]]])] = Nil
+  private var open = false
+
+  def getAggregateBytes(aggregateId: String): scala.concurrent.Future[Option[Array[Byte]]] = {
+    val p = scala.concurrent.Promise[Option[Array[Byte]]]()
+    val first = lock.synchronized { waiting = (aggregateId, p) :: waiting; val f = !open; open = true; f }
+    if (first) scala.concurrent.Future {
+      Thread.sleep(windowMicros / 1000, ((windowMicros % 1000) * 1000).toInt)
+      val batch = lock.synchronized { val b = waiting.reverse; waiting = Nil; open = false; b }
+      try {
+        val rows = store.getBatch(batch.map { case (id, _) => Bytes.wrap(id.getBytes("UTF-8")) })
+        batch.zip(rows).foreach { case ((_, pr), row) => pr.success(Option(row)) }
+      } catch { case e: Throwable => batch.foreach { case (_, pr) => pr.failure(e) } }
+    }
+    p.future
   }
 }

@@ -24,6 +24,9 @@ object Native {
   @native def loadKeys(handle: Long, keys: ByteBuffer, keyOffsets: ByteBuffer, nAgg: Long): Int // sgr_load_keys
   /** returns null for None, the program bytes otherwise; throws on a non-OK status */
   @native def get(handle: Long, key: Array[Byte]): Array[Byte]                     // sgr_get
+  /** n ids (keys[keyOffsets(i) until keyOffsets(i+1)], u32 offsets) in one device call: row i of `out` = program bytes
+   * (stateBytes - 8, zero for None / unknown), flags(i) = SGR_ST_* (0 for an unknown id); returns the status */
+  @native def getBatch(handle: Long, keys: ByteBuffer, keyOffsets: ByteBuffer, n: Long, out: ByteBuffer, flags: ByteBuffer): Int // sgr_get_batch
   @native def exportStates(handle: Long, out: ByteBuffer, changedBits: ByteBuffer): Int // sgr_export_states
   @native def partitionForKey(key: Array[Byte], numPartitions: Int, upToColon: Boolean): Int // sgr_partition_for_key_utf8
 

@@ -301,70 +301,6 @@ __global__ void dg_key_copy_kernel(const uint2* __restrict__ key_ref, const uint
   for (uint32_t k = part; k < ref.y; k += 8) dst[k] = src[k];
 }
 
-__device__ __forceinline__ unsigned long long hash_id(const uint8_t* k, uint32_t len) {
-  unsigned long long h = 0x9e3779b97f4a7c15ull ^ ((unsigned long long)len * 0xff51afd7ed558ccdull);
-  while (len >= 8) {
-    unsigned long long w = 0;
-    for (int q = 7; q >= 0; --q) w = (w << 8) | k[q];
-    h = (h ^ w) * 0x9fb21c651e98df25ull; h ^= h >> 32; k += 8; len -= 8;
-  }
-  if (len) {
-    unsigned long long w = 0;
-    for (int q = (int)len - 1; q >= 0; --q) w = (w << 8) | k[q];
-    h = (h ^ w) * 0x9fb21c651e98df25ull; h ^= h >> 32;
-  }
-  h *= 0xc4ceb9fe1a85ec53ull; h ^= h >> 29;
-  return h ? h : 1ull;
-}
-
-__device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) {
-  uint32_t v;
-  asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p));
-  return v;
-}
-
-// id -> dense index. Returns 0xffffffff when the dictionary is full (the call then fails as a whole).
-__device__ uint32_t intern(const DgDict& d, const uint8_t* id, uint32_t len) {
-  const unsigned long long h = hash_id(id, len);
-  uint64_t pos = h & d.slots_mask;
-  for (uint64_t probes = 0; probes <= d.slots_mask; ++probes, pos = (pos + 1) & d.slots_mask) {
-    unsigned long long tag = __ldcg(d.tags + pos);
-    if (tag == 0ull) {
-      tag = atomicCAS(d.tags + pos, 0ull, h);
-      if (tag == 0ull) {   // this thread owns the slot: the id is new
-        const unsigned long long idx = atomicAdd(d.ctl + 0, 1ull);
-        const unsigned long long need = ((unsigned long long)len + 7) & ~7ull;
-        const unsigned long long off = atomicAdd(d.ctl + 1, need);
-        if (idx >= d.max_keys || off + need > d.arena_cap) {
-          atomicAdd(d.ctl + 5, 1ull);
-          __threadfence();
-          atomicExch(d.slot_idx + pos, 0xffffffffu);
-          return 0xffffffffu;
-        }
-        for (uint32_t k = 0; k < len; ++k) d.arena[off + k] = id[k];
-        d.key_ref[idx] = make_uint2((uint32_t)(off >> 3), len);
-        __threadfence();
-        atomicExch(d.slot_idx + pos, (uint32_t)idx + 1u);
-        return (uint32_t)idx;
-      }
-    }
-    if (tag != h) continue;
-    uint32_t v;
-    while ((v = ld_volatile_u32(d.slot_idx + pos)) == 0u) __nanosleep(40);   // the owner is still writing the id
-    if (v == 0xffffffffu) return 0xffffffffu;
-    __threadfence();
-    // (L2 loads: an L1 line fetched before the owner wrote its part would be stale)
-    const uint2 ref = __ldcg(d.key_ref + (v - 1u));
-    if (ref.y != len) continue;                                               // same 64-bit hash, another id: keep probing
-    const uint8_t* have = d.arena + ((unsigned long long)ref.x << 3);
-    bool same = true;
-    for (uint32_t k = 0; k < len && same; ++k) same = __ldcg(have + k) == id[k];
-    if (same) return v - 1u;
-  }
-  atomicAdd(d.ctl + 5, 1ull);
-  return 0xffffffffu;
-}
-
 __global__ void __launch_bounds__(kThreads) dg_parse_kernel(const __grid_constant__ DgParse p) {
   const uint32_t i = p.rec_begin + blockIdx.x * kThreads + threadIdx.x;
   if (i >= p.n_records) return;

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "id_dict.cuh"
+
 namespace sgr {
 
 // error codes a kernel leaves in DgBatch::err (0 = fine); dingest.cu turns them into messages
@@ -27,18 +29,6 @@ struct DgBatch {
   uint64_t arena_off;    // in (decode pass): where the decompressed section goes
   uint32_t err;          // out: DgErr
   uint32_t err_record;   // out: record index the error refers to
-};
-
-struct DgDict {           // device id dictionary: open addressing on a 64-bit hash, ids compared byte for byte
-  unsigned long long* tags;   // [slots] 0 = empty, else the id's hash (never 0)
-  uint32_t* slot_idx;         // [slots] dense index + 1 once the owner has published the id (0 = not yet)
-  uint2* key_ref;             // [max_keys] (arena offset in 8-byte units, length) of dense index i
-  uint8_t* arena;             // id bytes, 8-byte aligned entries
-  unsigned long long* ctl;    // [0] n_keys [1] arena bytes used [2] records dropped as markers [3] null values [4] duplicates
-                              // [5] dictionary overflow (keys or arena) [6] packed records written (non-holes)
-                              // [8] [9] [10] decode arena: bytes claimed, capacity, overflow flag (dg_launch_crc_size_fast)
-  uint64_t slots_mask;        // slots - 1 (power of two)
-  uint64_t max_keys, arena_cap;
 };
 
 struct DgParse {

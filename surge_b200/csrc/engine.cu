@@ -20,6 +20,7 @@
 #include "fold_kernels.cuh"
 #include "fold_rows.cuh"
 #include "group_kernels.cuh"
+#include "id_index.cuh"
 #include "incremental.cuh"
 #include "keytable.h"
 #include "route_push.cuh"
@@ -129,6 +130,13 @@ struct sgr_engine {
   std::vector<uint32_t> ing_key_offs;
   const void* ing_keys_from = nullptr;      // whose dictionary the appended ids mirror (an sgr_ingest or an sgr_dingest)
   std::atomic<bool> keys_stale{false};
+  uint64_t keys_epoch = 0;                  // bumped (under keys_mu) whenever the key table is replaced rather than appended to
+  // sgr_get_batch: the device id index, kept up to date lazily like the host KeyTable (under op_mu, then keys_mu), and its
+  // staging: one page-locked buffer (ids and queries up, results down) and one device buffer (queries, results)
+  IdIndex id_index;
+  void* gb_host = nullptr;
+  size_t gb_host_cap = 0;
+  DevBuf gb_dev;
   // Every call that changes the engine (loads, folds, table growth) and the snapshot refresh of a reader hold op_mu:
   // a reader never sees a table being freed or swapped, and a snapshot is only marked clean for the generation it copied.
   std::recursive_mutex op_mu;
@@ -495,6 +503,8 @@ int32_t sgr_destroy(sgr_engine* e) {
   e->bulk_scratch.release(); e->bulk_err_ids.release(); e->bulk_counters.release(); e->hash_out.release();
   if (e->dist) dist_destroy(e->dist);
   e->part_flags.release(); e->part_data.release(); e->redo_ids.release(); e->run_counters.release();
+  e->id_index.release(); e->gb_dev.release();
+  if (e->gb_host) cudaFreeHost(e->gb_host);
   cudaEventDestroy(e->ev0); cudaEventDestroy(e->ev1); cudaEventDestroy(e->ev2); cudaEventDestroy(e->ev3);
   cudaStreamDestroy(e->stream);
   delete e;
@@ -807,6 +817,7 @@ int32_t sgr_load_keys(sgr_engine* e, const uint8_t* keys, const uint32_t* key_of
   if (!kt->build(keys, key_offsets, n_agg, &err)) return fail(e, SGR_ERR_INVALID, "%s", err.c_str());
   std::lock_guard<std::mutex> lk(e->keys_mu);
   e->ing_keys_from = nullptr; e->ing_key_bytes.clear(); e->ing_key_offs.clear();
+  ++e->keys_epoch;
   e->keys_stale.store(false, std::memory_order_release);
   std::atomic_store(&e->keys, std::shared_ptr<const KeyTable>(kt));
   return SGR_OK;
@@ -851,7 +862,7 @@ static void pinned_free(void* p) { cudaFreeHost(p); }
 // the hash index is rebuilt lazily by the first sgr_get that follows (a restore polls thousands of times before anybody reads)
 static int32_t sgr_append_keys_upto(sgr_engine* e, const void* owner, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n_keys) {
   std::lock_guard<std::mutex> lk(e->keys_mu);
-  if (e->ing_keys_from != owner) { e->ing_keys_from = owner; e->ing_key_bytes.clear(); e->ing_key_offs.assign(1, 0u); }
+  if (e->ing_keys_from != owner) { e->ing_keys_from = owner; e->ing_key_bytes.clear(); e->ing_key_offs.assign(1, 0u); ++e->keys_epoch; }
   const uint64_t have = e->ing_key_offs.size() - 1;
   if (n_keys > have) {
     e->ing_key_bytes.insert(e->ing_key_bytes.end(), keys + key_offsets[have], keys + key_offsets[n_keys]);
@@ -865,7 +876,7 @@ static int32_t sgr_append_keys_upto(sgr_engine* e, const void* owner, const uint
 int32_t sgr_append_keys(sgr_engine* e, const void* owner, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n_new) {
   if (!e || !key_offsets || (!keys && n_new && key_offsets[n_new])) return fail(e, SGR_ERR_INVALID, "null argument");
   std::lock_guard<std::mutex> lk(e->keys_mu);
-  if (e->ing_keys_from != owner) { e->ing_keys_from = owner; e->ing_key_bytes.clear(); e->ing_key_offs.assign(1, 0u); }
+  if (e->ing_keys_from != owner) { e->ing_keys_from = owner; e->ing_key_bytes.clear(); e->ing_key_offs.assign(1, 0u); ++e->keys_epoch; }
   if (n_new) {
     e->ing_key_bytes.insert(e->ing_key_bytes.end(), keys + key_offsets[0], keys + key_offsets[n_new]);
     const uint32_t shift = e->ing_key_offs.back() - key_offsets[0];
@@ -947,6 +958,79 @@ int32_t sgr_get(sgr_engine* e, const uint8_t* key, uint32_t klen, void* out, uin
     return SGR_OK;
   }
   return sgr_get_index(e, (uint64_t)idx, out, cap, outlen, exists, nullptr, nullptr);
+}
+
+static size_t round16(size_t v) { return (v + 15) & ~(size_t)15; }
+
+int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n, void* out, uint64_t cap, uint32_t* flags,
+                      int64_t* indices) {
+  if (!e || (n && (!key_offsets || !out)) || (n && !keys && key_offsets[n] != key_offsets[0])) return fail(e, SGR_ERR_INVALID, "null argument");
+  for (uint64_t i = 0; i < n; ++i)
+    if (key_offsets[i + 1] < key_offsets[i]) return fail(e, SGR_ERR_INVALID, "key_offsets not monotone at %llu", (unsigned long long)i);
+  // one table generation for the whole batch: no load or fold runs while it is read, and an enqueued fold is waited for
+  OpLock op_lock(e);
+  int32_t rc = use_device(e); if (rc) return rc;
+  rc = finish_fold(e); if (rc) return rc;
+  if (!e->states_valid) return fail(e, SGR_ERR_STATE, "state store is not readable: no fold has completed");
+  const uint32_t sb = e->program.state_bytes, user = sb - 8;
+  if (cap / user < n) return fail(e, SGR_ERR_CAPACITY, "%llu rows of %u bytes do not fit in %llu bytes", (unsigned long long)n, user, (unsigned long long)cap);
+  if (!n) return SGR_OK;
+
+  // layout: pinned [ids to index | query offsets | query bytes | results], device [results | query offsets | query bytes]
+  const uint64_t q0 = key_offsets[0], q_bytes = key_offsets[n] - q0;
+  const size_t up_offs = round16((n + 1) * 4), up = up_offs + round16(q_bytes);
+  const size_t r_idx = 32, r_flags = r_idx + n * 8, r_rows = r_flags + round16(n * 4), down = r_rows + round16(n * user);
+  IdIndex& x = e->id_index;
+  {
+    std::lock_guard<std::mutex> lk(e->keys_mu);
+    // the ids sgr_get would read: those appended by an ingest, else the table of sgr_load_keys (or none)
+    std::shared_ptr<const KeyTable> kt;
+    const uint8_t* kb = nullptr; const uint32_t* ko = nullptr; uint64_t kn = 0;
+    if (!e->ing_key_offs.empty()) { kb = e->ing_key_bytes.data(); ko = e->ing_key_offs.data(); kn = e->ing_key_offs.size() - 1; }
+    else if ((kt = std::atomic_load(&e->keys))) { kb = kt->bytes(); ko = kt->offsets(); kn = kt->size(); }
+    if (kn >= 0xffffffffull) return fail(e, SGR_ERR_UNSUPPORTED, "the device id index holds fewer than 2^32 - 1 ids");
+    if (!x.valid || x.epoch != e->keys_epoch || kn < x.n) { x.n = 0; x.arena_used = 0; x.epoch = e->keys_epoch; }
+    bool mono = true;
+    const size_t ids = kn > x.n ? round16(id_index_stage_bytes(ko, x.n, kn, &mono)) : 0;
+    if (!mono) { x.valid = false; return fail(e, SGR_ERR_INVALID, "key_offsets not monotone"); }
+    if (ids + up + down > e->gb_host_cap) {
+      if (e->gb_host) cudaFreeHost(e->gb_host);
+      e->gb_host = nullptr; e->gb_host_cap = 0;
+      const size_t want = ids + up + down + (ids + up + down) / 2;
+      CUDA_TRY(e, cudaHostAlloc(&e->gb_host, want, cudaHostAllocPortable));
+      e->gb_host_cap = want;
+    }
+    CUDA_TRY(e, e->gb_dev.reserve(down + up));
+    CUDA_TRY(e, cudaMemsetAsync(e->gb_dev.p, 0, 32, e->stream));
+    if (kn > x.n) {
+      x.valid = false;   // until the insert reports no duplicate id
+      cudaError_t ce = id_index_append(x, kb, ko, kn, e->gb_host, (unsigned long long*)e->gb_dev.p, e->stream);
+      if (ce != cudaSuccess) return fail(e, ce == cudaErrorMemoryAllocation ? SGR_ERR_OOM : SGR_ERR_CUDA, "id index: %s", cudaGetErrorString(ce));
+    }
+  }
+  uint8_t* hq = (uint8_t*)e->gb_host + (e->gb_host_cap - up - down);   // (behind the ids: the stream may still be copying them)
+  uint8_t* hd = hq + up;
+  uint8_t* dd = (uint8_t*)e->gb_dev.p;
+  uint32_t* qo = (uint32_t*)hq;
+  for (uint64_t i = 0; i <= n; ++i) qo[i] = key_offsets[i] - (uint32_t)q0;
+  if (q_bytes) memcpy(hq + up_offs, keys + q0, q_bytes);
+  CUDA_TRY(e, cudaMemcpyAsync(dd + down, hq, up, cudaMemcpyHostToDevice, e->stream));
+  cudaError_t ce = id_index_probe(x, dd + down + up_offs, (const uint32_t*)(dd + down), n, (long long*)(dd + r_idx), e->stream);
+  if (ce == cudaSuccess)
+    ce = id_index_gather((const uint8_t*)e->states.p, sb, e->states_n, (const long long*)(dd + r_idx), n, dd + r_rows, (uint32_t*)(dd + r_flags),
+                         (unsigned long long*)dd + 2, e->stream);
+  if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "get_batch launch: %s", cudaGetErrorString(ce));
+  CUDA_TRY(e, cudaMemcpyAsync(hd, dd, down, cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+  const unsigned long long* ctl = (const unsigned long long*)hd;
+  if (ctl[0]) { x.valid = false; return fail(e, SGR_ERR_INVALID, "duplicate aggregate id in key table"); }
+  if (ctl[1]) { x.valid = false; return fail(e, SGR_ERR_CUDA, "id index: %llu ids found no free slot", ctl[1]); }
+  x.valid = true;
+  if (ctl[2]) return fail(e, SGR_ERR_INVALID, "aggregate index %llu out of range", ctl[2] - 1);
+  memcpy(out, hd + r_rows, n * user);
+  if (flags) memcpy(flags, hd + r_flags, n * 4);
+  if (indices) memcpy(indices, hd + r_idx, n * 8);
+  return SGR_OK;
 }
 
 int32_t sgr_export_states(sgr_engine* e, void* out, uint64_t cap, uint8_t* exists_bits, uint8_t* changed_bits, uint8_t* error_bits) {

@@ -50,6 +50,9 @@ class KeyTable {
     return -1;
   }
   uint64_t size() const { return n_; }
+  // the table's ids back to back: key i = bytes()[offsets()[i] .. offsets()[i + 1])
+  const uint8_t* bytes() const { return bytes_.data(); }
+  const uint32_t* offsets() const { return offs_.data(); }
   // key i as (pointer, length)
   const uint8_t* key(uint64_t i, uint32_t* len) const { *len = offs_[i + 1] - offs_[i]; return bytes_.data() + offs_[i]; }
 

@@ -221,6 +221,24 @@ class ReplayEngine:
                                    C.byref(outlen), C.byref(exists)))
         return bytes(buf.raw[:outlen.value]) if exists.value else None
 
+    def get_many(self, keys: Sequence[str], arrays: bool = False):
+        """getAggregateBytes for many ids in one call, served from the device table (sgr_get_batch): a list of Optional[bytes],
+        the same as get() for each id. arrays=True: (states u8[n, state_bytes - 8], flags u32[n], indices i64[n]) instead, with
+        zero rows for None states and unknown ids, flags 0 and index -1 for unknown ids."""
+        enc = [k.encode("utf-8") for k in keys]
+        n = len(enc)
+        offs = np.zeros(n + 1, dtype=np.uint32)
+        np.cumsum([len(b) for b in enc], out=offs[1:])
+        blob = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8)
+        states = np.zeros((n, max(self.state_bytes - 8, 0)), dtype=np.uint8)
+        flags = np.zeros(n, dtype=np.uint32)
+        indices = np.zeros(n, dtype=np.int64)
+        self._ck(self._lib.sgr_get_batch(self._h, blob.ctypes.data, offs.ctypes.data, n, states.ctypes.data, states.nbytes,
+                                         flags.ctypes.data, indices.ctypes.data))
+        if arrays:
+            return states, flags, indices
+        return [states[i].tobytes() if flags[i] & N.ST_EXISTS else None for i in range(n)]
+
     def get_index(self, agg: int) -> Tuple[Optional[bytes], int, int]:
         """(program bytes or None, flags, err_idx) of one dense aggregate index."""
         buf = C.create_string_buffer(N.MAX_STATE_BYTES)

@@ -20,6 +20,7 @@ from __future__ import annotations
 
 import importlib
 import threading
+import time
 from concurrent.futures import Future, ThreadPoolExecutor
 from typing import Callable, Dict, Iterable, Iterator, List, Optional, Sequence, Tuple
 
@@ -306,12 +307,36 @@ class GpuReplayKeyValueStore:
             return self._unflushed[key]
         if not self._folded:
             raise InvalidStateStoreException(N.SGR_ERR_STATE, f"store {self._name} has not been restored yet")
-        b = self._engine.get(key)
+        return self._decode(key, self._engine.get(key))
+
+    def _decode(self, key: str, b: Optional[bytes]) -> Optional[bytes]:
         if b is None:
             return None
         if self._codec is not None:
             return self._codec.from_packed(key, b)
         return self._formatter(key, b) if self._formatter else b
+
+    def get_many(self, keys: Sequence[str]) -> List[Optional[bytes]]:
+        """get() for many keys: each key is answered from the overlay, then the unflushed puts, like get(); the rest go to the
+        device in one sgr_get_batch call and through the codec / formatter."""
+        if not self._open:
+            raise InvalidStateStoreException(N.SGR_ERR_STATE, f"store {self._name} is not open")
+        keys = list(keys)
+        out: List[Optional[bytes]] = [None] * len(keys)
+        rest = []
+        for i, key in enumerate(keys):
+            if key in self._overlay:
+                out[i] = self._overlay[key]
+            elif key in self._unflushed:
+                out[i] = self._unflushed[key]
+            else:
+                rest.append(i)
+        if rest:
+            if not self._folded:
+                raise InvalidStateStoreException(N.SGR_ERR_STATE, f"store {self._name} has not been restored yet")
+            for i, b in zip(rest, self._engine.get_many([keys[i] for i in rest])):
+                out[i] = self._decode(keys[i], b)
+        return out
 
     def all(self) -> Iterator[Tuple[str, bytes]]:
         with self._lock:
@@ -344,14 +369,52 @@ class GpuReplayKeyValueStore:
 
 class AggregateStateStore:
     """The narrow seam PersistentActor consumes (AggregateStateStoreKafkaStreams.scala:83-89):
-    getAggregateBytes(aggregateId): Future[Option[Array[Byte]]] served from a 32-thread pool (ThreadPools.scala:9-11)."""
+    getAggregateBytes(aggregateId): Future[Option[Array[Byte]]] served from a 32-thread pool (ThreadPools.scala:9-11).
 
-    def __init__(self, store: GpuReplayKeyValueStore, threads: int = 32):
+    coalesce_reads_us > 0: getAggregateBytes calls that arrive within that many microseconds of the first one are answered together
+    by one store.get_many (one device call), each future with its own row, or every future of the batch with the batch's
+    exception. A node that starts makes one recovery read per aggregate that receives a command; this turns those one-id calls
+    into batches without changing the callers. 0 (the default): every call is one store.get on the pool."""
+
+    def __init__(self, store: GpuReplayKeyValueStore, threads: int = 32, coalesce_reads_us: int = 0):
         self._store = store
         self._pool = ThreadPoolExecutor(max_workers=threads, thread_name_prefix="surge-io")
+        self._window_s = coalesce_reads_us / 1e6
+        self._batch_lock = threading.Lock()
+        self._batch: Optional[List[Tuple[str, Future]]] = None   # reads waiting for the open window
 
     def getAggregateBytes(self, aggregateId: str) -> "Future[Optional[bytes]]":  # noqa: N802,N803
-        return self._pool.submit(self._store.get, aggregateId)
+        if self._window_s <= 0:
+            return self._pool.submit(self._store.get, aggregateId)
+        fut: Future = Future()
+        with self._batch_lock:
+            opens = self._batch is None
+            if opens:
+                self._batch = []
+            self._batch.append((aggregateId, fut))
+        if opens:
+            self._pool.submit(self._read_window)
+        return fut
+
+    def _read_window(self) -> None:
+        time.sleep(self._window_s)
+        with self._batch_lock:
+            batch, self._batch = self._batch, None
+        live = [(k, f) for k, f in batch if f.set_running_or_notify_cancel()]
+        if not live:
+            return
+        try:
+            rows = self._store.get_many([k for k, _ in live])
+        except BaseException as ex:  # noqa: BLE001 - every caller of the batch sees its failure
+            for _, f in live:
+                f.set_exception(ex)
+            return
+        for (_, f), row in zip(live, rows):
+            f.set_result(row)
+
+    def getAggregateBytesBatch(self, aggregateIds: Sequence[str]) -> "Future[List[Optional[bytes]]]":  # noqa: N802,N803
+        """Recovery reads of many ids in one device call (store.get_many)."""
+        return self._pool.submit(self._store.get_many, list(aggregateIds))
 
     def healthCheck(self) -> dict:  # noqa: N802
         return {"name": "aggregate-state-store", "status": "up" if self._store.isOpen() else "down"}
