@@ -266,6 +266,34 @@ int32_t sgr_get_index(sgr_engine* e, uint64_t agg, void* out, uint32_t cap,
 int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n,
                       void* out, uint64_t cap, uint32_t* flags, int64_t* indices);
 
+/* Changed-state export: the aggregates the last fold changed (SGR_ST_CHANGED, "newState != oldState") or failed (SGR_ST_ERROR,
+ * the handler threw and the state was kept), with their ids, compacted on the device and handed over in pages: what the
+ * reference's actors publish to the state topic after a poll (PersistentActor.scala:252-263), without copying the whole table.
+ * select: a non-empty subset of SGR_ST_CHANGED | SGR_ST_ERROR; a row is reported when flags & select != 0.
+ * A page holds the selected rows in ascending dense index from cur->next on, at most max_rows of them and at most ids_cap id
+ * bytes; cur->next comes back as the first selected row that did not fit, or n_agg when the scan reached the end. Row i of the
+ * page: rows[i] (state_bytes - 8 bytes; all zero for a None state, the tombstone case CHANGED without EXISTS), flags[i],
+ * err_idx[i], indices[i] (its dense index) and its id ids[id_offsets[i] .. id_offsets[i+1]) from the key table sgr_get /
+ * sgr_get_batch read. A row at or past cur->n_keys has no id: a zero-length span, told apart from the id "" by its index.
+ * Buffers: rows max_rows x (state_bytes - 8), flags / err_idx max_rows x u32, indices max_rows x i64, id_offsets max_rows + 1
+ * u32, ids ids_cap bytes (NULL when ids_cap == 0); *n_rows = the rows written.
+ * One export is one table generation: start with cur = {0}; the first page records the generation and the key-table epoch in
+ * cur->token and later pages pass it back. After any fold, grow or sgr_set_initial_states, or sgr_load_keys or a new ingest
+ * owner, a later page fails with SGR_ERR_STATE and writes nothing. Appended ids and reads do not end an export.
+ * Holds the operation lock and waits for an sgr_fold_async, as sgr_get_batch does. SGR_ERR_STATE before any fold;
+ * SGR_ERR_INVALID on NULL arguments, a bad select, max_rows == 0 or cur->next > n_agg; SGR_ERR_CAPACITY (nothing written,
+ * the cursor unchanged) when the first selected row's id alone exceeds ids_cap; SGR_ERR_UNSUPPORTED on a routed engine
+ * (sgr_dist_init), whose rows are local slots. */
+typedef struct sgr_changes_cursor {
+  uint64_t next;     /* in/out: first dense index not yet reported; 0 starts an export; n_agg when the export is complete */
+  uint64_t token;    /* in/out: 0 on the first page; the engine sets it and later pages pass it back */
+  uint64_t n_keys;   /* out: size of the key table the page was read against */
+  uint64_t reserved;
+} sgr_changes_cursor;
+int32_t sgr_export_changes(sgr_engine* e, uint32_t select, sgr_changes_cursor* cur, uint64_t max_rows, void* rows,
+                           uint32_t* flags, uint32_t* err_idx, int64_t* indices, uint8_t* ids, uint64_t ids_cap,
+                           uint32_t* id_offsets, uint64_t* n_rows);
+
 /* Export the whole state table (n_agg * state_bytes) and, optionally, bitmaps
  * (bit i of byte i/8, LSB first). Any out pointer may be NULL. */
 int32_t sgr_export_states(sgr_engine* e, void* out, uint64_t cap,

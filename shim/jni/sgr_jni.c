@@ -97,6 +97,31 @@ JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_getBatch(JNIEnv* env, jobject
   if (rc != SGR_OK) throw_for(env, H(h), rc);
   return rc;
 }
+/* One page of sgr_export_changes. cursor: direct buffer of 4 u64 (next, token, nKeys, reserved), read and updated in place;
+ * flags / errIdx / indices / idOffsets: direct buffers of maxRows u32 / u32 / i64 / maxRows + 1 u32; rows: maxRows x
+ * (state_bytes - 8) bytes; ids: a direct buffer whose capacity is the page's id-byte budget. Returns the rows written, or -1
+ * after throwing (InvalidStateStoreException when the table changed since the export's first page). */
+JNIEXPORT jlong JNICALL Java_surge_gpu_Native_00024_exportChanges(JNIEnv* env, jobject o, jlong h, jint select, jobject cursor, jlong max_rows,
+                                                                  jobject rows, jobject flags, jobject err_idx, jobject indices, jobject ids,
+                                                                  jobject id_offsets) {
+  int ok = 1;
+  if (max_rows <= 0 || max_rows > INT64_MAX / (8 * SGR_MAX_STATE_BYTES)) { bad_arg(env, "maxRows must be positive"); return -1; }
+  uint32_t sb = 0;
+  const jlong user = sgr_states_device(H(h), 0, 0, &sb) == SGR_OK ? (jlong)sb - 8 : 0;   /* (no table yet: the call below says so) */
+  sgr_changes_cursor* cur = (sgr_changes_cursor*)direct(env, cursor, (jlong)sizeof(sgr_changes_cursor), "cursor: direct buffer of 4 u64", &ok);
+  void* rw = ok ? direct(env, rows, max_rows * user, "rows: direct buffer shorter than maxRows states", &ok) : 0;
+  uint32_t* fl = ok ? (uint32_t*)direct(env, flags, max_rows * 4, "flags: direct buffer of maxRows u32", &ok) : 0;
+  uint32_t* er = ok ? (uint32_t*)direct(env, err_idx, max_rows * 4, "errIdx: direct buffer of maxRows u32", &ok) : 0;
+  int64_t* ix = ok ? (int64_t*)direct(env, indices, max_rows * 8, "indices: direct buffer of maxRows i64", &ok) : 0;
+  uint32_t* io = ok ? (uint32_t*)direct(env, id_offsets, (max_rows + 1) * 4, "idOffsets: direct buffer of maxRows + 1 u32", &ok) : 0;
+  uint8_t* id = ok ? (uint8_t*)direct(env, ids, 1, "ids: direct buffer", &ok) : 0;
+  if (!ok) return -1;
+  uint64_t n = 0;
+  int32_t rc = sgr_export_changes(H(h), (uint32_t)select, cur, (uint64_t)max_rows, rw, fl, er, ix, id, (uint64_t)(*env)->GetDirectBufferCapacity(env, ids),
+                                  io, &n);
+  if (rc != SGR_OK) { throw_for(env, H(h), rc); return -1; }
+  return (jlong)n;
+}
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_exportStates(JNIEnv* env, jobject o, jlong h, jobject out, jobject changed) {
   return sgr_export_states(H(h), (*env)->GetDirectBufferAddress(env, out), (uint64_t)(*env)->GetDirectBufferCapacity(env, out), 0,
                            changed ? (uint8_t*)(*env)->GetDirectBufferAddress(env, changed) : 0, 0);

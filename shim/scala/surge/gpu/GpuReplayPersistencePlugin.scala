@@ -91,7 +91,12 @@ class GpuReplayPersistencePlugin extends SurgeKafkaStreamsPersistencePlugin {
   }
 }
 
-class GpuReplayKeyValueStore(storeName: String) extends KeyValueStore[Bytes, Array[Byte]] {
+/** onChanges(changed, failed): called once by every flush() that folded, before it returns, with what the reference's actors
+ *  would publish for that fold (PersistentActor.scala:252-263): changed = (id, serialized state through the codec, or null for a
+ *  state that became None), failed = (id, err_idx) for the aggregates whose handler threw. Rebuilding a state topic from the
+ *  events topic produces these records; producing them to Kafka is the caller's. */
+class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, Array[Byte])], Seq[(String, Int)]) => Unit] = None)
+    extends KeyValueStore[Bytes, Array[Byte]] {
   private val log = LoggerFactory.getLogger(getClass)
   private val reg = GpuFoldPrograms.current
   private var handle: Long = 0L
@@ -185,7 +190,43 @@ class GpuReplayKeyValueStore(storeName: String) extends KeyValueStore[Bytes, Arr
       }
       if (keys.size() != loadedKeys) loadKeyTable() // new ids inside the current capacity
       unflushed.clear()
+      onChanges.foreach(reportChanges)
     } finally lock.writeLock().unlock()
+  }
+
+  /** The CHANGED and ERROR rows of the fold that just ran, paged from the device (sgr_export_changes); spare capacity slots
+   *  (past the ids this store assigned) are left out. */
+  private def reportChanges(listener: (Seq[(String, Array[Byte])], Seq[(String, Int)]) => Unit): Unit = {
+    val user = reg.program.duplicate().order(ByteOrder.LITTLE_ENDIAN).getInt(0) - 8 // state_bytes is the first field
+    val pageRows = 65536
+    val cursor = ByteBuffer.allocateDirect(32).order(ByteOrder.LITTLE_ENDIAN)
+    val rows = ByteBuffer.allocateDirect(user * pageRows)
+    val flags = ByteBuffer.allocateDirect(4 * pageRows).order(ByteOrder.LITTLE_ENDIAN)
+    val errs = ByteBuffer.allocateDirect(4 * pageRows).order(ByteOrder.LITTLE_ENDIAN)
+    val indices = ByteBuffer.allocateDirect(8 * pageRows).order(ByteOrder.LITTLE_ENDIAN)
+    val idOffsets = ByteBuffer.allocateDirect(4 * (pageRows + 1)).order(ByteOrder.LITTLE_ENDIAN)
+    val ids = ByteBuffer.allocateDirect(4 << 20)
+    val changed = scala.collection.mutable.ArrayBuffer[(String, Array[Byte])]()
+    val failed = scala.collection.mutable.ArrayBuffer[(String, Int)]()
+    do {
+      val n = Native.exportChanges(handle, 2 | 4, cursor, pageRows.toLong, rows, flags, errs, indices, ids, idOffsets).toInt // CHANGED | ERROR
+      var i = 0
+      while (i < n) {
+        val slot = indices.getLong(8 * i)
+        if (slot < keys.size()) { // the key table is this store's ids in slot order
+          val id = keys.get(slot.toInt)
+          val fl = flags.getInt(4 * i)
+          if ((fl & 2) != 0) changed += id -> (if ((fl & 1) != 0) {
+            val packed = new Array[Byte](user)
+            rows.position(i * user); rows.get(packed)
+            reg.codec.fromPacked(id, packed)
+          } else null)
+          if ((fl & 4) != 0) failed += id -> errs.getInt(4 * i)
+        }
+        i += 1
+      }
+    } while (cursor.getLong(0) < capacity) // next == n_agg: the export is complete
+    listener(changed.toSeq, failed.toSeq)
   }
 
   /** Make room for the keys seen so far: the table is resized on the device, content kept, new slots None (sgr_grow_states). */

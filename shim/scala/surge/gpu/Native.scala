@@ -28,6 +28,12 @@ object Native {
    * (stateBytes - 8, zero for None / unknown), flags(i) = SGR_ST_* (0 for an unknown id); returns the status */
   @native def getBatch(handle: Long, keys: ByteBuffer, keyOffsets: ByteBuffer, n: Long, out: ByteBuffer, flags: ByteBuffer): Int // sgr_get_batch
   @native def exportStates(handle: Long, out: ByteBuffer, changedBits: ByteBuffer): Int // sgr_export_states
+  /** one page of the rows whose flags meet `select` (SGR_ST_CHANGED = 2 | SGR_ST_ERROR = 4), from the cursor (4 u64: next, token,
+   * nKeys, reserved; start with zeros) on: row i = rows (stateBytes - 8), flags(i), errIdx(i), indices(i) and its id
+   * ids[idOffsets(i) until idOffsets(i+1)]; the ids buffer's capacity is the page's id-byte budget. Returns the rows written and
+   * advances the cursor (next == nAgg: done); throws InvalidStateStoreException when the table changed since the first page */
+  @native def exportChanges(handle: Long, select: Int, cursor: ByteBuffer, maxRows: Long, rows: ByteBuffer, flags: ByteBuffer, errIdx: ByteBuffer,
+                            indices: ByteBuffer, ids: ByteBuffer, idOffsets: ByteBuffer): Long // sgr_export_changes
   @native def partitionForKey(key: Array[Byte], numPartitions: Int, upToColon: Boolean): Int // sgr_partition_for_key_utf8
 
   // raw record batches in, committed offsets out (include/sgr.h "ingest")

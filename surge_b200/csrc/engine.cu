@@ -15,6 +15,7 @@
 
 #include "../../include/sgr.h"
 #include "bulk_fold.cuh"
+#include "changes.cuh"
 #include "devbuf.h"
 #include "dist.cuh"
 #include "fold_kernels.cuh"
@@ -137,6 +138,7 @@ struct sgr_engine {
   void* gb_host = nullptr;
   size_t gb_host_cap = 0;
   DevBuf gb_dev;
+  DevBuf ch_tiles;                          // sgr_export_changes: per-tile totals and bases (changes.cuh)
   // Every call that changes the engine (loads, folds, table growth) and the snapshot refresh of a reader hold op_mu:
   // a reader never sees a table being freed or swapped, and a snapshot is only marked clean for the generation it copied.
   std::recursive_mutex op_mu;
@@ -503,7 +505,7 @@ int32_t sgr_destroy(sgr_engine* e) {
   e->bulk_scratch.release(); e->bulk_err_ids.release(); e->bulk_counters.release(); e->hash_out.release();
   if (e->dist) dist_destroy(e->dist);
   e->part_flags.release(); e->part_data.release(); e->redo_ids.release(); e->run_counters.release();
-  e->id_index.release(); e->gb_dev.release();
+  e->id_index.release(); e->gb_dev.release(); e->ch_tiles.release();
   if (e->gb_host) cudaFreeHost(e->gb_host);
   cudaEventDestroy(e->ev0); cudaEventDestroy(e->ev1); cudaEventDestroy(e->ev2); cudaEventDestroy(e->ev3);
   cudaStreamDestroy(e->stream);
@@ -962,6 +964,50 @@ int32_t sgr_get(sgr_engine* e, const uint8_t* key, uint32_t klen, void* out, uin
 
 static size_t round16(size_t v) { return (v + 15) & ~(size_t)15; }
 
+// Bring the device id index up to the key table sgr_get would read (the ids an ingest appended, else the table of
+// sgr_load_keys, or none): ids appended since the last call are staged at the front of the page-locked buffer and inserted; a
+// replaced table is indexed from id 0. Also makes room for `host_extra` page-locked bytes behind the staged ids (the caller's,
+// at gb_host + gb_host_cap - host_extra) and `dev_bytes` in gb_dev, whose first 32 bytes are zeroed for the insert's control
+// words. Enqueued on the stream only: the caller synchronises and hands those words to id_index_settle. Caller holds op_mu.
+static int32_t id_index_update(sgr_engine* e, size_t host_extra, size_t dev_bytes) {
+  IdIndex& x = e->id_index;
+  std::lock_guard<std::mutex> lk(e->keys_mu);
+  std::shared_ptr<const KeyTable> kt;
+  const uint8_t* kb = nullptr; const uint32_t* ko = nullptr; uint64_t kn = 0;
+  if (!e->ing_key_offs.empty()) { kb = e->ing_key_bytes.data(); ko = e->ing_key_offs.data(); kn = e->ing_key_offs.size() - 1; }
+  else if ((kt = std::atomic_load(&e->keys))) { kb = kt->bytes(); ko = kt->offsets(); kn = kt->size(); }
+  if (kn >= 0xffffffffull) return fail(e, SGR_ERR_UNSUPPORTED, "the device id index holds fewer than 2^32 - 1 ids");
+  if (!x.valid || x.epoch != e->keys_epoch || kn < x.n) { x.n = 0; x.arena_used = 0; x.epoch = e->keys_epoch; }
+  bool mono = true;
+  const size_t ids = kn > x.n ? round16(id_index_stage_bytes(ko, x.n, kn, &mono)) : 0;
+  if (!mono) { x.valid = false; return fail(e, SGR_ERR_INVALID, "key_offsets not monotone"); }
+  if (ids + host_extra > e->gb_host_cap) {
+    if (e->gb_host) cudaFreeHost(e->gb_host);
+    e->gb_host = nullptr; e->gb_host_cap = 0;
+    const size_t want = ids + host_extra + (ids + host_extra) / 2;
+    CUDA_TRY(e, cudaHostAlloc(&e->gb_host, want, cudaHostAllocPortable));
+    e->gb_host_cap = want;
+  }
+  CUDA_TRY(e, e->gb_dev.reserve(dev_bytes));
+  CUDA_TRY(e, cudaMemsetAsync(e->gb_dev.p, 0, 32, e->stream));
+  if (kn > x.n) {
+    x.valid = false;   // until the insert reports no duplicate id
+    cudaError_t ce = id_index_append(x, kb, ko, kn, e->gb_host, (unsigned long long*)e->gb_dev.p, e->stream);
+    if (ce != cudaSuccess) return fail(e, ce == cudaErrorMemoryAllocation ? SGR_ERR_OOM : SGR_ERR_CUDA, "id index: %s", cudaGetErrorString(ce));
+  }
+  return SGR_OK;
+}
+
+// The insert's control words (gb_dev's first two u64, copied back after a synchronisation): [0] duplicate ids, [1] ids that
+// found no free slot. Either one leaves the index to be rebuilt by the next call.
+static int32_t id_index_settle(sgr_engine* e, const unsigned long long* ctl) {
+  IdIndex& x = e->id_index;
+  if (ctl[0]) { x.valid = false; return fail(e, SGR_ERR_INVALID, "duplicate aggregate id in key table"); }
+  if (ctl[1]) { x.valid = false; return fail(e, SGR_ERR_CUDA, "id index: %llu ids found no free slot", ctl[1]); }
+  x.valid = true;
+  return SGR_OK;
+}
+
 int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n, void* out, uint64_t cap, uint32_t* flags,
                       int64_t* indices) {
   if (!e || (n && (!key_offsets || !out)) || (n && !keys && key_offsets[n] != key_offsets[0])) return fail(e, SGR_ERR_INVALID, "null argument");
@@ -981,33 +1027,7 @@ int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_of
   const size_t up_offs = round16((n + 1) * 4), up = up_offs + round16(q_bytes);
   const size_t r_idx = 32, r_flags = r_idx + n * 8, r_rows = r_flags + round16(n * 4), down = r_rows + round16(n * user);
   IdIndex& x = e->id_index;
-  {
-    std::lock_guard<std::mutex> lk(e->keys_mu);
-    // the ids sgr_get would read: those appended by an ingest, else the table of sgr_load_keys (or none)
-    std::shared_ptr<const KeyTable> kt;
-    const uint8_t* kb = nullptr; const uint32_t* ko = nullptr; uint64_t kn = 0;
-    if (!e->ing_key_offs.empty()) { kb = e->ing_key_bytes.data(); ko = e->ing_key_offs.data(); kn = e->ing_key_offs.size() - 1; }
-    else if ((kt = std::atomic_load(&e->keys))) { kb = kt->bytes(); ko = kt->offsets(); kn = kt->size(); }
-    if (kn >= 0xffffffffull) return fail(e, SGR_ERR_UNSUPPORTED, "the device id index holds fewer than 2^32 - 1 ids");
-    if (!x.valid || x.epoch != e->keys_epoch || kn < x.n) { x.n = 0; x.arena_used = 0; x.epoch = e->keys_epoch; }
-    bool mono = true;
-    const size_t ids = kn > x.n ? round16(id_index_stage_bytes(ko, x.n, kn, &mono)) : 0;
-    if (!mono) { x.valid = false; return fail(e, SGR_ERR_INVALID, "key_offsets not monotone"); }
-    if (ids + up + down > e->gb_host_cap) {
-      if (e->gb_host) cudaFreeHost(e->gb_host);
-      e->gb_host = nullptr; e->gb_host_cap = 0;
-      const size_t want = ids + up + down + (ids + up + down) / 2;
-      CUDA_TRY(e, cudaHostAlloc(&e->gb_host, want, cudaHostAllocPortable));
-      e->gb_host_cap = want;
-    }
-    CUDA_TRY(e, e->gb_dev.reserve(down + up));
-    CUDA_TRY(e, cudaMemsetAsync(e->gb_dev.p, 0, 32, e->stream));
-    if (kn > x.n) {
-      x.valid = false;   // until the insert reports no duplicate id
-      cudaError_t ce = id_index_append(x, kb, ko, kn, e->gb_host, (unsigned long long*)e->gb_dev.p, e->stream);
-      if (ce != cudaSuccess) return fail(e, ce == cudaErrorMemoryAllocation ? SGR_ERR_OOM : SGR_ERR_CUDA, "id index: %s", cudaGetErrorString(ce));
-    }
-  }
+  rc = id_index_update(e, up + down, down + up); if (rc) return rc;
   uint8_t* hq = (uint8_t*)e->gb_host + (e->gb_host_cap - up - down);   // (behind the ids: the stream may still be copying them)
   uint8_t* hd = hq + up;
   uint8_t* dd = (uint8_t*)e->gb_dev.p;
@@ -1023,13 +1043,99 @@ int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_of
   CUDA_TRY(e, cudaMemcpyAsync(hd, dd, down, cudaMemcpyDeviceToHost, e->stream));
   CUDA_TRY(e, cudaStreamSynchronize(e->stream));
   const unsigned long long* ctl = (const unsigned long long*)hd;
-  if (ctl[0]) { x.valid = false; return fail(e, SGR_ERR_INVALID, "duplicate aggregate id in key table"); }
-  if (ctl[1]) { x.valid = false; return fail(e, SGR_ERR_CUDA, "id index: %llu ids found no free slot", ctl[1]); }
-  x.valid = true;
+  rc = id_index_settle(e, ctl); if (rc) return rc;
   if (ctl[2]) return fail(e, SGR_ERR_INVALID, "aggregate index %llu out of range", ctl[2] - 1);
   memcpy(out, hd + r_rows, n * user);
   if (flags) memcpy(flags, hd + r_flags, n * 4);
   if (indices) memcpy(indices, hd + r_idx, n * 8);
+  return SGR_OK;
+}
+
+// The table generation and the key-table epoch a page is read against (generation >= 1 once a table exists).
+static uint64_t changes_token(uint64_t generation, uint64_t keys_epoch) { return ((generation & ((1ull << 40) - 1)) << 24) | (keys_epoch & 0xffffffull); }
+
+int32_t sgr_export_changes(sgr_engine* e, uint32_t select, sgr_changes_cursor* cur, uint64_t max_rows, void* rows, uint32_t* flags,
+                           uint32_t* err_idx, int64_t* indices, uint8_t* ids, uint64_t ids_cap, uint32_t* id_offsets, uint64_t* n_rows) {
+  if (!e || !cur || !rows || !flags || !err_idx || !indices || !id_offsets || !n_rows || (!ids && ids_cap)) return fail(e, SGR_ERR_INVALID, "null argument");
+  if (!select || (select & ~(uint32_t)(SGR_ST_CHANGED | SGR_ST_ERROR)))
+    return fail(e, SGR_ERR_INVALID, "select 0x%x is not a non-empty subset of SGR_ST_CHANGED | SGR_ST_ERROR", select);
+  if (!max_rows) return fail(e, SGR_ERR_INVALID, "max_rows is 0");
+  // one table generation per call, and the token ties the pages of one export to it
+  OpLock op_lock(e);
+  if (e->dist) return fail(e, SGR_ERR_UNSUPPORTED, "the rows of a routed engine are local slots: sgr_export_changes does not map them to ids");
+  int32_t rc = use_device(e); if (rc) return rc;
+  rc = finish_fold(e); if (rc) return rc;
+  if (!e->states_valid) return fail(e, SGR_ERR_STATE, "state store is not readable: no fold has completed");
+  const uint64_t n_agg = e->states_n, next = cur->next;
+  if (next > n_agg) return fail(e, SGR_ERR_INVALID, "cursor %llu is past the table's %llu aggregates", (unsigned long long)next, (unsigned long long)n_agg);
+  if (n_agg >= 0xffffffffull) return fail(e, SGR_ERR_UNSUPPORTED, "sgr_export_changes reads tables of fewer than 2^32 - 1 aggregates");
+  if (cur->token) {
+    uint64_t epoch;
+    { std::lock_guard<std::mutex> lk(e->keys_mu); epoch = e->keys_epoch; }
+    if (cur->token != changes_token(e->generation.load(std::memory_order_acquire), epoch))
+      return fail(e, SGR_ERR_STATE, "the table or its key table changed since the first page of this export: start again from 0");
+  }
+  const uint32_t sb = e->program.state_bytes, user = sb - 8;
+  // control words: [0, 32) of gb_dev the id index insert's, [32, 64) the page cut's; they come back behind the staged ids
+  rc = id_index_update(e, 64, 64); if (rc) return rc;
+  const IdIndex& x = e->id_index;
+  const uint64_t token = changes_token(e->generation.load(std::memory_order_acquire), x.epoch);
+  const uint2* key_ref = (const uint2*)x.key_ref.p;
+  const uint64_t n_keys = x.n;
+  const uint8_t* states = (const uint8_t*)e->states.p;
+  const uint64_t nt = (n_agg + kChangesTile - 1) / kChangesTile - next / kChangesTile;
+  if (nt) CUDA_TRY(e, e->ch_tiles.reserve(nt * 16));
+  unsigned long long* tiles = (unsigned long long*)e->ch_tiles.p;
+  cudaError_t ce = changes_count_cut(states, sb, n_agg, key_ref, n_keys, select, next, max_rows, ids_cap, tiles, (unsigned long long*)e->gb_dev.p + 4,
+                                     e->stream);
+  if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "export_changes launch: %s", cudaGetErrorString(ce));
+  uint8_t* hctl = (uint8_t*)e->gb_host + (e->gb_host_cap - 64);
+  CUDA_TRY(e, cudaMemcpyAsync(hctl, e->gb_dev.p, 64, cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+  unsigned long long ctl[8];
+  memcpy(ctl, hctl, sizeof ctl);
+  rc = id_index_settle(e, ctl); if (rc) return rc;
+  const uint64_t page = nt ? ctl[4 + kChCtlRows] : 0, bytes = nt ? ctl[4 + kChCtlBytes] : 0;
+  const uint64_t new_next = nt ? ctl[4 + kChCtlNext] : n_agg, page_tiles = nt ? ctl[4 + kChCtlTiles] : 0;
+  if (!page && new_next < n_agg)
+    return fail(e, SGR_ERR_CAPACITY, "the id of aggregate %llu does not fit in %llu id bytes", (unsigned long long)new_next, (unsigned long long)ids_cap);
+  if (page) {
+    // device (behind the control words) and page-locked alike: indices | flags | err_idx | id offsets | program bytes | ids
+    const size_t o_fl = round16(page * 8), o_err = o_fl + round16(page * 4), o_off = o_err + round16(page * 4);
+    const size_t o_rows = o_off + round16((page + 1) * 4), o_ids = o_rows + round16(page * user), total = o_ids + round16(bytes);
+    CUDA_TRY(e, e->gb_dev.reserve(64 + total));
+    if (total > e->gb_host_cap) {   // (the stream is idle: nothing is still copying from it)
+      cudaFreeHost(e->gb_host);
+      e->gb_host = nullptr; e->gb_host_cap = 0;
+      CUDA_TRY(e, cudaHostAlloc(&e->gb_host, total + total / 2, cudaHostAllocPortable));
+      e->gb_host_cap = total + total / 2;
+    }
+    uint8_t* dd = (uint8_t*)e->gb_dev.p + 64;
+    ce = changes_compact(states, sb, n_agg, key_ref, n_keys, select, next, tiles, nt, page_tiles, page, (long long*)dd, (uint32_t*)(dd + o_err),
+                         (uint32_t*)(dd + o_off), e->stream);
+    // (every compacted index is below n_agg: the gather's out-of-range word, gb_dev's third u64, stays unread)
+    if (ce == cudaSuccess)
+      ce = id_index_gather(states, sb, n_agg, (const long long*)dd, page, dd + o_rows, (uint32_t*)(dd + o_fl), (unsigned long long*)e->gb_dev.p + 2,
+                           e->stream);
+    if (ce == cudaSuccess)
+      ce = changes_copy_ids((const long long*)dd, (const uint32_t*)(dd + o_off), page, key_ref, (const uint8_t*)x.arena.p, n_keys, dd + o_ids, e->stream);
+    if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "export_changes launch: %s", cudaGetErrorString(ce));
+    const uint8_t* hd = (const uint8_t*)e->gb_host;
+    CUDA_TRY(e, cudaMemcpyAsync(e->gb_host, dd, total, cudaMemcpyDeviceToHost, e->stream));
+    CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+    memcpy(indices, hd, page * 8);
+    memcpy(flags, hd + o_fl, page * 4);
+    memcpy(err_idx, hd + o_err, page * 4);
+    memcpy(id_offsets, hd + o_off, (page + 1) * 4);
+    memcpy(rows, hd + o_rows, page * user);
+    if (bytes) memcpy(ids, hd + o_ids, bytes);
+  } else {
+    id_offsets[0] = 0;
+  }
+  *n_rows = page;
+  cur->next = new_next;
+  cur->token = token;
+  cur->n_keys = n_keys;
   return SGR_OK;
 }
 

@@ -7,7 +7,7 @@ entry points and are borrowed, not copied.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional, Sequence, Tuple
+from typing import Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -238,6 +238,35 @@ class ReplayEngine:
         if arrays:
             return states, flags, indices
         return [states[i].tobytes() if flags[i] & N.ST_EXISTS else None for i in range(n)]
+
+    def export_changes(self, select: int = N.ST_CHANGED, page_rows: Optional[int] = 1 << 20,
+                       page_id_bytes: int = 64 << 20) -> Iterator[Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray, List[Optional[str]]]]:
+        """The aggregates the last fold changed (select=ST_CHANGED) or failed (ST_ERROR, or both), compacted on the device
+        (sgr_export_changes). Yields pages of (indices i64[n], flags u32[n], err_idx u32[n], rows u8[n, state_bytes - 8], ids) in
+        ascending dense index; ids[i] is the aggregate id (str), or None for a row past the key table. A row is all zero when its
+        state is None. A page holds at most page_rows rows (None: the whole table) and page_id_bytes id bytes. Every page of one
+        export reads the same table: a fold, grow, set_initial_states or load_keys between two pages raises
+        InvalidStateStoreException (SGR_ERR_STATE) from the next one."""
+        n_agg = self.n_aggregates()
+        cap = max(1, n_agg if page_rows is None else min(int(page_rows), max(n_agg, 1)))
+        user = self.state_bytes - 8
+        cur = N.sgr_changes_cursor()
+        n = C.c_uint64()
+        while True:
+            rows = np.empty((cap, user), dtype=np.uint8)
+            flags, err = np.empty(cap, dtype=np.uint32), np.empty(cap, dtype=np.uint32)
+            idx = np.empty(cap, dtype=np.int64)
+            offs = np.empty(cap + 1, dtype=np.uint32)
+            blob = np.empty(max(int(page_id_bytes), 1), dtype=np.uint8)
+            self._ck(self._lib.sgr_export_changes(self._h, int(select), C.byref(cur), cap, rows.ctypes.data, flags.ctypes.data, err.ctypes.data,
+                                                  idx.ctypes.data, blob.ctypes.data, int(page_id_bytes), offs.ctypes.data, C.byref(n)))
+            k, n_keys = int(n.value), int(cur.n_keys)
+            raw = blob[:int(offs[k])].tobytes() if k else b""
+            ids = [raw[offs[i]:offs[i + 1]].decode("utf-8") if idx[i] < n_keys else None for i in range(k)]
+            if k:
+                yield idx[:k], flags[:k], err[:k], rows[:k], ids
+            if cur.next >= n_agg:
+                return
 
     def get_index(self, agg: int) -> Tuple[Optional[bytes], int, int]:
         """(program bytes or None, flags, err_idx) of one dense aggregate index."""

@@ -72,6 +72,10 @@ class sgr_stats(C.Structure):
                 ("fold_launches", C.c_uint32), ("reserved", C.c_uint32 * 7)]
 
 
+class sgr_changes_cursor(C.Structure):
+    _fields_ = [("next", C.c_uint64), ("token", C.c_uint64), ("n_keys", C.c_uint64), ("reserved", C.c_uint64)]
+
+
 class sgr_ingest_stats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("n_bytes", "n_trailing_bytes", "n_batches", "n_records", "n_markers", "n_null_values",
                                           "n_control_batches", "n_aborted_batches", "n_aborted_records", "n_duplicates", "n_new_keys",
@@ -116,6 +120,8 @@ ABI = [
     ("sgr_get_index", C.c_int32, [_P, C.c_uint64, _P, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_int32),
                                   C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
     ("sgr_get_batch", C.c_int32, [_P, _P, _P, C.c_uint64, _P, C.c_uint64, _P, _P]),
+    ("sgr_export_changes", C.c_int32, [_P, C.c_uint32, C.POINTER(sgr_changes_cursor), C.c_uint64, _P, _P, _P, _P, _P, C.c_uint64, _P,
+                                       C.POINTER(C.c_uint64)]),
     ("sgr_export_states", C.c_int32, [_P, _P, C.c_uint64, _P, _P, _P]),
     ("sgr_states_device", C.c_int32, [_P, C.POINTER(_P), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
     ("sgr_events_device", C.c_int32, [_P, C.POINTER(_P), C.POINTER(C.c_uint64), C.POINTER(_P)]),

@@ -133,8 +133,14 @@ class GpuReplayKeyValueStore:
     """
 
     def __init__(self, name: str, program: N.sgr_fold_program, device: int = 0, state_formatter: Optional[Callable[[str, bytes], bytes]] = None,
-                 codec: Optional[StateCodec] = None):
+                 codec: Optional[StateCodec] = None,
+                 on_changes: Optional[Callable[[List[Tuple[str, Optional[bytes]]], List[Tuple[str, int]]], None]] = None):
         self._name = name
+        # on_changes(changed, failed): called once by every flush() that folded, before it returns, with what the reference's
+        # actors would publish for that fold (PersistentActor.scala:252-263): changed = [(id, serialized state or None)], decoded
+        # like get(), None for a state that became None; failed = [(id, err_idx)] for the aggregates whose handler threw. Values
+        # put() keeps in the overlay (a store without a codec) are not folded, so they are never reported.
+        self._on_changes = on_changes
         # with a codec, put()/delete() are records of the STATE topic folded on the GPU as snapshot / tombstone events (feed (i) of
         # the Scala store): flush() — which Kafka Streams calls before it commits offsets — makes them readable from the table
         self._codec = codec
@@ -234,6 +240,7 @@ class GpuReplayKeyValueStore:
             if self._ingest is not None:
                 self._engine.fold_ingested(self._ingest)
                 self._folded = True
+                self._report_changes()
                 return
             if not self._pending and self._folded:
                 return
@@ -258,6 +265,25 @@ class GpuReplayKeyValueStore:
                 self._engine.load_keys(self._keys + [f"\0unused-{i}" for i in range(n_keys, self._capacity)])
                 self._keys_loaded = (n_keys, self._capacity)
             self._unflushed.clear()
+            self._report_changes()
+
+    def _report_changes(self) -> None:
+        """on_changes for the fold that just ran: its CHANGED and ERROR rows, paged from the device (sgr_export_changes). Spare
+        capacity slots (ids past the ones this store assigned) never appear."""
+        if self._on_changes is None:
+            return
+        n_ids = None if self._ingest is not None else len(self._keys)
+        changed: List[Tuple[str, Optional[bytes]]] = []
+        failed: List[Tuple[str, int]] = []
+        for idx, flags, err, rows, ids in self._engine.export_changes(N.ST_CHANGED | N.ST_ERROR):
+            for i, key in enumerate(ids):
+                if key is None or (n_ids is not None and idx[i] >= n_ids):
+                    continue
+                if flags[i] & N.ST_CHANGED:
+                    changed.append((key, self._decode(key, rows[i].tobytes()) if flags[i] & N.ST_EXISTS else None))
+                if flags[i] & N.ST_ERROR:
+                    failed.append((key, int(err[i])))
+        self._on_changes(changed, failed)
 
     # -- KeyValueStore
     def _state_record(self, key: str, value: Optional[bytes]) -> None:
