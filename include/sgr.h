@@ -294,6 +294,33 @@ int32_t sgr_export_changes(sgr_engine* e, uint32_t select, sgr_changes_cursor* c
                            uint32_t* flags, uint32_t* err_idx, int64_t* indices, uint8_t* ids, uint64_t ids_cap,
                            uint32_t* id_offsets, uint64_t* n_rows);
 
+/* Ordered scan of the live table: the rows whose state exists (SGR_ST_EXISTS), in Bytes order of their aggregate ids (unsigned
+ * lexicographic over the UTF-8 bytes, a prefix before any longer id), whose id lies in [from, to]: Kafka Streams'
+ * KeyValueStore.range / all over the store's Bytes keys, served from the table on the device.
+ * Bounds: from == NULL is no lower bound; a non-NULL from with from_len 0 is the id "", which from_exclusive != 0 leaves out
+ * (from_exclusive drops the id equal to from, whatever it is). to == NULL is no upper bound; to is inclusive. from > to gives an
+ * empty page.
+ * A page holds, from the lower bound on, at most max_rows rows and at most ids_cap id bytes. Row i of the page: rows[i]
+ * (state_bytes - 8 program bytes), flags[i] (SGR_ST_*; EXISTS is always set, ERROR when the last fold's handler threw and kept
+ * the state), indices[i] (its dense index) and its id ids[id_offsets[i] .. id_offsets[i+1]). *n_rows = the rows written; *more
+ * = 1 exactly when a live row in range was left out of the page.
+ * Pages carry no cursor: the caller continues with the page's last id as from and from_exclusive = 1. Each page is read against
+ * one table generation (the call holds the operation lock and waits for an sgr_fold_async, as sgr_get_batch does), but the
+ * pages of one scan may come from different generations when folds run between them. An id live at both ends of such a scan
+ * is reported exactly once; one created or deleted in between may or may not appear.
+ * Rows: the ids of the key table sgr_get_batch reads (sgr_load_keys, or the ids an ingest appended). Rows at or past n_agg,
+ * rows without SGR_ST_EXISTS and rows past the key table never appear. The order lives on the device next to the id index
+ * and is brought up to date by the first scan after the key table changes: appended ids are sorted and merged in, a replaced
+ * key table is ordered again.
+ * Buffers: rows max_rows x (state_bytes - 8), flags max_rows x u32 (optional), indices max_rows x i64 (optional), id_offsets
+ * max_rows + 1 u32, ids ids_cap bytes (NULL when ids_cap == 0).
+ * SGR_ERR_STATE before any fold; SGR_ERR_INVALID on NULL buffers, max_rows == 0 or a duplicate id in the key table;
+ * SGR_ERR_CAPACITY (nothing written) when the first row's id alone exceeds ids_cap; SGR_ERR_UNSUPPORTED on a routed engine
+ * (sgr_dist_init), whose rows are local slots, and for tables of 2^32 - 1 rows or more. */
+int32_t sgr_scan(sgr_engine* e, const uint8_t* from, uint32_t from_len, int32_t from_exclusive, const uint8_t* to, uint32_t to_len,
+                 uint64_t max_rows, void* rows, uint32_t* flags, int64_t* indices, uint8_t* ids, uint64_t ids_cap,
+                 uint32_t* id_offsets, uint64_t* n_rows, int32_t* more);
+
 /* Export the whole state table (n_agg * state_bytes) and, optionally, bitmaps
  * (bit i of byte i/8, LSB first). Any out pointer may be NULL. */
 int32_t sgr_export_states(sgr_engine* e, void* out, uint64_t cap,

@@ -122,6 +122,36 @@ JNIEXPORT jlong JNICALL Java_surge_gpu_Native_00024_exportChanges(JNIEnv* env, j
   if (rc != SGR_OK) { throw_for(env, H(h), rc); return -1; }
   return (jlong)n;
 }
+/* One page of sgr_scan. from / to: byte arrays, or null for an open end; fromExclusive leaves the id equal to from out. rows:
+ * maxRows x (state_bytes - 8) bytes; flags / indices / idOffsets: direct buffers of maxRows u32 / maxRows i64 / maxRows + 1 u32;
+ * ids: a direct buffer whose capacity is the page's id-byte budget. Returns 2 * (rows written) + 1 when a live row in range was
+ * left out of the page (+ 0 when the scan is complete), or -1 after throwing. */
+JNIEXPORT jlong JNICALL Java_surge_gpu_Native_00024_scan(JNIEnv* env, jobject o, jlong h, jbyteArray from, jboolean from_exclusive, jbyteArray to,
+                                                         jlong max_rows, jobject rows, jobject flags, jobject indices, jobject ids, jobject id_offsets) {
+  static const uint8_t empty = 0;
+  int ok = 1;
+  if (max_rows <= 0 || max_rows > INT64_MAX / (8 * SGR_MAX_STATE_BYTES)) { bad_arg(env, "maxRows must be positive"); return -1; }
+  uint32_t sb = 0;
+  const jlong user = sgr_states_device(H(h), 0, 0, &sb) == SGR_OK ? (jlong)sb - 8 : 0;   /* (no table yet: the call below says so) */
+  void* rw = direct(env, rows, max_rows * user, "rows: direct buffer shorter than maxRows states", &ok);
+  uint32_t* fl = ok ? (uint32_t*)direct(env, flags, max_rows * 4, "flags: direct buffer of maxRows u32", &ok) : 0;
+  int64_t* ix = ok ? (int64_t*)direct(env, indices, max_rows * 8, "indices: direct buffer of maxRows i64", &ok) : 0;
+  uint32_t* io = ok ? (uint32_t*)direct(env, id_offsets, (max_rows + 1) * 4, "idOffsets: direct buffer of maxRows + 1 u32", &ok) : 0;
+  uint8_t* id = ok ? (uint8_t*)direct(env, ids, 1, "ids: direct buffer", &ok) : 0;
+  if (!ok) return -1;
+  const jsize from_len = from ? (*env)->GetArrayLength(env, from) : 0, to_len = to ? (*env)->GetArrayLength(env, to) : 0;
+  jbyte* f = from ? (*env)->GetByteArrayElements(env, from, 0) : 0;
+  jbyte* t = to ? (*env)->GetByteArrayElements(env, to, 0) : 0;
+  uint64_t n = 0;
+  int32_t more = 0;
+  int32_t rc = sgr_scan(H(h), from ? (f ? (const uint8_t*)f : &empty) : 0, (uint32_t)from_len, from_exclusive ? 1 : 0,
+                        to ? (t ? (const uint8_t*)t : &empty) : 0, (uint32_t)to_len, (uint64_t)max_rows, rw, fl, ix, id,
+                        (uint64_t)(*env)->GetDirectBufferCapacity(env, ids), io, &n, &more);
+  if (f) (*env)->ReleaseByteArrayElements(env, from, f, JNI_ABORT);
+  if (t) (*env)->ReleaseByteArrayElements(env, to, t, JNI_ABORT);
+  if (rc != SGR_OK) { throw_for(env, H(h), rc); return -1; }
+  return (jlong)(2 * n + (more ? 1 : 0));
+}
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_exportStates(JNIEnv* env, jobject o, jlong h, jobject out, jobject changed) {
   return sgr_export_states(H(h), (*env)->GetDirectBufferAddress(env, out), (uint64_t)(*env)->GetDirectBufferCapacity(env, out), 0,
                            changed ? (uint8_t*)(*env)->GetDirectBufferAddress(env, changed) : 0, 0);

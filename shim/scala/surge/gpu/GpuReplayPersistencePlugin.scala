@@ -297,27 +297,76 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
     out.toSeq
   }
 
-  /** Snapshot of the keys in Bytes order (unsigned lexicographic over the UTF-8 bytes), values resolved lazily through get(). */
+  /** The live entries in Bytes order (unsigned lexicographic over the UTF-8 bytes) with from <= id <= to (null: that end open):
+   *  pages of sgr_scan, pulled from the device as the iterator advances, merged with the unflushed puts, which answer first as
+   *  in get() (a deleted one hides the device row). Each page resumes after the last id of the one before, so a fold between two
+   *  pages is fine. */
   private def orderedIterator(from: Bytes, to: Bytes): KeyValueIterator[Bytes, Array[Byte]] = {
     if (!open) throw new InvalidStateStoreException(s"store $storeName is not open")
+    def inside(b: Bytes) = (from == null || from.compareTo(b) <= 0) && (to == null || b.compareTo(to) <= 0)
     lock.readLock().lock()
-    val sorted: Array[Bytes] =
+    val (host, nIds, deviceReadable) =
       try {
-        val all = new util.TreeSet[Bytes]() // Bytes.compareTo is the store order of Kafka Streams
-        keys.forEach(k => all.add(Bytes.wrap(k.getBytes("UTF-8"))))
-        unflushed.keySet().forEach(k => all.add(Bytes.wrap(k.getBytes("UTF-8"))))
-        val view = if (from == null && to == null) all else all.subSet(if (from == null) all.first() else from, true, if (to == null) all.last() else to, true)
-        view.toArray(new Array[Bytes](0))
+        val m = new util.TreeMap[Bytes, Option[Array[Byte]]]() // Bytes.compareTo is the store order of Kafka Streams
+        unflushed.forEach((k, v) => { val b = Bytes.wrap(k.getBytes("UTF-8")); if (inside(b)) m.put(b, v) })
+        // the ids the engine's key table names: `keys` runs ahead of it between putEvent() and the end of flush(), and a slot
+        // the fold has filled still carries its spare-slot placeholder id until loadKeyTable() has run
+        (m.entrySet().toArray(new Array[util.Map.Entry[Bytes, Option[Array[Byte]]]](0)), math.max(loadedKeys, 0).toLong, folded)
       } finally lock.readLock().unlock()
+    val user = reg.program.duplicate().order(ByteOrder.LITTLE_ENDIAN).getInt(0) - 8 // state_bytes is the first field
+    val pageRows = 4096
     new KeyValueIterator[Bytes, Array[Byte]] {
-      private var i = 0
+      private val rows = ByteBuffer.allocateDirect(user * pageRows)
+      private val flags = ByteBuffer.allocateDirect(4 * pageRows).order(ByteOrder.LITTLE_ENDIAN)
+      private val indices = ByteBuffer.allocateDirect(8 * pageRows).order(ByteOrder.LITTLE_ENDIAN)
+      private val idOffsets = ByteBuffer.allocateDirect(4 * (pageRows + 1)).order(ByteOrder.LITTLE_ENDIAN)
+      private val ids = ByteBuffer.allocateDirect(1 << 20)
+      private val toBytes = if (to == null) null else to.get()
+      private var resume: Array[Byte] = if (from == null) null else from.get()
+      private var resumeExclusive = false
+      private var deviceMore = deviceReadable // an empty table before the first flush, as get() answers
+      private val pageKeys = scala.collection.mutable.ArrayBuffer[Bytes]()
+      private val pageValues = scala.collection.mutable.ArrayBuffer[Array[Byte]]()
+      private var d = 0
+      private var h = 0
       private var nextKv: KeyValue[Bytes, Array[Byte]] = _
+
+      private def fillPage(): Unit = while (d >= pageKeys.size && deviceMore) {
+        pageKeys.clear(); pageValues.clear(); d = 0
+        val r = Native.scan(handle, resume, resumeExclusive, toBytes, pageRows.toLong, rows, flags, indices, ids, idOffsets)
+        val n = (r >> 1).toInt
+        deviceMore = (r & 1) != 0
+        var i = 0
+        while (i < n) {
+          val lo = idOffsets.getInt(4 * i); val hi = idOffsets.getInt(4 * (i + 1))
+          val idBytes = new Array[Byte](hi - lo)
+          ids.position(lo); ids.get(idBytes)
+          if (indices.getLong(8 * i) < nIds) { // spare capacity slots are not this store's ids
+            val packed = new Array[Byte](user)
+            rows.position(i * user); rows.get(packed)
+            val value = reg.codec.fromPacked(new String(idBytes, "UTF-8"), packed)
+            if (value != null) { pageKeys += Bytes.wrap(idBytes); pageValues += value } // a null value is skipped, as get() => null was
+          }
+          if (i == n - 1) { resume = idBytes; resumeExclusive = true }
+          i += 1
+        }
+      }
+
       private def advance(): Unit = {
         nextKv = null
-        while (nextKv == null && i < sorted.length) {
-          val v = get(sorted(i)) // deleted / None entries are skipped, like tombstoned RocksDB keys
-          if (v != null) nextKv = new KeyValue(sorted(i), v)
-          i += 1
+        while (nextKv == null) {
+          fillPage()
+          val dk = if (d < pageKeys.size) pageKeys(d) else null
+          val hk = if (h < host.length) host(h).getKey else null
+          if (dk == null && hk == null) return
+          if (dk == null || (hk != null && hk.compareTo(dk) <= 0)) {
+            if (dk != null && hk.equals(dk)) d += 1 // the unflushed value answers for this id
+            host(h).getValue.foreach(v => nextKv = new KeyValue(hk, v.clone()))
+            h += 1
+          } else {
+            nextKv = new KeyValue(dk, pageValues(d))
+            d += 1
+          }
         }
       }
       advance()

@@ -34,6 +34,12 @@ object Native {
    * advances the cursor (next == nAgg: done); throws InvalidStateStoreException when the table changed since the first page */
   @native def exportChanges(handle: Long, select: Int, cursor: ByteBuffer, maxRows: Long, rows: ByteBuffer, flags: ByteBuffer, errIdx: ByteBuffer,
                             indices: ByteBuffer, ids: ByteBuffer, idOffsets: ByteBuffer): Long // sgr_export_changes
+  /** one page of the live rows (SGR_ST_EXISTS) whose id lies in [from, to] (null: that end open; fromExclusive leaves from out),
+   * in Bytes order of the ids: row i = rows (stateBytes - 8), flags(i), indices(i) and its id ids[idOffsets(i) until
+   * idOffsets(i+1)]; the ids buffer's capacity is the page's id-byte budget. Returns 2 * rows written + 1 when a live row in range
+   * was left out (continue from the page's last id, exclusive), + 0 when the scan is complete */
+  @native def scan(handle: Long, from: Array[Byte], fromExclusive: Boolean, to: Array[Byte], maxRows: Long, rows: ByteBuffer, flags: ByteBuffer,
+                   indices: ByteBuffer, ids: ByteBuffer, idOffsets: ByteBuffer): Long // sgr_scan
   @native def partitionForKey(key: Array[Byte], numPartitions: Int, upToColon: Boolean): Int // sgr_partition_for_key_utf8
 
   // raw record batches in, committed offsets out (include/sgr.h "ingest")

@@ -22,6 +22,7 @@
 #include "fold_rows.cuh"
 #include "group_kernels.cuh"
 #include "id_index.cuh"
+#include "id_order.cuh"
 #include "incremental.cuh"
 #include "keytable.h"
 #include "route_push.cuh"
@@ -138,7 +139,8 @@ struct sgr_engine {
   void* gb_host = nullptr;
   size_t gb_host_cap = 0;
   DevBuf gb_dev;
-  DevBuf ch_tiles;                          // sgr_export_changes: per-tile totals and bases (changes.cuh)
+  DevBuf ch_tiles;                          // sgr_export_changes, sgr_scan: per-tile totals and bases (changes.cuh)
+  IdOrder id_order;                         // sgr_scan: the index's ids in Bytes order, brought up to date by the first scan after they change
   // Every call that changes the engine (loads, folds, table growth) and the snapshot refresh of a reader hold op_mu:
   // a reader never sees a table being freed or swapped, and a snapshot is only marked clean for the generation it copied.
   std::recursive_mutex op_mu;
@@ -505,7 +507,7 @@ int32_t sgr_destroy(sgr_engine* e) {
   e->bulk_scratch.release(); e->bulk_err_ids.release(); e->bulk_counters.release(); e->hash_out.release();
   if (e->dist) dist_destroy(e->dist);
   e->part_flags.release(); e->part_data.release(); e->redo_ids.release(); e->run_counters.release();
-  e->id_index.release(); e->gb_dev.release(); e->ch_tiles.release();
+  e->id_index.release(); e->id_order.release(); e->gb_dev.release(); e->ch_tiles.release();
   if (e->gb_host) cudaFreeHost(e->gb_host);
   cudaEventDestroy(e->ev0); cudaEventDestroy(e->ev1); cudaEventDestroy(e->ev2); cudaEventDestroy(e->ev3);
   cudaStreamDestroy(e->stream);
@@ -977,7 +979,7 @@ static int32_t id_index_update(sgr_engine* e, size_t host_extra, size_t dev_byte
   if (!e->ing_key_offs.empty()) { kb = e->ing_key_bytes.data(); ko = e->ing_key_offs.data(); kn = e->ing_key_offs.size() - 1; }
   else if ((kt = std::atomic_load(&e->keys))) { kb = kt->bytes(); ko = kt->offsets(); kn = kt->size(); }
   if (kn >= 0xffffffffull) return fail(e, SGR_ERR_UNSUPPORTED, "the device id index holds fewer than 2^32 - 1 ids");
-  if (!x.valid || x.epoch != e->keys_epoch || kn < x.n) { x.n = 0; x.arena_used = 0; x.epoch = e->keys_epoch; }
+  if (!x.valid || x.epoch != e->keys_epoch || kn < x.n) { x.n = 0; x.arena_used = 0; x.epoch = e->keys_epoch; ++x.builds; }
   bool mono = true;
   const size_t ids = kn > x.n ? round16(id_index_stage_bytes(ko, x.n, kn, &mono)) : 0;
   if (!mono) { x.valid = false; return fail(e, SGR_ERR_INVALID, "key_offsets not monotone"); }
@@ -1086,8 +1088,8 @@ int32_t sgr_export_changes(sgr_engine* e, uint32_t select, sgr_changes_cursor* c
   const uint64_t nt = (n_agg + kChangesTile - 1) / kChangesTile - next / kChangesTile;
   if (nt) CUDA_TRY(e, e->ch_tiles.reserve(nt * 16));
   unsigned long long* tiles = (unsigned long long*)e->ch_tiles.p;
-  cudaError_t ce = changes_count_cut(states, sb, n_agg, key_ref, n_keys, select, next, max_rows, ids_cap, tiles, (unsigned long long*)e->gb_dev.p + 4,
-                                     e->stream);
+  cudaError_t ce = changes_count_cut(states, sb, n_agg, nullptr, key_ref, n_keys, select, next, n_agg, nullptr, max_rows, ids_cap, tiles,
+                                     (unsigned long long*)e->gb_dev.p + 4, e->stream);
   if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "export_changes launch: %s", cudaGetErrorString(ce));
   uint8_t* hctl = (uint8_t*)e->gb_host + (e->gb_host_cap - 64);
   CUDA_TRY(e, cudaMemcpyAsync(hctl, e->gb_dev.p, 64, cudaMemcpyDeviceToHost, e->stream));
@@ -1111,8 +1113,8 @@ int32_t sgr_export_changes(sgr_engine* e, uint32_t select, sgr_changes_cursor* c
       e->gb_host_cap = total + total / 2;
     }
     uint8_t* dd = (uint8_t*)e->gb_dev.p + 64;
-    ce = changes_compact(states, sb, n_agg, key_ref, n_keys, select, next, tiles, nt, page_tiles, page, (long long*)dd, (uint32_t*)(dd + o_err),
-                         (uint32_t*)(dd + o_off), e->stream);
+    ce = changes_compact(states, sb, n_agg, nullptr, key_ref, n_keys, select, next, n_agg, tiles, nt, page_tiles, page, (long long*)dd,
+                         (uint32_t*)(dd + o_err), (uint32_t*)(dd + o_off), e->stream);
     // (every compacted index is below n_agg: the gather's out-of-range word, gb_dev's third u64, stays unread)
     if (ce == cudaSuccess)
       ce = id_index_gather(states, sb, n_agg, (const long long*)dd, page, dd + o_rows, (uint32_t*)(dd + o_fl), (unsigned long long*)e->gb_dev.p + 2,
@@ -1136,6 +1138,105 @@ int32_t sgr_export_changes(sgr_engine* e, uint32_t select, sgr_changes_cursor* c
   cur->next = new_next;
   cur->token = token;
   cur->n_keys = n_keys;
+  return SGR_OK;
+}
+
+int32_t sgr_scan(sgr_engine* e, const uint8_t* from, uint32_t from_len, int32_t from_exclusive, const uint8_t* to, uint32_t to_len,
+                 uint64_t max_rows, void* rows, uint32_t* flags, int64_t* indices, uint8_t* ids, uint64_t ids_cap, uint32_t* id_offsets,
+                 uint64_t* n_rows, int32_t* more) {
+  if (!e || !rows || !id_offsets || !n_rows || !more || (!ids && ids_cap)) return fail(e, SGR_ERR_INVALID, "null argument");
+  if (!max_rows) return fail(e, SGR_ERR_INVALID, "max_rows is 0");
+  // one table generation per page; pages carry no state, so a scan resumes across folds by itself
+  OpLock op_lock(e);
+  if (e->dist) return fail(e, SGR_ERR_UNSUPPORTED, "the rows of a routed engine are local slots: sgr_scan does not map them to ids");
+  int32_t rc = use_device(e); if (rc) return rc;
+  rc = finish_fold(e); if (rc) return rc;
+  if (!e->states_valid) return fail(e, SGR_ERR_STATE, "state store is not readable: no fold has completed");
+  const uint64_t n_agg = e->states_n;
+  if (n_agg >= 0xffffffffull) return fail(e, SGR_ERR_UNSUPPORTED, "sgr_scan reads tables of fewer than 2^32 - 1 aggregates");
+  const uint32_t sb = e->program.state_bytes, user = sb - 8;
+  // gb_dev: [0, 32) the id index insert's control words, [32, 64) the page cut's, [64, 80) the range of positions, [96, ...) the
+  // bounds' bytes (each 16-byte aligned). The words come back to, and the bounds go up from, the page-locked bytes behind the ids.
+  const size_t q_from = from ? round16(from_len) : 0, q_to = to ? round16(to_len) : 0, extra = 96 + q_from + q_to;
+  rc = id_index_update(e, extra, extra); if (rc) return rc;
+  const IdIndex& x = e->id_index;
+  IdOrder& o = e->id_order;
+  uint8_t* hx = (uint8_t*)e->gb_host + (e->gb_host_cap - extra);
+  unsigned long long ctl[12];
+  if (o.builds != x.builds || o.n != x.n) {
+    // the order is made from the ids the index holds: the insert must have found no duplicate first
+    CUDA_TRY(e, cudaMemcpyAsync(hx, e->gb_dev.p, 32, cudaMemcpyDeviceToHost, e->stream));
+    CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+    memcpy(ctl, hx, 32);
+    rc = id_index_settle(e, ctl); if (rc) return rc;
+    if (o.builds != x.builds) { o.n = 0; o.builds = x.builds; }
+    const cudaError_t ce = id_order_update(o, (const uint2*)x.key_ref.p, (const uint8_t*)x.arena.p, x.n, e->stream);
+    if (ce != cudaSuccess) return fail(e, ce == cudaErrorMemoryAllocation ? SGR_ERR_OOM : SGR_ERR_CUDA, "id order: %s", cudaGetErrorString(ce));
+  }
+  const uint64_t n = o.n;
+  const uint2* key_ref = (const uint2*)x.key_ref.p;
+  const uint8_t* arena = (const uint8_t*)x.arena.p;
+  const uint8_t* states = (const uint8_t*)e->states.p;
+  const uint32_t* order = (const uint32_t*)o.order.p;
+  uint8_t* dd = (uint8_t*)e->gb_dev.p;
+  unsigned long long* d_range = (unsigned long long*)(dd + 64);
+  const uint64_t nt = (n + kChangesTile - 1) / kChangesTile;
+  if (n) {
+    if (from_len && from) memcpy(hx + 96, from, from_len);
+    if (to_len && to) memcpy(hx + 96 + q_from, to, to_len);
+    if (q_from + q_to) CUDA_TRY(e, cudaMemcpyAsync(dd + 96, hx + 96, q_from + q_to, cudaMemcpyHostToDevice, e->stream));
+    CUDA_TRY(e, e->ch_tiles.reserve(nt * 16));
+    // the range is found and the page cut on the device; one read-back brings both
+    cudaError_t ce = id_order_bounds(o, key_ref, arena, from ? dd + 96 : nullptr, from_len, from_exclusive != 0, to ? dd + 96 + q_from : nullptr,
+                                     to_len, d_range, e->stream);
+    if (ce == cudaSuccess)
+      ce = changes_count_cut(states, sb, n_agg, order, key_ref, x.n, SGR_ST_EXISTS, 0, n, d_range, max_rows, ids_cap,
+                             (unsigned long long*)e->ch_tiles.p, (unsigned long long*)dd + 4, e->stream);
+    if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "scan launch: %s", cudaGetErrorString(ce));
+  }
+  CUDA_TRY(e, cudaMemcpyAsync(hx, dd, 96, cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+  memcpy(ctl, hx, 96);
+  rc = id_index_settle(e, ctl); if (rc) return rc;
+  const uint64_t lo = n ? ctl[8] : 0, hi = n ? ctl[9] : 0;
+  const uint64_t page = n ? ctl[4 + kChCtlRows] : 0, bytes = n ? ctl[4 + kChCtlBytes] : 0;
+  const uint64_t stop = n ? ctl[4 + kChCtlNext] : 0, page_tiles = n ? ctl[4 + kChCtlTiles] : 0;
+  if (!page && stop < hi)
+    return fail(e, SGR_ERR_CAPACITY, "the id at position %llu of the order does not fit in %llu id bytes", (unsigned long long)stop,
+                (unsigned long long)ids_cap);
+  if (page) {
+    // device (behind the control words) and page-locked alike: indices | flags | err_idx (unused) | id offsets | program bytes | ids
+    const size_t o_fl = round16(page * 8), o_err = o_fl + round16(page * 4), o_off = o_err + round16(page * 4);
+    const size_t o_rows = o_off + round16((page + 1) * 4), o_ids = o_rows + round16(page * user), total = o_ids + round16(bytes);
+    CUDA_TRY(e, e->gb_dev.reserve(96 + total));
+    if (total > e->gb_host_cap) {   // (the stream is idle: nothing is still copying from it)
+      cudaFreeHost(e->gb_host);
+      e->gb_host = nullptr; e->gb_host_cap = 0;
+      CUDA_TRY(e, cudaHostAlloc(&e->gb_host, total + total / 2, cudaHostAllocPortable));
+      e->gb_host_cap = total + total / 2;
+    }
+    uint8_t* dp = (uint8_t*)e->gb_dev.p + 96;
+    cudaError_t ce = changes_compact(states, sb, n_agg, order, key_ref, x.n, SGR_ST_EXISTS, lo, hi, (const unsigned long long*)e->ch_tiles.p, nt,
+                                     page_tiles, page, (long long*)dp, (uint32_t*)(dp + o_err), (uint32_t*)(dp + o_off), e->stream);
+    // (every compacted index is below n_agg: the gather's out-of-range word, gb_dev's third u64, stays unread)
+    if (ce == cudaSuccess)
+      ce = id_index_gather(states, sb, n_agg, (const long long*)dp, page, dp + o_rows, (uint32_t*)(dp + o_fl), (unsigned long long*)e->gb_dev.p + 2,
+                           e->stream);
+    if (ce == cudaSuccess) ce = changes_copy_ids((const long long*)dp, (const uint32_t*)(dp + o_off), page, key_ref, arena, x.n, dp + o_ids, e->stream);
+    if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "scan launch: %s", cudaGetErrorString(ce));
+    const uint8_t* hd = (const uint8_t*)e->gb_host;
+    CUDA_TRY(e, cudaMemcpyAsync(e->gb_host, dp, total, cudaMemcpyDeviceToHost, e->stream));
+    CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+    if (indices) memcpy(indices, hd, page * 8);
+    if (flags) memcpy(flags, hd + o_fl, page * 4);
+    memcpy(id_offsets, hd + o_off, (page + 1) * 4);
+    memcpy(rows, hd + o_rows, page * user);
+    if (bytes) memcpy(ids, hd + o_ids, bytes);
+  } else {
+    id_offsets[0] = 0;
+  }
+  *n_rows = page;
+  *more = stop < hi ? 1 : 0;
   return SGR_OK;
 }
 

@@ -2,7 +2,8 @@
 //
 // Two owners use this one layout and probe: the device ingest interns ids as it parses records (intern: the dense index comes
 // from an atomic counter, csrc/dingest_kernels.cu), and the engine's id index (csrc/id_index.cu) inserts ids whose dense index
-// is their position in the key table (insert_at) and answers batched recovery reads (find).
+// is their position in the key table (insert_at) and answers batched recovery reads (find). The id order of the ordered scan
+// (csrc/id_order.cu) compares ids in Bytes order with cmp_ids.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -135,6 +136,28 @@ __device__ __forceinline__ long long find(const DgDict& d, const uint8_t* id, ui
     if (same) return (long long)(v - 1u);
   }
   return -1;
+}
+
+// The 8 bytes at p (8-byte aligned) as a big-endian word: p[0] is the most significant byte.
+__device__ __forceinline__ unsigned long long be_word(const uint8_t* p) {
+  const uint2 v = *reinterpret_cast<const uint2*>(p);
+  return ((unsigned long long)__byte_perm(v.x, 0, 0x0123) << 32) | __byte_perm(v.y, 0, 0x0123);
+}
+
+// Bytes order of two ids (unsigned lexicographic, a prefix before any longer id): < 0, 0 or > 0 as a sorts before, equal to or
+// after b. Both start 8-byte aligned and are readable in whole words up to their length rounded up to 8 (arena entries, or a
+// staged query); bytes past an id's length are masked off, whatever they hold.
+__device__ __forceinline__ int cmp_ids(const uint8_t* a, uint32_t la, const uint8_t* b, uint32_t lb) {
+  const uint32_t n = la < lb ? la : lb;
+  for (uint32_t k = 0; k < n; k += 8) {
+    unsigned long long wa = be_word(a + k), wb = be_word(b + k);
+    if (n - k < 8) {
+      const unsigned long long keep = ~0ull << (64 - 8 * (n - k));
+      wa &= keep; wb &= keep;
+    }
+    if (wa != wb) return wa < wb ? -1 : 1;
+  }
+  return la < lb ? -1 : (la > lb ? 1 : 0);
 }
 
 }  // namespace

@@ -18,6 +18,7 @@ struct IdIndex {
   uint64_t n = 0;            // ids [0, n) of the key table are indexed
   uint64_t arena_used = 0;   // bytes (8-byte aligned entries)
   uint64_t epoch = 0;        // which key table the ids come from (sgr_engine::keys_epoch)
+  uint64_t builds = 0;       // counts the times the index started again from id 0 (the id order, id_order.cuh, follows it)
   bool valid = false;        // false: rebuild from id 0 before the next read
 
   DgDict dict(unsigned long long* ctl) const {

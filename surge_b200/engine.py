@@ -268,6 +268,38 @@ class ReplayEngine:
             if cur.next >= n_agg:
                 return
 
+    def scan(self, frm: Optional[str] = None, to: Optional[str] = None, page_rows: int = 1 << 20,
+             page_id_bytes: int = 64 << 20) -> Iterator[Tuple[np.ndarray, np.ndarray, np.ndarray, List[str]]]:
+        """The live aggregates (their state exists) whose id lies in [frm, to], in Bytes order of the ids (sgr_scan); None leaves
+        that end open. Yields pages of (indices i64[n], flags u32[n], rows u8[n, state_bytes - 8], ids), at most page_rows rows
+        and page_id_bytes id bytes each. Each page resumes after the last id of the one before, so folds between pages are
+        fine: an id live throughout is reported exactly once."""
+        n_agg = self.n_aggregates()
+        cap = max(1, min(int(page_rows), max(n_agg, 1)))
+        user = self.state_bytes - 8
+        lo = None if frm is None else frm.encode("utf-8")
+        hi = None if to is None else to.encode("utf-8")
+        hi_buf = None if hi is None else C.create_string_buffer(hi, max(len(hi), 1))
+        exclusive = 0
+        n, more = C.c_uint64(), C.c_int32()
+        while True:
+            rows = np.empty((cap, user), dtype=np.uint8)
+            flags = np.empty(cap, dtype=np.uint32)
+            idx = np.empty(cap, dtype=np.int64)
+            offs = np.empty(cap + 1, dtype=np.uint32)
+            blob = np.empty(max(int(page_id_bytes), 1), dtype=np.uint8)
+            lo_buf = None if lo is None else C.create_string_buffer(lo, max(len(lo), 1))
+            self._ck(self._lib.sgr_scan(self._h, lo_buf, 0 if lo is None else len(lo), exclusive, hi_buf, 0 if hi is None else len(hi), cap,
+                                        rows.ctypes.data, flags.ctypes.data, idx.ctypes.data, blob.ctypes.data, int(page_id_bytes),
+                                        offs.ctypes.data, C.byref(n), C.byref(more)))
+            k = int(n.value)
+            if k:
+                raw = blob[:int(offs[k])].tobytes()
+                yield idx[:k], flags[:k], rows[:k], [raw[offs[i]:offs[i + 1]].decode("utf-8") for i in range(k)]
+                lo, exclusive = raw[offs[k - 1]:offs[k]], 1
+            if not more.value:
+                return
+
     def get_index(self, agg: int) -> Tuple[Optional[bytes], int, int]:
         """(program bytes or None, flags, err_idx) of one dense aggregate index."""
         buf = C.create_string_buffer(N.MAX_STATE_BYTES)

@@ -365,19 +365,80 @@ class GpuReplayKeyValueStore:
         return out
 
     def all(self) -> Iterator[Tuple[str, bytes]]:
-        with self._lock:
-            # KeyValueStore[Bytes, _] iterates in Bytes order: unsigned lexicographic over the UTF-8 key bytes
-            keys = sorted(set(self._ingest.keys() if self._ingest is not None else self._keys) | set(self._overlay) | set(self._unflushed),
-                          key=lambda k: k.encode("utf-8"))
-        for k in keys:
-            v = self.get(k)
-            if v is not None:
-                yield k, v
+        return self._entries(None, None, decode=True)
 
     def range(self, frm: str, to: str) -> Iterator[Tuple[str, bytes]]:
-        lo, hi = frm.encode("utf-8"), to.encode("utf-8")
-        for k, v in self.all():
-            if lo <= k.encode("utf-8") <= hi:
+        return self._entries(frm, to, decode=True)
+
+    def _entries(self, frm: Optional[str], to: Optional[str], decode: bool) -> Iterator[Tuple[str, Optional[bytes]]]:
+        """(id, value) of the live entries with frm <= id <= to (None: that end open) in Bytes order, the order a
+        KeyValueStore[Bytes, _] iterates in: unsigned lexicographic over the UTF-8 bytes. The device pages of engine.scan are
+        merged with the overlay and the unflushed puts, which answer first as in get(); a None there hides the device row. decode:
+        values as get() returns them, else the packed program bytes."""
+        lo = None if frm is None else frm.encode("utf-8")
+        hi = None if to is None else to.encode("utf-8")
+
+        def inside(kb: bytes) -> bool:
+            return (lo is None or lo <= kb) and (hi is None or kb <= hi)
+
+        def check_open():
+            if not self._open:
+                raise InvalidStateStoreException(N.SGR_ERR_STATE, f"store {self._name} is not open")
+
+        with self._lock:
+            host = dict(self._unflushed)
+            host.update(self._overlay)
+            if not self._open:
+                # as the earlier get() per id: a closed store raises at its first id and yields nothing when it holds none
+                if host or (self._ingest.keys() if self._ingest is not None else self._keys):
+                    check_open()
+                return
+            folded = self._folded
+            n_ids = None if self._ingest is not None else max(self._keys_loaded[0], 0)   # the ids in the engine's key table
+            unread = [] if folded else [k for k in (self._ingest.keys() if self._ingest is not None else self._keys) if k not in host]
+        hosted = sorted((kb, k, v) for k, v in host.items() if inside(kb := k.encode("utf-8")))
+
+        def device() -> Iterator[Tuple[bytes, str, Optional[bytes]]]:
+            if not folded:
+                # not restored yet: get() of a device id raises. The earlier range() filtered all(), so the first such id raises
+                # where it sorts, in the range or not, after the overlay and unflushed entries of the range that sort before it
+                for kb, k in sorted((k.encode("utf-8"), k) for k in unread):
+                    yield kb, k, None
+                    raise InvalidStateStoreException(N.SGR_ERR_STATE, f"store {self._name} has not been restored yet")
+                return
+            if lo is not None and hi is not None and lo > hi:
+                return
+            try:
+                for idx, _, rows, ids in self._engine.scan(frm, to):
+                    for i, k in enumerate(ids):
+                        if n_ids is None or idx[i] < n_ids:   # spare capacity slots are not this store's ids
+                            yield k.encode("utf-8"), k, rows[i].tobytes()
+            except N.SgrError:
+                check_open()   # closed while the iteration ran: what get() raised for the next id
+                raise
+
+        dev = device()
+        h = 0
+        for kb, k, packed in dev:
+            while h < len(hosted) and hosted[h][0] < kb:
+                check_open()
+                if hosted[h][2] is not None:
+                    yield hosted[h][1], hosted[h][2]
+                h += 1
+            check_open()
+            if h < len(hosted) and hosted[h][0] == kb:
+                if hosted[h][2] is not None:
+                    yield k, hosted[h][2]
+                h += 1
+                continue
+            if packed is None:   # (an id of a store that has not been restored: the device iterator raises next)
+                continue
+            v = self._decode(k, packed) if decode else packed
+            if v is not None:
+                yield k, v
+        for _, k, v in hosted[h:]:
+            check_open()
+            if v is not None:
                 yield k, v
 
     def restoreAll(self, records: Iterable[Tuple[Optional[str], bytes]]) -> None:  # noqa: N802
@@ -386,7 +447,7 @@ class GpuReplayKeyValueStore:
         self.restore(records)
 
     def approximateNumEntries(self) -> int:  # noqa: N802
-        return sum(1 for _ in self.all())
+        return sum(1 for _ in self._entries(None, None, decode=False))
 
     @property
     def engine(self) -> ReplayEngine:
