@@ -527,7 +527,13 @@ int32_t sgr_append_keys(sgr_engine* e, const void* owner, const uint8_t* keys, c
  * read_committed bookkeeping (control batches, aborted transactions, partition positions). csrc/ingest.cpp is its checker
  * (tests/test_gpu_dingest.py: identical states, ids, offsets and statistics on the same bytes).
  *   - value framing: SGR_VALUE_PACKED only (protobuf / JSON values: use the host ingest);
- *   - programs in the sort-free class (16-byte state, class 0): dropped records stay in place as holes the fold skips;
+ *   - every fixed-record program is accepted. Dropped records (flush markers, duplicates, null values without a tombstone type)
+ *     stay in place as holes. Sort-free programs skip the holes in the atomic fold; the others group the live records on the
+ *     device first (K5, holes left out), at one extra pass over the poll's records. err_idx counts the aggregate's live events of
+ *     the poll, as the host decoder does. For those others a poll whose records were all dropped folds nothing and leaves the
+ *     last fold's flags, as the host decoder does; a sort-free program runs its fold and clears them. All or nothing covers
+ *     refusals before the fold (corruption, dictionary full); an error inside the fold itself (a CUDA failure, a replay-list
+ *     overflow) can leave the previous poll's CHANGED / ERROR flags already cleared;
  *   - dense indices are stable per id but follow no arrival-order promise (they come from an atomic counter);
  *   - polls are processed in groups of SGR_DINGEST_GROUP (default 8192) batches, each group one chain of launches on one of eight
  *     streams; batches decompress into an arena of 3x the wire bytes (a poll that compresses better is decoded a second time from

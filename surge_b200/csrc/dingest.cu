@@ -13,8 +13,9 @@
 //          is enqueued on one of a few streams behind the copy that brought the group's last byte: no host round trip inside
 //          the chain, so groups decode while later fetches are still crossing PCIe and while the host walks their headers.
 // fold   = the chain of the remainder, one synchronisation, the verdicts (any error: nothing of the poll is applied), table
-//          growth, new ids to the engine's key table, the sort-free fold of the decoded records onto the live table; only
-//          then do the partitions' positions advance. All or nothing.
+//          growth, new ids to the engine's key table, the fold of the decoded records onto the live table (sort-free programs
+//          skip the holes in the atomic fold, the others group the live records first); only then do the partitions'
+//          positions advance. All or nothing.
 // The arena the batches decompress into is sized from the wire bytes (3x); if a poll compresses better than that the claims
 // overflow, the flag comes back with the verdicts and the poll is decoded again from an exact host-side layout.
 #include <cuda_runtime.h>
@@ -34,6 +35,7 @@
 #include "../../include/sgr.h"
 #include "devbuf.h"
 #include "dingest_kernels.cuh"
+#include "engine_internal.h"
 
 using namespace sgr;
 
@@ -591,7 +593,7 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
     }
     lap(3);
     int32_t rc_fold = SGR_OK;
-    if (nrec) rc_fold = sgr_fold_incremental_device(g->eng, g->out.b.p, nrec);
+    if (nrec) rc_fold = fold_decoded_poll(g->eng, g->out.b.p, nrec, st.n_records);
     if (appender.joinable()) appender.join();
     if (rc_fold) { dfail(g, rc_fold, "engine: %s", sgr_last_error(g->eng)); discard_poll(g); return rc_fold; }
     if (rc_append) { dfail(g, rc_append, "engine: %s", sgr_last_error(g->eng)); discard_poll(g); return rc_append; }

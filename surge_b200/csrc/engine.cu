@@ -18,6 +18,7 @@
 #include "changes.cuh"
 #include "devbuf.h"
 #include "dist.cuh"
+#include "engine_internal.h"
 #include "fold_kernels.cuh"
 #include "fold_rows.cuh"
 #include "group_kernels.cuh"
@@ -759,13 +760,19 @@ static int32_t fold_incremental_atomic(sgr_engine* e, const void* d_records, uin
   return SGR_OK;
 }
 
-static int32_t fold_incremental_impl(sgr_engine* e, const void* d_records, uint64_t n_records) {
+// holes: the batch is a poll of the device ingest, whose dropped records stay in place with agg == ~0, and n_live of its
+// records are not holes. The sort-free kernel skips holes; the group-by leaves them out of the CSR, so they are neither folded,
+// nor counted as events, nor in err_idx. A grouped poll without live records folds nothing: the last fold's flags stay.
+static int32_t fold_incremental_impl(sgr_engine* e, const void* d_records, uint64_t n_records, bool holes, uint64_t n_live) {
   if (e->program.record_kind != SGR_REC_FIXED64) return fail(e, SGR_ERR_UNSUPPORTED, "incremental batches take fixed 64-byte records");
   if (!e->states_valid) return fail(e, SGR_ERR_NOT_LOADED, "incremental fold needs a live state table (fold or set_initial_states first)");
   { int32_t rc0 = finish_fold(e); if (rc0) return rc0; }
   if (folds_sort_free(e)) return fold_incremental_atomic(e, d_records, n_records);
-  e->inc_atomic_prev_valid = false;
   const uint64_t n_agg = e->states_n;
+  if (holes && (n_agg >= (1ull << 32) || n_records >= (1ull << 32)))
+    return fail(e, SGR_ERR_UNSUPPORTED, "group-by is limited to 2^32 records/aggregates");
+  if (holes && n_live == 0) return SGR_OK;
+  e->inc_atomic_prev_valid = false;
   CUDA_TRY(e, e->inc_offsets.reserve((n_records + 2) * 8));
   CUDA_TRY(e, e->inc_ids.reserve((n_records + 1) * 4));
   DevBuf& grouped = e->group.batch_records;
@@ -774,16 +781,17 @@ static int32_t fold_incremental_impl(sgr_engine* e, const void* d_records, uint6
   // per-batch flags (CHANGED/ERROR) of the aggregates touched by the previous batch are cleared
   if (e->inc_prev_n) clear_batch_flags((uint8_t*)e->states.p, e->program.state_bytes, (const uint32_t*)e->inc_prev_ids.p, e->inc_prev_n, e->stream);
   else clear_batch_flags((uint8_t*)e->states.p, e->program.state_bytes, nullptr, n_agg, e->stream);
-  unsigned long long bad = 0;
+  unsigned long long bad = 0, n_holes = 0;
   uint64_t n_touched = 0;
   cudaError_t ce = group_by_agg_stable(e->group, (const uint8_t*)d_records, n_records, n_agg, (uint8_t*)grouped.p,
                                        (uint64_t*)e->inc_offsets.p, (uint32_t*)e->inc_ids.p, &n_touched,
-                                       (unsigned long long*)e->counters.p, e->stream, &bad);
+                                       (unsigned long long*)e->counters.p, e->stream, &bad, holes ? &n_holes : nullptr);
   if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "group-by: %s", cudaGetErrorString(ce));
   CUDA_TRY(e, cudaEventRecord(e->ev3, e->stream));
   if (bad) return fail(e, SGR_ERR_INVALID, "%llu records carry an aggregate index >= n_agg", bad);
+  const uint64_t live_bytes = (n_records - n_holes) * 64;
   int32_t rc = enqueue_fold(e, (const uint8_t*)grouped.p, (const uint64_t*)e->inc_offsets.p, (const uint32_t*)e->inc_ids.p, n_touched, true,
-                            n_records * 64, true, 0, n_records * 64);
+                            live_bytes, true, 0, live_bytes);
   if (rc) return rc;
   rc = finish_fold(e); if (rc) return rc;
   CUDA_TRY(e, cudaEventElapsedTime(&e->stats.ms_group, e->ev2, e->ev3));
@@ -794,13 +802,17 @@ static int32_t fold_incremental_impl(sgr_engine* e, const void* d_records, uint6
   return SGR_OK;
 }
 
-int32_t sgr_fold_incremental_device(sgr_engine* e, const void* d_records, uint64_t n_records) {
+static int32_t fold_incremental_device(sgr_engine* e, const void* d_records, uint64_t n_records, bool holes, uint64_t n_live) {
   OpLock op_lock(e);
   if (!e || (!d_records && n_records)) return fail(e, SGR_ERR_INVALID, "null argument");
   if (!e->has_program) return fail(e, SGR_ERR_NO_PROGRAM, "no fold program registered");
   int32_t rc = use_device(e); if (rc) return rc;
   e->stats.ms_h2d = 0;
-  return fold_incremental_impl(e, d_records, n_records);
+  return fold_incremental_impl(e, d_records, n_records, holes, n_live);
+}
+
+int32_t sgr_fold_incremental_device(sgr_engine* e, const void* d_records, uint64_t n_records) {
+  return fold_incremental_device(e, d_records, n_records, false, n_records);
 }
 
 int32_t sgr_fold_incremental(sgr_engine* e, const void* records, uint64_t n_records) {
@@ -810,7 +822,7 @@ int32_t sgr_fold_incremental(sgr_engine* e, const void* records, uint64_t n_reco
   int32_t rc = use_device(e); if (rc) return rc;
   CUDA_TRY(e, e->inc_records.reserve(n_records * 64));
   CUDA_TRY(e, cudaMemcpyAsync(e->inc_records.p, records, n_records * 64, cudaMemcpyHostToDevice, e->stream));
-  return fold_incremental_impl(e, e->inc_records.p, n_records);
+  return fold_incremental_impl(e, e->inc_records.p, n_records, false, n_records);
 }
 
 int32_t sgr_load_keys(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n_agg) {
@@ -1641,3 +1653,7 @@ int32_t sgr_stream(sgr_engine* e, void** stream) {
 }
 
 }  // extern "C"
+
+int32_t sgr::fold_decoded_poll(sgr_engine* e, const void* d_records, uint64_t n_records, uint64_t n_live) {
+  return fold_incremental_device(e, d_records, n_records, true, n_live);
+}

@@ -25,12 +25,26 @@ constexpr int kPerWarp = kTile / kWarps;  // 512 keys per warp
 constexpr int kRounds = kPerWarp / 32;    // 16
 
 // ---------------------------------------------------------------- keys
+// kHoles: a hole (agg == ~0, a record the device decode dropped) gets the key n_agg, one past the table, so that every hole
+// sorts behind every live record; holes are counted in bad[2] (one atomic per warp), apart from the bad records in bad[0].
+template <bool kHoles>
 __global__ void extract_keys_kernel(const uint8_t* __restrict__ rec, uint32_t n, uint64_t n_agg,
                                     uint32_t* __restrict__ keys, unsigned long long* __restrict__ bad) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const unsigned long long agg = *reinterpret_cast<const unsigned long long*>(rec + (size_t)i * 64 + 8);
-  if (agg >= n_agg) atomicAdd(bad, 1ull);
+  unsigned long long agg = *reinterpret_cast<const unsigned long long*>(rec + (size_t)i * 64 + 8);
+  if (kHoles) {
+    const bool hole = agg == ~0ull;
+    const uint32_t m = __ballot_sync(__activemask(), hole);
+    if (hole) {
+      if ((threadIdx.x & 31) == __ffs(m) - 1) atomicAdd(bad + 2, (unsigned long long)__popc(m));
+      agg = n_agg;
+    } else if (agg >= n_agg) {
+      atomicAdd(bad, 1ull);
+    }
+  } else if (agg >= n_agg) {
+    atomicAdd(bad, 1ull);
+  }
   keys[i] = (uint32_t)agg;
 }
 
@@ -209,10 +223,16 @@ __global__ void heads_kernel(const uint32_t* __restrict__ sorted, uint32_t n, ui
   if (j >= n) return;
   heads[j] = (j == 0 || sorted[j] != sorted[j - 1]) ? 1u : 0u;
 }
+// kHoles: the n_holes holes sort last and are left out; a poll of holes only leaves n_touched == 0 (zeroed with the counters)
+template <bool kHoles>
 __global__ void compact_kernel(const uint32_t* __restrict__ sorted, uint32_t n, const uint32_t* __restrict__ heads,
                                const uint32_t* __restrict__ pos, uint32_t* __restrict__ ids, uint64_t* __restrict__ offsets,
-                               unsigned long long* __restrict__ n_touched) {
+                               unsigned long long* __restrict__ n_touched, const unsigned long long* __restrict__ n_holes) {
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (kHoles) {
+    n -= (uint32_t)*n_holes;
+    if (n == 0 && j == 0) offsets[0] = 0;
+  }
   if (j >= n) return;
   if (heads[j]) { ids[pos[j]] = sorted[j]; offsets[pos[j]] = (uint64_t)j * 64; }
   if (j == n - 1) {
@@ -223,8 +243,12 @@ __global__ void compact_kernel(const uint32_t* __restrict__ sorted, uint32_t n, 
 }
 
 // ---------------------------------------------------------------- gather: out[j] = rec[idx[j]], 4 lanes x 16 bytes per record
-__global__ void gather_records_kernel(const uint8_t* __restrict__ rec, const uint32_t* __restrict__ idx, uint32_t n, uint8_t* __restrict__ out) {
+// kHoles: only the n - n_holes live records move (the holes sort last)
+template <bool kHoles>
+__global__ void gather_records_kernel(const uint8_t* __restrict__ rec, const uint32_t* __restrict__ idx, uint32_t n, uint8_t* __restrict__ out,
+                                      const unsigned long long* __restrict__ n_holes) {
   const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (kHoles) n -= (uint32_t)*n_holes;
   const uint64_t j = t >> 2;
   if (j >= n) return;
   const uint32_t part = (uint32_t)t & 3u;
@@ -258,11 +282,12 @@ void clear_batch_flags(uint8_t* d_states, uint32_t state_bytes, const uint32_t* 
 cudaError_t group_by_agg_stable(GroupScratch& sc, const uint8_t* d_records, uint64_t n64, uint64_t n_agg,
                                 uint8_t* d_out_records, uint64_t* d_out_offsets, uint32_t* d_touched_ids,
                                 uint64_t* n_touched, unsigned long long* d_counters, cudaStream_t st,
-                                unsigned long long* bad_out) {
+                                unsigned long long* bad_out, unsigned long long* holes_out) {
   const uint32_t n = (uint32_t)n64;
   cudaError_t e;
   *bad_out = 0;
   if (n_touched) *n_touched = 0;
+  if (holes_out) *holes_out = 0;
   if (n == 0) {
     // empty batch: every aggregate has an empty segment
     if (!d_touched_ids) {
@@ -281,10 +306,13 @@ cudaError_t group_by_agg_stable(GroupScratch& sc, const uint8_t* d_records, uint
   uint32_t* tmp = (uint32_t*)sc.scan_tmp.p;
 
   if ((e = cudaMemsetAsync(d_counters, 0, 64, st)) != cudaSuccess) return e;
-  extract_keys_kernel<<<cdiv(n, 256), 256, 0, st>>>(d_records, n, n_agg, ka, d_counters + 4);
+  if (holes_out) extract_keys_kernel<true><<<cdiv(n, 256), 256, 0, st>>>(d_records, n, n_agg, ka, d_counters + 4);
+  else extract_keys_kernel<false><<<cdiv(n, 256), 256, 0, st>>>(d_records, n, n_agg, ka, d_counters + 4);
 
+  // the keys run up to n_agg - 1, or up to n_agg with holes
+  const uint64_t key_end = holes_out ? n_agg + 1 : n_agg;
   int bits = 1;
-  while (bits < 32 && (1ull << bits) < n_agg) ++bits;
+  while (bits < 32 && (1ull << bits) < key_end) ++bits;
   for (int shift = 0; shift < bits; shift += 8) {
     radix_hist_kernel<<<nblocks, kThreads, 0, st>>>(ka, n, shift, hist, nblocks);
     if ((e = exclusive_scan_u32(hist, hist, 256 * nblocks, tmp, st)) != cudaSuccess) return e;
@@ -294,7 +322,9 @@ cudaError_t group_by_agg_stable(GroupScratch& sc, const uint8_t* d_records, uint
     t = ka; ka = kb; kb = t;
     t = ia; ia = ib; ib = t;
   }
-  // ka/ia now hold the sorted keys and the arrival indices in CSR order
+  // ka/ia now hold the sorted keys and the arrival indices in CSR order, holes last (the full-mode lower bound of n_agg is
+  // the first hole, so offsets[n_agg] ends the CSR before them)
+  const unsigned long long* d_holes = d_counters + 6;
   if (!d_touched_ids) {
     offsets_full_kernel<<<cdiv(n_agg + 1, 256), 256, 0, st>>>(ka, n, n_agg, d_out_offsets);
   } else {
@@ -303,15 +333,18 @@ cudaError_t group_by_agg_stable(GroupScratch& sc, const uint8_t* d_records, uint
     uint32_t* pos = heads + n;
     heads_kernel<<<cdiv(n, 256), 256, 0, st>>>(ka, n, heads);
     if ((e = exclusive_scan_u32(heads, pos, n, tmp, st)) != cudaSuccess) return e;
-    compact_kernel<<<cdiv(n, 256), 256, 0, st>>>(ka, n, heads, pos, d_touched_ids, d_out_offsets, d_counters + 5);
+    if (holes_out) compact_kernel<true><<<cdiv(n, 256), 256, 0, st>>>(ka, n, heads, pos, d_touched_ids, d_out_offsets, d_counters + 5, d_holes);
+    else compact_kernel<false><<<cdiv(n, 256), 256, 0, st>>>(ka, n, heads, pos, d_touched_ids, d_out_offsets, d_counters + 5, nullptr);
   }
-  gather_records_kernel<<<cdiv((uint64_t)n * 4, 256), 256, 0, st>>>(d_records, ia, n, d_out_records);
+  if (holes_out) gather_records_kernel<true><<<cdiv((uint64_t)n * 4, 256), 256, 0, st>>>(d_records, ia, n, d_out_records, d_holes);
+  else gather_records_kernel<false><<<cdiv((uint64_t)n * 4, 256), 256, 0, st>>>(d_records, ia, n, d_out_records, nullptr);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  unsigned long long h[2];
-  if ((e = cudaMemcpyAsync(h, d_counters + 4, 16, cudaMemcpyDeviceToHost, st)) != cudaSuccess) return e;
+  unsigned long long h[3];
+  if ((e = cudaMemcpyAsync(h, d_counters + 4, holes_out ? 24 : 16, cudaMemcpyDeviceToHost, st)) != cudaSuccess) return e;
   if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return e;
   *bad_out = h[0];
   if (n_touched) *n_touched = h[1];
+  if (holes_out) *holes_out = h[2];
   return cudaSuccess;
 }
 
