@@ -526,7 +526,12 @@ int32_t sgr_append_keys(sgr_engine* e, const void* owner, const uint8_t* keys, c
  * the fold run on the engine's device (csrc/dingest_kernels.cu); the host walks the 61-byte batch headers and keeps the
  * read_committed bookkeeping (control batches, aborted transactions, partition positions). csrc/ingest.cpp is its checker
  * (tests/test_gpu_dingest.py: identical states, ids, offsets and statistics on the same bytes).
- *   - value framing: SGR_VALUE_PACKED only (protobuf / JSON values: use the host ingest);
+ *   - value framing: as the host ingest's (sgr_dingest_set_value_framing, sgr_dingest_set_json_packer): the packed event, the
+ *     protobuf Event's payload or a flat JSON object through a registered member table, converted inside the parse kernel with
+ *     the host decoder's results and refusal texts ("offset N, record r: JSON event: unknown event class"). Both settings survive
+ *     sgr_dingest_reset and are refused with SGR_ERR_STATE between a submit and its fold. JSON compresses better than packed
+ *     values: under protobuf / JSON framing a poll that needed the exact-layout repeat raises the arena claim for the next polls
+ *     (to the power of two at or above the ratio it showed, at most 16x the wire bytes);
  *   - every fixed-record program is accepted. Dropped records (flush markers, duplicates, null values without a tombstone type)
  *     stay in place as holes. Sort-free programs skip the holes in the atomic fold; the others group the live records on the
  *     device first (K5, holes left out), at one extra pass over the poll's records. err_idx counts the aggregate's live events of
@@ -557,6 +562,10 @@ int32_t sgr_dingest_create(sgr_engine* e, uint64_t max_keys, uint64_t max_id_byt
 int32_t sgr_dingest_destroy(sgr_dingest* g);
 const char* sgr_dingest_last_error(const sgr_dingest* g);
 int32_t sgr_dingest_set_null_value_type(sgr_dingest* g, int32_t event_type);
+/* as sgr_ingest_set_value_framing / sgr_ingest_set_json_packer, validated alike; SGR_ERR_STATE while a poll is pending */
+int32_t sgr_dingest_set_value_framing(sgr_dingest* g, int32_t framing);          /* SGR_VALUE_PACKED | _PROTOBUF_EVENT | _JSON */
+int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, const sgr_json_event* events,
+                                    uint32_t n_events, int32_t unknown_type);
 int32_t sgr_dingest_set_aborted(sgr_dingest* g, int32_t partition, const int64_t* producer_ids, const int64_t* first_offsets, uint64_t n);
 int32_t sgr_dingest_submit(sgr_dingest* g, int32_t partition, const void* data, uint64_t nbytes, sgr_ingest_stats* stats);
 /* decode + intern + fold everything submitted since the last fold onto the engine's live table (grown as ids appear), publish
@@ -568,7 +577,7 @@ int32_t sgr_dingest_offsets(sgr_dingest* g, int32_t partition, int64_t* decoded_
 int32_t sgr_dingest_reset(sgr_dingest* g);
 /* host-clock milliseconds of the last sgr_dingest_fold: [0] wait for the copies and for every group's chain (CRC, lz4 decode +
  * record walk, record parse + id interning — launched by the submits behind the copies), [1] a repeat from an exact arena
- * layout when the 3x estimate was too small (normally 0), [2] unused, [3] launch of the new ids' gather and download,
+ * layout when the arena claims were too small (normally 0), [2] unused, [3] launch of the new ids' gather and download,
  * [4] table growth + fold, with the ids handed to the key table by a helper thread meanwhile, [5] the whole call. */
 int32_t sgr_dingest_last_timing(sgr_dingest* g, float* ms8);
 int32_t sgr_dingest_get_stats(sgr_dingest* g, sgr_ingest_stats* out);

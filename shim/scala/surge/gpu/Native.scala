@@ -55,10 +55,11 @@ object Native {
   /** Array(decodedNext, foldedNext) */
   @native def ingestOffsets(ingest: Long, partition: Int): Array[Long]             // sgr_ingest_offsets
 
-  // the same bytes decoded ON THE DEVICE: only the wire bytes cross PCIe (include/sgr.h "device ingest"); packed values only
+  // the same bytes decoded ON THE DEVICE: only the wire bytes cross PCIe (include/sgr.h "device ingest")
   @native def dingestCreate(handle: Long, maxKeys: Long, maxIdBytes: Long): Long   // sgr_dingest_create (maxIdBytes 0 = 32 per id)
   @native def dingestDestroy(dingest: Long): Int                                   // sgr_dingest_destroy
   @native def dingestSetNullValueType(dingest: Long, eventType: Int): Int          // sgr_dingest_set_null_value_type
+  @native def dingestSetValueFraming(dingest: Long, framing: Int): Int             // sgr_dingest_set_value_framing (0 packed, 1 protobuf Event, 2 JSON)
   @native def dingestSetAborted(dingest: Long, partition: Int, producerIds: Array[Long], firstOffsets: Array[Long]): Int // sgr_dingest_set_aborted
   /** queues one fetch response's bytes (a DIRECT buffer, untouched until dingestFold returns); returns the data batches queued */
   @native def dingestSubmit(dingest: Long, partition: Int, data: ByteBuffer, nbytes: Long): Long // sgr_dingest_submit

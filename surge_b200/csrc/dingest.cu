@@ -17,7 +17,9 @@
 //          skip the holes in the atomic fold, the others group the live records first); only then do the partitions'
 //          positions advance. All or nothing.
 // The arena the batches decompress into is sized from the wire bytes (3x); if a poll compresses better than that the claims
-// overflow, the flag comes back with the verdicts and the poll is decoded again from an exact host-side layout.
+// overflow, the flag comes back with the verdicts and the poll is decoded again from an exact host-side layout. Protobuf and
+// JSON values (sgr_dingest_set_value_framing) are converted to packed events inside the parse kernel (value_framing.h); JSON
+// compresses better than packed values, so under those framings the claim multiple adapts (claim_mult).
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -79,6 +81,12 @@ struct sgr_dingest {
   std::map<int32_t, PartState> parts;       // committed view (after the last successful fold)
   std::map<int32_t, PartState> staged;      // view after the submissions of the current poll
   int32_t null_value_type = -1;
+  int32_t value_framing = SGR_VALUE_PACKED;
+  DevBuf json_table;                        // SGR_VALUE_JSON: member table (vf::Class[], vf::Field[], names) on the device
+  vf::Table json{};                         // ... its view; n_classes == 0 until a packer is registered
+  // arena claim of an lz4 batch, in multiples of its compressed size: 3 for packed values; under protobuf / JSON framing raised
+  // after a poll that needed the exact-layout repeat, to the power of two at or above the largest ratio it showed (at most 16)
+  uint32_t claim_mult = 3;
   // staged submissions
   KeepBuf wire;
   // descriptors of the poll's data batches, in PAGE-LOCKED memory: every copy of them is a true asynchronous DMA (a copy from
@@ -154,7 +162,11 @@ int32_t dfail(sgr_dingest* g, int32_t code, const char* fmt, ...) {
     if (_e != cudaSuccess) return dfail((g), _e == cudaErrorMemoryAllocation ? SGR_ERR_OOM : SGR_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(_e)); \
   } while (0)
 
-const char* dg_err_text(uint32_t e) {
+std::string dg_err_text(uint32_t e) {
+  if ((e & 0xffu) == DG_VALUE_FRAMING) {   // the host decoder's text: JSON reasons follow "JSON event: "
+    const uint32_t why = e >> 8;
+    return std::string(why == vf::NOT_PROTOBUF ? "" : "JSON event: ") + vf::reason_text(why);
+  }
   switch (e) {
     case DG_CRC: return "CRC-32C mismatch";
     case DG_LZ4_HEADER: return "bad LZ4 frame header";
@@ -207,6 +219,7 @@ DgParse parse_args(sgr_dingest* g) {
   p.wire = (const uint8_t*)g->wire.b.p; p.arena = (const uint8_t*)g->arena.b.p;
   p.batches = (DgBatch*)g->d_batches.b.p;
   p.rec_off = (const uint32_t*)g->rec_off.b.p; p.rec_batch = (const uint32_t*)g->rec_batch.b.p; p.out = (uint8_t*)g->out.b.p; p.null_value_type = g->null_value_type;
+  p.value_framing = g->value_framing; p.json = g->json;
   p.dict.tags = (unsigned long long*)g->tags.p; p.dict.slot_idx = (uint32_t*)g->slot_idx.p; p.dict.key_ref = (uint2*)g->key_ref.p;
   p.dict.arena = (uint8_t*)g->id_arena.p; p.dict.ctl = (unsigned long long*)g->ctl.p; p.dict.slots_mask = g->slots - 1;
   p.dict.max_keys = g->max_keys; p.dict.arena_cap = g->arena_cap;
@@ -227,6 +240,8 @@ cudaError_t set_arena_capacity(sgr_dingest* g) {
   return cudaMemcpy((unsigned long long*)g->ctl.p + 9, &cap, 8, cudaMemcpyHostToDevice);
 }
 
+uint32_t claim_multiple(const sgr_dingest* g) { return g->value_framing == SGR_VALUE_PACKED ? 3u : g->claim_mult; }
+
 // Enqueue descriptors-up -> crc_size (+ arena claim) -> decode_walk -> parse for the batches [launched_batches, batch_end) —
 // record slots [launched_records, rec_end) — behind `landed` (the copy of the last fetch that contributes to the group).
 int32_t launch_group(sgr_dingest* g, uint64_t batch_end, uint64_t rec_end, cudaEvent_t landed) {
@@ -237,7 +252,7 @@ int32_t launch_group(sgr_dingest* g, uint64_t batch_end, uint64_t rec_end, cudaE
   DG_TRY(g, grow_keeping(g, g->rec_off, r0 * 4, rec_end * 4 + 64));
   DG_TRY(g, grow_keeping(g, g->rec_batch, r0 * 4, rec_end * 4 + 64));
   DG_TRY(g, grow_keeping(g, g->out, r0 * 64, rec_end * 64 + 64));
-  const uint64_t arena_want = 3 * (uint64_t)g->wire.b.cap + 512;
+  const uint64_t arena_want = (uint64_t)claim_multiple(g) * g->wire.b.cap + 512;
   if (g->arena.b.cap < arena_want) {
     DG_TRY(g, grow_keeping(g, g->arena, b0 ? g->arena.b.cap : 0, arena_want));
     DG_TRY(g, set_arena_capacity(g));
@@ -262,7 +277,7 @@ int32_t launch_group(sgr_dingest* g, uint64_t batch_end, uint64_t rec_end, cudaE
     DG_TRY(g, dg_copy_from_mapped_host(mapped, db, nb * sizeof(DgBatch), s));
   }
   if (rec_end > r0) DG_TRY(g, cudaMemsetAsync((uint32_t*)g->rec_batch.b.p + r0, 0xff, (rec_end - r0) * 4, s));
-  DG_TRY(g, dg_launch_crc_size_fast((const uint8_t*)g->wire.b.p, db, (uint32_t)nb, (unsigned long long*)g->ctl.p + 8, s));
+  DG_TRY(g, dg_launch_crc_size_fast((const uint8_t*)g->wire.b.p, db, (uint32_t)nb, (unsigned long long*)g->ctl.p + 8, claim_multiple(g), s));
   if (tl) DG_TRY(g, cudaEventRecord(tl[1], s));
   DG_TRY(g, dg_launch_decode_walk_fast((const uint8_t*)g->wire.b.p, (uint8_t*)g->arena.b.p, db, (uint32_t)nb, (uint32_t)b0, (uint32_t*)g->rec_off.b.p, (uint32_t*)g->rec_batch.b.p, (unsigned long long*)g->ctl.p + 8, s));
   if (tl) DG_TRY(g, cudaEventRecord(tl[2], s));
@@ -322,7 +337,7 @@ int32_t sgr_dingest_destroy(sgr_dingest* g) {
   if (g->h_keys) cudaFreeHost(g->h_keys);
   g->batches.release();
   g->wire.b.release(); g->d_batches.b.release(); g->arena.b.release(); g->rec_off.b.release(); g->rec_batch.b.release(); g->out.b.release();
-  g->key_offs_dev.release(); g->key_bytes_dev.release();
+  g->key_offs_dev.release(); g->key_bytes_dev.release(); g->json_table.release();
   g->tags.release(); g->slot_idx.release(); g->key_ref.release(); g->id_arena.release(); g->ctl.release();
   if (g->h_ctl) cudaFreeHost(g->h_ctl);
   delete g;
@@ -334,6 +349,59 @@ const char* sgr_dingest_last_error(const sgr_dingest* g) { return g ? g->last_er
 int32_t sgr_dingest_set_null_value_type(sgr_dingest* g, int32_t event_type) {
   if (!g || event_type >= (int32_t)SGR_MAX_TYPES) return dfail(g, SGR_ERR_INVALID, "event type out of range");
   g->null_value_type = event_type < 0 ? -1 : event_type;
+  return SGR_OK;
+}
+
+// Both settings are refused while a poll is pending: its groups were parsed at submit time, and the exact-layout repeat parses
+// again at fold time; one poll must not be decoded two ways.
+int32_t sgr_dingest_set_value_framing(sgr_dingest* g, int32_t framing) {
+  if (!g || (framing != SGR_VALUE_PACKED && framing != SGR_VALUE_PROTOBUF_EVENT && framing != SGR_VALUE_JSON)) return dfail(g, SGR_ERR_INVALID, "unknown value framing %d", framing);
+  if (!g->subs.empty()) return dfail(g, SGR_ERR_STATE, "the value framing cannot change between a submit and its fold");
+  if (framing == SGR_VALUE_JSON && !g->json.n_classes) return dfail(g, SGR_ERR_INVALID, "register a JSON packer first (sgr_dingest_set_json_packer)");
+  g->value_framing = framing;
+  return SGR_OK;
+}
+
+int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, const sgr_json_event* events, uint32_t n_events, int32_t unknown_type) {
+  if (!g || !discriminator || (n_events && !events)) return dfail(g, SGR_ERR_INVALID, "null argument");
+  if (!g->subs.empty()) return dfail(g, SGR_ERR_STATE, "the JSON packer cannot change between a submit and its fold");
+  if (unknown_type >= (int32_t)SGR_MAX_TYPES) return dfail(g, SGR_ERR_INVALID, "unknown_type out of range");
+  if (!*discriminator && n_events != 1) return dfail(g, SGR_ERR_INVALID, "without a discriminator member exactly one class can be registered");
+  // the same checks as sgr_ingest_set_json_packer; the table goes to the device as classes, fields, then the names
+  std::vector<vf::Class> classes;
+  std::vector<vf::Field> fields;
+  std::string names = discriminator;
+  for (uint32_t i = 0; i < n_events; ++i) {
+    const sgr_json_event& e = events[i];
+    if (!e.type_name || e.event_type >= SGR_MAX_TYPES || e.n_fields > SGR_JSON_MAX_FIELDS) return dfail(g, SGR_ERR_INVALID, "JSON event %u: bad type name, type index or field count", i);
+    classes.push_back(vf::Class{(uint32_t)names.size(), (uint32_t)strlen(e.type_name), e.event_type, (uint32_t)fields.size(), e.n_fields});
+    names += e.type_name;
+    for (uint32_t f = 0; f < e.n_fields; ++f) {
+      const sgr_json_field& jf = e.fields[f];
+      const uint32_t size = jf.kind == SGR_JSON_I32 ? 4u : jf.kind == SGR_JSON_UUID ? 16u : jf.kind == SGR_JSON_PSTR ? jf.len : 8u;
+      // a member may land on the sequence number (+4, Int only) or anywhere in the payload (+16 .. +64); never on type or agg
+      const bool ok = jf.name && jf.kind <= SGR_JSON_PSTR && jf.dst_off % 4 == 0 && size >= 4 && size % 4 == 0 &&
+                      ((jf.dst_off == 4 && jf.kind == SGR_JSON_I32) || (jf.dst_off >= 16 && jf.dst_off + size <= 64));
+      if (!ok) return dfail(g, SGR_ERR_INVALID, "JSON event %u field %u: bad name, kind, length or record offset", i, f);
+      fields.push_back(vf::Field{(uint32_t)names.size(), (uint32_t)strlen(jf.name), jf.kind, jf.dst_off, size});
+      names += jf.name;
+    }
+  }
+  const size_t cls_bytes = classes.size() * sizeof(vf::Class), fld_bytes = fields.size() * sizeof(vf::Field);
+  std::vector<uint8_t> blob(cls_bytes + fld_bytes + names.size() + 1);
+  if (cls_bytes) memcpy(blob.data(), classes.data(), cls_bytes);
+  if (fld_bytes) memcpy(blob.data() + cls_bytes, fields.data(), fld_bytes);
+  memcpy(blob.data() + cls_bytes + fld_bytes, names.data(), names.size());
+  DG_TRY(g, sync_all(g));   // (no kernel of an earlier poll may still read the old table)
+  DevBuf nb;
+  DG_TRY(g, nb.reserve(blob.size()));
+  const cudaError_t ce = cudaMemcpy(nb.p, blob.data(), blob.size(), cudaMemcpyHostToDevice);
+  if (ce != cudaSuccess) { nb.release(); DG_TRY(g, ce); }
+  g->json_table.release();
+  g->json_table = nb;
+  const uint8_t* base = (const uint8_t*)nb.p;
+  g->json = vf::Table{base + cls_bytes + fld_bytes, (const vf::Class*)base, (const vf::Field*)(base + cls_bytes), (uint32_t)classes.size(), 0,
+                      (uint32_t)strlen(discriminator), unknown_type < 0 ? -1 : unknown_type};
   return SGR_OK;
 }
 
@@ -503,17 +571,23 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
       // the arena claims overflowed (the poll compresses better than 3x): lay the arena out exactly and decode + parse again.
       // Ids the first attempt interned stay (an id is an id); its records are overwritten slot for slot.
       // (exact sizes first: the claim mode never measured them)
-      DG_TRY(g, dg_launch_crc_size_fast((const uint8_t*)g->wire.b.p, (DgBatch*)g->d_batches.b.p, nb, nullptr, g->stream));
+      DG_TRY(g, dg_launch_crc_size_fast((const uint8_t*)g->wire.b.p, (DgBatch*)g->d_batches.b.p, nb, nullptr, 0, g->stream));
       DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.b.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
       DG_TRY(g, cudaStreamSynchronize(g->stream));
       uint64_t need = 0;
+      double ratio = 0;
       for (uint32_t i = 0; i < nb; ++i) {
         DgBatch& b = g->batches[i];
         if (b.err == DG_ARENA_FULL) b.err = DG_OK;
-        if (b.err) { const int32_t rc = dfail(g, SGR_ERR_INVALID, "offset %lld: %s", (long long)b.base_offset, dg_err_text(b.err)); discard_poll(g); return rc; }
+        if (b.err) { const int32_t rc = dfail(g, SGR_ERR_INVALID, "offset %lld: %s", (long long)b.base_offset, dg_err_text(b.err).c_str()); discard_poll(g); return rc; }
         b.err_record = 0;
-        if (b.codec == 3) { b.arena_off = need; need += ((uint64_t)b.dsize + 15) & ~15ull; }
+        if (b.codec == 3) {
+          b.arena_off = need; need += ((uint64_t)b.dsize + 15) & ~15ull;
+          ratio = std::max(ratio, (double)b.dsize / (double)std::max<uint64_t>(1, b.total_len - kBatchHeader));
+        }
       }
+      if (g->value_framing != SGR_VALUE_PACKED)
+        while (g->claim_mult < 16 && (double)g->claim_mult < ratio) g->claim_mult = g->claim_mult < 4 ? 4 : 2 * g->claim_mult;
       g->arena.used = 0;
       DG_TRY(g, g->arena.ensure(need + 512, g->stream));
       DG_TRY(g, set_arena_capacity(g));
@@ -535,7 +609,7 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
     for (uint32_t i = 0; i < nb; ++i) if (g->batches[i].codec == 3 && !g->batches[i].err) st.n_decompressed_bytes += g->batches[i].dsize;
     for (uint32_t i = 0; i < nb; ++i)
       if (g->batches[i].err) {
-        const int32_t rc = dfail(g, SGR_ERR_INVALID, "offset %lld, record %u: %s", (long long)g->batches[i].base_offset, g->batches[i].err_record, dg_err_text(g->batches[i].err));
+        const int32_t rc = dfail(g, SGR_ERR_INVALID, "offset %lld, record %u: %s", (long long)g->batches[i].base_offset, g->batches[i].err_record, dg_err_text(g->batches[i].err).c_str());
         // ids interned by this failed poll stay in the dictionary (harmless: an id is an id); the records are dropped
         discard_poll(g); return rc;
       }

@@ -184,10 +184,10 @@ __device__ uint32_t crc32c_ring(const uint32_t (*tab)[256], RingIn& in, const ui
 }
 
 // arena_ctl (optional): [0] bytes claimed so far, [1] capacity, [2] set when a claim (or, later, a batch in its slot) did not fit.
-// With it: CRC only, and every lz4 batch leaves the kernel with an arena slot of 3x its compressed size. Without it: CRC and the
-// exact decoded size (an lz4 walk that only adds up lengths); the host then lays the arena out.
+// With it: CRC only, and every lz4 batch leaves the kernel with an arena slot of claim_mult x its compressed size. Without it: CRC
+// and the exact decoded size (an lz4 walk that only adds up lengths); the host then lays the arena out.
 __device__ __forceinline__ void crc_size_one(const uint32_t (*tab)[256], RingIn& in, const uint8_t* __restrict__ wire, DgBatch* __restrict__ batches, uint32_t i,
-                                             unsigned long long* __restrict__ arena_ctl) {
+                                             unsigned long long* __restrict__ arena_ctl, uint32_t claim_mult) {
   const DgBatch bt = batches[i];
   const uint8_t* b = wire + bt.src_off;
   uint32_t err = DG_OK, dsize = bt.total_len - 61u;
@@ -195,9 +195,9 @@ __device__ __forceinline__ void crc_size_one(const uint32_t (*tab)[256], RingIn&
   if (crc32c_ring(tab, in, b + 21, (uint64_t)bt.total_len - 21) != bt.stored_crc) err = DG_CRC;
   else if (bt.codec == 3) {
     if (arena_ctl) {
-      // claim mode: no size walk. The slot is 3x the compressed bytes (what the arena is sized for as a whole); a batch that
-      // decodes to more reports DG_ARENA_FULL from the decode kernel and the poll is repeated from exact sizes.
-      const unsigned long long cap = min(3ull * (bt.total_len - 61u) + 64ull, 0xfffffff0ull);
+      // claim mode: no size walk. The slot is claim_mult x the compressed bytes (what the arena is sized for as a whole); a batch
+      // that decodes to more reports DG_ARENA_FULL from the decode kernel and the poll is repeated from exact sizes.
+      const unsigned long long cap = min((unsigned long long)claim_mult * (bt.total_len - 61u) + 64ull, 0xfffffff0ull);
       const unsigned long long need = (cap + 15ull) & ~15ull;
       dsize = (uint32_t)cap;   // (the slot's capacity until the decode kernel replaces it by the decoded size)
       arena_off = atomicAdd(arena_ctl + 0, need);
@@ -217,7 +217,7 @@ __device__ __forceinline__ void crc_size_one(const uint32_t (*tab)[256], RingIn&
 }
 
 __global__ void __launch_bounds__(kFastThreads) dg_crc_size_fast_kernel(const uint8_t* __restrict__ wire, DgBatch* __restrict__ batches, uint32_t n,
-                                                                        unsigned long long* __restrict__ arena_ctl) {
+                                                                        unsigned long long* __restrict__ arena_ctl, uint32_t claim_mult) {
   __shared__ uint32_t tab[8][256];
   __shared__ uint4 ring[kRingChunks][kFastThreads];
   for (int i = threadIdx.x; i < 8 * 256; i += kFastThreads) (&tab[0][0])[i] = (&g_crc_tab[0][0])[i];
@@ -226,7 +226,7 @@ __global__ void __launch_bounds__(kFastThreads) dg_crc_size_fast_kernel(const ui
   if (i >= n) return;
   RingIn in;
   in.init(&ring[0][0]);
-  crc_size_one(tab, in, wire, batches, i, arena_ctl);
+  crc_size_one(tab, in, wire, batches, i, arena_ctl, claim_mult);
   asm volatile("cp.async.wait_all;" ::: "memory");   // chunks requested ahead of the last byte land before the CTA's memory goes
 }
 
@@ -301,6 +301,9 @@ __global__ void dg_key_copy_kernel(const uint2* __restrict__ key_ref, const uint
   for (uint32_t k = part; k < ref.y; k += 8) dst[k] = src[k];
 }
 
+// kFraming (SGR_VALUE_*): the packed instantiation copies the value as it is; the others convert it first (value_framing.h),
+// after the null-value check and before the 8..56 length check, in the host decoder's order.
+template <int32_t kFraming>
 __global__ void __launch_bounds__(kThreads) dg_parse_kernel(const __grid_constant__ DgParse p) {
   const uint32_t i = p.rec_begin + blockIdx.x * kThreads + threadIdx.x;
   if (i >= p.n_records) return;
@@ -322,7 +325,7 @@ __global__ void __launch_bounds__(kThreads) dg_parse_kernel(const __grid_constan
   const int32_t offset_delta = q.varint();
   const int32_t key_len = q.varint();
   const uint8_t* key = key_len > 0 ? q.bytes((uint64_t)key_len) : nullptr;
-  const int32_t val_len = q.varint();
+  int32_t val_len = q.varint();
   const uint8_t* val = val_len > 0 ? q.bytes((uint64_t)val_len) : nullptr;
   const int32_t n_headers = q.varint();
   for (int32_t h = 0; q.ok && h < n_headers; ++h) {
@@ -333,6 +336,15 @@ __global__ void __launch_bounds__(kThreads) dg_parse_kernel(const __grid_constan
   if (bt.base_offset + offset_delta < bt.min_offset) { atomicAdd(p.dict.ctl + 4, 1ull); return; }      // refetch after a restart
   if (key_len <= 0) { atomicAdd(p.dict.ctl + 2, 1ull); return; }                                        // the producer's flush record
   if (val_len < 0 && p.null_value_type < 0) { atomicAdd(p.dict.ctl + 3, 1ull); return; }
+  uint8_t converted[56];
+  if constexpr (kFraming != vf::PACKED) {
+    if (val_len >= 0) {
+      uint32_t n = 0;
+      const uint32_t why = vf::convert(kFraming, p.json, val, (uint32_t)val_len, converted, &val, &n);
+      if (why) { if (atomicCAS(&bt.err, 0u, (uint32_t)DG_VALUE_FRAMING | (why << 8)) == 0u) bt.err_record = r; return; }
+      val_len = (int32_t)n;   // (a protobuf payload lies inside the value: at most 2^31 - 1 bytes)
+    }
+  }
   if (val_len >= 0 && (val_len < 8 || val_len > 56)) { if (atomicCAS(&bt.err, 0u, (uint32_t)DG_VALUE_LENGTH) == 0u) bt.err_record = r; return; }
   uint32_t id_len = (uint32_t)key_len;
   for (uint32_t k = 0; k < (uint32_t)key_len; ++k) if (key[k] == ':') { id_len = k; break; }          // PartitionStringUpToColon
@@ -374,10 +386,10 @@ cudaError_t dg_copy_from_mapped_host(const void* host_mapped, void* dst, uint64_
 
 cudaError_t dg_prepare() { return ensure_crc_tables(); }
 
-cudaError_t dg_launch_crc_size_fast(const uint8_t* wire, DgBatch* batches, uint32_t n, unsigned long long* arena_ctl, cudaStream_t st) {
+cudaError_t dg_launch_crc_size_fast(const uint8_t* wire, DgBatch* batches, uint32_t n, unsigned long long* arena_ctl, uint32_t claim_mult, cudaStream_t st) {
   cudaError_t e = ensure_crc_tables();
   if (e != cudaSuccess || !n) return e;
-  dg_crc_size_fast_kernel<<<(n + kFastThreads - 1) / kFastThreads, kFastThreads, 0, st>>>(wire, batches, n, arena_ctl);
+  dg_crc_size_fast_kernel<<<(n + kFastThreads - 1) / kFastThreads, kFastThreads, 0, st>>>(wire, batches, n, arena_ctl, claim_mult);
   return cudaGetLastError();
 }
 
@@ -403,7 +415,13 @@ cudaError_t dg_gather_keys(const DgDict& d, uint64_t from, uint32_t n, uint32_t*
 
 cudaError_t dg_launch_parse(const DgParse& p, cudaStream_t st) {
   if (p.n_records <= p.rec_begin) return cudaSuccess;
-  dg_parse_kernel<<<(p.n_records - p.rec_begin + kThreads - 1) / kThreads, kThreads, 0, st>>>(p);
+  const uint32_t blocks = (p.n_records - p.rec_begin + kThreads - 1) / kThreads;
+  switch (p.value_framing) {
+    case vf::PACKED: dg_parse_kernel<vf::PACKED><<<blocks, kThreads, 0, st>>>(p); break;
+    case vf::PROTOBUF_EVENT: dg_parse_kernel<vf::PROTOBUF_EVENT><<<blocks, kThreads, 0, st>>>(p); break;
+    case vf::JSON: dg_parse_kernel<vf::JSON><<<blocks, kThreads, 0, st>>>(p); break;
+    default: return cudaErrorInvalidValue;
+  }
   return cudaGetLastError();
 }
 

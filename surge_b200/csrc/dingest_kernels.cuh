@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 #include "id_dict.cuh"
+#include "value_framing.h"
 
 namespace sgr {
 
@@ -12,6 +13,7 @@ enum DgErr : uint32_t {
   DG_OK = 0, DG_CRC = 1, DG_LZ4_HEADER = 2, DG_LZ4_BLOCK = 3, DG_LZ4_SEQUENCE = 4, DG_LZ4_CHECKSUM = 5, DG_LZ4_TOO_LARGE = 6,
   DG_RECORD_LENGTH = 7, DG_RECORD_MALFORMED = 8, DG_RECORD_COUNT = 9, DG_VALUE_LENGTH = 10, DG_ID_LENGTH = 11, DG_STRAY_BYTES = 12,
   DG_ARENA_FULL = 13,   // not a data error: the batch's arena claim did not fit (the host lays the arena out exactly and repeats)
+  DG_VALUE_FRAMING = 14,   // a protobuf / JSON value was refused: err = DG_VALUE_FRAMING | vf::Reason << 8
 };
 
 // One data batch that survived the host's header walk (control batches, aborted transactions and anything below the partition's
@@ -43,6 +45,8 @@ struct DgParse {
   uint8_t* out;                  // [n_records] packed 64-byte records; dropped records become holes (agg == ~0)
   int32_t null_value_type;       // -1: keyed records with a null value are dropped; else they become events of this type
   DgDict dict;
+  int32_t value_framing;         // SGR_VALUE_*: how a value wraps the packed event (selects the kernel's instantiation)
+  vf::Table json;                // SGR_VALUE_JSON: the registered member table, in device memory
 };
 
 cudaError_t dg_launch_parse(const DgParse& p, cudaStream_t st);
@@ -51,7 +55,8 @@ cudaError_t dg_copy_from_mapped_host(const void* host_mapped, void* dst, uint64_
 cudaError_t dg_prepare();   // uploads the CRC tables (a synchronous copy: call it before anything runs on other streams)
 // The two thread-per-batch kernels read wire and arena through a ring that runs up to 256 bytes past a batch's last byte: both
 // buffers need that much room past their content.
-cudaError_t dg_launch_crc_size_fast(const uint8_t* wire, DgBatch* batches, uint32_t n, unsigned long long* arena_ctl, cudaStream_t st);
+// With arena_ctl, every lz4 batch claims claim_mult x its compressed size of arena.
+cudaError_t dg_launch_crc_size_fast(const uint8_t* wire, DgBatch* batches, uint32_t n, unsigned long long* arena_ctl, uint32_t claim_mult, cudaStream_t st);
 // batches: the sub-array to process (n of them), whose first element has index `index_base` in the full array (what rec_batch records);
 // arena_ctl as given to dg_launch_crc_size_fast for the same batches (nullptr: dsize is exact, not a slot capacity)
 cudaError_t dg_launch_decode_walk_fast(const uint8_t* wire, uint8_t* arena, DgBatch* batches, uint32_t n, uint32_t index_base, uint32_t* rec_off, uint32_t* rec_batch,

@@ -13,7 +13,7 @@ from typing import Dict, Sequence, Tuple
 import numpy as np
 
 from . import native as N
-from .ingest import IngestError, _as_pointer
+from .ingest import IngestError, _as_pointer, json_events
 
 
 class DeviceIngest:
@@ -48,6 +48,14 @@ class DeviceIngest:
 
     def set_null_value_type(self, event_type: int) -> None:
         self._check(self._lib.sgr_dingest_set_null_value_type(self._h, event_type))
+
+    def set_value_framing(self, framing: int) -> None:
+        """N.VALUE_PACKED, N.VALUE_PROTOBUF_EVENT or N.VALUE_JSON (after set_json_packer), as Ingest.set_value_framing."""
+        self._check(self._lib.sgr_dingest_set_value_framing(self._h, framing))
+
+    def set_json_packer(self, discriminator: str, events: Sequence[Tuple[str, int, Sequence[Tuple]]], unknown_type: int = -1) -> None:
+        """The member table of JSON values, with the arguments of Ingest.set_json_packer."""
+        self._check(self._lib.sgr_dingest_set_json_packer(self._h, discriminator.encode("utf-8"), json_events(events), len(events), unknown_type))
 
     def set_aborted(self, partition: int, aborted: Sequence[Tuple[int, int]]) -> None:
         if not aborted:

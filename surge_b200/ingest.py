@@ -28,6 +28,24 @@ def _as_pointer(data) -> C.c_void_p:
     return C.c_void_p(np.frombuffer(data, dtype=np.uint8).ctypes.data)
 
 
+def json_events(events: Sequence[Tuple[str, int, Sequence[Tuple]]]):
+    """the sgr_json_event array of a JSON packer (Ingest.set_json_packer's `events`)"""
+    arr = (N.sgr_json_event * max(len(events), 1))()
+    for i, (type_name, event_type, fields) in enumerate(events):
+        arr[i].type_name = type_name.encode("utf-8")
+        arr[i].event_type = event_type
+        arr[i].n_fields = len(fields)
+        if len(fields) > 8:
+            raise IngestError(N.SGR_ERR_INVALID, "at most 8 numeric members per event")
+        for j, spec in enumerate(fields):
+            name, kind, dst_off = spec[:3]
+            arr[i].fields[j].name = name.encode("utf-8")
+            arr[i].fields[j].kind = kind
+            arr[i].fields[j].dst_off = dst_off
+            arr[i].fields[j].len = spec[3] if len(spec) > 3 else 0      # slot size of a JSON_PSTR member
+    return arr
+
+
 class Ingest:
     def __init__(self):
         self._lib = N.load_library()
@@ -64,20 +82,7 @@ class Ingest:
         """events = [(class name, event type index, [(member name, N.JSON_I32 | JSON_I64 | JSON_F64 | JSON_UUID, record byte offset) or
         (member name, N.JSON_PSTR, record byte offset, slot bytes)])].
         Switches nothing by itself: follow with set_value_framing(N.VALUE_JSON)."""
-        arr = (N.sgr_json_event * max(len(events), 1))()
-        for i, (type_name, event_type, fields) in enumerate(events):
-            arr[i].type_name = type_name.encode("utf-8")
-            arr[i].event_type = event_type
-            arr[i].n_fields = len(fields)
-            if len(fields) > 8:
-                raise IngestError(N.SGR_ERR_INVALID, "at most 8 numeric members per event")
-            for j, spec in enumerate(fields):
-                name, kind, dst_off = spec[:3]
-                arr[i].fields[j].name = name.encode("utf-8")
-                arr[i].fields[j].kind = kind
-                arr[i].fields[j].dst_off = dst_off
-                arr[i].fields[j].len = spec[3] if len(spec) > 3 else 0      # slot size of a JSON_PSTR member
-        self._check(self._lib.sgr_ingest_set_json_packer(self._h, discriminator.encode("utf-8"), arr, len(events), unknown_type))
+        self._check(self._lib.sgr_ingest_set_json_packer(self._h, discriminator.encode("utf-8"), json_events(events), len(events), unknown_type))
 
     def set_null_value_type(self, event_type: int) -> None:
         """State-topic mode: null-valued records become events of `event_type` (the program's tombstone rule); -1 drops them."""
