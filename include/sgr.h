@@ -554,7 +554,13 @@ int32_t sgr_append_keys(sgr_engine* e, const void* owner, const uint8_t* keys, c
  *     counting as duplicates. A control batch may be lz4-compressed; its marker is read after decompression. The order holds
  *     per batch: in a fetch with several bad batches the device may report the header-level refusal of a later batch (magic,
  *     codec, length) where the host reports the content error (CRC, lz4, records) of an earlier one. Either way nothing of the
- *     poll is applied.
+ *     poll is applied;
+ *   - inside a batch, a refused record (malformed, its value refused by the framing, outside 8..56 bytes, id too long) is
+ *     reported as the host reports it: the batch's lowest such record, with the host's reason ("offset N, record r: ..."),
+ *     whichever record the device happened to check first. The record walk (a record length that runs past the batch, stray
+ *     bytes after the last record, a recordsCount that does not fit) runs over the whole batch before any record is parsed,
+ *     so a batch with a walk error AND an earlier refused record gets the walk's reason on the device and that record's on
+ *     the host, which checks record by record. The code (SGR_ERR_INVALID) is the same and nothing is applied.
  * poll loop:  sgr_dingest_set_aborted* -> sgr_dingest_submit(partition, bytes)* -> sgr_dingest_fold.
  * `data` of a submit must stay valid until the fold returns (with page-locked memory the copy is one asynchronous DMA). */
 typedef struct sgr_dingest sgr_dingest;

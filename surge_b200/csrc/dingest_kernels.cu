@@ -212,8 +212,7 @@ __device__ __forceinline__ void crc_size_one(const uint32_t (*tab)[256], RingIn&
   if (!err && !(bt.codec == 3 && arena_ctl) && (uint64_t)bt.n_records > (uint64_t)dsize / 7 + 1) err = DG_RECORD_COUNT;   // every record is at least 7 bytes on the wire
   batches[i].dsize = dsize;
   if (arena_ctl) batches[i].arena_off = arena_off;
-  batches[i].err = err;
-  batches[i].err_record = 0;
+  batches[i].err = (uint16_t)err;
 }
 
 __global__ void __launch_bounds__(kFastThreads) dg_crc_size_fast_kernel(const uint8_t* __restrict__ wire, DgBatch* __restrict__ batches, uint32_t n,
@@ -235,6 +234,7 @@ __global__ void __launch_bounds__(kFastThreads) dg_crc_size_fast_kernel(const ui
 __device__ __forceinline__ void decode_walk_one(RingIn& in, const uint8_t* __restrict__ wire, uint8_t* arena, DgBatch* __restrict__ batches, uint32_t i, uint32_t index_base,
                                                 uint32_t* __restrict__ rec_off, uint32_t* __restrict__ rec_batch, unsigned long long* __restrict__ arena_ctl) {
   const DgBatch bt = batches[i];
+  batches[i].rec_err = kNoRecErr;
   if (bt.err) return;
   const uint8_t* sect = wire + bt.src_off + 61;
   uint64_t sect_len = (uint64_t)bt.total_len - 61;
@@ -243,10 +243,10 @@ __device__ __forceinline__ void decode_walk_one(RingIn& in, const uint8_t* __res
     const uint32_t e = lzf::frame<true>(in, sect, sect_len, arena + bt.arena_off, bt.dsize, &len);
     if (arena_ctl) {   // bt.dsize was the capacity of a claimed slot
       if (e == DG_LZ4_TOO_LARGE) { arena_ctl[2] = 1ull; batches[i].err = DG_ARENA_FULL; return; }   // (or a block past its maximum: the exact pass tells)
-      if (e) { batches[i].err = e; return; }
+      if (e) { batches[i].err = (uint16_t)e; return; }
       if ((uint64_t)bt.n_records > len / 7 + 1) { batches[i].err = DG_RECORD_COUNT; return; }
       batches[i].dsize = (uint32_t)len;
-    } else if (e || len != bt.dsize) { batches[i].err = e ? e : DG_LZ4_BLOCK; return; }
+    } else if (e || len != bt.dsize) { batches[i].err = (uint16_t)(e ? e : DG_LZ4_BLOCK); return; }
     sect = arena + bt.arena_off; sect_len = len;
   }
   in.seek(sect);
@@ -267,11 +267,11 @@ __device__ __forceinline__ void decode_walk_one(RingIn& in, const uint8_t* __res
       ok = ok && pos + used <= sect_len;
     }
     const int32_t len = (int32_t)(raw >> 1) ^ -(int32_t)(raw & 1u);
-    if (!ok || len < 0 || (uint64_t)len > sect_len - (pos + used)) { batches[i].err = DG_RECORD_LENGTH; batches[i].err_record = r; return; }
+    if (!ok || len < 0 || (uint64_t)len > sect_len - (pos + used)) { batches[i].err = DG_RECORD_LENGTH; batches[i].rec_err = ((unsigned long long)r << 32) | DG_RECORD_LENGTH; return; }
     rec_off[bt.rec_base + r] = (uint32_t)pos; rec_batch[bt.rec_base + r] = index_base + i;
     pos += used + (uint64_t)len;
   }
-  if (pos != sect_len) { batches[i].err = DG_STRAY_BYTES; batches[i].err_record = bt.n_records; }
+  if (pos != sect_len) { batches[i].err = DG_STRAY_BYTES; batches[i].rec_err = ((unsigned long long)bt.n_records << 32) | DG_STRAY_BYTES; }
 }
 
 __global__ void __launch_bounds__(kFastThreads) dg_decode_walk_fast_kernel(const uint8_t* __restrict__ wire, uint8_t* arena, DgBatch* __restrict__ batches,
@@ -299,6 +299,12 @@ __global__ void dg_key_copy_kernel(const uint2* __restrict__ key_ref, const uint
   const uint8_t* src = arena + ((unsigned long long)ref.x << 3);
   uint8_t* dst = out + offs[i];
   for (uint32_t k = part; k < ref.y; k += 8) dst[k] = src[k];
+}
+
+// A refused record leaves (index << 32) | reason in the batch's rec_err; the lowest index wins, whichever thread gets there
+// first, as the host decoder reports the first bad record of a batch.
+__device__ __forceinline__ void refuse_record(DgBatch& bt, uint32_t r, uint32_t code) {
+  atomicMin(&bt.rec_err, ((unsigned long long)r << 32) | code);
 }
 
 // kFraming (SGR_VALUE_*): the packed instantiation copies the value as it is; the others convert it first (value_framing.h),
@@ -332,7 +338,7 @@ __global__ void __launch_bounds__(kThreads) dg_parse_kernel(const __grid_constan
     const int32_t hk = q.varint(); if (hk < 0) { q.ok = false; break; } q.bytes((uint64_t)hk);
     const int32_t hv = q.varint(); if (hv > 0) q.bytes((uint64_t)hv);
   }
-  if (!q.ok || q.pos != q.n || n_headers < 0) { if (atomicCAS(&bt.err, 0u, (uint32_t)DG_RECORD_MALFORMED) == 0u) bt.err_record = r; return; }
+  if (!q.ok || q.pos != q.n || n_headers < 0) { refuse_record(bt, r, DG_RECORD_MALFORMED); return; }
   if (bt.base_offset + offset_delta < bt.min_offset) { atomicAdd(p.dict.ctl + 4, 1ull); return; }      // refetch after a restart
   if (key_len <= 0) { atomicAdd(p.dict.ctl + 2, 1ull); return; }                                        // the producer's flush record
   if (val_len < 0 && p.null_value_type < 0) { atomicAdd(p.dict.ctl + 3, 1ull); return; }
@@ -341,14 +347,14 @@ __global__ void __launch_bounds__(kThreads) dg_parse_kernel(const __grid_constan
     if (val_len >= 0) {
       uint32_t n = 0;
       const uint32_t why = vf::convert(kFraming, p.json, val, (uint32_t)val_len, converted, &val, &n);
-      if (why) { if (atomicCAS(&bt.err, 0u, (uint32_t)DG_VALUE_FRAMING | (why << 8)) == 0u) bt.err_record = r; return; }
+      if (why) { refuse_record(bt, r, (uint32_t)DG_VALUE_FRAMING | (why << 8)); return; }
       val_len = (int32_t)n;   // (a protobuf payload lies inside the value: at most 2^31 - 1 bytes)
     }
   }
-  if (val_len >= 0 && (val_len < 8 || val_len > 56)) { if (atomicCAS(&bt.err, 0u, (uint32_t)DG_VALUE_LENGTH) == 0u) bt.err_record = r; return; }
+  if (val_len >= 0 && (val_len < 8 || val_len > 56)) { refuse_record(bt, r, DG_VALUE_LENGTH); return; }
   uint32_t id_len = (uint32_t)key_len;
   for (uint32_t k = 0; k < (uint32_t)key_len; ++k) if (key[k] == ':') { id_len = k; break; }          // PartitionStringUpToColon
-  if (id_len >= (1u << 24)) { if (atomicCAS(&bt.err, 0u, (uint32_t)DG_ID_LENGTH) == 0u) bt.err_record = r; return; }
+  if (id_len >= (1u << 24)) { refuse_record(bt, r, DG_ID_LENGTH); return; }
   const uint32_t idx = intern(p.dict, key, id_len);
   if (idx == 0xffffffffu) return;   // dictionary full: counted in ctl[5], the whole call fails
   uint32_t w[16];

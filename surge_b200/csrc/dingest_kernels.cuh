@@ -8,12 +8,12 @@
 
 namespace sgr {
 
-// error codes a kernel leaves in DgBatch::err (0 = fine); dingest.cu turns them into messages
+// error codes a kernel leaves in DgBatch::err or, for one record, in DgBatch::rec_err (0 = fine); dingest.cu turns them into messages
 enum DgErr : uint32_t {
   DG_OK = 0, DG_CRC = 1, DG_LZ4_HEADER = 2, DG_LZ4_BLOCK = 3, DG_LZ4_SEQUENCE = 4, DG_LZ4_CHECKSUM = 5, DG_LZ4_TOO_LARGE = 6,
   DG_RECORD_LENGTH = 7, DG_RECORD_MALFORMED = 8, DG_RECORD_COUNT = 9, DG_VALUE_LENGTH = 10, DG_ID_LENGTH = 11, DG_STRAY_BYTES = 12,
   DG_ARENA_FULL = 13,   // not a data error: the batch's arena claim did not fit (the host lays the arena out exactly and repeats)
-  DG_VALUE_FRAMING = 14,   // a protobuf / JSON value was refused: err = DG_VALUE_FRAMING | vf::Reason << 8
+  DG_VALUE_FRAMING = 14,   // a protobuf / JSON value was refused: the code is DG_VALUE_FRAMING | vf::Reason << 8
 };
 
 // One data batch that survived the host's header walk (control batches, aborted transactions and anything below the partition's
@@ -24,14 +24,19 @@ struct DgBatch {
   int64_t min_offset;    // records below this offset were decoded by an earlier call: duplicates, dropped
   uint32_t total_len;    // 12 + batchLength
   uint32_t n_records;    // recordsCount of the header
-  uint32_t codec;        // 0 none, 3 lz4
   uint32_t stored_crc;   // CRC-32C field of the header
   uint32_t rec_base;     // index of the batch's first record in the per-record tables
   uint32_t dsize;        // out (size pass): decompressed bytes of the records section (lz4), else its stored length
+  uint16_t codec;        // 0 none, 3 lz4
+  uint16_t err;          // out: DgErr of the batch as a whole (CRC, lz4, the record walk); parse runs only when it is 0
   uint64_t arena_off;    // in (decode pass): where the decompressed section goes
-  uint32_t err;          // out: DgErr
-  uint32_t err_record;   // out: record index the error refers to
+  // out: (record << 32) | DgErr of the record an error refers to, ~0 for none (set by the walk). The walk's own errors name
+  // their record here; a parse thread that refuses its record takes the atomicMin, so the batch reports its LOWEST refused
+  // record, the one the host decoder, which checks records in order, stops at
+  unsigned long long rec_err;
 };
+static_assert(sizeof(DgBatch) == 64, "one descriptor per 64 bytes: the descriptor arrays cross PCIe every poll");
+constexpr unsigned long long kNoRecErr = ~0ull;
 
 struct DgParse {
   const uint8_t* wire;
