@@ -266,6 +266,31 @@ int32_t sgr_get_index(sgr_engine* e, uint64_t agg, void* out, uint32_t cap,
 int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n,
                       void* out, uint64_t cap, uint32_t* flags, int64_t* indices);
 
+/* Keyed state writes: a batch of state-topic records applied to the table on the device, the KTable a state topic restores
+ * (SurgeStateStoreConsumer.scala:57-76: last write wins per key, a null value deletes, SurgeModel.scala:62-64).
+ * Record i, in arrival order: id keys[key_offsets[i] .. key_offsets[i+1]) (any bytes, "" included), and either the row
+ * rows + i * (state_bytes - 8) (the program bytes) or, when present[i] == 0, a tombstone (its row is not read).
+ * The table ends as if each record had been folded in order as a snapshot event (SGR_CREATE + SET of every program byte) or a
+ * SGR_TOMBSTONE event: the last record per id decides its row. A row gets SGR_ST_EXISTS and its own bytes; a tombstone leaves
+ * None (program bytes zero, no EXISTS). SGR_ST_CHANGED compares the end state with the state before the batch, field by
+ * field, as a new instance: Double fields with == (NaN is never equal to itself, 0.0 == -0.0), the rest bitwise. So
+ * snap(x), tomb, snap(x) on an existing x is not CHANGED, nor is a tombstone of a None state. The rows the batch writes have
+ * SGR_ST_ERROR and err_idx cleared. The call is a fold for everything scoped to the last fold: the rows it does not write lose
+ * CHANGED and ERROR, the generation advances (an export in progress ends with SGR_ERR_STATE; sgr_get snapshots are refreshed).
+ * Ids: known ids are looked up in the device id index of sgr_get_batch. New ids get dense indices n_keys, n_keys + 1, ... in
+ * order of first appearance in the batch (a tombstone of an unknown id is one too, with a None row), are inserted into that
+ * index and appended to the key table sgr_get / sgr_get_batch / sgr_export_changes / sgr_scan read, and the table grows to
+ * hold them (new rows None, as sgr_grow_states). *n_new_ids (optional): the ids appended. Works for every program (16 to 128
+ * byte states, FIXED64 or VAR16 records: rows are states, not records), and on an engine without a table, which it creates.
+ * Key table: one of sgr_load_keys, one built by earlier put batches, or none. SGR_ERR_STATE (nothing applied) when it mirrors
+ * an ingest's id dictionary (sgr_fold_ingested, the device ingest, sgr_append_keys), which numbers new ids itself;
+ * SGR_ERR_UNSUPPORTED on a routed engine (sgr_dist_init).
+ * All or nothing: SGR_ERR_INVALID on NULL arguments, non-monotone key_offsets or a duplicate id in the key table;
+ * SGR_ERR_CAPACITY when the key table would reach 2^32 - 1 ids or pass 4 GiB of id bytes; SGR_ERR_UNSUPPORTED for n >= 2^32;
+ * n == 0 is a no-op. Holds the operation lock and waits for an sgr_fold_async, as sgr_get_batch does. */
+int32_t sgr_put_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n,
+                      const void* rows, const uint8_t* present, uint64_t* n_new_ids);
+
 /* Changed-state export: the aggregates the last fold changed (SGR_ST_CHANGED, "newState != oldState") or failed (SGR_ST_ERROR,
  * the handler threw and the state was kept), with their ids, compacted on the device and handed over in pages: what the
  * reference's actors publish to the state topic after a poll (PersistentActor.scala:252-263), without copying the whole table.

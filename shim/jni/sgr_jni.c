@@ -97,6 +97,27 @@ JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_getBatch(JNIEnv* env, jobject
   if (rc != SGR_OK) throw_for(env, H(h), rc);
   return rc;
 }
+/* One sgr_put_batch. keys / keyOffsets as for getBatch; rows: a direct buffer of n x (stateBytes - 8) bytes, stateBytes being
+ * the registered program's (checked against the table's when there is one); present: a direct buffer of n bytes (0 = a
+ * tombstone). Returns the ids appended, or -1 after throwing (InvalidStateStoreException on a key table of an ingest). */
+JNIEXPORT jlong JNICALL Java_surge_gpu_Native_00024_putBatch(JNIEnv* env, jobject o, jlong h, jobject keys, jobject offs, jlong n, jobject rows,
+                                                             jint state_bytes, jobject present) {
+  int ok = 1;
+  if (n < 0 || n > INT64_MAX / SGR_MAX_STATE_BYTES) { bad_arg(env, "n must be non-negative"); return -1; }
+  if (state_bytes < 16 || state_bytes > (jint)SGR_MAX_STATE_BYTES) { bad_arg(env, "stateBytes out of range"); return -1; }
+  uint32_t sb = 0;
+  if (sgr_states_device(H(h), 0, 0, &sb) == SGR_OK && sb != (uint32_t)state_bytes) { bad_arg(env, "stateBytes is not the program's"); return -1; }
+  const uint32_t* ko = (const uint32_t*)direct(env, offs, (n + 1) * 4, "keyOffsets: direct buffer of (n + 1) u32", &ok);
+  if (!ok) return -1;
+  const uint8_t* k = ko[n] ? (const uint8_t*)direct(env, keys, (jlong)ko[n], "keys: direct buffer shorter than keyOffsets[n]", &ok) : 0;
+  const void* r = ok ? direct(env, rows, n * (state_bytes - 8), "rows: direct buffer of n x (stateBytes - 8) bytes", &ok) : 0;
+  const uint8_t* p = ok ? (const uint8_t*)direct(env, present, n, "present: direct buffer of n bytes", &ok) : 0;
+  if (!ok) return -1;
+  uint64_t n_new = 0;
+  int32_t rc = sgr_put_batch(H(h), k, ko, (uint64_t)n, r, p, &n_new);
+  if (rc != SGR_OK) { throw_for(env, H(h), rc); return -1; }
+  return (jlong)n_new;
+}
 /* One page of sgr_export_changes. cursor: direct buffer of 4 u64 (next, token, nKeys, reserved), read and updated in place;
  * flags / errIdx / indices / idOffsets: direct buffers of maxRows u32 / u32 / i64 / maxRows + 1 u32; rows: maxRows x
  * (state_bytes - 8) bytes; ids: a direct buffer whose capacity is the page's id-byte budget. Returns the rows written, or -1

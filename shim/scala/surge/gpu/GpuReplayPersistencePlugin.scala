@@ -48,8 +48,8 @@ import surge.kafka.streams.SurgeKafkaStreamsPersistencePlugin
 /** serialized state bytes (what the topic and the actors hold) <-> the packed program bytes of the GPU table */
 trait GpuStateCodec {
 
-  /** program bytes of the state struct: sgr_fold_program.state_bytes - 8. At most 48 for this shim (one fixed 64-byte snapshot
-   *  record carries them at +16); wider states need VAR16 snapshot records (include/sgr.h), not wired here. */
+  /** program bytes of the state struct: sgr_fold_program.state_bytes - 8. At most 48 with snapshot rules (one fixed 64-byte
+   *  snapshot record carries them at +16); a registration without them (state-topic store, sgr_put_batch) takes up to 120. */
   def programBytes: Int
 
   /** aggregateReadFormatting.readState, then the packed layout of surge_b200/formats.py for the model */
@@ -63,12 +63,25 @@ trait GpuStateCodec {
  *  model's event classes PLUS one CREATE+SET rule `snapshotType` that copies program bytes from +16 and one TOMBSTONE rule
  *  `tombstoneType`; surge_b200/dsl.py emits both with `with_snapshot_rules`) and the codec. */
 object GpuFoldPrograms {
-  final case class Registration(program: ByteBuffer, codec: GpuStateCodec, snapshotType: Int, tombstoneType: Int)
+  /** snapshotType / tombstoneType of a registration without snapshot rules */
+  final val NoSnapshotRules = -1
+  final case class Registration(program: ByteBuffer, codec: GpuStateCodec, snapshotType: Int, tombstoneType: Int) {
+    /** no snapshot rules: the store takes records of the STATE topic only, applied on the device by sgr_put_batch */
+    def stateTopic: Boolean = snapshotType == NoSnapshotRules
+  }
   @volatile private var registration: Option[Registration] = None
   def register(packedSgrFoldProgram: ByteBuffer, codec: GpuStateCodec, snapshotType: Int, tombstoneType: Int): Unit = {
-    require(codec.programBytes > 0 && codec.programBytes <= 48 && codec.programBytes % 4 == 0, "snapshot records carry at most 48 program bytes")
+    if (snapshotType == NoSnapshotRules || tombstoneType == NoSnapshotRules) {
+      require(snapshotType == tombstoneType, "a registration names both the snapshot and the tombstone type, or neither")
+      require(codec.programBytes > 0 && codec.programBytes <= 120 && codec.programBytes % 4 == 0, "a state holds at most 120 program bytes")
+    } else {
+      require(codec.programBytes > 0 && codec.programBytes <= 48 && codec.programBytes % 4 == 0, "snapshot records carry at most 48 program bytes")
+    }
     registration = Some(Registration(packedSgrFoldProgram, codec, snapshotType, tombstoneType))
   }
+  /** a state-topic store: no snapshot rules, states of any width the engine folds */
+  def register(packedSgrFoldProgram: ByteBuffer, codec: GpuStateCodec): Unit =
+    register(packedSgrFoldProgram, codec, NoSnapshotRules, NoSnapshotRules)
   def current: Registration = registration.getOrElse(throw new IllegalStateException("no GPU fold program registered for this model"))
 }
 
@@ -106,6 +119,8 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
   private val lock = new ReentrantReadWriteLock()
   private val pending = new java.io.ByteArrayOutputStream()
   private var pendingRecords = 0L
+  // a state-topic store's pending records in arrival order: (id, packed program bytes, or null for a tombstone)
+  private val statePuts = new util.ArrayList[(String, Array[Byte])]()
   private val keyIndex = new util.HashMap[String, java.lang.Long]() // aggregate id -> dense slot (first-seen order)
   private val keys = new util.ArrayList[String]()
   // read-your-writes between put() and flush(): the not-yet-folded value of a key (None = deleted)
@@ -154,7 +169,12 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
     if (id.isEmpty) return // the producer's flush record: empty key, empty value (KafkaProducerActorImpl.scala:321-329)
     lock.writeLock().lock()
     try {
-      if (value == null) appendRecord(reg.tombstoneType, 0, slotOf(id), null)
+      if (reg.stateTopic) {
+        val packed = if (value == null) null else reg.codec.toPacked(id, value)
+        require(packed == null || packed.length <= reg.codec.programBytes, "the packed state is wider than the program's bytes")
+        slotOf(id) // (the device numbers new ids in first-appearance order too: keys stays the key table)
+        statePuts.add(id -> packed)
+      } else if (value == null) appendRecord(reg.tombstoneType, 0, slotOf(id), null)
       else appendRecord(reg.snapshotType, 0, slotOf(id), reg.codec.toPacked(id, value))
       unflushed.put(id, Option(value))
     } finally lock.writeLock().unlock()
@@ -165,6 +185,7 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
     require(packedEvent.length >= 8 && packedEvent.length <= 56, "packed event: u32 type, u32 seq, up to 48 payload bytes")
     val id = recordKey.takeWhile(_ != ':') // PartitionStringUpToColon, KafkaPartitioner.scala:38-42
     val b = ByteBuffer.wrap(packedEvent).order(ByteOrder.LITTLE_ENDIAN)
+    if (reg.stateTopic) throw new IllegalStateException("this store takes records of the state topic only (no snapshot rules registered)")
     lock.writeLock().lock()
     try {
       appendRecord(b.getInt(0), b.getInt(4), slotOf(id), util.Arrays.copyOfRange(packedEvent, 8, packedEvent.length))
@@ -180,6 +201,7 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
   override def flush(): Unit = {
     lock.writeLock().lock()
     try {
+      if (reg.stateTopic) { flushPuts(); return }
       if (pendingRecords == 0L && folded) return
       val batch = pending.toByteArray; pending.reset()
       val n = pendingRecords; pendingRecords = 0L
@@ -192,6 +214,36 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
       unflushed.clear()
       onChanges.foreach(reportChanges)
     } finally lock.writeLock().unlock()
+  }
+
+  /** A state-topic store's flush: every pending record in ONE sgr_put_batch, which interns new ids on the device and grows the
+   *  table to them; no key table is loaded. */
+  private def flushPuts(): Unit = {
+    if (statePuts.isEmpty && folded) return
+    val n = statePuts.size()
+    if (n == 0) check(Native.growStates(handle, 0L)) // nothing to restore: an empty table, readable
+    else {
+      val user = reg.program.duplicate().order(ByteOrder.LITTLE_ENDIAN).getInt(0) - 8
+      val blob = new java.io.ByteArrayOutputStream()
+      val offs = ByteBuffer.allocateDirect((n + 1) * 4).order(ByteOrder.LITTLE_ENDIAN)
+      val rows = ByteBuffer.allocateDirect(math.max(n * user, 1))
+      val present = ByteBuffer.allocateDirect(n)
+      offs.putInt(0)
+      var i = 0
+      while (i < n) {
+        val (id, packed) = statePuts.get(i)
+        blob.write(id.getBytes("UTF-8")); offs.putInt(blob.size())
+        if (packed != null) { rows.position(i * user); rows.put(packed) }
+        present.put(i, (if (packed != null) 1 else 0).toByte)
+        i += 1
+      }
+      val kb = ByteBuffer.allocateDirect(math.max(blob.size(), 1)); kb.put(blob.toByteArray); kb.flip(); offs.flip(); rows.clear()
+      Native.putBatch(handle, kb, offs, n.toLong, rows, user + 8, present) // throws on failure
+      statePuts.clear()
+    }
+    capacity = keys.size().toLong; loadedKeys = keys.size(); folded = true
+    unflushed.clear()
+    onChanges.foreach(reportChanges)
   }
 
   /** The CHANGED and ERROR rows of the fold that just ran, paged from the device (sgr_export_changes); spare capacity slots

@@ -27,6 +27,10 @@ object Native {
   /** n ids (keys[keyOffsets(i) until keyOffsets(i+1)], u32 offsets) in one device call: row i of `out` = program bytes
    * (stateBytes - 8, zero for None / unknown), flags(i) = SGR_ST_* (0 for an unknown id); returns the status */
   @native def getBatch(handle: Long, keys: ByteBuffer, keyOffsets: ByteBuffer, n: Long, out: ByteBuffer, flags: ByteBuffer): Int // sgr_get_batch
+  /** n state-topic records in arrival order (ids as for getBatch): row i = rows[i * (stateBytes - 8), +stateBytes - 8), or a
+   * tombstone when present(i) == 0; the last write per id wins on the device. Returns the ids appended to the key table (in
+   * first-appearance order); throws InvalidStateStoreException when the key table mirrors an ingest */
+  @native def putBatch(handle: Long, keys: ByteBuffer, keyOffsets: ByteBuffer, n: Long, rows: ByteBuffer, stateBytes: Int, present: ByteBuffer): Long // sgr_put_batch
   @native def exportStates(handle: Long, out: ByteBuffer, changedBits: ByteBuffer): Int // sgr_export_states
   /** one page of the rows whose flags meet `select` (SGR_ST_CHANGED = 2 | SGR_ST_ERROR = 4), from the cursor (4 u64: next, token,
    * nKeys, reserved; start with zeros) on: row i = rows (stateBytes - 8), flags(i), errIdx(i), indices(i) and its id

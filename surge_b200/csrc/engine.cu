@@ -26,6 +26,7 @@
 #include "id_order.cuh"
 #include "incremental.cuh"
 #include "keytable.h"
+#include "put_batch.cuh"
 #include "route_push.cuh"
 
 using namespace sgr;
@@ -152,6 +153,9 @@ struct sgr_engine {
   DevBuf gb_dev;
   DevBuf ch_tiles;                          // sgr_export_changes, sgr_scan: per-tile totals and bases (changes.cuh)
   IdOrder id_order;                         // sgr_scan: the index's ids in Bytes order, brought up to date by the first scan after they change
+  // sgr_put_batch: the batch's scratch (put_batch.cuh), and the last-write word of each table row (u32, zero between batches)
+  DevBuf pb_scratch, pb_last;
+  uint64_t pb_last_n = 0;                   // rows pb_last covers
   // Every call that changes the engine (loads, folds, table growth) and the snapshot refresh of a reader hold op_mu:
   // a reader never sees a table being freed or swapped, and a snapshot is only marked clean for the generation it copied.
   std::recursive_mutex op_mu;
@@ -499,6 +503,7 @@ int32_t sgr_destroy(sgr_engine* e) {
   if (e->dist) dist_destroy(e->dist);
   e->part_flags.release(); e->part_data.release(); e->redo_ids.release(); e->run_counters.release();
   e->id_index.release(); e->id_order.release(); e->gb_dev.release(); e->ch_tiles.release();
+  e->pb_scratch.release(); e->pb_last.release();
   if (e->gb_host) cudaFreeHost(e->gb_host);
   cudaEventDestroy(e->ev0); cudaEventDestroy(e->ev1); cudaEventDestroy(e->ev2); cudaEventDestroy(e->ev3);
   cudaStreamDestroy(e->stream);
@@ -1070,6 +1075,172 @@ int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_of
   memcpy(out, hd + r_rows, n * user);
   if (flags) memcpy(flags, hd + r_flags, n * 4);
   if (indices) memcpy(indices, hd + r_idx, n * 8);
+  return SGR_OK;
+}
+
+// What ing_keys_from names while the key table is the one sgr_put_batch appends to: ids the engine numbered itself, with no
+// ingest dictionary behind them (a table of sgr_load_keys becomes one, unchanged, at the first put batch)
+static const char kPutKeysOwner = 0;
+
+// Grow the live table to n_agg rows for sgr_put_batch, keeping its rows; rows past them are None. Capacity grows by at least
+// half, so that batches adding a few ids each do not copy the table every time. Without a table, a new one of None rows. The
+// last-write words (pb_last) cover every row.
+static int32_t put_grow_table(sgr_engine* e, uint64_t n_agg) {
+  const size_t sb = e->program.state_bytes;
+  const uint64_t have = e->states_valid ? e->states_n : 0;
+  if (n_agg > have) {
+    if (e->states.cap < n_agg * sb) {
+      struct Guard { DevBuf b; ~Guard() { b.release(); } } guard;   // frees the old table on success, the new one on failure
+      DevBuf& nb = guard.b;
+      const size_t half = e->states.cap + e->states.cap / 2;
+      CUDA_TRY(e, nb.reserve(n_agg * sb > half ? n_agg * sb : half));
+      if (have) CUDA_TRY(e, cudaMemcpyAsync(nb.p, e->states.p, have * sb, cudaMemcpyDeviceToDevice, e->stream));
+      CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+      std::swap(e->states, nb);
+    }
+    CUDA_TRY(e, cudaMemsetAsync((uint8_t*)e->states.p + have * sb, 0, (n_agg - have) * sb, e->stream));
+    e->states_n = n_agg;
+    e->states_valid = true;
+  }
+  if (e->pb_last_n < e->states_n) {
+    CUDA_TRY(e, e->pb_last.reserve(e->states.cap / sb * 4));
+    CUDA_TRY(e, cudaMemsetAsync(e->pb_last.p, 0, e->pb_last.cap, e->stream));
+    e->pb_last_n = e->pb_last.cap / 4;
+  }
+  return SGR_OK;
+}
+
+// sgr_put_batch once the batch's ids are resolved and known to fit (p: the batch on the device, n_new new ids taking
+// new_aligned arena bytes; its positions come back at hd + r_pos and its control words at hd + r_pb). Applies it and appends the
+// new ids to the host key table. On failure the caller has the id index rebuilt from the host key table, which is unchanged.
+static int32_t put_batch_commit(sgr_engine* e, const PutBatch& p, uint64_t n_new, uint64_t new_aligned, const uint8_t* keys,
+                                const uint32_t* key_offsets, uint8_t* hd, size_t r_pb, size_t r_pos) {
+  IdIndex& x = e->id_index;
+  const uint32_t sb = e->program.state_bytes;
+  const uint64_t n = p.n, n_keys = p.n_keys;
+  // the flags the previous operation left: its touched list when it kept one, else the whole table
+  if (e->states_valid) {
+    if (e->inc_prev_n) clear_batch_flags((uint8_t*)e->states.p, sb, (const uint32_t*)e->inc_prev_ids.p, e->inc_prev_n, e->stream);
+    else clear_batch_flags((uint8_t*)e->states.p, sb, nullptr, e->states_n, e->stream);
+  }
+  int32_t rc = put_grow_table(e, n_keys + n_new); if (rc) return rc;
+  CUDA_TRY(e, e->inc_ids.reserve(n * 4));   // this batch's touched list (the previous one is inc_prev_ids)
+  CUDA_TRY(e, cudaEventRecord(e->ev0, e->stream));
+  x.arena_used += new_aligned;
+  cudaError_t ce = id_index_insert(x, n_keys + n_new, (unsigned long long*)e->gb_dev.p + kCtlDup, e->stream);
+  if (ce == cudaSuccess) ce = put_batch_apply(p, (uint8_t*)e->states.p, e->dprog, (uint32_t*)e->pb_last.p, (uint32_t*)e->inc_ids.p, e->stream);
+  if (ce != cudaSuccess) return fail(e, ce == cudaErrorMemoryAllocation ? SGR_ERR_OOM : SGR_ERR_CUDA, "put_batch: %s", cudaGetErrorString(ce));
+  CUDA_TRY(e, cudaEventRecord(e->ev1, e->stream));
+  CUDA_TRY(e, cudaMemcpyAsync(hd, e->gb_dev.p, 8 * kCtlCut, cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(e, cudaMemcpyAsync(hd + r_pb, p.ctl, 64, cudaMemcpyDeviceToHost, e->stream));
+  if (n_new) CUDA_TRY(e, cudaMemcpyAsync(hd + r_pos, p.new_pos, n_new * 4, cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+  unsigned long long ctl[kCtlCut], pb[8];
+  memcpy(ctl, hd, sizeof ctl);
+  memcpy(pb, hd + r_pb, sizeof pb);
+  rc = id_index_settle(e, ctl); if (rc) return rc;
+  {
+    std::lock_guard<std::mutex> lk(e->keys_mu);
+    if (e->ing_keys_from != &kPutKeysOwner) {
+      // the table of sgr_load_keys (or none) goes on as the put batches' table: same ids, same epoch, the index stays
+      std::shared_ptr<const KeyTable> kt = std::atomic_load(&e->keys);
+      const uint64_t kn = kt ? kt->size() : 0;
+      e->ing_key_bytes.assign(kn ? kt->bytes() : nullptr, kn ? kt->bytes() + kt->offsets()[kn] : nullptr);
+      if (kn) e->ing_key_offs.assign(kt->offsets(), kt->offsets() + kn + 1);
+      else e->ing_key_offs.assign(1, 0u);
+      e->ing_keys_from = &kPutKeysOwner;
+    }
+    const uint32_t* pos = (const uint32_t*)(hd + r_pos);
+    for (uint64_t k = 0; k < n_new; ++k) {
+      const uint32_t b = key_offsets[pos[k]], len = key_offsets[pos[k] + 1] - b;
+      e->ing_key_bytes.insert(e->ing_key_bytes.end(), keys + b, keys + b + len);
+      e->ing_key_offs.push_back(e->ing_key_offs.back() + len);
+    }
+    if (n_new) e->keys_stale.store(true, std::memory_order_release);
+  }
+  // what the next incremental fold or put batch clears: the rows this batch wrote
+  std::swap(e->inc_ids, e->inc_prev_ids);
+  e->inc_prev_n = pb[kPbTouched];
+  e->inc_atomic_prev_valid = false;
+  e->stats.n_aggregates = pb[kPbTouched]; e->stats.n_events = n; e->stats.n_errors = 0; e->stats.n_long_segments = 0;
+  e->stats.event_bytes = n * (sb - 8); e->stats.algorithmic_bytes = n * (sb - 8) + 2ull * sb * pb[kPbTouched];
+  e->stats.ms_h2d = 0; e->stats.ms_group = 0; e->stats.fold_launches = 2;
+  CUDA_TRY(e, cudaEventElapsedTime(&e->stats.ms_fold, e->ev0, e->ev1));
+  mark_dirty(e);
+  return SGR_OK;
+}
+
+int32_t sgr_put_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n, const void* rows, const uint8_t* present,
+                      uint64_t* n_new_ids) {
+  if (!e || (n && (!key_offsets || !rows || !present)) || (n && !keys && key_offsets[n] != key_offsets[0]))
+    return fail(e, SGR_ERR_INVALID, "null argument");
+  if (n >= (1ull << 32)) return fail(e, SGR_ERR_UNSUPPORTED, "a put batch holds fewer than 2^32 records");
+  uint64_t q_aligned = 0;   // the batch's ids as arena entries
+  for (uint64_t i = 0; i < n; ++i) {
+    if (key_offsets[i + 1] < key_offsets[i]) return fail(e, SGR_ERR_INVALID, "key_offsets not monotone at %llu", (unsigned long long)i);
+    q_aligned += ((uint64_t)(key_offsets[i + 1] - key_offsets[i]) + 7) & ~7ull;
+  }
+  if (n_new_ids) *n_new_ids = 0;
+  if (!n) return SGR_OK;
+  OpLock op_lock(e);
+  if (!e->has_program) return fail(e, SGR_ERR_NO_PROGRAM, "register a fold program first");
+  if (e->dist) return fail(e, SGR_ERR_UNSUPPORTED, "the rows of a routed engine are local slots: sgr_put_batch does not map ids to them");
+  uint64_t key_bytes = 0;
+  {
+    std::lock_guard<std::mutex> lk(e->keys_mu);
+    if (e->ing_keys_from && e->ing_keys_from != &kPutKeysOwner)
+      return fail(e, SGR_ERR_STATE, "the key table mirrors an ingest's id dictionary, which numbers new ids itself");
+    std::shared_ptr<const KeyTable> kt;
+    if (!e->ing_key_offs.empty()) key_bytes = e->ing_key_offs.back();
+    else if ((kt = std::atomic_load(&e->keys))) key_bytes = kt->size() ? kt->offsets()[kt->size()] : 0;
+  }
+  int32_t rc = use_device(e); if (rc) return rc;
+  rc = finish_fold(e); if (rc) return rc;
+  const uint32_t user = e->program.state_bytes - 8;
+  // page-locked and device alike: offsets (from 0) | id bytes | rows | tombstone marks, one copy up; back come the index's
+  // control words, the batch's (PutBatch::ctl) and the new ids' positions
+  const uint64_t q0 = key_offsets[0], q_bytes = key_offsets[n] - q0;
+  const size_t o_ids = round16((n + 1) * 4), o_rows = o_ids + round16(q_bytes), o_present = o_rows + round16(n * user), up = o_present + round16(n);
+  const size_t r_pb = 8 * kCtlCut, r_pos = r_pb + 64, down = r_pos + round16(n * 4);
+  rc = id_index_update(e, up + down, kPayloadOff + up); if (rc) return rc;
+  IdIndex& x = e->id_index;
+  uint8_t* hq = (uint8_t*)e->gb_host + (e->gb_host_cap - up - down);   // (behind the ids the index update may still be copying)
+  uint8_t* hd = hq + up;
+  uint32_t* qo = (uint32_t*)hq;
+  for (uint64_t i = 0; i <= n; ++i) qo[i] = key_offsets[i] - (uint32_t)q0;
+  if (q_bytes) memcpy(hq + o_ids, keys + q0, q_bytes);
+  memcpy(hq + o_rows, rows, n * user);
+  memcpy(hq + o_present, present, n);
+  uint8_t* dd = (uint8_t*)e->gb_dev.p + kPayloadOff;
+  CUDA_TRY(e, cudaMemcpyAsync(dd, hq, up, cudaMemcpyHostToDevice, e->stream));
+  PutBatch p;
+  p.offs = (const uint32_t*)dd; p.ids = dd + o_ids; p.rows = dd + o_rows; p.present = dd + o_present;
+  p.n = (uint32_t)n; p.n_keys = x.n;
+  CUDA_TRY(e, e->pb_scratch.reserve(put_batch_scratch_bytes(n)));
+  put_batch_carve(p, e->pb_scratch.p, n);
+  // every id of the batch may be new: room for their refs and bytes behind the resident ones, which do not move
+  cudaError_t ce = id_index_reserve(x, x.n + n, x.arena_used + q_aligned + 8, e->stream);
+  if (ce == cudaSuccess) ce = put_batch_resolve(x, x.arena_used, p, e->stream);
+  if (ce != cudaSuccess) { x.valid = false; return fail(e, ce == cudaErrorMemoryAllocation ? SGR_ERR_OOM : SGR_ERR_CUDA, "put_batch: %s", cudaGetErrorString(ce)); }
+  CUDA_TRY(e, cudaMemcpyAsync(hd, e->gb_dev.p, 8 * kCtlCut, cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(e, cudaMemcpyAsync(hd + r_pb, p.ctl, 64, cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+  unsigned long long ctl[kCtlCut], pb[8];
+  memcpy(ctl, hd, sizeof ctl);
+  memcpy(pb, hd + r_pb, sizeof pb);
+  rc = id_index_settle(e, ctl); if (rc) return rc;
+  if (pb[kPbFull]) return fail(e, SGR_ERR_CUDA, "put_batch: %llu ids found no slot in the batch table", pb[kPbFull]);
+  // nothing is applied yet: the limits of the key table are checked against the exact new ids
+  const uint64_t n_new = pb[kPbNewIds];
+  if (x.n + n_new >= 0xffffffffull)
+    return fail(e, SGR_ERR_CAPACITY, "%llu ids and %llu new ones: a key table holds fewer than 2^32 - 1 ids", (unsigned long long)x.n,
+                (unsigned long long)n_new);
+  if (key_bytes + pb[kPbNewBytes] > 0xffffffffull)
+    return fail(e, SGR_ERR_CAPACITY, "%llu id bytes and %llu new ones: a key table holds at most 4 GiB of ids", (unsigned long long)key_bytes,
+                pb[kPbNewBytes]);
+  rc = put_batch_commit(e, p, n_new, pb[kPbNewIds + 1], keys, key_offsets, hd, r_pb, r_pos);
+  if (rc) { x.valid = false; return rc; }
+  if (n_new_ids) *n_new_ids = n_new;
   return SGR_OK;
 }
 

@@ -252,27 +252,9 @@ fold_stream_kernel(const __grid_constant__ FoldArgs a, const __grid_constant__ D
     } else {
       // shouldPublish = state.stateOpt != context.state
       uint32_t changed = exists != exists0;
-      if (exists && exists0) {
-        if (prog->n_f64 == 0) {
-          for (uint32_t w = 0; w < user_words; ++w) changed |= (st[w * THREADS] != st0[w * THREADS]);
-        } else {
-          // JVM Double ==: f64 fields compare numerically (0.0 == -0.0, NaN != NaN), the rest bitwise. Case-class
-          // equals starts with `this eq that`: when no event built a new instance (empty segment, or only rules without
-          // ops) the state IS the old object and equal to itself even if it holds a NaN.
-          for (uint32_t w = 0; w < user_words; ++w) {
-            bool is_f64 = false;
-            for (uint32_t f = 0; f < prog->n_f64; ++f) is_f64 |= (w == prog->f64_word[f]) || (w == prog->f64_word[f] + 1);
-            if (!is_f64) changed |= (st[w * THREADS] != st0[w * THREADS]);
-          }
-          for (uint32_t f = 0; f < prog->n_f64; ++f) {
-            const uint32_t w = prog->f64_word[f];
-            const uint32_t xl = st[w * THREADS], xh = st[(w + 1) * THREADS], yl = st0[w * THREADS], yh = st0[(w + 1) * THREADS];
-            const double x = __hiloint2double((int)xh, (int)xl);
-            const double y = __hiloint2double((int)yh, (int)yl);
-            changed |= !(x == y) && (copied || xl != yl || xh != yh);
-          }
-        }
-      }
+      if (exists && exists0)
+        changed |= program_words_differ(*prog, user_words, [=](uint32_t w) { return st[w * THREADS]; },
+                                        [=](uint32_t w) { return st0[w * THREADS]; }, copied);
       flags = exists | (changed ? SGR_ST_CHANGED : 0u);
     }
     const bool live = (flags & SGR_ST_EXISTS) != 0;

@@ -101,12 +101,22 @@ cudaError_t id_index_append(IdIndex& x, const uint8_t* bytes, const uint32_t* of
     pos += ((uint64_t)len + 7) & ~7ull;
   }
   cudaError_t e;
-  if ((e = grow_keep(x.key_ref, to * sizeof(uint2), from * sizeof(uint2), st)) != cudaSuccess) return e;
-  if ((e = grow_keep(x.arena, x.arena_used + pos + 8, x.arena_used, st)) != cudaSuccess) return e;
+  if ((e = id_index_reserve(x, to, x.arena_used + pos + 8, st)) != cudaSuccess) return e;
   if ((e = cudaMemcpyAsync((uint2*)x.key_ref.p + from, refs, n_new * sizeof(uint2), cudaMemcpyHostToDevice, st)) != cudaSuccess) return e;
   if (pos && (e = cudaMemcpyAsync((uint8_t*)x.arena.p + x.arena_used, arena, pos, cudaMemcpyHostToDevice, st)) != cudaSuccess) return e;
   x.arena_used += pos;
-  uint64_t insert_from = from;
+  return id_index_insert(x, to, d_ctl, st);
+}
+
+cudaError_t id_index_reserve(IdIndex& x, uint64_t ids, uint64_t arena_bytes, cudaStream_t st) {
+  cudaError_t e = grow_keep(x.key_ref, ids * sizeof(uint2), x.n * sizeof(uint2), st);
+  return e != cudaSuccess ? e : grow_keep(x.arena, arena_bytes, x.arena_used, st);
+}
+
+cudaError_t id_index_insert(IdIndex& x, uint64_t to, unsigned long long* d_ctl, cudaStream_t st) {
+  if (to <= x.n) return cudaSuccess;
+  cudaError_t e;
+  uint64_t insert_from = x.n;
   if (2 * to > x.slots) {
     // load factor past 1/2: a table of at least twice the ids, every resident id inserted again (nothing is uploaded twice)
     uint64_t slots = 1024;

@@ -40,6 +40,14 @@ uint64_t id_index_stage_bytes(const uint32_t* offs, uint64_t from, uint64_t to, 
 cudaError_t id_index_append(IdIndex& x, const uint8_t* bytes, const uint32_t* offs, uint64_t to, void* stage, unsigned long long* d_ctl,
                             cudaStream_t st);
 
+// Grow the resident id storage to hold `ids` refs and `arena_bytes` id bytes, keeping what the index holds (ids [0, x.n) and
+// x.arena_used bytes). Synchronises `st` when it moves them.
+cudaError_t id_index_reserve(IdIndex& x, uint64_t ids, uint64_t arena_bytes, cudaStream_t st);
+
+// Enqueue on `st`: insert ids [x.n, to), whose refs and bytes are already resident, and set x.n = to; rehashes every id from
+// id 0 when the load factor would pass 1/2. d_ctl as for id_index_append.
+cudaError_t id_index_insert(IdIndex& x, uint64_t to, unsigned long long* d_ctl, cudaStream_t st);
+
 // One thread per query id: its dense index, or -1. q_offs[n + 1] index the query bytes q.
 cudaError_t id_index_probe(const IdIndex& x, const uint8_t* q, const uint32_t* q_offs, uint64_t n, long long* idx, cudaStream_t st);
 

@@ -36,6 +36,33 @@ __host__ __device__ inline uint32_t pack_op(uint32_t opcode, uint32_t nwords, ui
 }
 
 #ifdef __CUDACC__
+// ---------------------------------------------------------------- the publish rule over the program words
+// shouldPublish = state.stateOpt != context.state for two states that both exist: word w of the new and the old state are
+// nw(w) and old(w), w < user_words. Words compare bitwise, except the JVM Double fields of the program, which compare as Double
+// == does (0.0 == -0.0, NaN != NaN). Case-class equals starts with `this eq that`: when no event built a new instance (`copied`
+// false: an empty segment, or only rules without ops) the state IS the old object and equal to itself even if it holds a NaN.
+template <class New, class Old>
+__device__ __forceinline__ uint32_t program_words_differ(const DevProgram& p, uint32_t user_words, New nw, Old old, uint32_t copied) {
+  uint32_t changed = 0;
+  if (p.n_f64 == 0) {
+    for (uint32_t w = 0; w < user_words; ++w) changed |= (nw(w) != old(w));
+  } else {
+    for (uint32_t w = 0; w < user_words; ++w) {
+      bool is_f64 = false;
+      for (uint32_t f = 0; f < p.n_f64; ++f) is_f64 |= (w == p.f64_word[f]) || (w == p.f64_word[f] + 1);
+      if (!is_f64) changed |= (nw(w) != old(w));
+    }
+    for (uint32_t f = 0; f < p.n_f64; ++f) {
+      const uint32_t w = p.f64_word[f];
+      const uint32_t xl = nw(w), xh = nw(w + 1), yl = old(w), yh = old(w + 1);
+      const double x = __hiloint2double((int)xh, (int)xl);
+      const double y = __hiloint2double((int)yh, (int)yl);
+      changed |= !(x == y) && (copied || xl != yl || xh != yh);
+    }
+  }
+  return changed;
+}
+
 // ---------------------------------------------------------------- PTX wrappers: mbarrier + 1-D TMA bulk copy
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));

@@ -239,6 +239,31 @@ class ReplayEngine:
             return states, flags, indices
         return [states[i].tobytes() if flags[i] & N.ST_EXISTS else None for i in range(n)]
 
+    def put_batch(self, ids: Sequence[str], rows, present=None) -> int:
+        """Records of a state topic, in arrival order, applied to the table on the device (sgr_put_batch): the last write per id
+        wins, a tombstone (present[i] false) leaves None. rows: u8[n, state_bytes - 8] (or n rows of bytes) holding the program
+        bytes; present: bool[n], None for all rows present. New ids get the next dense indices in order of first appearance and
+        join the key table get() / get_many() / export_changes() / scan() read. Returns the number of new ids."""
+        enc = [k.encode("utf-8") for k in ids]
+        n = len(enc)
+        user = self.state_bytes - 8
+        offs = np.zeros(n + 1, dtype=np.uint32)
+        np.cumsum([len(b) for b in enc], out=offs[1:])
+        blob = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8)
+        if isinstance(rows, np.ndarray):
+            r = np.ascontiguousarray(rows, dtype=np.uint8).reshape(n, user)
+        else:
+            r = np.zeros((n, user), dtype=np.uint8)
+            for i, b in enumerate(rows):
+                if b is not None:
+                    r[i, :len(b)] = np.frombuffer(b, dtype=np.uint8)
+        p = np.ones(n, dtype=np.uint8) if present is None else np.ascontiguousarray(present, dtype=bool).astype(np.uint8)
+        if r.size == 0:
+            r = np.zeros(1, dtype=np.uint8)
+        n_new = C.c_uint64()
+        self._ck(self._lib.sgr_put_batch(self._h, blob.ctypes.data, offs.ctypes.data, n, r.ctypes.data, p.ctypes.data, C.byref(n_new)))
+        return int(n_new.value)
+
     def export_changes(self, select: int = N.ST_CHANGED, page_rows: Optional[int] = 1 << 20,
                        page_id_bytes: int = 64 << 20) -> Iterator[Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray, List[Optional[str]]]]:
         """The aggregates the last fold changed (select=ST_CHANGED) or failed (ST_ERROR, or both), compacted on the device

@@ -120,6 +120,7 @@ ABI = [
     ("sgr_get_index", C.c_int32, [_P, C.c_uint64, _P, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_int32),
                                   C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
     ("sgr_get_batch", C.c_int32, [_P, _P, _P, C.c_uint64, _P, C.c_uint64, _P, _P]),
+    ("sgr_put_batch", C.c_int32, [_P, _P, _P, C.c_uint64, _P, _P, C.POINTER(C.c_uint64)]),
     ("sgr_export_changes", C.c_int32, [_P, C.c_uint32, C.POINTER(sgr_changes_cursor), C.c_uint64, _P, _P, _P, _P, _P, C.c_uint64, _P,
                                        C.POINTER(C.c_uint64)]),
     ("sgr_scan", C.c_int32, [_P, _P, C.c_uint32, C.c_int32, _P, C.c_uint32, C.c_uint64, _P, _P, _P, _P, C.c_uint64, _P,

@@ -116,10 +116,19 @@ def aggregate_id_of_record_key(key: str) -> str:
 class StateCodec:
     """serialized state bytes (what the state topic and the actors hold) <-> the packed program bytes of the GPU table
     (trait GpuStateCodec of shim/scala GpuReplayPersistencePlugin.scala). snapshot_type / tombstone_type are the two extra rules of
-    the registered fold program (programs.counter_program_with_snapshot_rules)."""
+    the registered fold program (programs.counter_program_with_snapshot_rules); a codec without them (both None) makes the store
+    a state-topic store, whose state records go to the table through sgr_put_batch (no extra rules, states of any width)."""
 
-    def __init__(self, to_packed: Callable[[str, bytes], bytes], from_packed: Callable[[str, bytes], bytes], snapshot_type: int, tombstone_type: int):
+    def __init__(self, to_packed: Callable[[str, bytes], bytes], from_packed: Callable[[str, bytes], bytes], snapshot_type: Optional[int] = None,
+                 tombstone_type: Optional[int] = None):
+        if (snapshot_type is None) != (tombstone_type is None):
+            raise ValueError("a codec names both the snapshot and the tombstone type, or neither")
         self.to_packed, self.from_packed, self.snapshot_type, self.tombstone_type = to_packed, from_packed, snapshot_type, tombstone_type
+
+    @property
+    def state_topic(self) -> bool:
+        """No snapshot rules: put()/delete() are applied by sgr_put_batch."""
+        return self.snapshot_type is None
 
 
 class GpuReplayKeyValueStore:
@@ -142,8 +151,12 @@ class GpuReplayKeyValueStore:
         # put() keeps in the overlay (a store without a codec) are not folded, so they are never reported.
         self._on_changes = on_changes
         # with a codec, put()/delete() are records of the STATE topic folded on the GPU as snapshot / tombstone events (feed (i) of
-        # the Scala store): flush() — which Kafka Streams calls before it commits offsets — makes them readable from the table
+        # the Scala store): flush() — which Kafka Streams calls before it commits offsets — makes them readable from the table.
+        # A codec without snapshot rules makes a state-topic store: flush() hands the pending records to one sgr_put_batch,
+        # which numbers new ids on the device in first-appearance order (the order _slot follows), so no key table is loaded
         self._codec = codec
+        self._state_topic = codec is not None and codec.state_topic
+        self._puts: List[Tuple[str, Optional[bytes]]] = []   # a state-topic store's pending records, packed, in arrival order
         self._unflushed: Dict[str, Optional[bytes]] = {}
         self._engine = ReplayEngine(device)
         self._engine.register_program(program)
@@ -201,6 +214,8 @@ class GpuReplayKeyValueStore:
         with self._lock:
             if self._ingest is not None:
                 raise N.SgrError(N.SGR_ERR_INVALID, "this store is already fed through restore_record_batches")
+            if self._state_topic:
+                raise N.SgrError(N.SGR_ERR_INVALID, "this store is fed through put() of state records (its codec has no snapshot rules)")
             rec = np.frombuffer(packed_event, dtype=np.uint8).copy()
             agg_id = aggregate_id_of_record_key(record_key)
             rec[8:16] = np.frombuffer(np.uint64(self._slot(agg_id)).tobytes(), dtype=np.uint8)
@@ -218,6 +233,8 @@ class GpuReplayKeyValueStore:
         would (SurgeStateStoreConsumer.scala:38) into the pending batch. flush() folds it. A store is fed either this
         way or through put_event, not both (each keeps its own id dictionary)."""
         with self._lock:
+            if self._state_topic:
+                raise N.SgrError(N.SGR_ERR_INVALID, "this store is fed through put() of state records (its codec has no snapshot rules)")
             if self._keys:
                 raise N.SgrError(N.SGR_ERR_INVALID, "this store is already fed through put_event")
             if self._ingest is None:
@@ -241,6 +258,9 @@ class GpuReplayKeyValueStore:
                 self._engine.fold_ingested(self._ingest)
                 self._folded = True
                 self._report_changes()
+                return
+            if self._state_topic:
+                self._flush_puts()
                 return
             if not self._pending and self._folded:
                 return
@@ -266,6 +286,26 @@ class GpuReplayKeyValueStore:
                 self._keys_loaded = (n_keys, self._capacity)
             self._unflushed.clear()
             self._report_changes()
+
+    def _flush_puts(self) -> None:
+        """A state-topic store's flush: every pending record in one sgr_put_batch (the first flush creates the table)."""
+        if not self._puts and self._folded:
+            return
+        puts, self._puts = self._puts, []
+        if puts:
+            user = self._engine.state_bytes - 8
+            rows = np.zeros((len(puts), user), dtype=np.uint8)
+            present = np.zeros(len(puts), dtype=bool)
+            for i, (_, packed) in enumerate(puts):
+                if packed is not None:
+                    rows[i, :len(packed)] = np.frombuffer(packed, dtype=np.uint8)
+                    present[i] = True
+            self._engine.put_batch([k for k, _ in puts], rows, present)
+        else:
+            self._engine.grow_states(0)   # nothing restored: an empty table, readable
+        self._folded = True
+        self._unflushed.clear()
+        self._report_changes()
 
     def _report_changes(self) -> None:
         """on_changes for the fold that just ran: its CHANGED and ERROR rows, paged from the device (sgr_export_changes). Spare
@@ -298,11 +338,23 @@ class GpuReplayKeyValueStore:
         self._pending.append(rec)
         self._unflushed[key] = value
 
+    def _state_put(self, key: str, value: Optional[bytes]) -> None:
+        packed = None
+        if value is not None:
+            packed = self._codec.to_packed(key, value)
+            if len(packed) > self._engine.state_bytes - 8:
+                raise ValueError(f"the state packs to {len(packed)} bytes; the program holds {self._engine.state_bytes - 8}")
+        self._slot(key)
+        self._puts.append((key, packed))
+        self._unflushed[key] = value
+
     def put(self, key: str, value: Optional[bytes]) -> None:
         if not key:      # the producer's flush record: empty key, empty value (KafkaProducerActorImpl.scala:321-329)
             return
         with self._lock:
-            if self._codec is not None:
+            if self._state_topic:
+                self._state_put(key, value)
+            elif self._codec is not None:
                 self._state_record(key, value)
             else:
                 self._overlay[key] = value
@@ -394,7 +446,8 @@ class GpuReplayKeyValueStore:
                     check_open()
                 return
             folded = self._folded
-            n_ids = None if self._ingest is not None else max(self._keys_loaded[0], 0)   # the ids in the engine's key table
+            # the ids in the engine's key table (a state-topic store's table has no spare slots)
+            n_ids = None if self._ingest is not None or self._state_topic else max(self._keys_loaded[0], 0)
             unread = [] if folded else [k for k in (self._ingest.keys() if self._ingest is not None else self._keys) if k not in host]
         hosted = sorted((kb, k, v) for k, v in host.items() if inside(kb := k.encode("utf-8")))
 
