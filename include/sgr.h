@@ -597,6 +597,41 @@ int32_t sgr_dingest_set_null_value_type(sgr_dingest* g, int32_t event_type);
 int32_t sgr_dingest_set_value_framing(sgr_dingest* g, int32_t framing);          /* SGR_VALUE_PACKED | _PROTOBUF_EVENT | _JSON */
 int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, const sgr_json_event* events,
                                     uint32_t n_events, int32_t unknown_type);
+/* Decode a compacted STATE topic instead of an events topic (on != 0; 0 goes back to events). The reference recovers by having
+ * Kafka Streams restore the state topic into a KTable (SurgeStateStoreConsumer.scala:57-76): key = the aggregate id as written
+ * (SurgeModel.scala:64), value = the serialized state, null deletes, the last write per key wins.
+ * When: SGR_ERR_STATE while a poll is pending, after any successful fold since create or sgr_dingest_reset (one dictionary and
+ * one set of positions belong to one topic), and once a JSON member table is registered (its offsets mean different things in
+ * the two modes: set the mode first). SGR_ERR_UNSUPPORTED on a routed engine (sgr_dist_init), as sgr_put_batch. The mode
+ * survives sgr_dingest_reset, as the value framing does.
+ * Records: everything a read_committed consumer does stays as in events mode (CRC first, control batches, aborted
+ * transactions, a trailing partial batch, duplicates below the partition's position, the positions of the lag gate). Then:
+ *   - the id is the WHOLE key, with no cut at ':' (shorter than 2^24 bytes);
+ *   - a null or empty key is the producer's flush marker: dropped, counted in n_markers. (The reference's KTable would hold
+ *     an entry for the empty key written by the producer's flush record, KafkaProducerActorImpl.scala:321-329; here it stays
+ *     a dropped marker, as everywhere in this library);
+ *   - a null value is a tombstone, counted in n_null_values and in n_records; sgr_dingest_set_null_value_type has no effect;
+ *   - any other value, after its framing, gives the row's program bytes: SGR_VALUE_PACKED, the value itself, 0 to
+ *     state_bytes - 8 bytes, zero-padded; SGR_VALUE_PROTOBUF_EVENT, the payload of the multilanguage
+ *     `State { string aggregateId = 1; bytes payload = 2; }` (Event's field numbers); SGR_VALUE_JSON, the members of the
+ *     registered table at PROGRAM byte offsets;
+ *   - a framed value longer than state_bytes - 8 is refused: "offset N, record r: state value of L bytes is longer than the
+ *     P program bytes of a row (state_bytes - 8)";
+ *   - n_records counts the live records: rows plus tombstones.
+ * JSON member table in this mode (sgr_dingest_set_json_packer, with a program registered): an empty discriminator and exactly
+ * one class (Json.toJson(state) writes no discriminator; its event_type and unknown_type are ignored); each member needs
+ * dst_off % 4 == 0, a size that is a multiple of 4 and at least 4, and dst_off + size <= state_bytes - 8, else SGR_ERR_INVALID.
+ * Apply: the poll is one sgr_put_batch over its live records in arrival order (submission order, then batch order, then record
+ * order): the last record per id decides its row (EXISTS with its bytes, or None for a tombstone); CHANGED compares with the
+ * state before the poll (Double fields with ==, the rest bitwise); the rows written have ERROR and err_idx cleared; rows the
+ * poll does not write lose CHANGED and ERROR; the generation advances and the rows written are what the next operation clears;
+ * an unknown id, one seen only in a tombstone included, gets a None row; the table grows to hold new ids. Dense indices come
+ * from the device dictionary, with no first-appearance promise; new ids reach the key table as in events mode, so sgr_get,
+ * sgr_get_batch, sgr_export_changes and sgr_scan read them. Every program works: 16- to 128-byte states, FIXED64 or VAR16.
+ * All or nothing as an events poll: a refusal applies nothing to the table, the positions or the statistics. A poll whose
+ * records were all dropped applies nothing to the table and leaves the last fold's flags (as an n == 0 put batch); its
+ * positions still advance. Slot [4] of sgr_dingest_last_timing is table growth + the apply. */
+int32_t sgr_dingest_set_state_topic(sgr_dingest* g, int32_t on);
 int32_t sgr_dingest_set_aborted(sgr_dingest* g, int32_t partition, const int64_t* producer_ids, const int64_t* first_offsets, uint64_t n);
 int32_t sgr_dingest_submit(sgr_dingest* g, int32_t partition, const void* data, uint64_t nbytes, sgr_ingest_stats* stats);
 /* decode + intern + fold everything submitted since the last fold onto the engine's live table (grown as ids appear), publish

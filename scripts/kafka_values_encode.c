@@ -10,8 +10,10 @@
 /* Records i = 0..n-1 with key keys[key_offs[i], key_offs[i + 1]) and value vals[val_offs[i], val_offs[i + 1]) of ONE
  * partition, as consecutive RecordBatches of recs_per_batch records from base_offset. Returns the bytes written, -1 when `cap`
  * is too small, -2 when memory runs out. A bound for cap: the key and value bytes + 32 per record + 160 per batch, plus 1/255. */
-int64_t kv_kafka_encode_values(const uint8_t* keys, const uint64_t* key_offs, const uint8_t* vals, const uint64_t* val_offs, uint64_t n,
-                               uint32_t recs_per_batch, int lz4, int64_t base_offset, uint8_t* out, uint64_t cap) {
+/* nulls (optional): nulls[i] != 0 writes a null value for record i (a tombstone on a compacted topic; its value bytes are not read). */
+int64_t kv_kafka_encode_values_nulls(const uint8_t* keys, const uint64_t* key_offs, const uint8_t* vals, const uint64_t* val_offs,
+                                     const uint8_t* nulls, uint64_t n, uint32_t recs_per_batch, int lz4, int64_t base_offset, uint8_t* out,
+                                     uint64_t cap) {
   if (!recs_per_batch) return -1;
   uint64_t body_cap = 0;
   uint8_t *body = NULL, *comp = NULL;
@@ -30,13 +32,14 @@ int64_t kv_kafka_encode_values(const uint8_t* keys, const uint64_t* key_offs, co
     uint64_t bl = 0;
     for (uint32_t d = 0; d < cnt; d++) {
       const uint64_t i = s + d;
-      const uint64_t kl = key_offs[i + 1] - key_offs[i], vl = val_offs[i + 1] - val_offs[i];
+      const int null_value = nulls && nulls[i];
+      const uint64_t kl = key_offs[i + 1] - key_offs[i], vl = null_value ? 0 : val_offs[i + 1] - val_offs[i];
       uint8_t head[24]; uint32_t h = 0;
       head[h++] = 0;                                   /* attributes */
       h += put_varlong(head + h, (int64_t)d);          /* timestampDelta */
       h += put_varint(head + h, (int32_t)d);           /* offsetDelta */
       uint8_t kv[10], vv[10];
-      const uint32_t kh = put_varint(kv, (int32_t)kl), vh = put_varint(vv, (int32_t)vl);
+      const uint32_t kh = put_varint(kv, (int32_t)kl), vh = put_varint(vv, null_value ? -1 : (int32_t)vl);
       const uint64_t r = h + kh + kl + vh + vl + 1;
       bl += put_varint(body + bl, (int32_t)r);
       memcpy(body + bl, head, h); bl += h;
@@ -64,4 +67,9 @@ int64_t kv_kafka_encode_values(const uint8_t* keys, const uint64_t* key_offs, co
   }
   free(body); free(comp);
   return (int64_t)op;
+}
+
+int64_t kv_kafka_encode_values(const uint8_t* keys, const uint64_t* key_offs, const uint8_t* vals, const uint64_t* val_offs, uint64_t n,
+                               uint32_t recs_per_batch, int lz4, int64_t base_offset, uint8_t* out, uint64_t cap) {
+  return kv_kafka_encode_values_nulls(keys, key_offs, vals, val_offs, NULL, n, recs_per_batch, lz4, base_offset, out, cap);
 }

@@ -241,6 +241,7 @@ JNIEXPORT jlong JNICALL Java_surge_gpu_Native_00024_dingestCreate(JNIEnv* env, j
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_dingestDestroy(JNIEnv* env, jobject o, jlong g) { return sgr_dingest_destroy(DG(g)); }
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_dingestSetNullValueType(JNIEnv* env, jobject o, jlong g, jint event_type) { return sgr_dingest_set_null_value_type(DG(g), event_type); }
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_dingestSetValueFraming(JNIEnv* env, jobject o, jlong g, jint framing) { return sgr_dingest_set_value_framing(DG(g), framing); }
+JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_dingestSetStateTopic(JNIEnv* env, jobject o, jlong g, jint on) { return sgr_dingest_set_state_topic(DG(g), on); }
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_dingestSetAborted(JNIEnv* env, jobject o, jlong g, jint partition, jlongArray pids, jlongArray firsts) {
   jsize n = (*env)->GetArrayLength(env, pids);
   if ((*env)->GetArrayLength(env, firsts) != n) return bad_arg(env, "producerIds and firstOffsets differ in length");

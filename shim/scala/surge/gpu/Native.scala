@@ -64,6 +64,7 @@ object Native {
   @native def dingestDestroy(dingest: Long): Int                                   // sgr_dingest_destroy
   @native def dingestSetNullValueType(dingest: Long, eventType: Int): Int          // sgr_dingest_set_null_value_type
   @native def dingestSetValueFraming(dingest: Long, framing: Int): Int             // sgr_dingest_set_value_framing (0 packed, 1 protobuf Event, 2 JSON)
+  @native def dingestSetStateTopic(dingest: Long, on: Int): Int                    // sgr_dingest_set_state_topic (1: compacted state topic, before the first fold)
   @native def dingestSetAborted(dingest: Long, partition: Int, producerIds: Array[Long], firstOffsets: Array[Long]): Int // sgr_dingest_set_aborted
   /** queues one fetch response's bytes (a DIRECT buffer, untouched until dingestFold returns); returns the data batches queued */
   @native def dingestSubmit(dingest: Long, partition: Int, data: ByteBuffer, nbytes: Long): Long // sgr_dingest_submit

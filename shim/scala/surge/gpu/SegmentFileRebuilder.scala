@@ -72,12 +72,20 @@ object SegmentFileRebuilder {
 /** One rebuild of one engine from partition directories `partition -> dir`. Not thread-safe; run it on the thread that owns the
  *  engine's mutating calls (the store's flush lock in GpuReplayKeyValueStore). */
 final class SegmentFileRebuilder(engine: Long, maxAggregates: Long, chunkBytes: Int = 64 << 20, pollBytes: Long = 1L << 30,
-                                 valueFraming: Int = 0) {   // sgr_dingest_set_value_framing: 0 packed, 1 protobuf Event
+                                 valueFraming: Int = 0,      // sgr_dingest_set_value_framing: 0 packed, 1 protobuf Event (State)
+                                 stateTopic: Boolean = false) { // sgr_dingest_set_state_topic: the partitions hold the compacted state topic
   import SegmentFileRebuilder._
   private val log = LoggerFactory.getLogger(getClass)
   // (JSON needs a member table, which has no JNI binding: checked before the handle exists, so a refusal leaks nothing)
   require(valueFraming == 0 || valueFraming == 1, s"value framing $valueFraming: 0 (packed) or 1 (protobuf Event)")
   private val dingest = Native.dingestCreate(engine, maxAggregates, 0L)
+  if (stateTopic) {   // before the first submit: the mode is fixed once a poll was folded
+    val rc = Native.dingestSetStateTopic(dingest, 1)
+    if (rc != 0) {
+      Native.dingestDestroy(dingest)
+      throw new IllegalStateException(s"sgr_dingest_set_state_topic failed: $rc")
+    }
+  }
   if (valueFraming != 0) {
     val rc = Native.dingestSetValueFraming(dingest, valueFraming)
     if (rc != 0) {

@@ -20,6 +20,8 @@
 // overflow, the flag comes back with the verdicts and the poll is decoded again from an exact host-side layout. Protobuf and
 // JSON values (sgr_dingest_set_value_framing) are converted to packed events inside the parse kernel (value_framing.h); JSON
 // compresses better than packed values, so under those framings the claim multiple adapts (claim_mult).
+// A compacted STATE topic (sgr_dingest_set_state_topic) takes the same chain; its parse writes rows of program bytes, and the
+// fold applies them last write wins with sgr_put_batch's kernels (put_decoded_poll) instead of folding events.
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -87,6 +89,12 @@ struct sgr_dingest {
   // arena claim of an lz4 batch, in multiples of its compressed size: 3 for packed values; under protobuf / JSON framing raised
   // after a poll that needed the exact-layout repeat, to the power of two at or above the largest ratio it showed (at most 16)
   uint32_t claim_mult = 3;
+  // a compacted STATE topic (sgr_dingest_set_state_topic): the whole key is the id, a value is the program bytes of a row, null
+  // deletes; a poll is applied last write wins (put_decoded_poll) instead of folded. Fixed before the first fold.
+  bool state_topic = false;
+  bool folded = false;                      // a fold succeeded since create / sgr_dingest_reset
+  uint32_t row_bytes = 0;                   // state mode: program bytes of a row (state_bytes - 8), read when a poll's first group launches
+  uint32_t json_row_end = 0;                // state mode: end of the registered JSON members in the row
   // staged submissions
   KeepBuf wire;
   // descriptors of the poll's data batches, in PAGE-LOCKED memory: every copy of them is a true asynchronous DMA (a copy from
@@ -121,6 +129,7 @@ struct sgr_dingest {
   // device scratch
   KeepBuf arena, d_batches;
   KeepBuf rec_off, rec_batch, out;          // per record slot; they keep their content when a later group needs them larger
+  KeepBuf st_idx, st_present;               // ... state mode: the slot's dense index (~0u: hole) and 0 / 1 (tombstone / row)
   DevBuf key_offs_dev, key_bytes_dev;
   // chains of launches per group of batches
   uint64_t launched_batches = 0;            // batches of this poll whose chain has been launched
@@ -162,10 +171,17 @@ int32_t dfail(sgr_dingest* g, int32_t code, const char* fmt, ...) {
     if (_e != cudaSuccess) return dfail((g), _e == cudaErrorMemoryAllocation ? SGR_ERR_OOM : SGR_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(_e)); \
   } while (0)
 
-std::string dg_err_text(uint32_t e) {
+std::string dg_err_text(const sgr_dingest* g, uint32_t e) {
   if ((e & 0xffu) == DG_VALUE_FRAMING) {   // the host decoder's text: JSON reasons follow "JSON event: "
     const uint32_t why = e >> 8;
     return std::string(why == vf::NOT_PROTOBUF ? "" : "JSON event: ") + vf::reason_text(why);
+  }
+  if ((e & 0xffu) == DG_STATE_LENGTH) {
+    char buf[160];
+    const uint32_t len = e >> 8;
+    snprintf(buf, sizeof buf, "state value of %s%u bytes is longer than the %u program bytes of a row (state_bytes - 8)", len == 0xffffffu ? "at least " : "",
+             len, g->row_bytes);
+    return buf;
   }
   switch (e) {
     case DG_CRC: return "CRC-32C mismatch";
@@ -223,6 +239,8 @@ DgParse parse_args(sgr_dingest* g) {
   p.dict.tags = (unsigned long long*)g->tags.p; p.dict.slot_idx = (uint32_t*)g->slot_idx.p; p.dict.key_ref = (uint2*)g->key_ref.p;
   p.dict.arena = (uint8_t*)g->id_arena.p; p.dict.ctl = (unsigned long long*)g->ctl.p; p.dict.slots_mask = g->slots - 1;
   p.dict.max_keys = g->max_keys; p.dict.arena_cap = g->arena_cap;
+  p.state_topic = g->state_topic; p.row_bytes = g->row_bytes;
+  p.idx = (uint32_t*)g->st_idx.b.p; p.present = (uint8_t*)g->st_present.b.p;
   return p;
 }
 
@@ -240,7 +258,8 @@ cudaError_t set_arena_capacity(sgr_dingest* g) {
   return cudaMemcpy((unsigned long long*)g->ctl.p + 9, &cap, 8, cudaMemcpyHostToDevice);
 }
 
-uint32_t claim_multiple(const sgr_dingest* g) { return g->value_framing == SGR_VALUE_PACKED ? 3u : g->claim_mult; }
+// (state values compress like JSON events: a state topic adapts the claim whatever its framing)
+uint32_t claim_multiple(const sgr_dingest* g) { return g->value_framing == SGR_VALUE_PACKED && !g->state_topic ? 3u : g->claim_mult; }
 
 // Enqueue descriptors-up -> crc_size (+ arena claim) -> decode_walk -> parse for the batches [launched_batches, batch_end) —
 // record slots [launched_records, rec_end) — behind `landed` (the copy of the last fetch that contributes to the group).
@@ -248,10 +267,24 @@ int32_t launch_group(sgr_dingest* g, uint64_t batch_end, uint64_t rec_end, cudaE
   const uint64_t b0 = g->launched_batches, nb = batch_end - b0;
   if (!nb) return SGR_OK;
   const uint64_t r0 = g->launched_records;
+  if (g->state_topic && !g->n_groups) {   // the poll's rows take the program's width, fixed until its fold
+    uint32_t sb = 0;
+    bool routed = false;
+    const int32_t rc = engine_program_state_bytes(g->eng, &sb, &routed);
+    if (rc || !sb) return dfail(g, rc ? rc : SGR_ERR_NO_PROGRAM, "state topic: register a fold program first");
+    if (routed) return dfail(g, SGR_ERR_UNSUPPORTED, "state topic: the rows of a routed engine are local slots");
+    if (g->json_row_end > sb - 8) return dfail(g, SGR_ERR_STATE, "state topic: the JSON members end at program byte %u, past the program's %u", g->json_row_end, sb - 8);
+    g->row_bytes = sb - 8;
+  }
+  const uint64_t stride = g->state_topic ? g->row_bytes : 64;
   DG_TRY(g, grow_keeping(g, g->d_batches, b0 * sizeof(DgBatch), batch_end * sizeof(DgBatch) + 64));
   DG_TRY(g, grow_keeping(g, g->rec_off, r0 * 4, rec_end * 4 + 64));
   DG_TRY(g, grow_keeping(g, g->rec_batch, r0 * 4, rec_end * 4 + 64));
-  DG_TRY(g, grow_keeping(g, g->out, r0 * 64, rec_end * 64 + 64));
+  DG_TRY(g, grow_keeping(g, g->out, r0 * stride, rec_end * stride + 64));
+  if (g->state_topic) {
+    DG_TRY(g, grow_keeping(g, g->st_idx, r0 * 4, rec_end * 4 + 64));
+    DG_TRY(g, grow_keeping(g, g->st_present, r0, rec_end + 64));
+  }
   const uint64_t arena_want = (uint64_t)claim_multiple(g) * g->wire.b.cap + 512;
   if (g->arena.b.cap < arena_want) {
     DG_TRY(g, grow_keeping(g, g->arena, b0 ? g->arena.b.cap : 0, arena_want));
@@ -337,6 +370,7 @@ int32_t sgr_dingest_destroy(sgr_dingest* g) {
   if (g->h_keys) cudaFreeHost(g->h_keys);
   g->batches.release();
   g->wire.b.release(); g->d_batches.b.release(); g->arena.b.release(); g->rec_off.b.release(); g->rec_batch.b.release(); g->out.b.release();
+  g->st_idx.b.release(); g->st_present.b.release();
   g->key_offs_dev.release(); g->key_bytes_dev.release(); g->json_table.release();
   g->tags.release(); g->slot_idx.release(); g->key_ref.release(); g->id_arena.release(); g->ctl.release();
   if (g->h_ctl) cudaFreeHost(g->h_ctl);
@@ -362,11 +396,32 @@ int32_t sgr_dingest_set_value_framing(sgr_dingest* g, int32_t framing) {
   return SGR_OK;
 }
 
+int32_t sgr_dingest_set_state_topic(sgr_dingest* g, int32_t on) {
+  if (!g) return SGR_ERR_INVALID;
+  if (!g->subs.empty()) return dfail(g, SGR_ERR_STATE, "the topic mode cannot change between a submit and its fold");
+  if (g->folded) return dfail(g, SGR_ERR_STATE, "the topic mode is fixed once a poll was folded (sgr_dingest_reset first)");
+  if (g->json.n_classes) return dfail(g, SGR_ERR_STATE, "set the topic mode before the JSON packer: its offsets mean different things in the two modes");
+  uint32_t sb = 0;
+  bool routed = false;
+  if (engine_program_state_bytes(g->eng, &sb, &routed) != SGR_OK) return dfail(g, SGR_ERR_INVALID, "engine");
+  if (routed) return dfail(g, SGR_ERR_UNSUPPORTED, "the rows of a routed engine are local slots: a state topic does not map ids to them");
+  g->state_topic = on != 0;
+  return SGR_OK;
+}
+
 int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, const sgr_json_event* events, uint32_t n_events, int32_t unknown_type) {
   if (!g || !discriminator || (n_events && !events)) return dfail(g, SGR_ERR_INVALID, "null argument");
   if (!g->subs.empty()) return dfail(g, SGR_ERR_STATE, "the JSON packer cannot change between a submit and its fold");
   if (unknown_type >= (int32_t)SGR_MAX_TYPES) return dfail(g, SGR_ERR_INVALID, "unknown_type out of range");
   if (!*discriminator && n_events != 1) return dfail(g, SGR_ERR_INVALID, "without a discriminator member exactly one class can be registered");
+  // state topic: Json.toJson(state) writes no discriminator, the one class is the state; members land at program byte offsets
+  uint32_t row_limit = 0, row_end = 0;
+  if (g->state_topic) {
+    if (*discriminator) return dfail(g, SGR_ERR_INVALID, "a state topic's JSON values carry no discriminator member");
+    bool routed = false;
+    if (engine_program_state_bytes(g->eng, &row_limit, &routed) != SGR_OK || !row_limit) return dfail(g, SGR_ERR_NO_PROGRAM, "state topic: register a fold program first");
+    row_limit -= 8;
+  }
   // the same checks as sgr_ingest_set_json_packer; the table goes to the device as classes, fields, then the names
   std::vector<vf::Class> classes;
   std::vector<vf::Field> fields;
@@ -379,10 +434,14 @@ int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, c
     for (uint32_t f = 0; f < e.n_fields; ++f) {
       const sgr_json_field& jf = e.fields[f];
       const uint32_t size = jf.kind == SGR_JSON_I32 ? 4u : jf.kind == SGR_JSON_UUID ? 16u : jf.kind == SGR_JSON_PSTR ? jf.len : 8u;
-      // a member may land on the sequence number (+4, Int only) or anywhere in the payload (+16 .. +64); never on type or agg
+      // a member may land on the sequence number (+4, Int only) or anywhere in the payload (+16 .. +64); never on type or agg.
+      // State topic: anywhere in the row's program bytes.
       const bool ok = jf.name && jf.kind <= SGR_JSON_PSTR && jf.dst_off % 4 == 0 && size >= 4 && size % 4 == 0 &&
-                      ((jf.dst_off == 4 && jf.kind == SGR_JSON_I32) || (jf.dst_off >= 16 && jf.dst_off + size <= 64));
-      if (!ok) return dfail(g, SGR_ERR_INVALID, "JSON event %u field %u: bad name, kind, length or record offset", i, f);
+                      (g->state_topic ? (uint64_t)jf.dst_off + size <= row_limit
+                                      : ((jf.dst_off == 4 && jf.kind == SGR_JSON_I32) || (jf.dst_off >= 16 && jf.dst_off + size <= 64)));
+      if (!ok) return dfail(g, SGR_ERR_INVALID, "JSON %s %u field %u: bad name, kind, length or %s offset", g->state_topic ? "state" : "event", i, f,
+                            g->state_topic ? "program byte" : "record");
+      row_end = std::max(row_end, jf.dst_off + size);
       fields.push_back(vf::Field{(uint32_t)names.size(), (uint32_t)strlen(jf.name), jf.kind, jf.dst_off, size});
       names += jf.name;
     }
@@ -402,6 +461,7 @@ int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, c
   const uint8_t* base = (const uint8_t*)nb.p;
   g->json = vf::Table{base + cls_bytes + fld_bytes, (const vf::Class*)base, (const vf::Field*)(base + cls_bytes), (uint32_t)classes.size(), 0,
                       (uint32_t)strlen(discriminator), unknown_type < 0 ? -1 : unknown_type};
+  g->json_row_end = row_end;
   return SGR_OK;
 }
 
@@ -579,14 +639,14 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
       for (uint32_t i = 0; i < nb; ++i) {
         DgBatch& b = g->batches[i];
         if (b.err == DG_ARENA_FULL) b.err = DG_OK;
-        if (b.err) { const int32_t rc = dfail(g, SGR_ERR_INVALID, "offset %lld: %s", (long long)b.base_offset, dg_err_text(b.err).c_str()); discard_poll(g); return rc; }
+        if (b.err) { const int32_t rc = dfail(g, SGR_ERR_INVALID, "offset %lld: %s", (long long)b.base_offset, dg_err_text(g, b.err).c_str()); discard_poll(g); return rc; }
         b.rec_err = kNoRecErr;
         if (b.codec == 3) {
           b.arena_off = need; need += ((uint64_t)b.dsize + 15) & ~15ull;
           ratio = std::max(ratio, (double)b.dsize / (double)std::max<uint64_t>(1, b.total_len - kBatchHeader));
         }
       }
-      if (g->value_framing != SGR_VALUE_PACKED)
+      if (g->value_framing != SGR_VALUE_PACKED || g->state_topic)
         while (g->claim_mult < 16 && (double)g->claim_mult < ratio) g->claim_mult = g->claim_mult < 4 ? 4 : 2 * g->claim_mult;
       g->arena.used = 0;
       DG_TRY(g, g->arena.ensure(need + 512, g->stream));
@@ -613,7 +673,7 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
       if (g->batches[i].err || g->batches[i].rec_err != kNoRecErr) {
         const DgBatch& b = g->batches[i];
         const uint32_t record = b.rec_err == kNoRecErr ? 0u : (uint32_t)(b.rec_err >> 32), code = b.err ? b.err : (uint32_t)b.rec_err;
-        const int32_t rc = dfail(g, SGR_ERR_INVALID, "offset %lld, record %u: %s", (long long)b.base_offset, record, dg_err_text(code).c_str());
+        const int32_t rc = dfail(g, SGR_ERR_INVALID, "offset %lld, record %u: %s", (long long)b.base_offset, record, dg_err_text(g, code).c_str());
         // ids interned by this failed poll stay in the dictionary (harmless: an id is an id); the records are dropped
         discard_poll(g); return rc;
       }
@@ -671,7 +731,8 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
     }
     lap(3);
     int32_t rc_fold = SGR_OK;
-    if (nrec) rc_fold = fold_decoded_poll(g->eng, g->out.b.p, nrec, st.n_records);
+    if (nrec && g->state_topic) rc_fold = put_decoded_poll(g->eng, g->out.b.p, (const uint32_t*)g->st_idx.b.p, (const uint8_t*)g->st_present.b.p, nrec, st.n_records);
+    else if (nrec) rc_fold = fold_decoded_poll(g->eng, g->out.b.p, nrec, st.n_records);
     if (appender.joinable()) appender.join();
     if (rc_fold) { dfail(g, rc_fold, "engine: %s", sgr_last_error(g->eng)); discard_poll(g); return rc_fold; }
     if (rc_append) { dfail(g, rc_append, "engine: %s", sgr_last_error(g->eng)); discard_poll(g); return rc_append; }
@@ -682,6 +743,7 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
   // ---- commit: the staged positions become the live ones and everything decoded is folded
   for (auto& kv : g->staged) { kv.second.folded_next = kv.second.decoded_next; }
   g->parts = g->staged;
+  g->folded = true;
   if (nb) DG_TRY(g, reset_poll_counters(g));
   clear_poll(g);
   sgr_ingest_stats& t = g->total;
@@ -696,6 +758,7 @@ int32_t sgr_dingest_reset(sgr_dingest* g) {
   if (!g) return SGR_ERR_INVALID;
   discard_poll(g);
   g->parts.clear(); g->staged.clear(); g->total = sgr_ingest_stats{}; g->keys_on_host = 0; g->id_bytes_on_host = 0; ++g->generation;
+  g->folded = false;   // (the topic mode stays, as the value framing does)
   DG_TRY(g, cudaMemsetAsync(g->tags.p, 0, g->slots * 8, g->stream));
   DG_TRY(g, cudaMemsetAsync(g->slot_idx.p, 0, g->slots * 4, g->stream));
   DG_TRY(g, cudaMemsetAsync(g->ctl.p, 0, 9 * 8, g->stream));                                  // ([9], the arena's capacity, stays)

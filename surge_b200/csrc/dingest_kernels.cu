@@ -307,16 +307,57 @@ __device__ __forceinline__ void refuse_record(DgBatch& bt, uint32_t r, uint32_t 
   atomicMin(&bt.rec_err, ((unsigned long long)r << 32) | code);
 }
 
+// One live record of a compacted state topic at slot i: the id is the whole key (no cut at ':'), a null value is a tombstone,
+// any other value (after its framing) is 0 .. row_bytes program bytes, zero-padded to the row. Counted as a record either way.
+template <int32_t kFraming>
+__device__ __forceinline__ void state_row(const DgParse& p, DgBatch& bt, uint32_t i, uint32_t r, const uint8_t* key, uint32_t key_len,
+                                          const uint8_t* val, int32_t val_len) {
+  uint8_t converted[vf::kStateRowMax];
+  if constexpr (kFraming != vf::PACKED) {
+    if (val_len >= 0) {
+      uint32_t n = 0;
+      const uint32_t why = vf::convert<vf::STATE>(kFraming, p.json, val, (uint32_t)val_len, converted, &val, &n);
+      if (why) { refuse_record(bt, r, (uint32_t)DG_VALUE_FRAMING | (why << 8)); return; }
+      val_len = kFraming == vf::JSON ? (int32_t)p.row_bytes : (int32_t)n;   // (the member table was checked against the row)
+    }
+  }
+  if (val_len > (int32_t)p.row_bytes) { refuse_record(bt, r, (uint32_t)DG_STATE_LENGTH | ((uint32_t)min(val_len, 0xffffff) << 8)); return; }
+  if (key_len >= (1u << 24)) { refuse_record(bt, r, DG_ID_LENGTH); return; }
+  const uint32_t idx = intern(p.dict, key, key_len);
+  if (idx == 0xffffffffu) return;   // dictionary full: counted in ctl[5], the whole call fails
+  if (val_len < 0) {
+    p.present[i] = 0;
+    atomicAdd(p.dict.ctl + 3, 1ull);
+  } else {
+    uint32_t* row = reinterpret_cast<uint32_t*>(p.out + (size_t)i * p.row_bytes);   // (row_bytes is a multiple of 4)
+    for (uint32_t w = 0; w < p.row_bytes / 4; ++w) {
+      uint32_t x = 0;
+      for (uint32_t b = 0; b < 4; ++b) if (4 * w + b < (uint32_t)val_len) x |= (uint32_t)val[4 * w + b] << (8 * b);
+      row[w] = x;
+    }
+    p.present[i] = 1;
+  }
+  p.idx[i] = idx;
+  const uint32_t grp = __activemask();
+  if ((threadIdx.x & 31) == (uint32_t)(__ffs(grp) - 1)) atomicAdd(p.dict.ctl + 6, (unsigned long long)__popc(grp));
+}
+
 // kFraming (SGR_VALUE_*): the packed instantiation copies the value as it is; the others convert it first (value_framing.h),
 // after the null-value check and before the 8..56 length check, in the host decoder's order.
-template <int32_t kFraming>
+// kState (a compacted state topic, DgParse::state_topic): the record becomes a row of the program bytes, its dense index and a
+// present byte instead of a packed event (state_row); the events instantiations compile as they did without it.
+template <int32_t kFraming, bool kState>
 __global__ void __launch_bounds__(kThreads) dg_parse_kernel(const __grid_constant__ DgParse p) {
   const uint32_t i = p.rec_begin + blockIdx.x * kThreads + threadIdx.x;
   if (i >= p.n_records) return;
   uint4* out = reinterpret_cast<uint4*>(p.out + (size_t)i * 64);
-  const uint4 zero = make_uint4(0, 0, 0, 0), hole = make_uint4(0, 0, 0xffffffffu, 0xffffffffu);
-  out[1] = zero; out[2] = zero; out[3] = zero;
-  out[0] = hole;
+  if constexpr (kState) {
+    p.idx[i] = ~0u;   // a hole until the record proves live
+  } else {
+    const uint4 zero = make_uint4(0, 0, 0, 0), hole = make_uint4(0, 0, 0xffffffffu, 0xffffffffu);
+    out[1] = zero; out[2] = zero; out[3] = zero;
+    out[0] = hole;
+  }
   const uint32_t bi = p.rec_batch[i];
   if (bi >= p.n_batches) return;    // a slot the walk never reached (its batch failed earlier)
   DgBatch& bt = p.batches[bi];
@@ -341,6 +382,10 @@ __global__ void __launch_bounds__(kThreads) dg_parse_kernel(const __grid_constan
   if (!q.ok || q.pos != q.n || n_headers < 0) { refuse_record(bt, r, DG_RECORD_MALFORMED); return; }
   if (bt.base_offset + offset_delta < bt.min_offset) { atomicAdd(p.dict.ctl + 4, 1ull); return; }      // refetch after a restart
   if (key_len <= 0) { atomicAdd(p.dict.ctl + 2, 1ull); return; }                                        // the producer's flush record
+  if constexpr (kState) {
+    state_row<kFraming>(p, bt, i, r, key, (uint32_t)key_len, val, val_len);
+    return;
+  }
   if (val_len < 0 && p.null_value_type < 0) { atomicAdd(p.dict.ctl + 3, 1ull); return; }
   uint8_t converted[56];
   if constexpr (kFraming != vf::PACKED) {
@@ -422,10 +467,13 @@ cudaError_t dg_gather_keys(const DgDict& d, uint64_t from, uint32_t n, uint32_t*
 cudaError_t dg_launch_parse(const DgParse& p, cudaStream_t st) {
   if (p.n_records <= p.rec_begin) return cudaSuccess;
   const uint32_t blocks = (p.n_records - p.rec_begin + kThreads - 1) / kThreads;
-  switch (p.value_framing) {
-    case vf::PACKED: dg_parse_kernel<vf::PACKED><<<blocks, kThreads, 0, st>>>(p); break;
-    case vf::PROTOBUF_EVENT: dg_parse_kernel<vf::PROTOBUF_EVENT><<<blocks, kThreads, 0, st>>>(p); break;
-    case vf::JSON: dg_parse_kernel<vf::JSON><<<blocks, kThreads, 0, st>>>(p); break;
+  switch (p.value_framing + (p.state_topic ? 3 : 0)) {
+    case vf::PACKED: dg_parse_kernel<vf::PACKED, false><<<blocks, kThreads, 0, st>>>(p); break;
+    case vf::PROTOBUF_EVENT: dg_parse_kernel<vf::PROTOBUF_EVENT, false><<<blocks, kThreads, 0, st>>>(p); break;
+    case vf::JSON: dg_parse_kernel<vf::JSON, false><<<blocks, kThreads, 0, st>>>(p); break;
+    case 3 + vf::PACKED: dg_parse_kernel<vf::PACKED, true><<<blocks, kThreads, 0, st>>>(p); break;
+    case 3 + vf::PROTOBUF_EVENT: dg_parse_kernel<vf::PROTOBUF_EVENT, true><<<blocks, kThreads, 0, st>>>(p); break;
+    case 3 + vf::JSON: dg_parse_kernel<vf::JSON, true><<<blocks, kThreads, 0, st>>>(p); break;
     default: return cudaErrorInvalidValue;
   }
   return cudaGetLastError();

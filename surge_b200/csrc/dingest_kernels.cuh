@@ -14,6 +14,7 @@ enum DgErr : uint32_t {
   DG_RECORD_LENGTH = 7, DG_RECORD_MALFORMED = 8, DG_RECORD_COUNT = 9, DG_VALUE_LENGTH = 10, DG_ID_LENGTH = 11, DG_STRAY_BYTES = 12,
   DG_ARENA_FULL = 13,   // not a data error: the batch's arena claim did not fit (the host lays the arena out exactly and repeats)
   DG_VALUE_FRAMING = 14,   // a protobuf / JSON value was refused: the code is DG_VALUE_FRAMING | vf::Reason << 8
+  DG_STATE_LENGTH = 15,    // state topic: a value longer than the program bytes; the code is DG_STATE_LENGTH | min(length, 2^24 - 1) << 8
 };
 
 // One data batch that survived the host's header walk (control batches, aborted transactions and anything below the partition's
@@ -52,6 +53,12 @@ struct DgParse {
   DgDict dict;
   int32_t value_framing;         // SGR_VALUE_*: how a value wraps the packed event (selects the kernel's instantiation)
   vf::Table json;                // SGR_VALUE_JSON: the registered member table, in device memory
+  // state topic (sgr_dingest_set_state_topic): `out` holds rows of row_bytes (state_bytes - 8) program bytes instead of packed
+  // records, with each slot's dense index (~0u: a hole) in idx and 0 (tombstone) / 1 (row) in present
+  bool state_topic;
+  uint32_t row_bytes;
+  uint32_t* idx;
+  uint8_t* present;
 };
 
 cudaError_t dg_launch_parse(const DgParse& p, cudaStream_t st);

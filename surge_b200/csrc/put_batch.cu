@@ -11,6 +11,7 @@
 //   resolve  one thread per record: its dense index; a first appearance also writes its key_ref, its bytes into the arena and
 //            its batch position into new_pos[k] (what the host appends to its key table: no id bytes come back)
 //   last     one thread per record: atomicMax(last[slot], position + 1)
+//            (last and write skip a slot of ~0u: the holes of a device-ingest poll of a state topic, put_decoded_poll)
 //   write    one thread per record: the record whose position + 1 is last[slot] zeroes last[slot], compares its row with the
 //            prior state (program_words_differ: the publish rule the fold kernels use) and writes the row, its flags and
 //            err_idx 0; the written indices are appended to `touched` by one atomic per warp
@@ -121,7 +122,7 @@ __global__ void __launch_bounds__(kThreads) pb_resolve_kernel(const PutBatch p, 
 
 __global__ void __launch_bounds__(kThreads) pb_last_kernel(const PutBatch p, uint32_t* __restrict__ last) {
   const uint64_t i = (uint64_t)blockIdx.x * kThreads + threadIdx.x;
-  if (i < p.n) atomicMax(last + p.slot[i], (uint32_t)i + 1u);
+  if (i < p.n && p.slot[i] != ~0u) atomicMax(last + p.slot[i], (uint32_t)i + 1u);   // (~0u: a hole of a device-ingest poll)
 }
 
 __global__ void __launch_bounds__(kThreads) pb_write_kernel(const PutBatch p, uint8_t* __restrict__ states, const __grid_constant__ DevProgram prog,
@@ -132,7 +133,7 @@ __global__ void __launch_bounds__(kThreads) pb_write_kernel(const PutBatch p, ui
   bool win = false;
   if (i < p.n) {
     sl = p.slot[i];
-    win = last[sl] == (uint32_t)i + 1u;   // (the winner zeroes the word: no other record of the slot ever reads its own position)
+    win = sl != ~0u && last[sl] == (uint32_t)i + 1u;   // (the winner zeroes the word: no other record of the slot ever reads its own position)
   }
   if (win) {
     last[sl] = 0u;

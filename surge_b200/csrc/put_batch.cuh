@@ -34,7 +34,7 @@ struct PutBatch {
   uint32_t* rank = nullptr;           // [n + 1] exclusive scan of first: rank[n] = new ids
   unsigned long long* alen = nullptr; // [n + 1] its 8-byte aligned length at a first appearance
   unsigned long long* aoff = nullptr; // [n + 1] exclusive scan of alen: its arena offset behind the resident ids
-  uint32_t* slot = nullptr;           // [n] the record's dense index after the batch
+  uint32_t* slot = nullptr;           // [n] the record's dense index after the batch (~0u: a hole, skipped by put_batch_apply)
   uint32_t* new_pos = nullptr;        // [n] batch position of new id k (k < rank[n]): index order
   unsigned long long* bt_tags = nullptr;   // batch table: hash tag (0 empty)
   uint32_t* bt_owner = nullptr;            // the first claimant's position + 1 (0: still publishing)

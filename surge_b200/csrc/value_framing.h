@@ -494,8 +494,16 @@ VF_HD uint32_t protobuf_payload(const uint8_t* v, uint32_t n, uint32_t* off, uin
   return OK;
 }
 
-// a flat JSON object -> out[56] (record bytes 0..7, then 16..63), as json_pack does
-VF_HD uint32_t json_pack(const Table& t, const uint8_t* v, uint32_t n, uint8_t out[56]) {
+// Where json_pack puts a member. RECORD: Field::dst_off is a record offset and out[56] holds record bytes 0..7, then 16..63 (the
+// class's event type goes to bytes 0..3), as the host decoder's json_pack does. STATE: Field::dst_off is a program byte offset
+// and out[kStateRowMax] holds the program bytes of a state row (state-topic values carry no event type).
+enum Layout : int { RECORD = 0, STATE = 1 };
+constexpr uint32_t kStateRowMax = 120;   // program bytes of the widest state (128 bytes)
+
+// a flat JSON object -> out, in layout kLayout
+template <int kLayout = RECORD>
+VF_HD uint32_t json_pack(const Table& t, const uint8_t* v, uint32_t n, uint8_t* out) {
+  constexpr int kOutBytes = kLayout == RECORD ? 56 : (int)kStateRowMax;
   Member mem[kMaxMembers];
   uint32_t n_members = 0;
   Scan sc{v, n, 0};
@@ -538,15 +546,15 @@ VF_HD uint32_t json_pack(const Table& t, const uint8_t* v, uint32_t n, uint8_t o
     for (uint32_t c = 0; c < t.n_classes && !ev; ++c)
       if (name_is(v + d->val_off, d->val_len, d->kind == 'S', t.names + t.classes[c].name_off, t.classes[c].name_len)) ev = &t.classes[c];
   }
-  for (int k = 0; k < 56; ++k) out[k] = 0;
+  for (int k = 0; k < kOutBytes; ++k) out[k] = 0;
   const uint32_t ty = ev ? ev->event_type : (uint32_t)t.unknown_type;
   if (!ev && t.unknown_type < 0) return UNKNOWN_CLASS;
-  out[0] = (uint8_t)ty; out[1] = (uint8_t)(ty >> 8); out[2] = (uint8_t)(ty >> 16); out[3] = (uint8_t)(ty >> 24);
+  if constexpr (kLayout == RECORD) { out[0] = (uint8_t)ty; out[1] = (uint8_t)(ty >> 8); out[2] = (uint8_t)(ty >> 16); out[3] = (uint8_t)(ty >> 24); }
   if (!ev) return OK;
   for (uint32_t fi = 0; fi < ev->n_fields; ++fi) {
     const Field& f = t.fields[ev->field_begin + fi];
     const Member* m = find(f.name_off, f.name_len);
-    uint8_t* dst = out + (f.dst_off < 8 ? f.dst_off : f.dst_off - 8);
+    uint8_t* dst = out + (kLayout == STATE ? f.dst_off : f.dst_off < 8 ? f.dst_off : f.dst_off - 8);
     if (f.kind == K_UUID || f.kind == K_PSTR) {
       if (!m || (m->kind != 's' && m->kind != 'S')) return STRING_MISSING;
       uint32_t sn = 0;
@@ -605,15 +613,18 @@ VF_HD uint32_t json_pack(const Table& t, const uint8_t* v, uint32_t n, uint8_t o
 
 // A non-null record value under `framing` (PROTOBUF_EVENT or JSON) -> the packed event value: on OK, *len bytes of it are at
 // *val (a part of the value itself, or out[56]). The caller applies the 8..56 length check, as the host decoder does next.
-VF_HD uint32_t convert(int32_t framing, const Table& t, const uint8_t* v, uint32_t n, uint8_t out[56], const uint8_t** val, uint32_t* len) {
+// Under the STATE layout the value is a state-topic value (the protobuf State message has Event's field numbers) and a JSON
+// object fills out[kStateRowMax]; the caller checks the length against its program bytes.
+template <int kLayout = RECORD>
+VF_HD uint32_t convert(int32_t framing, const Table& t, const uint8_t* v, uint32_t n, uint8_t* out, const uint8_t** val, uint32_t* len) {
   if (framing == PROTOBUF_EVENT) {
     uint32_t off;
     const uint32_t e = protobuf_payload(v, n, &off, len);
     *val = v + off;
     return e;
   }
-  *val = out; *len = 56;
-  return json_pack(t, v, n, out);
+  *val = out; *len = kLayout == RECORD ? 56 : kStateRowMax;
+  return json_pack<kLayout>(t, v, n, out);
 }
 
 }  // namespace vf

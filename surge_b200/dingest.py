@@ -21,6 +21,9 @@ class DeviceIngest:
         self._lib = N.load_library()
         self._engine = engine
         self._h = C.c_void_p()
+        eh = getattr(engine, "_h", None)
+        if not isinstance(eh, C.c_void_p) or not eh:
+            raise IngestError(N.SGR_ERR_INVALID, "a device ingest needs an open ReplayEngine")
         rc = self._lib.sgr_dingest_create(engine._h, int(max_keys), int(max_id_bytes), C.byref(self._h))
         if rc != N.SGR_OK:
             raise IngestError(rc, "sgr_dingest_create failed")
@@ -56,6 +59,12 @@ class DeviceIngest:
     def set_json_packer(self, discriminator: str, events: Sequence[Tuple[str, int, Sequence[Tuple]]], unknown_type: int = -1) -> None:
         """The member table of JSON values, with the arguments of Ingest.set_json_packer."""
         self._check(self._lib.sgr_dingest_set_json_packer(self._h, discriminator.encode("utf-8"), json_events(events), len(events), unknown_type))
+
+    def set_state_topic(self, on: bool = True) -> None:
+        """Decode a compacted state topic (include/sgr.h sgr_dingest_set_state_topic): the whole key is the id, a value is the
+        program bytes of a row (after its framing), null deletes, and fold() applies the poll last write wins. Set it before the
+        first fold and before set_json_packer, whose member offsets then are program byte offsets."""
+        self._check(self._lib.sgr_dingest_set_state_topic(self._h, 1 if on else 0))
 
     def set_aborted(self, partition: int, aborted: Sequence[Tuple[int, int]]) -> None:
         if not aborted:

@@ -169,6 +169,7 @@ ABI = [
     ("sgr_dingest_set_null_value_type", C.c_int32, [_P, C.c_int32]),
     ("sgr_dingest_set_value_framing", C.c_int32, [_P, C.c_int32]),
     ("sgr_dingest_set_json_packer", C.c_int32, [_P, C.c_char_p, C.POINTER(sgr_json_event), C.c_uint32, C.c_int32]),
+    ("sgr_dingest_set_state_topic", C.c_int32, [_P, C.c_int32]),
     ("sgr_dingest_set_aborted", C.c_int32, [_P, C.c_int32, _P, _P, C.c_uint64]),
     ("sgr_dingest_submit", C.c_int32, [_P, C.c_int32, _P, C.c_uint64, _P]),
     ("sgr_dingest_fold", C.c_int32, [_P, _P]),

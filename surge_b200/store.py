@@ -143,7 +143,8 @@ class GpuReplayKeyValueStore:
 
     def __init__(self, name: str, program: N.sgr_fold_program, device: int = 0, state_formatter: Optional[Callable[[str, bytes], bytes]] = None,
                  codec: Optional[StateCodec] = None,
-                 on_changes: Optional[Callable[[List[Tuple[str, Optional[bytes]]], List[Tuple[str, int]]], None]] = None):
+                 on_changes: Optional[Callable[[List[Tuple[str, Optional[bytes]]], List[Tuple[str, int]]], None]] = None,
+                 max_ids: int = 1 << 20):
         self._name = name
         # on_changes(changed, failed): called once by every flush() that folded, before it returns, with what the reference's
         # actors would publish for that fold (PersistentActor.scala:252-263): changed = [(id, serialized state or None)], decoded
@@ -153,8 +154,12 @@ class GpuReplayKeyValueStore:
         # with a codec, put()/delete() are records of the STATE topic folded on the GPU as snapshot / tombstone events (feed (i) of
         # the Scala store): flush() — which Kafka Streams calls before it commits offsets — makes them readable from the table.
         # A codec without snapshot rules makes a state-topic store: flush() hands the pending records to one sgr_put_batch,
-        # which numbers new ids on the device in first-appearance order (the order _slot follows), so no key table is loaded
+        # which numbers new ids on the device in first-appearance order (the order _slot follows), so no key table is loaded.
+        # A state-topic store may instead restore the topic's raw record batches (restore_record_batches): a DeviceIngest in
+        # state-topic mode decodes and applies them on the device, its id dictionary bounded by max_ids
         self._codec = codec
+        self._max_ids = int(max_ids)
+        self._dingest = None
         self._state_topic = codec is not None and codec.state_topic
         self._puts: List[Tuple[str, Optional[bytes]]] = []   # a state-topic store's pending records, packed, in arrival order
         self._unflushed: Dict[str, Optional[bytes]] = {}
@@ -194,6 +199,8 @@ class GpuReplayKeyValueStore:
     def close(self) -> None:
         with self._lock:
             self._open = False
+            if self._dingest is not None:
+                self._dingest.close()
             self._engine.close()
 
     # -- event ingestion
@@ -231,10 +238,20 @@ class GpuReplayKeyValueStore:
         """Raw bytes of one fetch response for `partition` (a concatenation of Kafka RecordBatch v2), plus the
         response's aborted transactions [(producerId, firstOffset)]: decoded natively as a read_committed consumer
         would (SurgeStateStoreConsumer.scala:38) into the pending batch. flush() folds it. A store is fed either this
-        way or through put_event, not both (each keeps its own id dictionary)."""
+        way or through put_event, not both (each keeps its own id dictionary).
+        A state-topic store (codec without snapshot rules) takes the fetches of the compacted state topic: decoded and applied
+        last write wins on the device (DeviceIngest in state-topic mode), fed this way or through put()/delete(), not both."""
         with self._lock:
             if self._state_topic:
-                raise N.SgrError(N.SGR_ERR_INVALID, "this store is fed through put() of state records (its codec has no snapshot rules)")
+                if self._keys:
+                    raise N.SgrError(N.SGR_ERR_INVALID, "this store is already fed through put() / delete() of state records")
+                if self._dingest is None:
+                    from .dingest import DeviceIngest
+
+                    self._dingest = DeviceIngest(self._engine, self._max_ids, 64 * self._max_ids)
+                    self._dingest.set_state_topic(True)
+                self._dingest.set_aborted(partition, aborted)
+                return self._dingest.submit(partition, data)
             if self._keys:
                 raise N.SgrError(N.SGR_ERR_INVALID, "this store is already fed through put_event")
             if self._ingest is None:
@@ -248,14 +265,20 @@ class GpuReplayKeyValueStore:
         (KafkaProducerActorImpl.scala:684-708 -> KafkaAdminClient.consumerLag, KafkaAdminClient.scala:44-56) reaches zero
         exactly when get() can serve the state."""
         with self._lock:
-            if self._ingest is None:
+            fed = self._dingest if self._dingest is not None else self._ingest
+            if fed is None:
                 return {int(p): 0 for p in partitions}
-            return {int(p): self._ingest.offsets(int(p))[1] for p in partitions}
+            return {int(p): fed.offsets(int(p))[1] for p in partitions}
 
     def flush(self) -> None:
         with self._lock:
             if self._ingest is not None:
                 self._engine.fold_ingested(self._ingest)
+                self._folded = True
+                self._report_changes()
+                return
+            if self._dingest is not None:
+                self._dingest.fold()
                 self._folded = True
                 self._report_changes()
                 return
@@ -312,7 +335,7 @@ class GpuReplayKeyValueStore:
         capacity slots (ids past the ones this store assigned) never appear."""
         if self._on_changes is None:
             return
-        n_ids = None if self._ingest is not None else len(self._keys)
+        n_ids = None if self._ingest is not None or self._dingest is not None else len(self._keys)
         changed: List[Tuple[str, Optional[bytes]]] = []
         failed: List[Tuple[str, int]] = []
         for idx, flags, err, rows, ids in self._engine.export_changes(N.ST_CHANGED | N.ST_ERROR):
@@ -352,6 +375,8 @@ class GpuReplayKeyValueStore:
         if not key:      # the producer's flush record: empty key, empty value (KafkaProducerActorImpl.scala:321-329)
             return
         with self._lock:
+            if self._dingest is not None:
+                raise N.SgrError(N.SGR_ERR_INVALID, "this store is already fed through restore_record_batches")
             if self._state_topic:
                 self._state_put(key, value)
             elif self._codec is not None:
