@@ -171,7 +171,9 @@ typedef struct sgr_stats {
   uint64_t n_long_segments; /* aggregates taken by the split (long-segment) path */
   float    ms_h2d;          /* host->device copy of the last load (0 for _device loads) */
   float    ms_group;        /* stable group-by of the last unsorted load */
-  float    ms_fold;         /* device time of the last fold (all its kernels) */
+  float    ms_fold;         /* device time of the last fold (all its kernels); a record-parallel fold queued behind a
+                               fold of the same log (sgr_fold_async) overlaps it and is timed from its first CTA's entry
+                               to its last warp's exit by %globaltimer, every other fold by CUDA events around it */
   float    ms_d2h;          /* device->host copy of the last export */
   uint32_t fold_launches;   /* kernels launched by the last fold */
   uint32_t reserved[7];
@@ -363,6 +365,11 @@ int32_t sgr_set_option(sgr_engine* e, const char* name, int64_t value);
 
 /* The CUDA stream (cudaStream_t) the engine launches on, so callers can record events. */
 int32_t sgr_stream(sgr_engine* e, void** stream);
+
+/* Measurement probe (scripts/fold_ceiling.py): enqueue on `stream` one launch that stages `bytes` of the device buffer
+ * `buf` into shared memory the way the default record-parallel fold does, and does nothing else. Warps take fixed
+ * spans (ticketed = 0) or chunks of chunk_bytes by ticket (ticketed = 1); ctl: 2 device u64, zero before the launch. */
+int32_t sgr_probe_read(const void* buf, uint64_t bytes, int32_t ticketed, uint64_t chunk_bytes, void* ctl, void* stream);
 
 /* ------------------------------------------------------------------ multi-GPU (one process per GPU, one node)
  * Aggregates are hash-partitioned across ranks exactly as Surge shards them across nodes

@@ -38,13 +38,17 @@ struct RowArgs {
   const uint8_t* states_in;     // optional prior states
   uint8_t* states_out;
   unsigned long long* counters; // [0] events applied, [1] aggregates in error, [3] segments queued for exact replay,
-                                // [4] records dropped after a throw, [6] grid-barrier arrivals (fold_runs)
-  unsigned long long* counters_next;  // fold_runs: the other counter block, zeroed for the next fold
+                                // [4] records dropped after a throw; fold_runs (16 words): [6] warps arrived,
+                                // [8] ~%globaltimer at the first CTA's entry (max of the complement),
+                                // [9] %globaltimer at the last warp's exit,
+                                // [10] chunk ticket, [11] replay cursor
+  unsigned long long* counters_next;  // fold_runs: the other counter block (16 words), zeroed for the next fold
   uint32_t* redo_ids;           // segments whose handler threw (replayed by the sequential kernel)
   uint64_t redo_cap;
-  uint32_t* part_flags;         // per warp: == epoch once its open transformer is published
-  uint32_t* part_data;          // per warp: m, v[W], ex | has_head<<2
+  uint32_t* part_flags;         // per warp (fold_runs: per chunk): == epoch once its open transformer is published
+  uint32_t* part_data;          // per warp (fold_runs: per chunk): m, v[W], ex | has_head<<2
   uint32_t epoch;
+  uint64_t chunk_steps;         // fold_runs: steps per chunk of the ticketed work order (run_variant_chunk_steps)
 };
 
 // false if the program is outside the transformer algebra (IF_EXISTS rules, 64-bit adds, f64 fields,
@@ -80,6 +84,11 @@ const char* run_variant_name(int v);
 int run_kernel_max_grid(int num_sms, int variant, const RowProgram& prog);
 int run_variant_step_bytes(int variant, const RowProgram& prog);
 int run_warps_per_cta();
-cudaError_t launch_fold_runs(const RowArgs& args, const RowProgram& prog, int variant, int grid, cudaStream_t stream);
+// steps per chunk of a log of `steps` steps folded by up to n_warps warps: at most chunk_bytes, small enough that every warp
+// gets a chunk, and at least the steps the variant stages ahead
+uint64_t run_variant_chunk_steps(int variant, const RowProgram& prog, uint64_t chunk_bytes, uint64_t steps, uint64_t n_warps);
+// one launch, replay included; overlap: it may start while the runs fold before it on the stream drains (programmatic
+// dependent launch), for a fold of the same log right behind another
+cudaError_t launch_fold_runs(const RowArgs& args, const RowProgram& prog, int variant, int grid, bool overlap, cudaStream_t stream);
 
 }  // namespace sgr

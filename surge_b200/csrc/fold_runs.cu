@@ -8,9 +8,9 @@
 // bracketing of the log-ordered product equals the sequential fold bit for bit.
 //
 // Shape (HBM-bound byte parse + segmented scan; no tensor cores):
-//   * the log is cut into byte-balanced spans, one per warp — a hot aggregate (Zipf skew) is
-//     spread over many warps instead of serialising one lane;
-//   * a warp walks its span in steps of 32*R records. The step's 2048*R bytes are staged into
+//   * the log is cut into byte-balanced chunks, handed out to warps in log order (work order
+//     below) — a hot aggregate (Zipf skew) is spread over many warps instead of serialising one lane;
+//   * a warp walks a chunk in steps of 32*R records. The step's 2048*R bytes are staged into
 //     shared memory with coalesced 16-byte cp.async copies (512 contiguous bytes per warp
 //     instruction), NSTAGE steps deep, no register staging;
 //   * the staging layout XOR-swizzles each record's 16-byte chunks with (record/R)&7, so that
@@ -23,8 +23,20 @@
 //     that flows into it; the scan's tail is the carry into the next step;
 //   * segment heads come from the CSR offsets: a window of 32 boundaries is read with coalesced
 //     8-byte loads and scattered into a per-step head bitmap + segment-id table in smem;
-//   * a segment that crosses a span boundary is finished by the warp that sees its end, after a
-//     decoupled look-back over the predecessors' published open transformers.
+//   * a segment that crosses a chunk boundary is finished by the warp that sees its end, after a
+//     decoupled look-back over the preceding chunks' published open transformers.
+//
+// Work order: the log is cut into chunks of a few steps (RowArgs::chunk_steps). Warp g takes chunk g first, then further
+// chunks in log order by an atomic ticket (counters[10]), the single-pass-scan pattern: a warp that finishes early takes
+// more, so the fold ends when HBM runs dry rather than when the slowest of fixed spans ends. A chunk only ever waits on
+// chunks handed out before it. There is no grid barrier either: a warp leaves when its last chunk is done, unless a
+// segment threw, in which case the warps still there replay the list once every warp has arrived (replay_segments).
+// A fold queued right behind a fold of the same log is launched with programmatic dependent launch: before
+// griddepcontrol.wait it reads only the program, the log and its offsets (table load, first boundary search, first steps
+// in flight), which the fold before it only reads too, so it overlaps that fold's tail; states, look-back buffers,
+// counters, the replay list and the ticket come after the wait. Behind any other work (a kernel that writes the log, a
+// copy) it is launched plainly and the wait is a no-op. The chunk size shrinks on small logs so that every resident warp
+// gets a chunk (run_variant_chunk_steps).
 #include <stdio.h>
 
 #include "../../include/sgr.h"
@@ -94,6 +106,14 @@ __device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) {
   uint32_t v;
   asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p));
   return v;
+}
+// programmatic dependent launch: no-ops when the grid was launched without the attribute
+__device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
 }
 
 // Finish one segment: apply the composed transformer to the prior state, write the state struct.
@@ -180,6 +200,32 @@ __host__ __device__ constexpr int warp_smem_bytes() {
          + 32 * 4;           // head bitmap (R words used) + pad
 }
 
+template <int W>
+__device__ __noinline__ void replay_segments(const RowArgs& a, const RowProgram& pg, const uint32_t* tab, int lane, unsigned long long n_redo);
+
+// Decoupled look-back (lane 0): compose the open transformers of the chunks before chunk c until one that contains a head.
+// They were all handed out before c, to warps that are running, and a chunk publishes without waiting on anyone.
+template <int W, int CLS>
+__device__ __forceinline__ Xf<W> look_back_chunks(const RowArgs& a, uint64_t c) {
+  Xf<W> pre = identity<W>();
+  while (c > 0) {
+    --c;
+    const uint32_t* pf = a.part_flags + c;
+    while (ld_volatile_u32(pf) != a.epoch) { __nanosleep(64); }
+    __threadfence();
+    const uint32_t* pd = a.part_data + c * (W + 2);
+    Xf<W> e;
+    e.m = ld_volatile_u32(pd);
+#pragma unroll
+    for (int w = 0; w < W; ++w) e.v[w] = ld_volatile_u32(pd + 1 + w);
+    const uint32_t tailw = ld_volatile_u32(pd + W + 1);
+    e.ex = tailw & 3u;
+    pre = compose<W, CLS>(e, pre);
+    if (tailw & 4u) break;
+  }
+  return pre;
+}
+
 // DIRECT: programs with many source words read each state word's source straight from the staged record instead of
 // pre-fetching NS slots and selecting (NS is then unused)
 template <int W, int R, int NSTAGE, int NS, int MINB, bool DIRECT, int CLS>
@@ -189,6 +235,9 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
   constexpr int STEP_RECS = 32 * R;
   extern __shared__ __align__(128) uint8_t smem_raw[];
   __shared__ __align__(16) uint32_t tab[16 * kTabStride];
+  // the next fold may be scheduled now: it waits for this grid to complete before it touches anything this one writes
+  grid_dep_launch();
+  const unsigned long long t_entry = global_ns();
   for (int i = threadIdx.x; i < 16 * kTabStride; i += kRunThreads) tab[i] = pg.tab[i];
   const uint32_t f64_mask = pg.f64_mask;
   __syncthreads();
@@ -206,40 +255,30 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
   const uint64_t base = a.log_begin;
   const uint64_t total_bytes = a.log_end - base;
   const uint64_t total_steps = (total_bytes + STEP_BYTES - 1) / STEP_BYTES;
-  const uint64_t spw = (total_steps + n_warps - 1) / n_warps;  // steps per warp
-  const uint64_t step0 = gw * spw;
-  const uint64_t step_end = step0 + spw < total_steps ? step0 + spw : total_steps;
-  const bool has_span = step0 < step_end;
-  const uint64_t wb = base + step0 * STEP_BYTES;
-  // the warp that owns the end of the log also finishes the last segment and trailing empty ones;
-  // with an empty log that is warp 0
-  const bool owns_end = has_span ? (step_end == total_steps) : (total_steps == 0 && gw == 0);
+  // >= NSTAGE-1 (and >= 1): the steps staged ahead never reach past the next chunk, whose ticket is drawn when the
+  // current chunk starts
+  const uint64_t cs = a.chunk_steps;
+  const uint64_t n_chunks = (total_steps + cs - 1) / cs;
+  constexpr uint64_t kNone = ~0ull;
 
-  // ---- first boundary of the span: kc = first k in [0, n_seg] with off[k] >= wb (32-ary search)
-  uint64_t kc = 0;
-  if (has_span && gw != 0) {
+  // ---- first boundary at or after byte wb: the first k in [0, n_seg] with off[k] >= wb (32-ary search)
+  auto first_boundary = [&](uint64_t wb) -> uint64_t {
     uint64_t lo = 0, hi = n_seg + 1;  // answer in [lo, hi]; hi == n_seg+1: no such boundary
     while (lo < hi) {
-      const uint64_t chunk = (hi - lo + 31) / 32;
-      const uint64_t p = lo + (uint64_t)lane * chunk;
+      const uint64_t part = (hi - lo + 31) / 32;
+      const uint64_t p = lo + (uint64_t)lane * part;
       const bool valid = p < hi;
       const bool ge = !valid || a.seg_offsets[p] >= wb;  // monotone in lane
       const uint32_t bal = __ballot_sync(0xffffffffu, ge);
-      if (bal == 0) { lo = lo + 31 * chunk + 1; continue; }
+      if (bal == 0) { lo = lo + 31 * part + 1; continue; }
       const int f = __ffs(bal) - 1;
       if (f == 0) { hi = lo; break; }
-      const uint64_t pf = lo + (uint64_t)f * chunk;
-      lo = lo + (uint64_t)(f - 1) * chunk + 1;
+      const uint64_t pf = lo + (uint64_t)f * part;
+      lo = lo + (uint64_t)(f - 1) * part + 1;
       hi = pf < hi ? pf : hi;
     }
-    kc = lo;
-  }
-
-  bool span_has_head = false;          // a segment head was seen in this span
-  bool inh_pending = false;            // the segment flowing into the span awaits the look-back (held by lane 0)
-  uint32_t inh_seg = 0;
-  Xf<W> inh_t = identity<W>();
-  Xf<W> carry = identity<W>();         // open transformer at the end of the previous step
+    return lo;
+  };
 
   // ---- staging: lane l, copy q of a step moves the 16-byte chunk g = q*32 + l (source order) to its
   //      swizzled place: record j = g>>2, chunk c = g&3 -> line j>>1, position (4*(j&1)+c) ^ ((j/R)&7)
@@ -263,14 +302,42 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
         if (sbyte + (uint64_t)q * 512 + (uint64_t)lane * 16 < total_bytes) cp_async16(dst + dst_q[q], src + q * 512);
     }
   };
-  // prologue: NSTAGE-1 steps in flight
-  if (has_span) {
-#pragma unroll
-    for (int s = 0; s < NSTAGE - 1; ++s) {
-      if (step0 + s < step_end) issue_step(step0 + s, s);
-      cp_async_commit();
+  // ---- issue side: steps are staged in the warp's own order, the current chunk's and then the next one's, so the pipeline
+  //      runs on across chunk boundaries. iss: the next step to stage, iss_end: the end of its chunk iss_chunk.
+  uint64_t chunk = gw < n_chunks ? gw : kNone;  // the chunk being folded: the first one fixed, later ones by ticket
+  uint64_t iss_chunk = chunk, iss = 0, iss_end = 0;
+  if (chunk != kNone) { iss = chunk * cs; iss_end = iss + cs < total_steps ? iss + cs : total_steps; }
+  uint64_t nxt = kNone;             // the chunk after the current one, once the ticket is read
+  bool nxt_pending = false;         // lane 0 holds a ticket not yet read
+  unsigned long long tk = 0;
+  auto resolve_next = [&]() {
+    if (!nxt_pending) return;
+    const unsigned long long t = __shfl_sync(0xffffffffu, tk, 0);
+    nxt = n_warps + t < n_chunks ? n_warps + t : kNone;
+    nxt_pending = false;
+  };
+  int ist = 0;
+  auto issue_next = [&]() {
+    if (iss == iss_end && iss_chunk != kNone) {
+      resolve_next();
+      if (nxt != kNone && nxt != iss_chunk) {
+        iss_chunk = nxt; iss = nxt * cs; iss_end = iss + cs < total_steps ? iss + cs : total_steps;
+      }
     }
+    if (iss < iss_end) {
+      issue_step(iss, ist);
+      ++iss;
+      if (++ist == NSTAGE) ist = 0;
+    }
+  };
+
+  // ---- before the wait: the first chunk's first steps in flight, its first boundary and boundary window
+#pragma unroll
+  for (int s = 0; s < NSTAGE - 1; ++s) {
+    issue_next();
+    cp_async_commit();
   }
+  uint64_t kc = (chunk != kNone && chunk != 0) ? first_boundary(base + chunk * cs * STEP_BYTES) : 0;
 
   // where lane i finds word (c,k) of a record of parity par: byte (((4*par + c) ^ (i&7)) << 4) + 4k of its 128-byte line
   constexpr int NSOFF = DIRECT ? 1 : NS;
@@ -289,222 +356,268 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
     win_b = k <= n_seg ? a.seg_offsets[k] : ~0ull;
     win_bn = k < n_seg ? a.seg_offsets[k + 1] : ~0ull;
   };
-  if (has_span) load_window();
+  if (chunk != kNone) load_window();
 
+  // ---- after the wait: the previous fold (and its replay) has completed; its states, counters and buffers are free
+  grid_dep_wait();
+  if (threadIdx.x == 0) atomicMax(a.counters + 8, ~t_entry);  // the earliest CTA entry, complemented (stats ms_fold)
+  if (gw == 0 && lane < 16) a.counters_next[lane] = 0ull;    // the next fold starts from clean counters without a memset
+  auto look_back = [&](uint64_t c) -> Xf<W> { return look_back_chunks<W, CLS>(a, c); };
+  // lane 0: a chunk's first segment, begun in an earlier chunk, is finished after the warp's next chunk (or at its exit),
+  // so the warp does not wait on a predecessor that is still being folded
+  bool dfr = false;
+  uint64_t dfr_chunk = 0;
+  uint32_t dfr_seg = 0;
+  Xf<W> dfr_t = identity<W>();
+
+  unsigned long long n_applied = 0;  // records of this warp's chunks
   int stage = 0;
-  for (uint64_t step = step0; step < step_end; ++step) {
-    // keep NSTAGE-1 steps in flight
-    {
-      const uint64_t ahead = step + (NSTAGE - 1);
-      int st = stage + (NSTAGE - 1); if (st >= NSTAGE) st -= NSTAGE;
-      if (ahead < step_end) issue_step(ahead, st);
+  uint64_t prev_chunk = kNone;
+  while (chunk != kNone) {
+    const uint64_t step0 = chunk * cs;
+    const uint64_t step_end = step0 + cs < total_steps ? step0 + cs : total_steps;
+    const uint64_t wb = base + step0 * STEP_BYTES;
+    if (iss_chunk != chunk) { iss_chunk = chunk; iss = step0; iss_end = step_end; }  // one stage: nothing was staged ahead
+    if (lane == 0) tk = atomicAdd(a.counters + 10, 1ull);  // the chunk after this one; read when the issue side reaches it
+    nxt_pending = true;
+    if (prev_chunk != kNone && chunk != prev_chunk + 1) {
+      // a chunk right after the previous one starts at the boundary where that one stopped
+      kc = chunk != 0 ? first_boundary(wb) : 0;
+      load_window();
+    }
+
+    bool span_has_head = false;          // a segment head was seen in this chunk
+    bool inh_pending = false;            // the segment flowing into the chunk awaits the look-back (held by lane 0)
+    uint32_t inh_seg = 0;
+    Xf<W> inh_t = identity<W>();
+    Xf<W> carry = identity<W>();         // open transformer at the end of the previous step
+
+    for (uint64_t step = step0; step < step_end; ++step) {
+      // keep NSTAGE-1 steps in flight
+      issue_next();
       cp_async_commit();
-    }
-    const uint64_t sb = base + step * (uint64_t)STEP_BYTES;
-    const uint64_t rem = a.log_end - sb;
-    const uint32_t span = rem < (uint64_t)STEP_BYTES ? (uint32_t)rem : (uint32_t)STEP_BYTES;
-    const int nvalid = (int)(span >> 6);
+      const uint64_t sb = base + step * (uint64_t)STEP_BYTES;
+      const uint64_t rem = a.log_end - sb;
+      const uint32_t span = rem < (uint64_t)STEP_BYTES ? (uint32_t)rem : (uint32_t)STEP_BYTES;
+      const int nvalid = (int)(span >> 6);
 
-    // ---- segment heads of this step: boundaries k with off[k] in [sb, sb+span) ----------------------
+      // ---- segment heads of this step: boundaries k with off[k] in [sb, sb+span) ----------------------
 #pragma unroll
-    for (int i = 0; i < R; ++i) { hs_end[i * 32 + lane] = 0xffffffffu; hs_start[i * 32 + lane] = 0u; }
-    if (lane < R) hmask[lane] = 0u;
-    __syncwarp();
-    while (true) {
-      const uint64_t k = kc + lane;
-      const uint64_t b = win_b, bn = win_bn;  // window at kc, loaded one step ahead
-      const uint64_t d = b - sb;  // >= 0 for every unconsumed boundary
-      const bool in = d < (uint64_t)span;
-      if (in) {
-        const uint32_t pos = (uint32_t)d >> 6;
-        atomicOr(&hmask[pos >> 5], 1u << (pos & 31));
-        atomicMax(&hs_start[pos], (uint32_t)k);                       // the last boundary at this offset starts the live segment
-        if (k > 0) atomicMin(&hs_end[pos], (uint32_t)k - 1u);         // the first one ends the previous segment
-        if (bn == b) finish_empty<W>(a, (uint32_t)k);                 // segment k is empty
-      }
-      const int cnt = __popc(__ballot_sync(0xffffffffu, in));
-      kc += cnt;
-      if (cnt) load_window();
-      if (cnt < 32) break;
-    }
-    __syncwarp();
-
-    // ---- wait for this step's bytes --------------------------------------------------------------------
-    cp_async_wait<NSTAGE - 1>();
-    __syncwarp();
-
-    // ---- lane run: R consecutive records, left to right -------------------------------------------------
-    const uint32_t sbase = stage0 + (uint32_t)stage * STEP_BYTES;
-    uint32_t hbits;
-    if (R >= 32) hbits = hmask[lane];
-    else hbits = (hmask[(lane * R) >> 5] >> ((lane * R) & 31)) & ((R >= 32) ? 0xffffffffu : ((1u << R) - 1u));
-    Xf<W> cur = identity<W>();
-    Xf<W> first = identity<W>();
-    uint32_t first_seg = 0xffffffffu;
-    bool have_first = false;
-#pragma unroll
-    for (int t = 0; t < R; ++t) {
-      const int p = lane * R + t;
-      if (hbits & (1u << t)) {
-        const uint32_t eseg = hs_end[p];
-        if (!have_first) { first = cur; first_seg = eseg; have_first = true; }
-        else if (eseg != 0xffffffffu) finish_segment<W>(a, f64_mask, eseg, cur);  // began and ended inside this run
-        cur = identity<W>();
-      }
-      if (p < nvalid) {
-        const uint32_t rec = sbase + (uint32_t)(p >> 1) * 128u;
-        const uint32_t lane7 = (uint32_t)(lane & 7), par4 = (uint32_t)(t & 1) * 4u;  // p&1 == t&1: R is even
-        uint32_t sv[DIRECT ? 1 : NS];
-        if (DIRECT) {
-          sv[0] = lds32(rec + soff[t & 1][0]);
-        } else {
-#pragma unroll
-          for (int s = 0; s < NS; ++s) sv[s] = lds32(rec + soff[t & 1][s]);
+      for (int i = 0; i < R; ++i) { hs_end[i * 32 + lane] = 0xffffffffu; hs_start[i * 32 + lane] = 0u; }
+      if (lane < R) hmask[lane] = 0u;
+      __syncwarp();
+      while (true) {
+        const uint64_t k = kc + lane;
+        const uint64_t b = win_b, bn = win_bn;  // window at kc, loaded one step ahead
+        const uint64_t d = b - sb;  // >= 0 for every unconsumed boundary
+        const bool in = d < (uint64_t)span;
+        if (in) {
+          const uint32_t pos = (uint32_t)d >> 6;
+          atomicOr(&hmask[pos >> 5], 1u << (pos & 31));
+          atomicMax(&hs_start[pos], (uint32_t)k);                       // the last boundary at this offset starts the live segment
+          if (k > 0) atomicMin(&hs_end[pos], (uint32_t)k - 1u);         // the first one ends the previous segment
+          if (bn == b) finish_empty<W>(a, (uint32_t)k);                 // segment k is empty
         }
-        const uint32_t type = sv[0];
-        uint4 e0 = make_uint4(0, 0, 0, 0);
-        if (type < 16u) e0 = *reinterpret_cast<const uint4*>(tab + type * kTabStride);
-        if (!(e0.x & 1u)) {
-          cur.m |= M_ERR;  // THROW rule or scala.MatchError
-        } else if (CLS == 1 && (e0.x & 4u) && cur.ex == EX_NONE) {
-          // IF_EXISTS event after a tombstone in this run: the state does not exist, the event is a no-op
-        } else {
-          if (CLS == 0 || !(e0.x & 4u)) cur.ex = (e0.x & 2u) ? EX_NONE : EX_SOME;  // an IF_EXISTS event leaves the exists-op as it is
-          uint32_t spec[W];
-          spec[0] = e0.y;
-          if (W > 1) spec[1] = e0.z;
-          if (W > 2) spec[2] = e0.w;
+        const int cnt = __popc(__ballot_sync(0xffffffffu, in));
+        kc += cnt;
+        if (cnt) load_window();
+        if (cnt < 32) break;
+      }
+      __syncwarp();
+
+      // ---- wait for this step's bytes --------------------------------------------------------------------
+      cp_async_wait<NSTAGE - 1>();
+      __syncwarp();
+
+      // ---- lane run: R consecutive records, left to right -------------------------------------------------
+      const uint32_t sbase = stage0 + (uint32_t)stage * STEP_BYTES;
+      uint32_t hbits;
+      if (R >= 32) hbits = hmask[lane];
+      else hbits = (hmask[(lane * R) >> 5] >> ((lane * R) & 31)) & ((R >= 32) ? 0xffffffffu : ((1u << R) - 1u));
+      Xf<W> cur = identity<W>();
+      Xf<W> first = identity<W>();
+      uint32_t first_seg = 0xffffffffu;
+      bool have_first = false;
 #pragma unroll
-          for (int w = 3; w < W; ++w) spec[w] = tab[type * kTabStride + 1 + w];
+      for (int t = 0; t < R; ++t) {
+        const int p = lane * R + t;
+        if (hbits & (1u << t)) {
+          const uint32_t eseg = hs_end[p];
+          if (!have_first) { first = cur; first_seg = eseg; have_first = true; }
+          else if (eseg != 0xffffffffu) finish_segment<W>(a, f64_mask, eseg, cur);  // began and ended inside this run
+          cur = identity<W>();
+        }
+        if (p < nvalid) {
+          const uint32_t rec = sbase + (uint32_t)(p >> 1) * 128u;
+          const uint32_t lane7 = (uint32_t)(lane & 7), par4 = (uint32_t)(t & 1) * 4u;  // p&1 == t&1: R is even
+          uint32_t sv[DIRECT ? 1 : NS];
+          if (DIRECT) {
+            sv[0] = lds32(rec + soff[t & 1][0]);
+          } else {
 #pragma unroll
-          for (int w = 0; w < W; ++w) {
-            uint32_t val = 0;
-            if (DIRECT) {
-              const uint32_t sl = spec[w] >> 3;
-              if (sl) { const uint32_t sw = pg.slot_word[sl]; val = lds32(rec + ((((par4 + (sw >> 2)) ^ lane7) << 4) | ((sw & 3u) << 2))); }
-            } else {
-#pragma unroll
-              for (int s = 1; s < NS; ++s) val = ((spec[w] >> 3) == (uint32_t)s) ? sv[s] : val;
-            }
-            if (spec[w] & 4u) val = 0u - val;
-            const uint32_t mode = spec[w] & 3u;
-            if (mode == 2u) cur.v[w] = val;
-            else if (mode == 1u) cur.v[w] += val;
-            cur.m |= mode << (2 * w);
+            for (int s = 0; s < NS; ++s) sv[s] = lds32(rec + soff[t & 1][s]);
           }
-          cur.m |= (e0.x & 8u) << 27;   // M_COPY: this rule builds a new instance (CREATE, or any field op)
+          const uint32_t type = sv[0];
+          uint4 e0 = make_uint4(0, 0, 0, 0);
+          if (type < 16u) e0 = *reinterpret_cast<const uint4*>(tab + type * kTabStride);
+          if (!(e0.x & 1u)) {
+            cur.m |= M_ERR;  // THROW rule or scala.MatchError
+          } else if (CLS == 1 && (e0.x & 4u) && cur.ex == EX_NONE) {
+            // IF_EXISTS event after a tombstone in this run: the state does not exist, the event is a no-op
+          } else {
+            if (CLS == 0 || !(e0.x & 4u)) cur.ex = (e0.x & 2u) ? EX_NONE : EX_SOME;  // an IF_EXISTS event leaves the exists-op as it is
+            uint32_t spec[W];
+            spec[0] = e0.y;
+            if (W > 1) spec[1] = e0.z;
+            if (W > 2) spec[2] = e0.w;
+#pragma unroll
+            for (int w = 3; w < W; ++w) spec[w] = tab[type * kTabStride + 1 + w];
+#pragma unroll
+            for (int w = 0; w < W; ++w) {
+              uint32_t val = 0;
+              if (DIRECT) {
+                const uint32_t sl = spec[w] >> 3;
+                if (sl) { const uint32_t sw = pg.slot_word[sl]; val = lds32(rec + ((((par4 + (sw >> 2)) ^ lane7) << 4) | ((sw & 3u) << 2))); }
+              } else {
+#pragma unroll
+                for (int s = 1; s < NS; ++s) val = ((spec[w] >> 3) == (uint32_t)s) ? sv[s] : val;
+              }
+              if (spec[w] & 4u) val = 0u - val;
+              const uint32_t mode = spec[w] & 3u;
+              if (mode == 2u) cur.v[w] = val;
+              else if (mode == 1u) cur.v[w] += val;
+              cur.m |= mode << (2 * w);
+            }
+            cur.m |= (e0.x & 8u) << 27;   // M_COPY: this rule builds a new instance (CREATE, or any field op)
+          }
         }
       }
-    }
-    // cur = transformer of the records after the run's last head (the whole run if it has none)
+      // cur = transformer of the records after the run's last head (the whole run if it has none)
 
-    // ---- once per step: segmented inclusive scan of the 32 lane transformers, in log order -------------
-    const uint32_t lane_heads = __ballot_sync(0xffffffffu, have_first);
-    Xf<W> sc = cur;
-    if (lane == 0 && !have_first) sc = compose<W, CLS>(carry, sc);
+      // ---- once per step: segmented inclusive scan of the 32 lane transformers, in log order -------------
+      const uint32_t lane_heads = __ballot_sync(0xffffffffu, have_first);
+      Xf<W> sc = cur;
+      if (lane == 0 && !have_first) sc = compose<W, CLS>(carry, sc);
 #pragma unroll
-    for (int dd = 1; dd < 32; dd <<= 1) {
-      const Xf<W> o = shfl_xf(sc, lane - dd);  // wraps for lane < dd; masked below
-      const int sh = lane >= dd ? lane - dd + 1 : 0;
-      const uint32_t window = (lane_heads >> sh) & ((1u << dd) - 1u);  // a head in lanes (lane-dd, lane]?
-      if (lane >= dd && window == 0) sc = compose<W, CLS>(o, sc);
-    }
-    // what flows INTO each lane's run: the scan value of the previous lane (lane 0: the carry)
-    Xf<W> cin = shfl_xf(sc, lane - 1);
-    if (lane == 0) cin = carry;
-    carry = shfl_xf(sc, 31);
-
-    // ---- the segment that ends at a run's first head needs what flowed in ----------------------------------
-    if (have_first && first_seg != 0xffffffffu) {
-      const Xf<W> tot = compose<W, CLS>(cin, first);
-      // the very first head of the span ends a segment that began in an earlier span: look-back needed
-      const bool is_span_first = !span_has_head && (lane_heads & ((1u << lane) - 1u)) == 0;
-      if (is_span_first && gw != 0) { inh_t = tot; inh_seg = first_seg; inh_pending = true; }
-      else finish_segment<W>(a, f64_mask, first_seg, tot);
-    }
-    if (lane_heads) {
-      // the pending look-back lives in the lane that saw the span's first head: move it to lane 0
-      if (!span_has_head) {
-        const int src = __ffs(lane_heads) - 1;
-        inh_t = shfl_xf(inh_t, src);
-        inh_seg = __shfl_sync(0xffffffffu, inh_seg, src);
-        inh_pending = __shfl_sync(0xffffffffu, (int)inh_pending, src) != 0;
+      for (int dd = 1; dd < 32; dd <<= 1) {
+        const Xf<W> o = shfl_xf(sc, lane - dd);  // wraps for lane < dd; masked below
+        const int sh = lane >= dd ? lane - dd + 1 : 0;
+        const uint32_t window = (lane_heads >> sh) & ((1u << dd) - 1u);  // a head in lanes (lane-dd, lane]?
+        if (lane >= dd && window == 0) sc = compose<W, CLS>(o, sc);
       }
-      span_has_head = true;
-    }
-    __syncwarp();
-    if (++stage == NSTAGE) stage = 0;
-  }
-  cp_async_wait<0>();
+      // what flows INTO each lane's run: the scan value of the previous lane (lane 0: the carry)
+      Xf<W> cin = shfl_xf(sc, lane - 1);
+      if (lane == 0) cin = carry;
+      carry = shfl_xf(sc, 31);
 
-  // ---- end of the log: the open segment and any trailing empty segments --------------------------------
-  // boundaries with off[k] == log_end were never a head inside a step; kc is the first of them.
-  bool end_needs_lookback = false;
-  if (owns_end) {
-    for (uint64_t k = kc + lane; k < n_seg; k += 32) finish_empty<W>(a, (uint32_t)k);  // segments kc..n_seg-1 are empty
-    if (kc >= 1 && total_steps > 0) {
-      // segment kc-1 is the last non-empty one; its transformer is the carry
-      if (span_has_head || gw == 0) { if (lane == 0) finish_segment<W>(a, f64_mask, (uint32_t)(kc - 1), carry); }
-      else end_needs_lookback = true;  // the whole span lies inside that segment
+      // ---- the segment that ends at a run's first head needs what flowed in ----------------------------------
+      if (have_first && first_seg != 0xffffffffu) {
+        const Xf<W> tot = compose<W, CLS>(cin, first);
+        // the very first head of the chunk ends a segment that began in an earlier chunk: look-back needed
+        const bool is_span_first = !span_has_head && (lane_heads & ((1u << lane) - 1u)) == 0;
+        if (is_span_first && chunk != 0) { inh_t = tot; inh_seg = first_seg; inh_pending = true; }
+        else finish_segment<W>(a, f64_mask, first_seg, tot);
+      }
+      if (lane_heads) {
+        // the pending look-back lives in the lane that saw the chunk's first head: move it to lane 0
+        if (!span_has_head) {
+          const int src = __ffs(lane_heads) - 1;
+          inh_t = shfl_xf(inh_t, src);
+          inh_seg = __shfl_sync(0xffffffffu, inh_seg, src);
+          inh_pending = __shfl_sync(0xffffffffu, (int)inh_pending, src) != 0;
+        }
+        span_has_head = true;
+      }
+      __syncwarp();
+      if (++stage == NSTAGE) stage = 0;
     }
-  }
 
-  // ---- publish this span's open transformer, then finish what needs the predecessors ---------------------
-  if (has_span) {
-    uint32_t* part_data = a.part_data + gw * (W + 2);
-    if (lane == 0) {
-      part_data[0] = carry.m;
+    // ---- end of the log: the open segment and any trailing empty segments --------------------------------
+    // boundaries with off[k] == log_end were never a head inside a step; kc is the first of them.
+    bool end_needs_lookback = false;
+    if (step_end == total_steps) {
+      for (uint64_t k = kc + lane; k < n_seg; k += 32) finish_empty<W>(a, (uint32_t)k);  // segments kc..n_seg-1 are empty
+      if (kc >= 1) {
+        // segment kc-1 is the last non-empty one; its transformer is the carry
+        if (span_has_head || chunk == 0) { if (lane == 0) finish_segment<W>(a, f64_mask, (uint32_t)(kc - 1), carry); }
+        else end_needs_lookback = true;  // the whole chunk lies inside that segment
+      }
+    }
+
+    // ---- publish this chunk's open transformer, then finish what needs the preceding chunks -----------------
+    {
+      uint32_t* part_data = a.part_data + chunk * (W + 2);
+      if (lane == 0) {
+        part_data[0] = carry.m;
 #pragma unroll
-      for (int w = 0; w < W; ++w) part_data[1 + w] = carry.v[w];
-      part_data[W + 1] = carry.ex | (span_has_head ? 4u : 0u);
-      __threadfence();
-      asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(a.part_flags + gw), "r"(a.epoch) : "memory");
-    }
-    if (lane == 0 && (inh_pending || end_needs_lookback)) {
-      // decoupled look-back: compose predecessors' open transformers until one that contains a head
-      Xf<W> pre = identity<W>();
-      uint64_t p = gw;
-      while (p > 0) {
-        --p;
-        const uint32_t* pf = a.part_flags + p;
-        while (ld_volatile_u32(pf) != a.epoch) { __nanosleep(64); }
+        for (int w = 0; w < W; ++w) part_data[1 + w] = carry.v[w];
+        part_data[W + 1] = carry.ex | (span_has_head ? 4u : 0u);
         __threadfence();
-        const uint32_t* pd = a.part_data + p * (W + 2);
-        Xf<W> e;
-        e.m = ld_volatile_u32(pd);
-#pragma unroll
-        for (int w = 0; w < W; ++w) e.v[w] = ld_volatile_u32(pd + 1 + w);
-        const uint32_t tailw = ld_volatile_u32(pd + W + 1);
-        e.ex = tailw & 3u;
-        pre = compose<W, CLS>(e, pre);
-        if (tailw & 4u) break;
+        asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(a.part_flags + chunk), "r"(a.epoch) : "memory");
       }
-      if (inh_pending) finish_segment<W>(a, f64_mask, inh_seg, compose<W, CLS>(pre, inh_t));
-      if (end_needs_lookback) finish_segment<W>(a, f64_mask, (uint32_t)(kc - 1), compose<W, CLS>(pre, carry));
+      if (lane == 0) {
+        // the previous chunk's look-back, left until now: its predecessors were folded while this chunk was
+        if (dfr) { finish_segment<W>(a, f64_mask, dfr_seg, compose<W, CLS>(look_back(dfr_chunk), dfr_t)); dfr = false; }
+        if (inh_pending) { dfr = true; dfr_chunk = chunk; dfr_seg = inh_seg; dfr_t = inh_t; }
+        // (a chunk without a head has no pending segment; the one that ends the log finishes the open one now)
+        if (end_needs_lookback) finish_segment<W>(a, f64_mask, (uint32_t)(kc - 1), compose<W, CLS>(look_back(chunk), carry));
+      }
+      __syncwarp();
     }
-  }
-  // every record of the span was applied; records of throwing segments are taken back by the replay below
-  if (lane == 0 && has_span) {
-    const uint64_t we = base + step_end * (uint64_t)STEP_BYTES < a.log_end ? base + step_end * (uint64_t)STEP_BYTES : a.log_end;
-    atomicAdd(a.counters + 0, (unsigned long long)((we - wb) >> 6));
-  }
+    // every record of the chunk was applied; records of throwing segments are taken back by the replay below
+    {
+      const uint64_t we = base + step_end * (uint64_t)STEP_BYTES < a.log_end ? base + step_end * (uint64_t)STEP_BYTES : a.log_end;
+      n_applied += (we - wb) >> 6;
+    }
+    prev_chunk = chunk;
+    resolve_next();
+    chunk = nxt;
+  }  // chunks
+  cp_async_wait<0>();
+  if (lane == 0 && dfr) finish_segment<W>(a, f64_mask, dfr_seg, compose<W, CLS>(look_back(dfr_chunk), dfr_t));
 
-  // ---- grid barrier (every warp of the grid is resident), then exact replay of the throwing segments ----
-  // A segment whose handler threw keeps its pre-batch state and reports the index of the throwing event
-  // (PersistentActor.scala:260-263); that needs the strictly sequential walk, done here one lane per segment.
+  // an empty log (every segment empty): warp 0 writes every state
+  if (n_chunks == 0 && gw == 0)
+    for (uint64_t k = lane; k < n_seg; k += 32) finish_empty<W>(a, (uint32_t)k);
+
+  // ---- arrival, then the exact replay of the throwing segments, without a grid barrier ----------------------------
+  // A warp that arrives while no segment is queued for replay leaves at once (its SM slot goes to the next fold). One that
+  // arrives after a throw waits for the others and helps with the replay; the last warp to arrive always does, so the
+  // replay list is complete whoever replays it.
+  unsigned long long arrived = 0, n_redo = 0;
   if (lane == 0) {
+    if (n_applied) atomicAdd(a.counters + 0, n_applied);
     __threadfence();
-    atomicAdd(a.counters + 6, 1ull);
-    while (ld_volatile_u64(a.counters + 6) < n_warps) { __nanosleep(128); }
+    arrived = atomicAdd(a.counters + 6, 1ull) + 1;
     __threadfence();
+    n_redo = ld_volatile_u64(a.counters + 3);
+    if (arrived < n_warps && n_redo != 0) {
+      while (ld_volatile_u64(a.counters + 6) < n_warps) { __nanosleep(128); }
+      __threadfence();
+      n_redo = ld_volatile_u64(a.counters + 3);
+    }
+    if (n_redo == 0) atomicMax(a.counters + 9, global_ns());
   }
-  __syncwarp();
-  if (gw == 0 && lane < 8) a.counters_next[lane] = 0ull;  // the next fold starts from clean counters without a memset
-  unsigned long long n_redo = ld_volatile_u64(a.counters + 3);
+  n_redo = __shfl_sync(0xffffffffu, n_redo, 0);
   if (n_redo == 0) return;
+  replay_segments<W>(a, pg, tab, lane, n_redo);
+}
+
+// ---- exact replay of the throwing segments the fold listed (counters[3] of them) -------------------------------------
+// A segment whose handler threw keeps its pre-batch state and reports the index of the throwing event
+// (PersistentActor.scala:260-263); that needs the strictly sequential walk, done here one lane per segment. The warps that
+// replay take 32 list entries at a time from a cursor (counters[11]).
+template <int W>
+__device__ __noinline__ void replay_segments(const RowArgs& a, const RowProgram& pg, const uint32_t* tab, int lane, unsigned long long n_redo) {
   if (n_redo > a.redo_cap) n_redo = a.redo_cap;  // overflow: the host re-runs the whole fold sequentially
   unsigned long long n_err = 0, n_dropped = 0;
-  for (unsigned long long i = gw * 32 + lane; i < n_redo; i += n_warps * 32) {
+  while (true) {
+    unsigned long long i0 = 0;
+    if (lane == 0) i0 = atomicAdd(a.counters + 11, 32ull);
+    i0 = __shfl_sync(0xffffffffu, i0, 0);
+    if (i0 >= n_redo) break;
+    const unsigned long long i = i0 + lane;
+    if (i >= n_redo) continue;
     const uint32_t seg = a.redo_ids[i];
     const uint64_t b = a.seg_offsets[seg], e = a.seg_offsets[(uint64_t)seg + 1];
     const uint64_t slot = a.seg_ids ? (uint64_t)a.seg_ids[seg] : (uint64_t)seg;
@@ -563,6 +676,8 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
   if (lane == 0) {
     if (n_err) atomicAdd(a.counters + 1, n_err);
     if (n_dropped) atomicAdd(a.counters + 4, n_dropped);
+    __threadfence();
+    atomicMax(a.counters + 9, global_ns());
   }
 }
 
@@ -610,12 +725,97 @@ int run_variant_step_bytes(int variant, const RowProgram& prog) {
 }
 int run_warps_per_cta() { return kRunWarps; }
 
-cudaError_t launch_fold_runs(const RowArgs& args, const RowProgram& prog, int variant, int grid, cudaStream_t stream) {
+uint64_t run_variant_chunk_steps(int variant, const RowProgram& prog, uint64_t chunk_bytes, uint64_t steps, uint64_t n_warps) {
+  if (variant < 0 || variant >= kNumRunVariants) variant = 0;
+  const bool wide = prog.user_words != 2 || prog.n_slots > 6 || prog.cls != 0;
+  const uint64_t ns = (uint64_t)(wide ? kWideStages : kRunVariants[variant].nstage);
+  const uint64_t lo = ns > 1 ? ns - 1 : 1;  // what is staged ahead stays inside the next chunk
+  uint64_t hi = chunk_bytes / (uint64_t)run_variant_step_bytes(variant, prog);
+  if (hi < lo) hi = lo;
+  const uint64_t fair = n_warps ? steps / n_warps : hi;  // a chunk for every warp on a small log
+  return fair < lo ? lo : (fair > hi ? hi : fair);
+}
+
+cudaError_t launch_fold_runs(const RowArgs& args, const RowProgram& prog, int variant, int grid, bool overlap, cudaStream_t stream) {
   if (variant < 0 || variant >= kNumRunVariants) variant = 0;
   const size_t smem = variant_smem(variant, prog);
   RunKernel k = variant_kernel(variant, prog);  // its smem attribute was set by run_kernel_max_grid
-  k<<<grid, kRunThreads, smem, stream>>>(args, prog);
-  return cudaGetLastError();
+  // overlap: the launch may begin while the fold before it drains (programmatic dependent launch); the kernel waits on the
+  // device for its predecessor before it touches anything that predecessor writes
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(kRunThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+  cfg.attrs = attr; cfg.numAttrs = overlap ? 1 : 0;
+  return cudaLaunchKernelEx(&cfg, k, args, prog);
 }
 
+namespace {
+// ---- read-ceiling probe (scripts/fold_ceiling.py) ----------------------------------------------------------------------
+// The default variant's staging alone — the same CTAs, warps and shared memory, 16-byte cp.async copies of 8 KiB steps,
+// two stages — over a buffer, with no fold work: the practical read ceiling of the fold on this card. Warps take fixed
+// spans (1/n of the buffer each) or chunks of chunk_steps steps by ticket (ctl[0], zero before the launch).
+template <bool TICKET>
+__global__ void __launch_bounds__(kRunThreads, 3) read_probe_kernel(const uint8_t* buf, uint64_t bytes, uint64_t chunk_steps, unsigned long long* ctl) {
+  constexpr int R = 4, NSTAGE = 2, STEP_BYTES = 2048 * R;
+  extern __shared__ __align__(128) uint8_t smem_raw[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t stage0 = smem_u32(smem_raw + (size_t)warp * warp_smem_bytes<R, NSTAGE>());
+  const uint64_t gw = (uint64_t)blockIdx.x * kRunWarps + warp, n_warps = (uint64_t)gridDim.x * kRunWarps;
+  const uint64_t total_steps = (bytes + STEP_BYTES - 1) / STEP_BYTES;
+  auto issue = [&](uint64_t s, int stage) {
+    const uint64_t sbyte = s * (uint64_t)STEP_BYTES;
+    const uint32_t dst = stage0 + (uint32_t)stage * STEP_BYTES + (uint32_t)lane * 16u;
+#pragma unroll
+    for (int q = 0; q < 4 * R; ++q)
+      if (sbyte + (uint64_t)q * 512 + (uint64_t)lane * 16 < bytes) cp_async16(dst + q * 512, buf + sbyte + q * 512 + lane * 16);
+  };
+  uint32_t acc = 0;
+  auto run = [&](uint64_t s0, uint64_t s1) {
+    if (s0 < s1) issue(s0, 0);
+    cp_async_commit();
+    int stage = 0;
+    for (uint64_t s = s0; s < s1; ++s) {
+      if (s + 1 < s1) issue(s + 1, stage ^ 1);
+      cp_async_commit();
+      cp_async_wait<NSTAGE - 1>();
+      __syncwarp();
+      acc ^= lds32(stage0 + (uint32_t)stage * STEP_BYTES + (uint32_t)lane * 4u);
+      __syncwarp();
+      stage ^= 1;
+    }
+    cp_async_wait<0>();
+  };
+  if (!TICKET) {
+    const uint64_t spw = (total_steps + n_warps - 1) / n_warps, s0 = gw * spw;
+    run(s0, s0 + spw < total_steps ? s0 + spw : total_steps);
+  } else {
+    const uint64_t n_chunks = (total_steps + chunk_steps - 1) / chunk_steps;
+    for (uint64_t c = gw; c < n_chunks;) {
+      const uint64_t s0 = c * chunk_steps;
+      run(s0, s0 + chunk_steps < total_steps ? s0 + chunk_steps : total_steps);
+      unsigned long long t = 0;
+      if (lane == 0) t = atomicAdd(ctl, 1ull);
+      c = n_warps + __shfl_sync(0xffffffffu, t, 0);
+    }
+  }
+  if (acc == 0x9e3779b9u) ctl[1] = acc;  // keeps the shared-memory reads
+}
+}  // namespace
+
 }  // namespace sgr
+
+extern "C" int32_t sgr_probe_read(const void* buf, uint64_t bytes, int32_t ticketed, uint64_t chunk_bytes, void* ctl, void* stream) {
+  using namespace sgr;
+  int dev = 0, n_sm = 0, per_sm = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return SGR_ERR_CUDA;
+  auto k = ticketed ? read_probe_kernel<true> : read_probe_kernel<false>;
+  const size_t smem = (size_t)kRunWarps * warp_smem_bytes<4, 2>();
+  if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kRunThreads, smem) != cudaSuccess || per_sm < 1)
+    return SGR_ERR_CUDA;
+  const uint64_t steps = chunk_bytes / 8192 > 2 ? chunk_bytes / 8192 : 2;
+  k<<<per_sm * n_sm, kRunThreads, smem, (cudaStream_t)stream>>>((const uint8_t*)buf, bytes, steps, (unsigned long long*)ctl);
+  return cudaGetLastError() == cudaSuccess ? SGR_OK : SGR_ERR_CUDA;
+}

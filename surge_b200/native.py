@@ -131,6 +131,7 @@ ABI = [
     ("sgr_get_stats", C.c_int32, [_P, C.POINTER(sgr_stats)]),
     ("sgr_set_option", C.c_int32, [_P, C.c_char_p, C.c_int64]),
     ("sgr_stream", C.c_int32, [_P, C.POINTER(_P)]),
+    ("sgr_probe_read", C.c_int32, [_P, C.c_uint64, C.c_int32, C.c_uint64, _P, _P]),
     ("sgr_dist_unique_id", C.c_int32, [_P]),
     ("sgr_dist_init", C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_uint64]),
     ("sgr_dist_set_partitions", C.c_int32, [_P, _P, C.c_uint64]),
