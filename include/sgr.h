@@ -655,6 +655,54 @@ int32_t sgr_dingest_reset(sgr_dingest* g);
 int32_t sgr_dingest_last_timing(sgr_dingest* g, float* ms8);
 int32_t sgr_dingest_get_stats(sgr_dingest* g, sgr_ingest_stats* out);
 
+/* ------------------------------------------------------------------ state values: rows written as the model's JSON state
+ * The store's reads and the records a republish produces are the model's serialized state (getAggregateBytes; the state topic's
+ * value, aggregateWriteFormatting.writeState, SurgeModel.scala:57-65). With a writer table the engine writes that value on the
+ * device, as Json.toJson(state) writes a case class of flat members: {"name":value,...}, members in table order, no whitespace
+ * (csrc/state_writer.h; restatement oracle/state_json.py):
+ *   SGR_JSON_I32 / _I64  plain decimal;  SGR_JSON_UUID  8-4-4-4-12 lowercase hex, most significant byte first;
+ *   SGR_JSON_PSTR        a string of the slot's first length-byte bytes (padding ignored);
+ *   SGR_JSON_F64         the shortest decimal that rounds back to the double (Python's repr digits, Double.toString's from
+ *                        JDK 19 on), trailing zeros stripped, plain for 1e-10 <= |v| <= 1e20, else BigDecimal.toString's
+ *                        scientific form (1.5E+21, 1E-11); 0.0 and -0.0 are 0;
+ *   SGR_JSON_ID          (writer tables only) the row's aggregate id; dst_off and len are ignored.
+ * Strings escape '"', '\\' and \b \t \n \f \r by their short forms and other characters below U+0020 as \u00XX (uppercase hex);
+ * every other byte is written as it is. Every value parses back to its row through the state-topic restore (JSON members,
+ * sgr_dingest_set_state_topic) and through any JSON parser, doubles equal by == (so -0.0 comes back as 0.0). The exact bytes
+ * play-json writes are NOT pinned (no JVM here): member order, integers, UUIDs and escaping follow a restatement, the digits
+ * of doubles are repr's, their layout is our reading of play-json's serializer.
+ * A row cannot be written, and the JVM's writeState throws too, when an F64 member holds NaN or an infinity, a PSTR length byte
+ * exceeds len - 1 or its bytes are not well-formed UTF-8, or (ID member) the id is not well-formed UTF-8 or the row has no id in
+ * the key table. */
+#define SGR_JSON_ID 5u
+/* Register the writer table: members in value order, at most 32. Each non-ID member needs dst_off % 4 == 0, a size (I32 4,
+ * I64 / F64 8, UUID 16, PSTR len) that is a multiple of 4 and at least 4, and dst_off + size <= state_bytes - 8, as a state
+ * topic's JSON member table does; at most one SGR_JSON_ID member; names non-empty, well-formed UTF-8 and distinct. The restore's
+ * table for the same values is this table without its ID member. n_members == 0 clears the writer. SGR_ERR_NO_PROGRAM before
+ * sgr_register_program, and a later sgr_register_program clears the writer; SGR_ERR_INVALID on a bad table (nothing changes);
+ * SGR_ERR_UNSUPPORTED on a routed engine (sgr_dist_init). */
+int32_t sgr_set_state_writer(sgr_engine* e, const sgr_json_field* members, uint32_t n_members);
+/* Three reads that return values instead of rows. Each matches its twin (sgr_get_batch, sgr_export_changes, sgr_scan) in
+ * locking, table generation, id-index update, paging, cursor / token and error codes, with the rows replaced by values
+ * (values_cap bytes) and value_offsets (rows + 1 u64): row i's value is values[value_offsets[i] .. value_offsets[i + 1]). A
+ * None row (no SGR_ST_EXISTS in flags; in an export, the tombstone: the (id, null) record) has an empty span. flags is required.
+ * SGR_ERR_STATE when no writer is set. A row that cannot be written fails the call with SGR_ERR_UNSUPPORTED and nothing written
+ * (for a page, the cursor unchanged); the message names the lowest such row (its position in the batch or page and its dense
+ * index), the member and the reason.
+ * sgr_get_batch_values: all or nothing; an unknown id has an empty span, flags 0 and index -1. SGR_ERR_CAPACITY (nothing
+ * written but *values_len, optional, = the bytes needed) when the values need more than values_cap bytes.
+ * sgr_export_changes_values / sgr_scan_values: a page also ends before the first selected row whose value does not fit in
+ * what is left of values_cap (cur->next names that row; *more is 1); SGR_ERR_CAPACITY (nothing written, the cursor unchanged)
+ * when the first row's value alone does not fit. */
+int32_t sgr_get_batch_values(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n, uint8_t* values, uint64_t values_cap,
+                             uint64_t* value_offsets, uint32_t* flags, int64_t* indices, uint64_t* values_len);
+int32_t sgr_export_changes_values(sgr_engine* e, uint32_t select, sgr_changes_cursor* cur, uint64_t max_rows, uint8_t* values,
+                                  uint64_t values_cap, uint64_t* value_offsets, uint32_t* flags, uint32_t* err_idx, int64_t* indices,
+                                  uint8_t* ids, uint64_t ids_cap, uint32_t* id_offsets, uint64_t* n_rows);
+int32_t sgr_scan_values(sgr_engine* e, const uint8_t* from, uint32_t from_len, int32_t from_exclusive, const uint8_t* to, uint32_t to_len,
+                        uint64_t max_rows, uint8_t* values, uint64_t values_cap, uint64_t* value_offsets, uint32_t* flags, int64_t* indices,
+                        uint8_t* ids, uint64_t ids_cap, uint32_t* id_offsets, uint64_t* n_rows, int32_t* more);
+
 /* building blocks, exported for the known-answer tests */
 uint32_t sgr_crc32c(const void* data, uint64_t nbytes);            /* RFC 3720 CRC-32C (SSE4.2 when present) */
 uint32_t sgr_crc32c_portable(const void* data, uint64_t nbytes);   /* table-driven twin */

@@ -173,6 +173,104 @@ JNIEXPORT jlong JNICALL Java_surge_gpu_Native_00024_scan(JNIEnv* env, jobject o,
   if (rc != SGR_OK) { throw_for(env, H(h), rc); return -1; }
   return (jlong)(2 * n + (more ? 1 : 0));
 }
+/* sgr_set_state_writer. table: a direct buffer of tableBytes bytes, per member (little endian) u32 kind (SGR_JSON_*), u32 program
+ * byte offset, u32 PSTR slot bytes, u32 name length, then the name's UTF-8 bytes; nMembers == 0 clears the writer. */
+JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_setStateWriter(JNIEnv* env, jobject o, jlong h, jobject table, jlong table_bytes, jint n_members) {
+  int ok = 1;
+  if (n_members < 0 || n_members > 32 || table_bytes < 0) return bad_arg(env, "nMembers: 0 to 32 members");
+  const uint8_t* t = n_members ? (const uint8_t*)direct(env, table, table_bytes, "table: direct buffer shorter than tableBytes", &ok) : 0;
+  if (!ok) return SGR_ERR_INVALID;
+  sgr_json_field f[32];
+  char name_buf[32][256];
+  jlong at = 0;
+  for (jint i = 0; i < n_members; ++i) {
+    uint32_t w[4];
+    if (table_bytes - at < 16) return bad_arg(env, "table: a member runs past tableBytes");
+    memcpy(w, t + at, 16);
+    at += 16;
+    if (w[0] > 255 || w[1] > 0xffff || w[3] > 255 || (jlong)w[3] > table_bytes - at) return bad_arg(env, "table: kind, offset or name length out of range");
+    memcpy(name_buf[i], t + at, w[3]);
+    name_buf[i][w[3]] = 0;
+    at += w[3];
+    if (strlen(name_buf[i]) != w[3]) return bad_arg(env, "table: a name holds a NUL byte");
+    memset(&f[i], 0, sizeof f[i]);
+    f[i].name = name_buf[i]; f[i].kind = (uint8_t)w[0]; f[i].dst_off = (uint16_t)w[1]; f[i].len = w[2];
+  }
+  int32_t rc = sgr_set_state_writer(H(h), f, (uint32_t)n_members);
+  if (rc != SGR_OK) throw_for(env, H(h), rc);
+  return rc;
+}
+/* One sgr_get_batch_values. keys / keyOffsets as for getBatch; values: a direct buffer whose capacity is the byte budget;
+ * valueOffsets: n + 1 u64; flags: n u32. Returns the value bytes written, or -(bytes needed) when values is too small (nothing
+ * written); throws on every other failure (a row the writer refuses, no writer: InvalidStateStoreException). */
+JNIEXPORT jlong JNICALL Java_surge_gpu_Native_00024_getBatchValues(JNIEnv* env, jobject o, jlong h, jobject keys, jobject offs, jlong n, jobject values,
+                                                                   jobject value_offsets, jobject flags) {
+  int ok = 1;
+  if (n < 0 || n > INT64_MAX / 16) { bad_arg(env, "n must be non-negative"); return 0; }
+  const uint32_t* ko = (const uint32_t*)direct(env, offs, (n + 1) * 4, "keyOffsets: direct buffer of (n + 1) u32", &ok);
+  if (!ok) return 0;
+  const uint8_t* k = ko[n] ? (const uint8_t*)direct(env, keys, (jlong)ko[n], "keys: direct buffer shorter than keyOffsets[n]", &ok) : 0;
+  uint64_t* vo = ok ? (uint64_t*)direct(env, value_offsets, (n + 1) * 8, "valueOffsets: direct buffer of (n + 1) u64", &ok) : 0;
+  uint32_t* fl = ok ? (uint32_t*)direct(env, flags, n * 4, "flags: direct buffer of n u32", &ok) : 0;
+  uint8_t* v = ok ? (uint8_t*)direct(env, values, 0, "values: direct buffer", &ok) : 0;
+  if (!ok) return 0;
+  uint64_t need = 0;
+  int32_t rc = sgr_get_batch_values(H(h), k, ko, (uint64_t)n, v, (uint64_t)(*env)->GetDirectBufferCapacity(env, values), vo, fl, 0, &need);
+  if (rc == SGR_ERR_CAPACITY) return -(jlong)need;
+  if (rc != SGR_OK) { throw_for(env, H(h), rc); return 0; }
+  return (jlong)need;
+}
+/* One page of sgr_export_changes_values: as exportChanges, with values (a direct buffer whose capacity is the page's value-byte
+ * budget) and valueOffsets (maxRows + 1 u64) in place of rows. Returns the rows written, or -1 after throwing. */
+JNIEXPORT jlong JNICALL Java_surge_gpu_Native_00024_exportChangesValues(JNIEnv* env, jobject o, jlong h, jint select, jobject cursor, jlong max_rows,
+                                                                        jobject values, jobject value_offsets, jobject flags, jobject err_idx,
+                                                                        jobject indices, jobject ids, jobject id_offsets) {
+  int ok = 1;
+  if (max_rows <= 0 || max_rows > INT64_MAX / 16) { bad_arg(env, "maxRows must be positive"); return -1; }
+  sgr_changes_cursor* cur = (sgr_changes_cursor*)direct(env, cursor, (jlong)sizeof(sgr_changes_cursor), "cursor: direct buffer of 4 u64", &ok);
+  uint8_t* v = ok ? (uint8_t*)direct(env, values, 1, "values: direct buffer", &ok) : 0;
+  uint64_t* vo = ok ? (uint64_t*)direct(env, value_offsets, (max_rows + 1) * 8, "valueOffsets: direct buffer of maxRows + 1 u64", &ok) : 0;
+  uint32_t* fl = ok ? (uint32_t*)direct(env, flags, max_rows * 4, "flags: direct buffer of maxRows u32", &ok) : 0;
+  uint32_t* er = ok ? (uint32_t*)direct(env, err_idx, max_rows * 4, "errIdx: direct buffer of maxRows u32", &ok) : 0;
+  int64_t* ix = ok ? (int64_t*)direct(env, indices, max_rows * 8, "indices: direct buffer of maxRows i64", &ok) : 0;
+  uint32_t* io = ok ? (uint32_t*)direct(env, id_offsets, (max_rows + 1) * 4, "idOffsets: direct buffer of maxRows + 1 u32", &ok) : 0;
+  uint8_t* id = ok ? (uint8_t*)direct(env, ids, 1, "ids: direct buffer", &ok) : 0;
+  if (!ok) return -1;
+  uint64_t n = 0;
+  int32_t rc = sgr_export_changes_values(H(h), (uint32_t)select, cur, (uint64_t)max_rows, v, (uint64_t)(*env)->GetDirectBufferCapacity(env, values), vo,
+                                         fl, er, ix, id, (uint64_t)(*env)->GetDirectBufferCapacity(env, ids), io, &n);
+  if (rc != SGR_OK) { throw_for(env, H(h), rc); return -1; }
+  return (jlong)n;
+}
+/* One page of sgr_scan_values: as scan, with values and valueOffsets (maxRows + 1 u64) in place of rows. Returns 2 * (rows
+ * written) + 1 when a live row in range was left out of the page (+ 0 when the scan is complete), or -1 after throwing. */
+JNIEXPORT jlong JNICALL Java_surge_gpu_Native_00024_scanValues(JNIEnv* env, jobject o, jlong h, jbyteArray from, jboolean from_exclusive, jbyteArray to,
+                                                               jlong max_rows, jobject values, jobject value_offsets, jobject flags, jobject indices,
+                                                               jobject ids, jobject id_offsets) {
+  static const uint8_t empty = 0;
+  int ok = 1;
+  if (max_rows <= 0 || max_rows > INT64_MAX / 16) { bad_arg(env, "maxRows must be positive"); return -1; }
+  uint8_t* v = (uint8_t*)direct(env, values, 1, "values: direct buffer", &ok);
+  uint64_t* vo = ok ? (uint64_t*)direct(env, value_offsets, (max_rows + 1) * 8, "valueOffsets: direct buffer of maxRows + 1 u64", &ok) : 0;
+  uint32_t* fl = ok ? (uint32_t*)direct(env, flags, max_rows * 4, "flags: direct buffer of maxRows u32", &ok) : 0;
+  int64_t* ix = ok ? (int64_t*)direct(env, indices, max_rows * 8, "indices: direct buffer of maxRows i64", &ok) : 0;
+  uint32_t* io = ok ? (uint32_t*)direct(env, id_offsets, (max_rows + 1) * 4, "idOffsets: direct buffer of maxRows + 1 u32", &ok) : 0;
+  uint8_t* id = ok ? (uint8_t*)direct(env, ids, 1, "ids: direct buffer", &ok) : 0;
+  if (!ok) return -1;
+  const jsize from_len = from ? (*env)->GetArrayLength(env, from) : 0, to_len = to ? (*env)->GetArrayLength(env, to) : 0;
+  jbyte* f = from ? (*env)->GetByteArrayElements(env, from, 0) : 0;
+  jbyte* t = to ? (*env)->GetByteArrayElements(env, to, 0) : 0;
+  uint64_t n = 0;
+  int32_t more = 0;
+  int32_t rc = sgr_scan_values(H(h), from ? (f ? (const uint8_t*)f : &empty) : 0, (uint32_t)from_len, from_exclusive ? 1 : 0,
+                               to ? (t ? (const uint8_t*)t : &empty) : 0, (uint32_t)to_len, (uint64_t)max_rows, v,
+                               (uint64_t)(*env)->GetDirectBufferCapacity(env, values), vo, fl, ix, id, (uint64_t)(*env)->GetDirectBufferCapacity(env, ids),
+                               io, &n, &more);
+  if (f) (*env)->ReleaseByteArrayElements(env, from, f, JNI_ABORT);
+  if (t) (*env)->ReleaseByteArrayElements(env, to, t, JNI_ABORT);
+  if (rc != SGR_OK) { throw_for(env, H(h), rc); return -1; }
+  return (jlong)(2 * n + (more ? 1 : 0));
+}
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_exportStates(JNIEnv* env, jobject o, jlong h, jobject out, jobject changed) {
   return sgr_export_states(H(h), (*env)->GetDirectBufferAddress(env, out), (uint64_t)(*env)->GetDirectBufferCapacity(env, out), 0,
                            changed ? (uint8_t*)(*env)->GetDirectBufferAddress(env, changed) : 0, 0);

@@ -65,7 +65,10 @@ trait GpuStateCodec {
 object GpuFoldPrograms {
   /** snapshotType / tombstoneType of a registration without snapshot rules */
   final val NoSnapshotRules = -1
-  final case class Registration(program: ByteBuffer, codec: GpuStateCodec, snapshotType: Int, tombstoneType: Int) {
+  /** one member of a JSON state writer table (sgr_set_state_writer): kind SGR_JSON_* (0 I32, 1 I64, 2 F64, 3 UUID, 4 PSTR, 5 the
+   *  aggregate id), program byte offset, PSTR slot bytes */
+  final case class WriterMember(name: String, kind: Int, offset: Int = 0, len: Int = 0)
+  final case class Registration(program: ByteBuffer, codec: GpuStateCodec, snapshotType: Int, tombstoneType: Int, writer: Seq[WriterMember] = Nil) {
     /** no snapshot rules: the store takes records of the STATE topic only, applied on the device by sgr_put_batch */
     def stateTopic: Boolean = snapshotType == NoSnapshotRules
   }
@@ -82,6 +85,13 @@ object GpuFoldPrograms {
   /** a state-topic store: no snapshot rules, states of any width the engine folds */
   def register(packedSgrFoldProgram: ByteBuffer, codec: GpuStateCodec): Unit =
     register(packedSgrFoldProgram, codec, NoSnapshotRules, NoSnapshotRules)
+  /** a state-topic store whose reads, iterators and onChanges take the model's JSON state from the device writer: the codec's
+   *  fromPacked is not called (its toPacked still packs what put() receives) */
+  def register(packedSgrFoldProgram: ByteBuffer, codec: GpuStateCodec, writer: Seq[WriterMember]): Unit = {
+    require(writer.nonEmpty && writer.size <= 32, "a writer table holds 1 to 32 members")
+    register(packedSgrFoldProgram, codec, NoSnapshotRules, NoSnapshotRules)
+    registration = registration.map(_.copy(writer = writer))
+  }
   def current: Registration = registration.getOrElse(throw new IllegalStateException("no GPU fold program registered for this model"))
 }
 
@@ -142,6 +152,16 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
   override def init(context: ProcessorContext, root: StateStore): Unit = {
     handle = Native.create(0) // throws when there is no usable GPU: no CPU fallback, the stream thread dies loudly
     check(Native.registerProgram(handle, reg.program))
+    if (reg.writer.nonEmpty) {
+      val t = new java.io.ByteArrayOutputStream()
+      reg.writer.foreach { m =>
+        val name = m.name.getBytes("UTF-8")
+        t.write(ByteBuffer.allocate(16).order(ByteOrder.LITTLE_ENDIAN).putInt(m.kind).putInt(m.offset).putInt(m.len).putInt(name.length).array())
+        t.write(name)
+      }
+      val tb = ByteBuffer.allocateDirect(math.max(t.size(), 1)); tb.put(t.toByteArray); tb.flip()
+      check(Native.setStateWriter(handle, tb, t.size().toLong, reg.writer.size))
+    }
     // The restore callback exists for stores with a changelog (SingleExceptionThrowingKeyValueStore.scala:84-86). This store has
     // none (enableLogging = false), so Kafka Streams never calls it; it is registered because StateStore.init must register the
     // root store, and it does the right thing if a future topology does restore through it.
@@ -260,15 +280,19 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
     val ids = ByteBuffer.allocateDirect(4 << 20)
     val changed = scala.collection.mutable.ArrayBuffer[(String, Array[Byte])]()
     val failed = scala.collection.mutable.ArrayBuffer[(String, Int)]()
+    val values = if (writes) ByteBuffer.allocateDirect(16 << 20) else null
+    val valueOffsets = if (writes) ByteBuffer.allocateDirect(8 * (pageRows + 1)).order(ByteOrder.LITTLE_ENDIAN) else null
     do {
-      val n = Native.exportChanges(handle, 2 | 4, cursor, pageRows.toLong, rows, flags, errs, indices, ids, idOffsets).toInt // CHANGED | ERROR
+      val n = (if (writes) Native.exportChangesValues(handle, 2 | 4, cursor, pageRows.toLong, values, valueOffsets, flags, errs, indices, ids, idOffsets)
+               else Native.exportChanges(handle, 2 | 4, cursor, pageRows.toLong, rows, flags, errs, indices, ids, idOffsets)).toInt // CHANGED | ERROR
       var i = 0
       while (i < n) {
         val slot = indices.getLong(8 * i)
         if (slot < keys.size()) { // the key table is this store's ids in slot order
           val id = keys.get(slot.toInt)
           val fl = flags.getInt(4 * i)
-          if ((fl & 2) != 0) changed += id -> (if ((fl & 1) != 0) {
+          if ((fl & 2) != 0) changed += id -> (if ((fl & 1) != 0 && writes) valueAt(values, valueOffsets, i)
+          else if ((fl & 1) != 0) {
             val packed = new Array[Byte](user)
             rows.position(i * user); rows.get(packed)
             reg.codec.fromPacked(id, packed)
@@ -279,6 +303,17 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
       }
     } while (cursor.getLong(0) < capacity) // next == n_agg: the export is complete
     listener(changed.toSeq, failed.toSeq)
+  }
+
+  /** with a writer table the device writes the model's JSON state (sgr_*_values) and fromPacked is not called */
+  private def writes: Boolean = reg.writer.nonEmpty
+
+  /** value i of a page of JSON values (u64 offsets) */
+  private def valueAt(values: ByteBuffer, valueOffsets: ByteBuffer, i: Int): Array[Byte] = {
+    val lo = valueOffsets.getLong(8 * i).toInt; val hi = valueOffsets.getLong(8 * (i + 1)).toInt
+    val v = new Array[Byte](hi - lo)
+    values.position(lo); values.get(v)
+    v
   }
 
   /** Make room for the keys seen so far: the table is resized on the device, content kept, new slots None (sgr_grow_states). */
@@ -314,6 +349,7 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
     val u = unflushed.get(id)
     if (u != null) return u.map(_.clone()).orNull
     if (!folded) return null // nothing was ever put: an empty table, not an error (KTable miss)
+    if (writes) return getBatch(Seq(key)).head
     val packed = Native.get(handle, key.get()) // null == None; InvalidStateStoreException while the table is being rebuilt
     if (packed == null) null else reg.codec.fromPacked(id, packed)
   }
@@ -335,8 +371,16 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
       offs.putInt(0)
       rest.foreach { i => blob.write(batch(i).get()); offs.putInt(blob.size()) }
       val kb = ByteBuffer.allocateDirect(math.max(blob.size(), 1)); kb.put(blob.toByteArray); kb.flip(); offs.flip()
-      val rows = ByteBuffer.allocateDirect(user * rest.size)
       val flags = ByteBuffer.allocateDirect(4 * rest.size).order(ByteOrder.LITTLE_ENDIAN)
+      if (writes) {
+        val valueOffsets = ByteBuffer.allocateDirect(8 * (rest.size + 1)).order(ByteOrder.LITTLE_ENDIAN)
+        var values = ByteBuffer.allocateDirect(64 * rest.size + 64)
+        var r = Native.getBatchValues(handle, kb, offs, rest.size.toLong, values, valueOffsets, flags)
+        if (r < 0) { values = ByteBuffer.allocateDirect((-r).toInt); r = Native.getBatchValues(handle, kb, offs, rest.size.toLong, values, valueOffsets, flags) }
+        rest.zipWithIndex.foreach { case (i, j) => if ((flags.getInt(4 * j) & 1) != 0) out(i) = valueAt(values, valueOffsets, j) }
+        return out.toSeq
+      }
+      val rows = ByteBuffer.allocateDirect(user * rest.size)
       check(Native.getBatch(handle, kb, offs, rest.size.toLong, rows, flags))
       rest.zipWithIndex.foreach { case (i, r) =>
         if ((flags.getInt(4 * r) & 1) != 0) { // SGR_ST_EXISTS
@@ -373,6 +417,8 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
       private val indices = ByteBuffer.allocateDirect(8 * pageRows).order(ByteOrder.LITTLE_ENDIAN)
       private val idOffsets = ByteBuffer.allocateDirect(4 * (pageRows + 1)).order(ByteOrder.LITTLE_ENDIAN)
       private val ids = ByteBuffer.allocateDirect(1 << 20)
+      private val values = if (writes) ByteBuffer.allocateDirect(4 << 20) else null
+      private val valueOffsets = if (writes) ByteBuffer.allocateDirect(8 * (pageRows + 1)).order(ByteOrder.LITTLE_ENDIAN) else null
       private val toBytes = if (to == null) null else to.get()
       private var resume: Array[Byte] = if (from == null) null else from.get()
       private var resumeExclusive = false
@@ -385,7 +431,8 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
 
       private def fillPage(): Unit = while (d >= pageKeys.size && deviceMore) {
         pageKeys.clear(); pageValues.clear(); d = 0
-        val r = Native.scan(handle, resume, resumeExclusive, toBytes, pageRows.toLong, rows, flags, indices, ids, idOffsets)
+        val r = if (writes) Native.scanValues(handle, resume, resumeExclusive, toBytes, pageRows.toLong, values, valueOffsets, flags, indices, ids, idOffsets)
+                else Native.scan(handle, resume, resumeExclusive, toBytes, pageRows.toLong, rows, flags, indices, ids, idOffsets)
         val n = (r >> 1).toInt
         deviceMore = (r & 1) != 0
         var i = 0
@@ -394,9 +441,11 @@ class GpuReplayKeyValueStore(storeName: String, onChanges: Option[(Seq[(String, 
           val idBytes = new Array[Byte](hi - lo)
           ids.position(lo); ids.get(idBytes)
           if (indices.getLong(8 * i) < nIds) { // spare capacity slots are not this store's ids
-            val packed = new Array[Byte](user)
-            rows.position(i * user); rows.get(packed)
-            val value = reg.codec.fromPacked(new String(idBytes, "UTF-8"), packed)
+            val value = if (writes) valueAt(values, valueOffsets, i) else {
+              val packed = new Array[Byte](user)
+              rows.position(i * user); rows.get(packed)
+              reg.codec.fromPacked(new String(idBytes, "UTF-8"), packed)
+            }
             if (value != null) { pageKeys += Bytes.wrap(idBytes); pageValues += value } // a null value is skipped, as get() => null was
           }
           if (i == n - 1) { resume = idBytes; resumeExclusive = true }

@@ -44,6 +44,19 @@ object Native {
    * was left out (continue from the page's last id, exclusive), + 0 when the scan is complete */
   @native def scan(handle: Long, from: Array[Byte], fromExclusive: Boolean, to: Array[Byte], maxRows: Long, rows: ByteBuffer, flags: ByteBuffer,
                    indices: ByteBuffer, ids: ByteBuffer, idOffsets: ByteBuffer): Long // sgr_scan
+  /** the JSON state writer (sgr_set_state_writer): per member (little endian) u32 SGR_JSON_* kind (5 = the aggregate id), u32
+   *  program byte offset, u32 PSTR slot bytes, u32 name length, the UTF-8 name; nMembers == 0 clears it */
+  @native def setStateWriter(handle: Long, table: ByteBuffer, tableBytes: Long, nMembers: Int): Int // sgr_set_state_writer
+  /** getBatch with JSON values: value i = values[valueOffsets(i) until valueOffsets(i+1)] (u64 offsets), empty for None / unknown
+   *  ids; returns the value bytes written, or -(bytes needed) when values is too small */
+  @native def getBatchValues(handle: Long, keys: ByteBuffer, keyOffsets: ByteBuffer, n: Long, values: ByteBuffer, valueOffsets: ByteBuffer,
+                             flags: ByteBuffer): Long // sgr_get_batch_values
+  /** exportChanges with JSON values in place of rows; the values buffer's capacity is the page's value-byte budget */
+  @native def exportChangesValues(handle: Long, select: Int, cursor: ByteBuffer, maxRows: Long, values: ByteBuffer, valueOffsets: ByteBuffer,
+                                  flags: ByteBuffer, errIdx: ByteBuffer, indices: ByteBuffer, ids: ByteBuffer, idOffsets: ByteBuffer): Long // sgr_export_changes_values
+  /** scan with JSON values in place of rows */
+  @native def scanValues(handle: Long, from: Array[Byte], fromExclusive: Boolean, to: Array[Byte], maxRows: Long, values: ByteBuffer,
+                         valueOffsets: ByteBuffer, flags: ByteBuffer, indices: ByteBuffer, ids: ByteBuffer, idOffsets: ByteBuffer): Long // sgr_scan_values
   @native def partitionForKey(key: Array[Byte], numPartitions: Int, upToColon: Boolean): Int // sgr_partition_for_key_utf8
 
   // raw record batches in, committed offsets out (include/sgr.h "ingest")

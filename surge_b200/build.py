@@ -17,7 +17,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libsgr.so")
 OBJ_DIR = os.path.join(HERE, "build")
 
-SOURCES = ["engine.cu", "fold_kernels.cu", "fold_rows.cu", "fold_runs.cu", "fold_vruns.cu", "group_kernels.cu", "incremental.cu", "bulk_fold.cu", "dist.cu", "route_push.cu", "dingest_kernels.cu", "dingest.cu", "id_index.cu", "id_order.cu", "changes.cu", "put_batch.cu", "partitioner.cpp", "ingest.cpp"]
+SOURCES = ["engine.cu", "fold_kernels.cu", "fold_rows.cu", "fold_runs.cu", "fold_vruns.cu", "group_kernels.cu", "incremental.cu", "bulk_fold.cu", "dist.cu", "route_push.cu", "dingest_kernels.cu", "dingest.cu", "id_index.cu", "id_order.cu", "changes.cu", "put_batch.cu", "state_values.cu", "partitioner.cpp", "ingest.cpp"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-Wall", "-Xptxas", "-v"]
 

@@ -325,6 +325,103 @@ class ReplayEngine:
             if not more.value:
                 return
 
+    # -- JSON state values (sgr_set_state_writer)
+    def set_state_writer(self, members) -> None:
+        """Register the table the value-returning reads write rows with: members in value order, each (name, N.JSON_*, program
+        byte offset[, slot bytes for JSON_PSTR]) or (name, N.JSON_ID) for the aggregate id. An empty table clears the writer."""
+        arr = (N.sgr_json_field * max(len(members), 1))()
+        names = [m[0].encode("utf-8") for m in members]
+        for i, m in enumerate(members):
+            arr[i].name = names[i]
+            arr[i].kind = m[1]
+            if m[1] != N.JSON_ID:
+                arr[i].dst_off = m[2]
+                arr[i].len = m[3] if len(m) > 3 else 0
+        self._ck(self._lib.sgr_set_state_writer(self._h, arr, len(members)))
+
+    @staticmethod
+    def _split_values(buf: np.ndarray, offs: np.ndarray, n: int) -> List[Optional[bytes]]:
+        raw = buf[:int(offs[n])].tobytes() if n else b""
+        return [raw[offs[i]:offs[i + 1]] if offs[i + 1] > offs[i] else None for i in range(n)]
+
+    def get_many_values(self, keys: Sequence[str], values_cap: Optional[int] = None) -> List[Optional[bytes]]:
+        """The JSON state value of each id (sgr_get_batch_values), None for a None state or an unknown id. values_cap: the byte
+        budget of one call (None: sized from the first attempt)."""
+        enc = [k.encode("utf-8") for k in keys]
+        n = len(enc)
+        offs = np.zeros(n + 1, dtype=np.uint32)
+        np.cumsum([len(b) for b in enc], out=offs[1:])
+        blob = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8)
+        flags = np.zeros(max(n, 1), dtype=np.uint32)
+        voffs = np.zeros(n + 1, dtype=np.uint64)
+        need = C.c_uint64()
+        cap = int(values_cap) if values_cap is not None else 64 * n + 64
+        while True:
+            buf = np.empty(max(cap, 1), dtype=np.uint8)
+            rc = self._lib.sgr_get_batch_values(self._h, blob.ctypes.data, offs.ctypes.data, n, buf.ctypes.data, cap, voffs.ctypes.data,
+                                                flags.ctypes.data, None, C.byref(need))
+            if rc == N.SGR_ERR_CAPACITY and values_cap is None:
+                cap = int(need.value)
+                continue
+            self._ck(rc)
+            return self._split_values(buf, voffs, n)
+
+    def export_changes_values(self, select: int = N.ST_CHANGED, max_rows: Optional[int] = 1 << 20, values_cap: int = 64 << 20,
+                              page_id_bytes: int = 64 << 20) -> Iterator[Tuple[np.ndarray, np.ndarray, np.ndarray, List[Optional[str]], List[Optional[bytes]]]]:
+        """export_changes with JSON values in place of rows (sgr_export_changes_values). Yields pages of (indices i64[n], flags
+        u32[n], err_idx u32[n], ids, values): values[i] is the row's JSON state, or None for a None state (the tombstone: the
+        (id, null) record of a republish). A page also ends before a value that does not fit in values_cap bytes."""
+        n_agg = self.n_aggregates()
+        cap = max(1, n_agg if max_rows is None else min(int(max_rows), max(n_agg, 1)))
+        cur = N.sgr_changes_cursor()
+        n = C.c_uint64()
+        while True:
+            buf = np.empty(max(int(values_cap), 1), dtype=np.uint8)
+            voffs = np.empty(cap + 1, dtype=np.uint64)
+            flags, err = np.empty(cap, dtype=np.uint32), np.empty(cap, dtype=np.uint32)
+            idx = np.empty(cap, dtype=np.int64)
+            offs = np.empty(cap + 1, dtype=np.uint32)
+            blob = np.empty(max(int(page_id_bytes), 1), dtype=np.uint8)
+            self._ck(self._lib.sgr_export_changes_values(self._h, int(select), C.byref(cur), cap, buf.ctypes.data, int(values_cap), voffs.ctypes.data,
+                                                         flags.ctypes.data, err.ctypes.data, idx.ctypes.data, blob.ctypes.data, int(page_id_bytes),
+                                                         offs.ctypes.data, C.byref(n)))
+            k, n_keys = int(n.value), int(cur.n_keys)
+            raw = blob[:int(offs[k])].tobytes() if k else b""
+            ids = [raw[offs[i]:offs[i + 1]].decode("utf-8") if idx[i] < n_keys else None for i in range(k)]
+            if k:
+                yield idx[:k], flags[:k], err[:k], ids, self._split_values(buf, voffs, k)
+            if cur.next >= n_agg:
+                return
+
+    def scan_values(self, frm: Optional[str] = None, to: Optional[str] = None, max_rows: int = 1 << 20, values_cap: int = 64 << 20,
+                    page_id_bytes: int = 64 << 20) -> Iterator[Tuple[np.ndarray, np.ndarray, List[str], List[bytes]]]:
+        """scan with JSON values in place of rows (sgr_scan_values). Yields pages of (indices i64[n], flags u32[n], ids, values)."""
+        n_agg = self.n_aggregates()
+        cap = max(1, min(int(max_rows), max(n_agg, 1)))
+        lo = None if frm is None else frm.encode("utf-8")
+        hi = None if to is None else to.encode("utf-8")
+        hi_buf = None if hi is None else C.create_string_buffer(hi, max(len(hi), 1))
+        exclusive = 0
+        n, more = C.c_uint64(), C.c_int32()
+        while True:
+            buf = np.empty(max(int(values_cap), 1), dtype=np.uint8)
+            voffs = np.empty(cap + 1, dtype=np.uint64)
+            flags = np.empty(cap, dtype=np.uint32)
+            idx = np.empty(cap, dtype=np.int64)
+            offs = np.empty(cap + 1, dtype=np.uint32)
+            blob = np.empty(max(int(page_id_bytes), 1), dtype=np.uint8)
+            lo_buf = None if lo is None else C.create_string_buffer(lo, max(len(lo), 1))
+            self._ck(self._lib.sgr_scan_values(self._h, lo_buf, 0 if lo is None else len(lo), exclusive, hi_buf, 0 if hi is None else len(hi), cap,
+                                               buf.ctypes.data, int(values_cap), voffs.ctypes.data, flags.ctypes.data, idx.ctypes.data,
+                                               blob.ctypes.data, int(page_id_bytes), offs.ctypes.data, C.byref(n), C.byref(more)))
+            k = int(n.value)
+            if k:
+                raw = blob[:int(offs[k])].tobytes()
+                yield idx[:k], flags[:k], [raw[offs[i]:offs[i + 1]].decode("utf-8") for i in range(k)], self._split_values(buf, voffs, k)
+                lo, exclusive = raw[offs[k - 1]:offs[k]], 1
+            if not more.value:
+                return
+
     def get_index(self, agg: int) -> Tuple[Optional[bytes], int, int]:
         """(program bytes or None, flags, err_idx) of one dense aggregate index."""
         buf = C.create_string_buffer(N.MAX_STATE_BYTES)

@@ -117,13 +117,19 @@ class StateCodec:
     """serialized state bytes (what the state topic and the actors hold) <-> the packed program bytes of the GPU table
     (trait GpuStateCodec of shim/scala GpuReplayPersistencePlugin.scala). snapshot_type / tombstone_type are the two extra rules of
     the registered fold program (programs.counter_program_with_snapshot_rules); a codec without them (both None) makes the store
-    a state-topic store, whose state records go to the table through sgr_put_batch (no extra rules, states of any width)."""
+    a state-topic store, whose state records go to the table through sgr_put_batch (no extra rules, states of any width).
+    writer: a JSON state writer table for ReplayEngine.set_state_writer, [(name, N.JSON_*, program offset[, slot bytes])] or
+    (name, N.JSON_ID): the store's reads and on_changes then take the model's JSON value from the device (sgr_get_batch_values,
+    sgr_scan_values, sgr_export_changes_values) instead of calling from_packed, which becomes optional."""
 
-    def __init__(self, to_packed: Callable[[str, bytes], bytes], from_packed: Callable[[str, bytes], bytes], snapshot_type: Optional[int] = None,
-                 tombstone_type: Optional[int] = None):
+    def __init__(self, to_packed: Callable[[str, bytes], bytes], from_packed: Optional[Callable[[str, bytes], bytes]] = None,
+                 snapshot_type: Optional[int] = None, tombstone_type: Optional[int] = None, writer: Optional[Sequence[Tuple]] = None):
         if (snapshot_type is None) != (tombstone_type is None):
             raise ValueError("a codec names both the snapshot and the tombstone type, or neither")
+        if from_packed is None and writer is None:
+            raise ValueError("a codec decodes rows with from_packed, or has the device write them with a writer table")
         self.to_packed, self.from_packed, self.snapshot_type, self.tombstone_type = to_packed, from_packed, snapshot_type, tombstone_type
+        self.writer = None if writer is None else list(writer)
 
     @property
     def state_topic(self) -> bool:
@@ -165,6 +171,10 @@ class GpuReplayKeyValueStore:
         self._unflushed: Dict[str, Optional[bytes]] = {}
         self._engine = ReplayEngine(device)
         self._engine.register_program(program)
+        # with a writer table, values leave the device as the model's JSON state and the host codec is not called
+        self._writer = codec is not None and codec.writer is not None
+        if self._writer:
+            self._engine.set_state_writer(codec.writer)
         self._formatter = state_formatter
         self._keys: List[str] = []
         self._index: Dict[str, int] = {}
@@ -331,19 +341,26 @@ class GpuReplayKeyValueStore:
         self._report_changes()
 
     def _report_changes(self) -> None:
-        """on_changes for the fold that just ran: its CHANGED and ERROR rows, paged from the device (sgr_export_changes). Spare
-        capacity slots (ids past the ones this store assigned) never appear."""
+        """on_changes for the fold that just ran: its CHANGED and ERROR rows, paged from the device (sgr_export_changes, or
+        sgr_export_changes_values with a writer table). Spare capacity slots (ids past the ones this store assigned) never appear."""
         if self._on_changes is None:
             return
         n_ids = None if self._ingest is not None or self._dingest is not None else len(self._keys)
         changed: List[Tuple[str, Optional[bytes]]] = []
         failed: List[Tuple[str, int]] = []
-        for idx, flags, err, rows, ids in self._engine.export_changes(N.ST_CHANGED | N.ST_ERROR):
+        if self._writer:
+            pages = ((idx, flags, err, vals, ids) for idx, flags, err, ids, vals in self._engine.export_changes_values(N.ST_CHANGED | N.ST_ERROR))
+        else:
+            pages = self._engine.export_changes(N.ST_CHANGED | N.ST_ERROR)
+        for idx, flags, err, rows, ids in pages:
             for i, key in enumerate(ids):
                 if key is None or (n_ids is not None and idx[i] >= n_ids):
                     continue
                 if flags[i] & N.ST_CHANGED:
-                    changed.append((key, self._decode(key, rows[i].tobytes()) if flags[i] & N.ST_EXISTS else None))
+                    if not flags[i] & N.ST_EXISTS:
+                        changed.append((key, None))
+                    else:
+                        changed.append((key, rows[i] if self._writer else self._decode(key, rows[i].tobytes())))
                 if flags[i] & N.ST_ERROR:
                     failed.append((key, int(err[i])))
         self._on_changes(changed, failed)
@@ -410,6 +427,8 @@ class GpuReplayKeyValueStore:
             return self._unflushed[key]
         if not self._folded:
             raise InvalidStateStoreException(N.SGR_ERR_STATE, f"store {self._name} has not been restored yet")
+        if self._writer:
+            return self._engine.get_many_values([key])[0]
         return self._decode(key, self._engine.get(key))
 
     def _decode(self, key: str, b: Optional[bytes]) -> Optional[bytes]:
@@ -421,7 +440,8 @@ class GpuReplayKeyValueStore:
 
     def get_many(self, keys: Sequence[str]) -> List[Optional[bytes]]:
         """get() for many keys: each key is answered from the overlay, then the unflushed puts, like get(); the rest go to the
-        device in one sgr_get_batch call and through the codec / formatter."""
+        device in one sgr_get_batch call and through the codec / formatter (or, with a writer table, as JSON values from one
+        sgr_get_batch_values call)."""
         if not self._open:
             raise InvalidStateStoreException(N.SGR_ERR_STATE, f"store {self._name} is not open")
         keys = list(keys)
@@ -437,8 +457,12 @@ class GpuReplayKeyValueStore:
         if rest:
             if not self._folded:
                 raise InvalidStateStoreException(N.SGR_ERR_STATE, f"store {self._name} has not been restored yet")
-            for i, b in zip(rest, self._engine.get_many([keys[i] for i in rest])):
-                out[i] = self._decode(keys[i], b)
+            if self._writer:
+                for i, v in zip(rest, self._engine.get_many_values([keys[i] for i in rest])):
+                    out[i] = v
+            else:
+                for i, b in zip(rest, self._engine.get_many([keys[i] for i in rest])):
+                    out[i] = self._decode(keys[i], b)
         return out
 
     def all(self) -> Iterator[Tuple[str, bytes]]:
@@ -451,7 +475,8 @@ class GpuReplayKeyValueStore:
         """(id, value) of the live entries with frm <= id <= to (None: that end open) in Bytes order, the order a
         KeyValueStore[Bytes, _] iterates in: unsigned lexicographic over the UTF-8 bytes. The device pages of engine.scan are
         merged with the overlay and the unflushed puts, which answer first as in get(); a None there hides the device row. decode:
-        values as get() returns them, else the packed program bytes."""
+        values as get() returns them (with a writer table, the device's JSON values of engine.scan_values), else the packed
+        program bytes."""
         lo = None if frm is None else frm.encode("utf-8")
         hi = None if to is None else to.encode("utf-8")
 
@@ -475,6 +500,7 @@ class GpuReplayKeyValueStore:
             n_ids = None if self._ingest is not None or self._state_topic else max(self._keys_loaded[0], 0)
             unread = [] if folded else [k for k in (self._ingest.keys() if self._ingest is not None else self._keys) if k not in host]
         hosted = sorted((kb, k, v) for k, v in host.items() if inside(kb := k.encode("utf-8")))
+        values = decode and self._writer
 
         def device() -> Iterator[Tuple[bytes, str, Optional[bytes]]]:
             if not folded:
@@ -487,10 +513,14 @@ class GpuReplayKeyValueStore:
             if lo is not None and hi is not None and lo > hi:
                 return
             try:
-                for idx, _, rows, ids in self._engine.scan(frm, to):
+                if values:
+                    pages = ((idx, vals, ids) for idx, _, ids, vals in self._engine.scan_values(frm, to))
+                else:
+                    pages = ((idx, rows, ids) for idx, _, rows, ids in self._engine.scan(frm, to))
+                for idx, rows, ids in pages:
                     for i, k in enumerate(ids):
                         if n_ids is None or idx[i] < n_ids:   # spare capacity slots are not this store's ids
-                            yield k.encode("utf-8"), k, rows[i].tobytes()
+                            yield k.encode("utf-8"), k, rows[i] if values else rows[i].tobytes()
             except N.SgrError:
                 check_open()   # closed while the iteration ran: what get() raised for the next id
                 raise
@@ -511,7 +541,7 @@ class GpuReplayKeyValueStore:
                 continue
             if packed is None:   # (an id of a store that has not been restored: the device iterator raises next)
                 continue
-            v = self._decode(k, packed) if decode else packed
+            v = self._decode(k, packed) if decode and not values else packed
             if v is not None:
                 yield k, v
         for _, k, v in hosted[h:]:
