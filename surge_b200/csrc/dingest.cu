@@ -684,15 +684,8 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
     st.n_markers = h[2]; st.n_null_values = h[3]; st.n_duplicates += h[4]; st.n_records = h[6]; st.n_new_keys = h[0] - g->keys_on_host;   // (ids a failed poll interned become visible with the next good one)
     // ---- grow the table for the new ids, hand their names to the engine's key table, fold
     const uint64_t n_keys = h[0];
-    void* d_states = nullptr; uint64_t n_agg = 0; uint32_t sb = 0;
-    const int32_t have = sgr_states_device(g->eng, &d_states, &n_agg, &sb);
-    if (have != SGR_OK || n_keys > n_agg) {
-      uint64_t cap = have == SGR_OK ? n_agg : 0;
-      if (cap < 1024) cap = 1024;
-      while (cap < n_keys) cap *= 2;
-      if (cap > g->max_keys && g->max_keys >= n_keys) cap = g->max_keys;
-      int32_t rc = sgr_grow_states(g->eng, cap);
-      if (rc) { dfail(g, rc, "engine: %s", sgr_last_error(g->eng)); discard_poll(g); return rc; }
+    if (const int32_t rc = grow_states_for_ids(g->eng, n_keys, g->max_keys)) {
+      dfail(g, rc, "engine: %s", sgr_last_error(g->eng)); discard_poll(g); return rc;
     }
     lap(4);
     // The new ids, gathered on the device into dense-index order, come down in two copies queued BEHIND nothing the fold needs

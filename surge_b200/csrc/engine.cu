@@ -52,6 +52,32 @@ struct Snapshot {
 // id_index_update zeroes the words before kCtlCut, and sgr_get_batch's results follow them. The scan's bounds and the page of
 // sgr_export_changes / sgr_scan start at byte kPayloadOff.
 constexpr size_t kCtlDup = 0, kCtlNoSlot = 1, kCtlGatherBad = 2, kCtlCut = 4, kCtlRange = 8, kPayloadOff = 96;
+
+// Which rows carry the CHANGED/ERROR flags the last operation set, so that the next one clears only those (clear_flagged). The
+// lists stay in the engine's buffers: a host list in inc_prev_ids, a device list in inc_touched[next ^ 1] with its count in the
+// matching inc_counters block.
+struct FlaggedRows {
+  enum Kind { kWholeTable, kNothing, kHostList, kDeviceList };
+  Kind kind = kWholeTable;
+  uint64_t n = 0;       // kHostList: the list's length
+  uint32_t upper = 0;   // kDeviceList: a bound on the list's length
+  int next = 0;         // the inc_touched buffer the next atomic micro-batch writes its list to
+  void forget() { kind = kWholeTable; }
+  void nothing() { kind = kNothing; }
+  void host_list(uint64_t count) { kind = kHostList; n = count; }
+  void device_list(uint32_t bound) { kind = kDeviceList; upper = bound; next ^= 1; }
+};
+
+// The fold enqueue_fold launched, for finish_fold: which kernel, on what, and where its counters are.
+struct PendingFold {
+  enum Kernel { kSequential, kRows, kRuns, kVarRuns };
+  Kernel kernel = kSequential;
+  bool stamped = false;   // timed by the kernel itself (counters[8], [9]) rather than by ev0 / ev1
+  bool prior = false;     // folded onto the live table in place
+  uint64_t n_seg = 0, event_bytes = 0;
+  const uint8_t* events = nullptr; const uint64_t* offsets = nullptr; const uint32_t* ids = nullptr;
+  const void* counters = nullptr;
+};
 }  // namespace
 
 struct sgr_engine {
@@ -81,13 +107,10 @@ struct sgr_engine {
   DevBuf counters;      // 8 x u64
   GroupScratch group;   // K5 scratch
   DevBuf inc_records, inc_offsets, inc_ids, inc_prev_ids;  // K6
-  uint64_t inc_prev_n = 0;
   // sort-free K6 (incremental.cu)
   DevBuf inc_scratch, inc_touched[2], inc_err_ids, inc_counters;
   uint64_t inc_scratch_slots = 0;
-  int inc_flip = 0;
-  bool inc_atomic_prev_valid = false;   // inc_touched[inc_flip^1] / its counter describe the previous batch
-  uint32_t inc_prev_upper = 0;
+  FlaggedRows flagged;
 
   // record-parallel path (fold_rows.cu)
   bool row_ok = false;            // program is inside the transformer algebra
@@ -100,16 +123,12 @@ struct sgr_engine {
   int run_counter_idx = 0;
   int64_t opt_run_chunk_bytes = 131072; // runs kernel: bytes of log per ticket (rounded to whole steps, at least NSTAGE);
                                         // on configs[1] 128 KiB beat 32 KiB and 512 KiB (scripts/fold_ceiling.py)
-  const void* pending_counters = nullptr;
   uint32_t epoch = 0;
   size_t part_flags_cap_seen = 0;
   bool offsets_aligned64 = false; // every segment offset == log_begin (mod 64)
   uint64_t log_begin = 0, log_end = 0, max_seg_bytes = 0;
-  bool fold_pending = false;      // a fold was enqueued and not yet finished
-  bool pending_rows_v1 = false, pending_var = false, pending_runs = false, pending_stamped = false;
-  bool pending_used_rows = false, pending_prior = false, pending_timed_group = false;
-  uint64_t pending_n_seg = 0, pending_event_bytes = 0;
-  const uint8_t* pending_events = nullptr; const uint64_t* pending_offsets = nullptr; const uint32_t* pending_ids = nullptr;
+  bool fold_pending = false;      // a fold was enqueued and not yet finished (it is `pending`)
+  PendingFold pending;
   cudaEvent_t ev2 = nullptr, ev3 = nullptr;
 
   int64_t opt_kernel = 0;         // 0 auto (runs if the program allows), 1 lane-sequential TMA kernel (fold_kernels.cu),
@@ -340,16 +359,13 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
   // A runs fold queued right behind a runs fold of the same log overlaps it (programmatic dependent launch): before its
   // griddepcontrol.wait it reads only the log, the offsets and the program, which the fold before it does not write. Behind
   // anything else (a group-by or decode kernel that writes the log, a copy) it is launched plainly.
-  const bool overlap = runs && e->fold_pending && e->pending_runs && e->pending_events == d_events && e->pending_offsets == d_offsets &&
-                       e->pending_ids == d_ids;
-  e->pending_counters = counters;
-  e->pending_var = false;
-  e->pending_runs = runs;
+  const bool overlap = runs && e->fold_pending && e->pending.kernel == PendingFold::kRuns && e->pending.events == d_events &&
+                       e->pending.offsets == d_offsets && e->pending.ids == d_ids;
   // an overlapping fold stamps its own start and end (counters[8], [9]): an event between two folds would keep the next
   // one from starting while this one drains. Every other fold is timed by CUDA events around its launch.
-  e->pending_stamped = overlap;
   if (!overlap) CUDA_TRY(e, cudaEventRecord(e->ev0, e->stream));
   uint32_t launches = 0;
+  PendingFold::Kernel kernel = PendingFold::kSequential;
   const bool use_var = e->row_ok && e->row_prog.user_words == 2 && e->row_prog.cls == 0 && e->program.record_kind == SGR_REC_VAR16 && e->d_rec_offsets && d_offsets == e->d_offsets && !use_prior &&
                        !d_ids && e->opt_kernel != 1 && n_seg > 0 && n_seg < (1ull << 32) && e->n_rec > 0;
   if (use_var) {
@@ -369,10 +385,10 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
       if (le != cudaSuccess) return fail(e, SGR_ERR_CUDA, "fold_vruns launch: %s", cudaGetErrorString(le));
       rc = launch_replay(e, d_events, d_offsets, d_ids, states_in, counters); if (rc) return rc;
       launches = 2;
-      e->pending_var = true;
+      kernel = PendingFold::kVarRuns;
     }
   }
-  if (n_seg && !e->pending_var) {
+  if (n_seg && kernel != PendingFold::kVarRuns) {
     if (use_rows) {
       const bool v1 = e->opt_kernel == 3;
       const int rv = (int)e->opt_run_variant;
@@ -409,6 +425,7 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
         rc = launch_replay(e, d_events, d_offsets, d_ids, states_in, counters); if (rc) return rc;
         launches = 2;
       }
+      kernel = runs ? PendingFold::kRuns : PendingFold::kRows;
     } else {
       FoldArgs a{};
       a.events = d_events; a.seg_offsets = d_offsets; a.seg_ids = d_ids; a.n_seg = n_seg;
@@ -422,9 +439,8 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
     }
   }
   if (!overlap) CUDA_TRY(e, cudaEventRecord(e->ev1, e->stream));
-  e->fold_pending = true; e->pending_used_rows = use_rows; e->pending_rows_v1 = use_rows && e->opt_kernel == 3; e->pending_prior = use_prior;
-  e->pending_n_seg = n_seg; e->pending_event_bytes = event_bytes;
-  e->pending_events = d_events; e->pending_offsets = d_offsets; e->pending_ids = d_ids;
+  e->fold_pending = true;
+  e->pending = PendingFold{kernel, overlap, use_prior, n_seg, event_bytes, d_events, d_offsets, d_ids, counters};
   e->stats.fold_launches = launches;
   return SGR_OK;
 }
@@ -433,23 +449,24 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
 int32_t finish_fold(sgr_engine* e) {
   if (!e->fold_pending) return SGR_OK;
   e->fold_pending = false;
+  PendingFold& p = e->pending;
   unsigned long long h[16] = {};
-  CUDA_TRY(e, cudaMemcpyAsync(h, e->pending_counters, e->pending_runs ? 128 : 64, cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(e, cudaMemcpyAsync(h, p.counters, p.kernel == PendingFold::kRuns ? 128 : 64, cudaMemcpyDeviceToHost, e->stream));
   CUDA_TRY(e, cudaStreamSynchronize(e->stream));
   // stamped: from the first CTA's entry (~counters[8]) to the last warp's exit, both %globaltimer nanoseconds
-  if (e->pending_stamped) e->stats.ms_fold = (h[8] && h[9] > ~h[8]) ? (float)((double)(h[9] - ~h[8]) * 1e-6) : 0.f;
+  if (p.stamped) e->stats.ms_fold = (h[8] && h[9] > ~h[8]) ? (float)((double)(h[9] - ~h[8]) * 1e-6) : 0.f;
   else CUDA_TRY(e, cudaEventElapsedTime(&e->stats.ms_fold, e->ev0, e->ev1));
-  if ((e->pending_var && (h[7] || h[3] > kRedoCap)) || (e->pending_used_rows && h[3] > kRedoCap)) {
+  if ((p.kernel == PendingFold::kVarRuns && h[7]) || (p.kernel != PendingFold::kSequential && h[3] > kRedoCap)) {
     // the variable-record kernel's directory/header view disagreed with the CSR, or more aggregates threw than the replay
     // list holds: the CSR is the source of truth, fold everything again on the sequential kernel
-    if (e->pending_prior) {
+    if (p.prior) {
       // the kernel has already overwritten the non-throwing aggregates in place: the table is half-applied. It must not be
       // served, and a retry must not double-apply — invalidate it (reads fail with SGR_ERR_STATE until the next full fold)
       e->states_valid = false; mark_dirty(e);
       return fail(e, SGR_ERR_UNSUPPORTED, "replay list overflow on an in-place incremental fold: state table invalidated, rebuild it");
     }
     FoldArgs a{};
-    a.events = e->pending_events; a.seg_offsets = e->pending_offsets; a.seg_ids = e->pending_ids; a.n_seg = e->pending_n_seg;
+    a.events = p.events; a.seg_offsets = p.offsets; a.seg_ids = p.ids; a.n_seg = p.n_seg;
     a.states_out = (uint8_t*)e->states.p; a.counters = (unsigned long long*)e->counters.p;
     CUDA_TRY(e, cudaMemsetAsync(e->counters.p, 0, 64, e->stream));
     CUDA_TRY(e, cudaEventRecord(e->ev2, e->stream));
@@ -462,18 +479,22 @@ int32_t finish_fold(sgr_engine* e) {
     float ms2 = 0; CUDA_TRY(e, cudaEventElapsedTime(&ms2, e->ev2, e->ev3));
     e->stats.ms_fold += ms2; e->stats.fold_launches += 1;
     // h now holds the sequential kernel's counters, which count only the events before each throw
-    e->pending_var = false; e->pending_used_rows = false;
+    p.kernel = PendingFold::kSequential;
   }
-  const uint64_t n_seg = e->pending_n_seg;
+  const uint64_t n_seg = p.n_seg;
   e->stats.n_aggregates = n_seg;
-  // runs kernel counts every record, the replay takes back what followed a throw; the rows kernel skips
-  // throwing segments, the replay adds what preceded the throw
-  e->stats.n_events = e->pending_var ? h[0] - h[4] + h[5] : !e->pending_used_rows ? h[0] : (e->pending_rows_v1 ? h[0] + h[5] : h[0] - h[4]);
+  switch (p.kernel) {
+    case PendingFold::kSequential: e->stats.n_events = h[0]; break;
+    // the runs kernel counts every record, the replay takes back what followed a throw; the rows kernel skips throwing
+    // segments, the replay adds what preceded the throw; the variable-record kernel does both
+    case PendingFold::kRuns: e->stats.n_events = h[0] - h[4]; break;
+    case PendingFold::kRows: e->stats.n_events = h[0] + h[5]; break;
+    case PendingFold::kVarRuns: e->stats.n_events = h[0] - h[4] + h[5]; break;
+  }
   e->stats.n_errors = h[1];
   e->stats.n_long_segments = h[2];
-  e->stats.event_bytes = e->pending_event_bytes;
-  e->stats.algorithmic_bytes = e->pending_event_bytes + 8 * (n_seg + 1) +
-                               (uint64_t)e->program.state_bytes * n_seg * (e->pending_prior ? 2 : 1) + (e->pending_ids ? 4 * n_seg : 0);
+  e->stats.event_bytes = p.event_bytes;
+  e->stats.algorithmic_bytes = p.event_bytes + 8 * (n_seg + 1) + (uint64_t)e->program.state_bytes * n_seg * (p.prior ? 2 : 1) + (p.ids ? 4 * n_seg : 0);
   return SGR_OK;
 }
 
@@ -689,7 +710,7 @@ int32_t sgr_set_initial_states(sgr_engine* e, const void* states, uint64_t n_agg
   CUDA_TRY(e, cudaMemcpyAsync(e->states.p, states, (size_t)n_agg * e->program.state_bytes, cudaMemcpyHostToDevice, e->stream));
   CUDA_TRY(e, cudaStreamSynchronize(e->stream));
   e->states_valid = true;
-  e->inc_atomic_prev_valid = false; e->inc_prev_n = 0;
+  e->flagged.forget();
   mark_dirty(e);
   return SGR_OK;
 }
@@ -707,8 +728,7 @@ static int32_t fold_begin(sgr_engine* e, bool pipelined) {
   rc = enqueue_fold(e, e->d_events, e->d_offsets, nullptr, e->n_agg, prior, e->event_bytes, e->offsets_aligned64, e->log_begin, e->log_end);
   if (rc) return rc;
   e->states_valid = true;
-  e->inc_prev_n = 0;
-  e->inc_atomic_prev_valid = false;
+  e->flagged.forget();
   mark_dirty(e);
   return SGR_OK;
 }
@@ -728,8 +748,45 @@ int32_t sgr_wait(sgr_engine* e) {
   return finish_fold(e);
 }
 
+// Exact replay of the slots that saw a throwing event in a sort-free fold: the batch is grouped once (K5) and exactly those
+// slots are folded sequentially onto their untouched prior states (exact err_idx, state kept: PersistentActor.scala:260-263).
+// h_throwing / h_dropped: aggregates in error, events dropped after their throw.
 static int32_t replay_throwing_slots(sgr_engine* e, const void* d_records, uint64_t n_records, uint64_t n_agg, const uint32_t* d_err_ids,
-                                     uint64_t n_err, unsigned long long* h_throwing, unsigned long long* h_dropped);
+                                     uint64_t n_err, unsigned long long* h_throwing, unsigned long long* h_dropped) {
+  DevBuf& grouped = e->group.batch_records;
+  CUDA_TRY(e, grouped.reserve(n_records * 64));
+  CUDA_TRY(e, e->inc_offsets.reserve((n_agg + 2) * 8));
+  unsigned long long bad = 0;
+  cudaError_t ce = group_by_agg_stable(e->group, (const uint8_t*)d_records, n_records, n_agg, (uint8_t*)grouped.p, (uint64_t*)e->inc_offsets.p,
+                                       nullptr, nullptr, (unsigned long long*)e->counters.p, e->stream, &bad);
+  if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "group-by (replay): %s", cudaGetErrorString(ce));
+  CUDA_TRY(e, cudaMemsetAsync(e->counters.p, 0, 64, e->stream));
+  FoldArgs a{};
+  a.events = (const uint8_t*)grouped.p; a.seg_offsets = (const uint64_t*)e->inc_offsets.p; a.n_seg = n_err;
+  a.seg_list = d_err_ids; a.states_in = (const uint8_t*)e->states.p; a.states_out = (uint8_t*)e->states.p;
+  a.counters = (unsigned long long*)e->counters.p;
+  FoldLaunchInfo info{};
+  cudaError_t le2 = launch_fold_stream(a, e->dprog, -1, e->num_sms, e->max_record_bytes, e->stream, &info);
+  if (le2 != cudaSuccess) return fail(e, SGR_ERR_CUDA, "replay launch: %s", cudaGetErrorString(le2));
+  unsigned long long h2[8];
+  CUDA_TRY(e, cudaMemcpyAsync(h2, e->counters.p, 64, cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+  *h_throwing = h2[1]; *h_dropped = h2[4];
+  return SGR_OK;
+}
+
+// Enqueue the clear of the flags e->flagged names, before an operation sets its own. The atomic micro-batch (`atomic`) clears a
+// device list in its own kernel and clears nothing on a fresh table; it gets back the bound on the list it is to clear (0:
+// none). Every other operation clears a host list, or else the whole table.
+static uint32_t clear_flagged(sgr_engine* e, bool atomic) {
+  const FlaggedRows& f = e->flagged;
+  if (atomic && f.kind == FlaggedRows::kDeviceList) return f.upper;
+  if (atomic && f.kind == FlaggedRows::kNothing) return 0;
+  const bool list = !atomic && f.kind == FlaggedRows::kHostList;
+  clear_batch_flags((uint8_t*)e->states.p, e->program.state_bytes, list ? (const uint32_t*)e->inc_prev_ids.p : nullptr, list ? f.n : e->states_n,
+                    e->stream);
+  return 0;
+}
 
 // The program folds sort-free on integer atomics (incremental.cu, bulk_fold.cu), both as micro-batches and as arrival-order logs.
 // (a 16-byte state that is one JVM Double compares with ==, not bitwise: it takes the sort-based path)
@@ -751,20 +808,15 @@ static int32_t fold_incremental_atomic(sgr_engine* e, const void* d_records, uin
   CUDA_TRY(e, e->inc_touched[0].reserve((n_agg + 1) * 4)); CUDA_TRY(e, e->inc_touched[1].reserve((n_agg + 1) * 4));
   CUDA_TRY(e, e->inc_err_ids.reserve((n_agg + 1) * 4));
   CUDA_TRY(e, e->inc_counters.reserve(256));
-  unsigned long long* cur = (unsigned long long*)e->inc_counters.p + 8 * e->inc_flip;
-  unsigned long long* prev = (unsigned long long*)e->inc_counters.p + 8 * (e->inc_flip ^ 1);
+  const int next = e->flagged.next;
+  unsigned long long* cur = (unsigned long long*)e->inc_counters.p + 8 * next;
+  unsigned long long* prev = (unsigned long long*)e->inc_counters.p + 8 * (next ^ 1);
   CUDA_TRY(e, cudaEventRecord(e->ev0, e->stream));
   CUDA_TRY(e, cudaMemsetAsync(cur, 0, 64, e->stream));
-  uint32_t prev_upper = 0;
-  if (!e->inc_atomic_prev_valid) {
-    // first batch after a full fold / set_initial_states / a sort-based batch: every slot may carry per-batch flags
-    clear_batch_flags((uint8_t*)e->states.p, e->program.state_bytes, nullptr, n_agg, e->stream);
-  } else {
-    prev_upper = e->inc_prev_upper;
-  }
+  const uint32_t prev_upper = clear_flagged(e, true);
   cudaError_t le = launch_incremental_atomic((const uint8_t*)d_records, (uint32_t)n_records, n_agg, e->inc_scratch.p, (uint8_t*)e->states.p,
-                                             (uint32_t*)e->inc_touched[e->inc_flip].p, (uint32_t*)e->inc_err_ids.p,
-                                             (const uint32_t*)e->inc_touched[e->inc_flip ^ 1].p, prev + 5, prev_upper, e->row_prog, cur, (unsigned long long)e->opt_replay_budget, e->stream);
+                                             (uint32_t*)e->inc_touched[next].p, (uint32_t*)e->inc_err_ids.p,
+                                             (const uint32_t*)e->inc_touched[next ^ 1].p, prev + 5, prev_upper, e->row_prog, cur, (unsigned long long)e->opt_replay_budget, e->stream);
   if (le != cudaSuccess) return fail(e, SGR_ERR_CUDA, "incremental launch: %s", cudaGetErrorString(le));
   CUDA_TRY(e, cudaEventRecord(e->ev1, e->stream));
   unsigned long long h[8];
@@ -780,10 +832,7 @@ static int32_t fold_incremental_atomic(sgr_engine* e, const void* d_records, uin
     if (rr) return rr;
     h[1] = thr; h[6] = drop;   // throwing slots, events dropped after their throw
   }
-  e->inc_atomic_prev_valid = true;
-  e->inc_prev_upper = (uint32_t)(h[5]);
-  e->inc_flip ^= 1;
-  e->inc_prev_n = 0;
+  e->flagged.device_list((uint32_t)h[5]);
   e->stats.ms_group = 0;
   e->stats.n_aggregates = h[5]; e->stats.n_errors = h[1]; e->stats.n_events = n_records - h[6];
   e->stats.event_bytes = n_records * 64; e->stats.n_long_segments = 0;
@@ -805,15 +854,13 @@ static int32_t fold_incremental_impl(sgr_engine* e, const void* d_records, uint6
   if (holes && (n_agg >= (1ull << 32) || n_records >= (1ull << 32)))
     return fail(e, SGR_ERR_UNSUPPORTED, "group-by is limited to 2^32 records/aggregates");
   if (holes && n_live == 0) return SGR_OK;
-  e->inc_atomic_prev_valid = false;
+  if (e->flagged.kind != FlaggedRows::kHostList) e->flagged.forget();   // this batch rewrites rows a device list does not name
   CUDA_TRY(e, e->inc_offsets.reserve((n_records + 2) * 8));
   CUDA_TRY(e, e->inc_ids.reserve((n_records + 1) * 4));
   DevBuf& grouped = e->group.batch_records;
   CUDA_TRY(e, grouped.reserve(n_records * 64));
   CUDA_TRY(e, cudaEventRecord(e->ev2, e->stream));
-  // per-batch flags (CHANGED/ERROR) of the aggregates touched by the previous batch are cleared
-  if (e->inc_prev_n) clear_batch_flags((uint8_t*)e->states.p, e->program.state_bytes, (const uint32_t*)e->inc_prev_ids.p, e->inc_prev_n, e->stream);
-  else clear_batch_flags((uint8_t*)e->states.p, e->program.state_bytes, nullptr, n_agg, e->stream);
+  clear_flagged(e, false);
   unsigned long long bad = 0, n_holes = 0;
   uint64_t n_touched = 0;
   cudaError_t ce = group_by_agg_stable(e->group, (const uint8_t*)d_records, n_records, n_agg, (uint8_t*)grouped.p,
@@ -828,9 +875,8 @@ static int32_t fold_incremental_impl(sgr_engine* e, const void* d_records, uint6
   if (rc) return rc;
   rc = finish_fold(e); if (rc) return rc;
   CUDA_TRY(e, cudaEventElapsedTime(&e->stats.ms_group, e->ev2, e->ev3));
-  // remember who was touched so the next batch can clear their per-batch flags
   std::swap(e->inc_ids, e->inc_prev_ids);
-  e->inc_prev_n = n_touched;
+  e->flagged.host_list(n_touched);
   mark_dirty(e);
   return SGR_OK;
 }
@@ -871,6 +917,25 @@ int32_t sgr_load_keys(sgr_engine* e, const uint8_t* keys, const uint32_t* key_of
   return SGR_OK;
 }
 
+// Grow the live table to n_agg rows (no fewer than it holds), keeping the rows of a valid table and making the others None, in a
+// new buffer of at least min_bytes only when the old one is too small (no device-wide synchronisation by cudaFree otherwise).
+static int32_t grow_table(sgr_engine* e, uint64_t n_agg, size_t min_bytes) {
+  const size_t sb = e->program.state_bytes, need = (size_t)n_agg * sb;
+  const uint64_t have = e->states_valid ? e->states_n : 0;
+  if (e->states.cap < need) {
+    struct Guard { DevBuf b; ~Guard() { b.release(); } } guard;   // frees the old table on success, the new one on failure
+    DevBuf& nb = guard.b;
+    CUDA_TRY(e, nb.reserve(need > min_bytes ? need : min_bytes));
+    if (have) CUDA_TRY(e, cudaMemcpyAsync(nb.p, e->states.p, have * sb, cudaMemcpyDeviceToDevice, e->stream));
+    CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+    std::swap(e->states, nb);
+  }
+  CUDA_TRY(e, cudaMemsetAsync((uint8_t*)e->states.p + have * sb, 0, need - have * sb, e->stream));
+  e->states_n = n_agg;
+  e->states_valid = true;
+  return SGR_OK;
+}
+
 int32_t sgr_grow_states(sgr_engine* e, uint64_t n_agg) {
   OpLock op_lock(e);
   if (!e) return SGR_ERR_INVALID;
@@ -878,27 +943,8 @@ int32_t sgr_grow_states(sgr_engine* e, uint64_t n_agg) {
   int32_t rc = use_device(e); if (rc) return rc;
   rc = before_load(e); if (rc) return rc;
   if (e->states_valid && n_agg <= e->states_n) return SGR_OK;
-  const size_t sb = e->program.state_bytes;
-  if (!e->states_valid && e->states.p && e->states.cap >= (size_t)n_agg * sb) {
-    // a table that was reset (sgr_set_initial_states(NULL)) and is large enough: all None, no reallocation, no device-wide
-    // synchronisation by cudaFree
-    CUDA_TRY(e, cudaMemsetAsync(e->states.p, 0, (size_t)n_agg * sb, e->stream));
-    e->states_n = n_agg; e->states_valid = true;
-    e->inc_atomic_prev_valid = false; e->inc_prev_n = 0;
-    mark_dirty(e);
-    return SGR_OK;
-  }
-  struct Guard { DevBuf b; ~Guard() { b.release(); } } guard;   // frees the old table on success, the new one on failure
-  DevBuf& nb = guard.b;
-  CUDA_TRY(e, nb.reserve((size_t)n_agg * sb));
-  const size_t keep = e->states_valid ? (size_t)e->states_n * sb : 0;
-  if (keep) CUDA_TRY(e, cudaMemcpyAsync(nb.p, e->states.p, keep, cudaMemcpyDeviceToDevice, e->stream));
-  CUDA_TRY(e, cudaMemsetAsync((uint8_t*)nb.p + keep, 0, (size_t)n_agg * sb - keep, e->stream));
-  CUDA_TRY(e, cudaStreamSynchronize(e->stream));
-  std::swap(e->states, nb);
-  e->states_n = n_agg;
-  e->states_valid = true;
-  e->inc_atomic_prev_valid = false; e->inc_prev_n = 0;
+  rc = grow_table(e, n_agg, 0); if (rc) return rc;
+  e->flagged.forget();
   mark_dirty(e);
   return SGR_OK;
 }
@@ -940,13 +986,7 @@ int32_t sgr_fold_ingested(sgr_engine* e, sgr_ingest* g) {
   const uint8_t* keys = nullptr; const uint32_t* key_offsets = nullptr; uint64_t n_keys = 0;
   if (sgr_ingest_pending(g, &recs, &n_records) || sgr_ingest_keys(g, &keys, &key_offsets, &n_keys))
     return fail(e, SGR_ERR_INVALID, "ingest: %s", sgr_ingest_last_error(g));
-  if (!e->states_valid || n_keys > e->states_n) {
-    // amortised doubling, like a hash table: the resize copies the table device to device
-    uint64_t cap = e->states_valid ? e->states_n : 0;
-    if (cap < 1024) cap = 1024;
-    while (cap < n_keys) cap *= 2;
-    int32_t rc = sgr_grow_states(e, cap); if (rc) return rc;
-  }
+  { int32_t rc = grow_states_for_ids(e, n_keys, UINT64_MAX); if (rc) return rc; }
   if (n_records) { int32_t rc = sgr_fold_incremental(e, recs, n_records); if (rc) return rc; }
   if (n_keys) append_keys(e, g, keys, key_offsets, n_keys, true);
   sgr_ingest_mark_folded(g);
@@ -1015,14 +1055,16 @@ static int32_t ensure_pinned(sgr_engine* e, size_t bytes) {
   return SGR_OK;
 }
 
-// The start of every device read, in this order: refuse a routed engine when asked, wait for an enqueued fold, and fail before
-// any fold. `api`: the entry point's name without "sgr_". Caller holds op_mu.
-static int32_t begin_read(sgr_engine* e, const char* api, bool refuse_routed) {
+// The start of every device read, in this order: refuse a routed engine when asked, wait for an enqueued fold, fail before
+// any fold, and fail a read of JSON values (`values`) without a state writer. `api`: the entry point's name without "sgr_".
+// Caller holds op_mu.
+static int32_t begin_read(sgr_engine* e, const char* api, bool refuse_routed, bool values) {
   if (refuse_routed && e->dist)
     return fail(e, SGR_ERR_UNSUPPORTED, "the rows of a routed engine are local slots: sgr_%s does not map them to ids", api);
   int32_t rc = use_device(e); if (rc) return rc;
   rc = finish_fold(e); if (rc) return rc;
   if (!e->states_valid) return fail(e, SGR_ERR_STATE, "state store is not readable: no fold has completed");
+  if (values && !e->writer.n) return fail(e, SGR_ERR_STATE, "sgr_%s: no state writer is set (sgr_set_state_writer)", api);
   return SGR_OK;
 }
 
@@ -1064,45 +1106,65 @@ static int32_t id_index_settle(sgr_engine* e, const unsigned long long* ctl) {
   return SGR_OK;
 }
 
-int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n, void* out, uint64_t cap, uint32_t* flags,
-                      int64_t* indices) {
-  if (!e || (n && (!key_offsets || !out)) || (n && !keys && key_offsets[n] != key_offsets[0])) return fail(e, SGR_ERR_INVALID, "null argument");
+// Where read_batch_front left a batch. Device, at dd: the results (`down` bytes: the id index's control words, then indices at
+// r_idx, flags at r_flags, program bytes at r_rows) | query offsets | query bytes (at q_ids). Page-locked, at hd (behind the
+// staged ids and queries): room for the results, then for sgr_get_batch_values' value control words.
+struct BatchRead {
+  std::unique_lock<std::recursive_mutex> op_lock;
+  uint8_t* hd = nullptr;
+  uint8_t* dd = nullptr;
+  size_t down = 0, q_ids = 0, r_idx = 0, r_flags = 0, r_rows = 0;
+};
+
+// The front of sgr_get_batch and sgr_get_batch_values, after their output checks: the key checks, begin_read, the refusal of a
+// batch whose program bytes do not fit in rows_cap bytes, then (n > 0) the staging of the queries and the probe + gather.
+// `values`: the batch is read as JSON values. `api`: the entry point's name without "sgr_".
+static int32_t read_batch_front(sgr_engine* e, const char* api, bool values, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n,
+                                uint64_t rows_cap, BatchRead* b) {
+  if ((n && !key_offsets) || (n && !keys && key_offsets[n] != key_offsets[0])) return fail(e, SGR_ERR_INVALID, "null argument");
   for (uint64_t i = 0; i < n; ++i)
     if (key_offsets[i + 1] < key_offsets[i]) return fail(e, SGR_ERR_INVALID, "key_offsets not monotone at %llu", (unsigned long long)i);
   // one table generation for the whole batch: no load or fold runs while it is read, and an enqueued fold is waited for
-  OpLock op_lock(e);
-  int32_t rc = begin_read(e, "get_batch", false); if (rc) return rc;
+  b->op_lock = std::unique_lock<std::recursive_mutex>(e->op_mu);
+  int32_t rc = begin_read(e, api, false, values); if (rc) return rc;
   const uint32_t sb = e->program.state_bytes, user = sb - 8;
-  if (cap / user < n) return fail(e, SGR_ERR_CAPACITY, "%llu rows of %u bytes do not fit in %llu bytes", (unsigned long long)n, user, (unsigned long long)cap);
+  if (rows_cap / user < n) return fail(e, SGR_ERR_CAPACITY, "%llu rows of %u bytes do not fit in %llu bytes", (unsigned long long)n, user, (unsigned long long)rows_cap);
   if (!n) return SGR_OK;
-
-  // layout: pinned [ids to index | query offsets | query bytes | results], device [results | query offsets | query bytes], where
-  // the results are the id index's control words, then indices | flags | program bytes
   const uint64_t q0 = key_offsets[0], q_bytes = key_offsets[n] - q0;
-  const size_t up_offs = round16((n + 1) * 4), up = up_offs + round16(q_bytes);
-  const size_t r_idx = 8 * kCtlCut, r_flags = r_idx + n * 8, r_rows = r_flags + round16(n * 4), down = r_rows + round16(n * user);
-  IdIndex& x = e->id_index;
-  rc = id_index_update(e, up + down, down + up); if (rc) return rc;
-  uint8_t* hq = (uint8_t*)e->gb_host + (e->gb_host_cap - up - down);   // (behind the ids: the stream may still be copying them)
-  uint8_t* hd = hq + up;
-  uint8_t* dd = (uint8_t*)e->gb_dev.p;
+  b->q_ids = round16((n + 1) * 4);
+  const size_t up = b->q_ids + round16(q_bytes);
+  b->r_idx = 8 * kCtlCut; b->r_flags = b->r_idx + n * 8; b->r_rows = b->r_flags + round16(n * 4); b->down = b->r_rows + round16(n * user);
+  const size_t host = up + b->down + (values ? 8 * kSvCtlWords : 0);
+  rc = id_index_update(e, host, b->down + up); if (rc) return rc;
+  uint8_t* hq = (uint8_t*)e->gb_host + (e->gb_host_cap - host);   // (behind the ids: the stream may still be copying them)
+  b->hd = hq + up;
+  uint8_t* dd = b->dd = (uint8_t*)e->gb_dev.p;
   uint32_t* qo = (uint32_t*)hq;
   for (uint64_t i = 0; i <= n; ++i) qo[i] = key_offsets[i] - (uint32_t)q0;
-  if (q_bytes) memcpy(hq + up_offs, keys + q0, q_bytes);
-  CUDA_TRY(e, cudaMemcpyAsync(dd + down, hq, up, cudaMemcpyHostToDevice, e->stream));
-  cudaError_t ce = id_index_probe(x, dd + down + up_offs, (const uint32_t*)(dd + down), n, (long long*)(dd + r_idx), e->stream);
+  if (q_bytes) memcpy(hq + b->q_ids, keys + q0, q_bytes);
+  CUDA_TRY(e, cudaMemcpyAsync(dd + b->down, hq, up, cudaMemcpyHostToDevice, e->stream));
+  cudaError_t ce = id_index_probe(e->id_index, dd + b->down + b->q_ids, (const uint32_t*)(dd + b->down), n, (long long*)(dd + b->r_idx), e->stream);
   if (ce == cudaSuccess)
-    ce = id_index_gather((const uint8_t*)e->states.p, sb, e->states_n, (const long long*)(dd + r_idx), n, dd + r_rows, (uint32_t*)(dd + r_flags),
-                         (unsigned long long*)dd + kCtlGatherBad, e->stream);
-  if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "get_batch launch: %s", cudaGetErrorString(ce));
-  CUDA_TRY(e, cudaMemcpyAsync(hd, dd, down, cudaMemcpyDeviceToHost, e->stream));
+    ce = id_index_gather((const uint8_t*)e->states.p, sb, e->states_n, (const long long*)(dd + b->r_idx), n, dd + b->r_rows,
+                         (uint32_t*)(dd + b->r_flags), (unsigned long long*)dd + kCtlGatherBad, e->stream);
+  if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "%s launch: %s", api, cudaGetErrorString(ce));
+  return SGR_OK;
+}
+
+int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n, void* out, uint64_t cap, uint32_t* flags,
+                      int64_t* indices) {
+  if (!e || (n && !out)) return fail(e, SGR_ERR_INVALID, "null argument");
+  BatchRead b;
+  int32_t rc = read_batch_front(e, "get_batch", false, keys, key_offsets, n, cap, &b);
+  if (rc || !n) return rc;
+  CUDA_TRY(e, cudaMemcpyAsync(b.hd, b.dd, b.down, cudaMemcpyDeviceToHost, e->stream));
   CUDA_TRY(e, cudaStreamSynchronize(e->stream));
-  const unsigned long long* ctl = (const unsigned long long*)hd;
+  const unsigned long long* ctl = (const unsigned long long*)b.hd;
   rc = id_index_settle(e, ctl); if (rc) return rc;
   if (ctl[kCtlGatherBad]) return fail(e, SGR_ERR_INVALID, "aggregate index %llu out of range", ctl[kCtlGatherBad] - 1);
-  memcpy(out, hd + r_rows, n * user);
-  if (flags) memcpy(flags, hd + r_flags, n * 4);
-  if (indices) memcpy(indices, hd + r_idx, n * 8);
+  memcpy(out, b.hd + b.r_rows, n * (e->program.state_bytes - 8));
+  if (flags) memcpy(flags, b.hd + b.r_flags, n * 4);
+  if (indices) memcpy(indices, b.hd + b.r_idx, n * 8);
   return SGR_OK;
 }
 
@@ -1172,46 +1234,24 @@ int32_t sgr_set_state_writer(sgr_engine* e, const sgr_json_field* members, uint3
 
 int32_t sgr_get_batch_values(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n, uint8_t* values, uint64_t values_cap,
                              uint64_t* value_offsets, uint32_t* flags, int64_t* indices, uint64_t* values_len) {
-  if (!e || !value_offsets || !flags || (!values && values_cap) || (n && !key_offsets) || (n && !keys && key_offsets[n] != key_offsets[0]))
-    return fail(e, SGR_ERR_INVALID, "null argument");
-  for (uint64_t i = 0; i < n; ++i)
-    if (key_offsets[i + 1] < key_offsets[i]) return fail(e, SGR_ERR_INVALID, "key_offsets not monotone at %llu", (unsigned long long)i);
-  OpLock op_lock(e);
-  int32_t rc = begin_read(e, "get_batch_values", false); if (rc) return rc;
-  if (!e->writer.n) return fail(e, SGR_ERR_STATE, "sgr_get_batch_values: no state writer is set (sgr_set_state_writer)");
+  if (!e || !value_offsets || !flags || (!values && values_cap)) return fail(e, SGR_ERR_INVALID, "null argument");
+  BatchRead b;
+  int32_t rc = read_batch_front(e, "get_batch_values", true, keys, key_offsets, n, UINT64_MAX, &b); if (rc) return rc;
   if (!n) { value_offsets[0] = 0; if (values_len) *values_len = 0; return SGR_OK; }
-  const uint32_t sb = e->program.state_bytes, user = sb - 8;
-  // as sgr_get_batch: pinned [ids to index | query offsets | query bytes | results | value control words], device [results |
-  // query offsets | query bytes]; the results are the id index's control words, then indices | flags | program bytes
-  const uint64_t q0 = key_offsets[0], q_bytes = key_offsets[n] - q0;
-  const size_t up_offs = round16((n + 1) * 4), up = up_offs + round16(q_bytes);
-  const size_t r_idx = 8 * kCtlCut, r_flags = r_idx + n * 8, r_rows = r_flags + round16(n * 4), down = r_rows + round16(n * user);
-  const size_t h_sv = up + down, h_extra = h_sv + 8 * kSvCtlWords;
-  IdIndex& x = e->id_index;
-  rc = id_index_update(e, h_extra, down + up); if (rc) return rc;
-  uint8_t* hq = (uint8_t*)e->gb_host + (e->gb_host_cap - h_extra);   // (behind the ids: the stream may still be copying them)
-  uint8_t* dd = (uint8_t*)e->gb_dev.p;
-  uint32_t* qo = (uint32_t*)hq;
-  for (uint64_t i = 0; i <= n; ++i) qo[i] = key_offsets[i] - (uint32_t)q0;
-  if (q_bytes) memcpy(hq + up_offs, keys + q0, q_bytes);
-  CUDA_TRY(e, cudaMemcpyAsync(dd + down, hq, up, cudaMemcpyHostToDevice, e->stream));
-  cudaError_t ce = id_index_probe(x, dd + down + up_offs, (const uint32_t*)(dd + down), n, (long long*)(dd + r_idx), e->stream);
-  if (ce == cudaSuccess)
-    ce = id_index_gather((const uint8_t*)e->states.p, sb, e->states_n, (const long long*)(dd + r_idx), n, dd + r_rows, (uint32_t*)(dd + r_flags),
-                         (unsigned long long*)dd + kCtlGatherBad, e->stream);
+  const uint8_t* dd = b.dd;
   // a query's id is the row's id: every found row has one
-  const SvRows r{dd + r_rows, user, (const uint32_t*)(dd + r_flags), (const long long*)(dd + r_idx), dd + down + up_offs, (const uint32_t*)(dd + down),
-                 ~0ull, n};
+  const SvRows r{dd + b.r_rows, e->program.state_bytes - 8, (const uint32_t*)(dd + b.r_flags), (const long long*)(dd + b.r_idx), dd + b.down + b.q_ids,
+                 (const uint32_t*)(dd + b.down), ~0ull, n};
   unsigned long long *d_offs = nullptr, *d_sv = nullptr;
-  if (ce == cudaSuccess) ce = e->sv_scratch.reserve(state_values_scratch_bytes(n));
+  cudaError_t ce = e->sv_scratch.reserve(state_values_scratch_bytes(n));
   if (ce == cudaSuccess) ce = state_values_measure(e->writer, r, ~0ull, e->sv_scratch.p, &d_offs, &d_sv, e->stream);
   if (ce != cudaSuccess) return fail(e, ce == cudaErrorMemoryAllocation ? SGR_ERR_OOM : SGR_ERR_CUDA, "get_batch_values launch: %s", cudaGetErrorString(ce));
-  CUDA_TRY(e, cudaMemcpyAsync(hq + up, dd, 8 * kCtlCut, cudaMemcpyDeviceToHost, e->stream));
-  CUDA_TRY(e, cudaMemcpyAsync(hq + h_sv, d_sv, 8 * kSvCtlWords, cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(e, cudaMemcpyAsync(b.hd, dd, 8 * kCtlCut, cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(e, cudaMemcpyAsync(b.hd + b.down, d_sv, 8 * kSvCtlWords, cudaMemcpyDeviceToHost, e->stream));
   CUDA_TRY(e, cudaStreamSynchronize(e->stream));
   unsigned long long ctl[kCtlCut], sv[kSvCtlWords];
-  memcpy(ctl, hq + up, sizeof ctl);
-  memcpy(sv, hq + h_sv, sizeof sv);
+  memcpy(ctl, b.hd, sizeof ctl);
+  memcpy(sv, b.hd + b.down, sizeof sv);
   rc = id_index_settle(e, ctl); if (rc) return rc;
   if (ctl[kCtlGatherBad]) return fail(e, SGR_ERR_INVALID, "aggregate index %llu out of range", ctl[kCtlGatherBad] - 1);
   if (sv[kSvRefused] < n) return writer_refusal(e, "get_batch_values", "batch", sv);
@@ -1224,15 +1264,15 @@ int32_t sgr_get_batch_values(sgr_engine* e, const uint8_t* keys, const uint32_t*
   ce = state_values_write(e->writer, r, n, d_offs, (uint8_t*)e->sv_values.p, e->stream);
   if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "get_batch_values launch: %s", cudaGetErrorString(ce));
   // pinned, from its start (the stream is idle): results | value offsets | values
-  const size_t h_offs = down, h_vals = h_offs + round16((n + 1) * 8);
+  const size_t h_offs = b.down, h_vals = h_offs + round16((n + 1) * 8);
   rc = ensure_pinned(e, h_vals + total); if (rc) return rc;
   uint8_t* hd = (uint8_t*)e->gb_host;
-  CUDA_TRY(e, cudaMemcpyAsync(hd, dd, r_rows, cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(e, cudaMemcpyAsync(hd, dd, b.r_rows, cudaMemcpyDeviceToHost, e->stream));
   CUDA_TRY(e, cudaMemcpyAsync(hd + h_offs, d_offs, (n + 1) * 8, cudaMemcpyDeviceToHost, e->stream));
   if (total) CUDA_TRY(e, cudaMemcpyAsync(hd + h_vals, e->sv_values.p, total, cudaMemcpyDeviceToHost, e->stream));
   CUDA_TRY(e, cudaStreamSynchronize(e->stream));
-  memcpy(flags, hd + r_flags, n * 4);
-  if (indices) memcpy(indices, hd + r_idx, n * 8);
+  memcpy(flags, hd + b.r_flags, n * 4);
+  if (indices) memcpy(indices, hd + b.r_idx, n * 8);
   memcpy(value_offsets, hd + h_offs, (n + 1) * 8);
   if (total) memcpy(values, hd + h_vals, total);
   if (values_len) *values_len = total;
@@ -1243,44 +1283,21 @@ int32_t sgr_get_batch_values(sgr_engine* e, const uint8_t* keys, const uint32_t*
 // ingest dictionary behind them (a table of sgr_load_keys becomes one, unchanged, at the first put batch)
 static const char kPutKeysOwner = 0;
 
-// Grow the live table to n_agg rows for sgr_put_batch, keeping its rows; rows past them are None. Capacity grows by at least
-// half, so that batches adding a few ids each do not copy the table every time. Without a table, a new one of None rows. The
-// last-write words (pb_last) cover every row.
-static int32_t put_grow_table(sgr_engine* e, uint64_t n_agg) {
+// The apply of a put batch, before its kernels: the flags the previous operation left are cleared, the table grows to n_agg
+// rows with the last-write words (pb_last) covering them, there is room for a touched list of n rows, and ev0 marks the start.
+// Shared by sgr_put_batch and put_decoded_poll.
+static int32_t put_apply_begin(sgr_engine* e, uint64_t n_agg, uint64_t n) {
   const size_t sb = e->program.state_bytes;
-  const uint64_t have = e->states_valid ? e->states_n : 0;
-  if (n_agg > have) {
-    if (e->states.cap < n_agg * sb) {
-      struct Guard { DevBuf b; ~Guard() { b.release(); } } guard;   // frees the old table on success, the new one on failure
-      DevBuf& nb = guard.b;
-      const size_t half = e->states.cap + e->states.cap / 2;
-      CUDA_TRY(e, nb.reserve(n_agg * sb > half ? n_agg * sb : half));
-      if (have) CUDA_TRY(e, cudaMemcpyAsync(nb.p, e->states.p, have * sb, cudaMemcpyDeviceToDevice, e->stream));
-      CUDA_TRY(e, cudaStreamSynchronize(e->stream));
-      std::swap(e->states, nb);
-    }
-    CUDA_TRY(e, cudaMemsetAsync((uint8_t*)e->states.p + have * sb, 0, (n_agg - have) * sb, e->stream));
-    e->states_n = n_agg;
-    e->states_valid = true;
+  if (e->states_valid) clear_flagged(e, false);
+  if (n_agg > (e->states_valid ? e->states_n : 0)) {
+    // capacity grows by at least half, so that batches adding a few ids each do not copy the table every time
+    int32_t rc = grow_table(e, n_agg, e->states.cap + e->states.cap / 2); if (rc) return rc;
   }
   if (e->pb_last_n < e->states_n) {
     CUDA_TRY(e, e->pb_last.reserve(e->states.cap / sb * 4));
     CUDA_TRY(e, cudaMemsetAsync(e->pb_last.p, 0, e->pb_last.cap, e->stream));
     e->pb_last_n = e->pb_last.cap / 4;
   }
-  return SGR_OK;
-}
-
-// The apply of a put batch, before its kernels: the flags the previous operation left are cleared (its touched list when it kept
-// one, else the whole table), the table grows to n_agg rows with pb_last covering them, there is room for a touched list of n
-// rows, and ev0 marks the start. Shared by sgr_put_batch and put_decoded_poll.
-static int32_t put_apply_begin(sgr_engine* e, uint64_t n_agg, uint64_t n) {
-  const uint32_t sb = e->program.state_bytes;
-  if (e->states_valid) {
-    if (e->inc_prev_n) clear_batch_flags((uint8_t*)e->states.p, sb, (const uint32_t*)e->inc_prev_ids.p, e->inc_prev_n, e->stream);
-    else clear_batch_flags((uint8_t*)e->states.p, sb, nullptr, e->states_n, e->stream);
-  }
-  int32_t rc = put_grow_table(e, n_agg); if (rc) return rc;
   CUDA_TRY(e, e->inc_ids.reserve(n * 4));   // this batch's touched list (the previous one is inc_prev_ids)
   CUDA_TRY(e, cudaEventRecord(e->ev0, e->stream));
   return SGR_OK;
@@ -1291,8 +1308,7 @@ static int32_t put_apply_begin(sgr_engine* e, uint64_t n_agg, uint64_t n) {
 static int32_t put_apply_end(sgr_engine* e, uint64_t n_live, uint64_t touched) {
   const uint32_t sb = e->program.state_bytes;
   std::swap(e->inc_ids, e->inc_prev_ids);
-  e->inc_prev_n = touched;
-  e->inc_atomic_prev_valid = false;
+  e->flagged.host_list(touched);
   e->stats.n_aggregates = touched; e->stats.n_events = n_live; e->stats.n_errors = 0; e->stats.n_long_segments = 0;
   e->stats.event_bytes = n_live * (sb - 8); e->stats.algorithmic_bytes = n_live * (sb - 8) + 2ull * sb * touched;
   e->stats.ms_h2d = 0; e->stats.ms_group = 0; e->stats.fold_launches = 2;
@@ -1524,8 +1540,7 @@ static int32_t export_changes_page(sgr_engine* e, const char* api, uint32_t sele
   if (!max_rows) return fail(e, SGR_ERR_INVALID, "max_rows is 0");
   // one table generation per call, and the token ties the pages of one export to it
   OpLock op_lock(e);
-  int32_t rc = begin_read(e, api, true); if (rc) return rc;
-  if (out.value_offsets && !e->writer.n) return fail(e, SGR_ERR_STATE, "sgr_%s: no state writer is set (sgr_set_state_writer)", api);
+  int32_t rc = begin_read(e, api, true, out.value_offsets != nullptr); if (rc) return rc;
   const uint64_t n_agg = e->states_n, next = cur->next;
   if (next > n_agg) return fail(e, SGR_ERR_INVALID, "cursor %llu is past the table's %llu aggregates", (unsigned long long)next, (unsigned long long)n_agg);
   if (n_agg >= 0xffffffffull) return fail(e, SGR_ERR_UNSUPPORTED, "sgr_export_changes reads tables of fewer than 2^32 - 1 aggregates");
@@ -1583,8 +1598,7 @@ static int32_t scan_page(sgr_engine* e, const char* api, const uint8_t* from, ui
   if (!max_rows) return fail(e, SGR_ERR_INVALID, "max_rows is 0");
   // one table generation per page; pages carry no state, so a scan resumes across folds by itself
   OpLock op_lock(e);
-  int32_t rc = begin_read(e, api, true); if (rc) return rc;
-  if (out.value_offsets && !e->writer.n) return fail(e, SGR_ERR_STATE, "sgr_%s: no state writer is set (sgr_set_state_writer)", api);
+  int32_t rc = begin_read(e, api, true, out.value_offsets != nullptr); if (rc) return rc;
   const uint64_t n_agg = e->states_n;
   if (n_agg >= 0xffffffffull) return fail(e, SGR_ERR_UNSUPPORTED, "sgr_scan reads tables of fewer than 2^32 - 1 aggregates");
   // the control words come back to, and the bounds' bytes (each 16-byte aligned, at kPayloadOff in gb_dev) go up from, the
@@ -1713,33 +1727,6 @@ int32_t sgr_get_stats(sgr_engine* e, sgr_stats* out) {
   return SGR_OK;
 }
 
-// Exact replay of the slots that saw a throwing event in a sort-free fold: the batch is grouped once (K5) and exactly those
-// slots are folded sequentially onto their untouched prior states (exact err_idx, state kept: PersistentActor.scala:260-263).
-// h_throwing / h_dropped: aggregates in error, events dropped after their throw.
-static int32_t replay_throwing_slots(sgr_engine* e, const void* d_records, uint64_t n_records, uint64_t n_agg, const uint32_t* d_err_ids,
-                                     uint64_t n_err, unsigned long long* h_throwing, unsigned long long* h_dropped) {
-  DevBuf& grouped = e->group.batch_records;
-  CUDA_TRY(e, grouped.reserve(n_records * 64));
-  CUDA_TRY(e, e->inc_offsets.reserve((n_agg + 2) * 8));
-  unsigned long long bad = 0;
-  cudaError_t ce = group_by_agg_stable(e->group, (const uint8_t*)d_records, n_records, n_agg, (uint8_t*)grouped.p, (uint64_t*)e->inc_offsets.p,
-                                       nullptr, nullptr, (unsigned long long*)e->counters.p, e->stream, &bad);
-  if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "group-by (replay): %s", cudaGetErrorString(ce));
-  CUDA_TRY(e, cudaMemsetAsync(e->counters.p, 0, 64, e->stream));
-  FoldArgs a{};
-  a.events = (const uint8_t*)grouped.p; a.seg_offsets = (const uint64_t*)e->inc_offsets.p; a.n_seg = n_err;
-  a.seg_list = d_err_ids; a.states_in = (const uint8_t*)e->states.p; a.states_out = (uint8_t*)e->states.p;
-  a.counters = (unsigned long long*)e->counters.p;
-  FoldLaunchInfo info{};
-  cudaError_t le2 = launch_fold_stream(a, e->dprog, -1, e->num_sms, e->max_record_bytes, e->stream, &info);
-  if (le2 != cudaSuccess) return fail(e, SGR_ERR_CUDA, "replay launch: %s", cudaGetErrorString(le2));
-  unsigned long long h2[8];
-  CUDA_TRY(e, cudaMemcpyAsync(h2, e->counters.p, 64, cudaMemcpyDeviceToHost, e->stream));
-  CUDA_TRY(e, cudaStreamSynchronize(e->stream));
-  *h_throwing = h2[1]; *h_dropped = h2[4];
-  return SGR_OK;
-}
-
 static int32_t ensure_bulk_buffers(sgr_engine* e, uint64_t n_agg) {
   if (e->bulk_scratch_slots != n_agg || !e->bulk_scratch.p) {
     const size_t need = bulk_scratch_bytes(e->bulk_lay, n_agg);
@@ -1791,10 +1778,10 @@ static int32_t fold_arrival_order(sgr_engine* e, const uint8_t* d_records, uint6
     e->states_valid = true;
     e->loaded = false;
     if (e->bulk_ok && e->opt_bulk && n_records < (1ull << 30)) {
-      e->inc_atomic_prev_valid = false; e->inc_prev_n = 0;   // the next micro-batch clears every slot's per-batch flags
+      e->flagged.forget();
       return fold_bulk(e, d_records, n_records, n_agg);
     }
-    e->inc_atomic_prev_valid = true; e->inc_prev_upper = 0;   // a fresh all-None table: no per-batch flags to clear
+    e->flagged.nothing();   // a fresh all-None table: the micro-batch kernel has no flags to clear
     rc = fold_incremental_atomic(e, d_records, n_records);
     if (rc) return rc;
     e->stats.ms_group = 0;
@@ -1897,7 +1884,7 @@ int32_t sgr_dist_route_and_fold(sgr_engine* e, const void* d_records, uint64_t n
     rc = ensure_states(e, n_local); if (rc) return rc;
     rc = ensure_bulk_buffers(e, n_local); if (rc) return rc;
     CUDA_TRY(e, cudaMemsetAsync(e->states.p, 0, (size_t)n_local * e->program.state_bytes, e->stream));
-    e->states_valid = true; e->loaded = false; e->inc_atomic_prev_valid = false; e->inc_prev_n = 0;
+    e->states_valid = true; e->loaded = false; e->flagged.forget();
     PushFoldArgs pf{};
     pf.prog = &e->row_prog; pf.lay = &e->bulk_lay; pf.scratch = e->bulk_scratch.p; pf.states = (uint8_t*)e->states.p;
     pf.err_ids = (uint32_t*)e->bulk_err_ids.p; pf.counters = (unsigned long long*)e->bulk_counters.p; pf.n_slots = n_local;
@@ -2109,6 +2096,18 @@ int32_t sgr::put_decoded_poll(sgr_engine* e, const void* d_rows, const uint32_t*
   CUDA_TRY(e, cudaMemcpyAsync(pb, p.ctl, 64, cudaMemcpyDeviceToHost, e->stream));
   CUDA_TRY(e, cudaStreamSynchronize(e->stream));
   return put_apply_end(e, n_live, pb[kPbTouched]);
+}
+
+int32_t sgr::grow_states_for_ids(sgr_engine* e, uint64_t n_keys, uint64_t limit) {
+  OpLock op_lock(e);
+  if (!e) return SGR_ERR_INVALID;
+  if (e->states_valid && n_keys <= e->states_n) return SGR_OK;
+  // amortised doubling, like a hash table: the resize copies the table device to device
+  uint64_t cap = e->states_valid ? e->states_n : 0;
+  if (cap < 1024) cap = 1024;
+  while (cap < n_keys) cap *= 2;
+  if (cap > limit && limit >= n_keys) cap = limit;
+  return sgr_grow_states(e, cap);
 }
 
 int32_t sgr::engine_program_state_bytes(sgr_engine* e, uint32_t* state_bytes, bool* routed) {

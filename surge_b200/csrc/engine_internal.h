@@ -19,6 +19,10 @@ int32_t fold_decoded_poll(sgr_engine* e, const void* d_records, uint64_t n_recor
 // batch. The table already holds every index (the ingest grew it). n_live == 0: nothing is applied, the last fold's flags stay.
 int32_t put_decoded_poll(sgr_engine* e, const void* d_rows, const uint32_t* d_slots, const uint8_t* d_present, uint64_t n_slots, uint64_t n_live);
 
+// sgr_grow_states for the n_keys ids an ingest has numbered, unless the table holds them already: the rows double from 1024
+// until they do (a restore of many polls copies the table only a few times), but stop at `limit` when limit >= n_keys.
+int32_t grow_states_for_ids(sgr_engine* e, uint64_t n_keys, uint64_t limit);
+
 // The registered program's state bytes (0 without a program) and whether the engine is routed (sgr_dist_init).
 int32_t engine_program_state_bytes(sgr_engine* e, uint32_t* state_bytes, bool* routed);
 
