@@ -579,6 +579,9 @@ int32_t sgr_append_keys(sgr_engine* e, const void* owner, const uint8_t* keys, c
  *     poll with SGR_ERR_CAPACITY and applies nothing;
  *   - a refused poll applies nothing to the table, the positions or the statistics, but ids it interned stay in the device
  *     dictionary (they count against max_keys, and the next good poll reports them in n_new_keys);
+ *   - after SGR_ERR_CAPACITY the dictionary holds at most max_keys ids in at most max_id_bytes id bytes, and each of them is an
+ *     id that arrived; a later poll of ids it holds folds as usual, and a poll with an id it did not admit fails again, until
+ *     sgr_dingest_reset;
  *   - refusals follow the host decoder, which checks each batch in the order Kafka's consumer does: the CRC-32C first (a damaged
  *     batch is SGR_ERR_INVALID whatever else it claims); a batch of an aborted transaction is then skipped unread (its codec is
  *     not looked at, it is not decompressed); any other batch is SGR_ERR_UNSUPPORTED for a codec other than none / lz4, control

@@ -681,9 +681,11 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
       const int32_t rc = dfail(g, SGR_ERR_CAPACITY, "device id dictionary full (%llu ids / %llu id bytes allowed): create the device ingest with larger bounds", (unsigned long long)g->max_keys, (unsigned long long)g->arena_cap);
       discard_poll(g); return rc;
     }
-    st.n_markers = h[2]; st.n_null_values = h[3]; st.n_duplicates += h[4]; st.n_records = h[6]; st.n_new_keys = h[0] - g->keys_on_host;   // (ids a failed poll interned become visible with the next good one)
+    // ctl[0] and ctl[1] also count the claims a full dictionary refused (intern): the ids admitted are the first max_keys dense
+    // indices at most, their bytes within arena_cap
+    const uint64_t n_keys = std::min<uint64_t>(h[0], g->max_keys), id_bytes = std::min<uint64_t>(h[1], g->arena_cap);
+    st.n_markers = h[2]; st.n_null_values = h[3]; st.n_duplicates += h[4]; st.n_records = h[6]; st.n_new_keys = n_keys - g->keys_on_host;   // (ids a failed poll interned become visible with the next good one)
     // ---- grow the table for the new ids, hand their names to the engine's key table, fold
-    const uint64_t n_keys = h[0];
     if (const int32_t rc = grow_states_for_ids(g->eng, n_keys, g->max_keys)) {
       dfail(g, rc, "engine: %s", sgr_last_error(g->eng)); discard_poll(g); return rc;
     }
@@ -694,7 +696,7 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
     int32_t rc_append = SGR_OK;
     if (n_keys > g->keys_on_host) {
       const uint64_t add = n_keys - g->keys_on_host;
-      const uint64_t id_bytes_max = h[1] - g->id_bytes_on_host;   // (an upper bound: arena entries are padded to 8 bytes)
+      const uint64_t id_bytes_max = id_bytes - g->id_bytes_on_host;   // (an upper bound: arena entries are padded to 8 bytes)
       DG_TRY(g, g->key_offs_dev.reserve((add + 2) * 4 + (2 * (add / 4096 + 2) + 4 * 4096) * 4));
       DG_TRY(g, g->key_bytes_dev.reserve(id_bytes_max + 64));
       uint32_t* d_offs = (uint32_t*)g->key_offs_dev.p;
@@ -729,7 +731,7 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
     if (appender.joinable()) appender.join();
     if (rc_fold) { dfail(g, rc_fold, "engine: %s", sgr_last_error(g->eng)); discard_poll(g); return rc_fold; }
     if (rc_append) { dfail(g, rc_append, "engine: %s", sgr_last_error(g->eng)); discard_poll(g); return rc_append; }
-    g->keys_on_host = n_keys; g->id_bytes_on_host = h[1];
+    g->keys_on_host = n_keys; g->id_bytes_on_host = id_bytes;
   }
   lap(4);
   g->ms[5] = std::chrono::duration<float, std::milli>(Clk::now() - t_begin).count();

@@ -4,6 +4,9 @@
 // from an atomic counter, csrc/dingest_kernels.cu), and the engine's id index (csrc/id_index.cu) inserts ids whose dense index
 // is their position in the key table (insert_at) and answers batched recovery reads (find). The id order of the ordered scan
 // (csrc/id_order.cu) compares ids in Bytes order with cmp_ids.
+//
+// tests/fuzz/id_dict_main.cpp builds this header for the host (SGR_ID_DICT_HOST, with single-threaded stand-ins for the atomics
+// and cache-hinted loads) and checks intern, insert_at and find against a Python dict on ids built to share one tag.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -23,7 +26,7 @@ struct DgDict {           // device id dictionary: open addressing on a 64-bit h
   uint64_t max_keys, arena_cap;
 };
 
-#ifdef __CUDACC__
+#if defined(__CUDACC__) || defined(SGR_ID_DICT_HOST)
 namespace {
 
 __device__ __forceinline__ unsigned long long hash_id(const uint8_t* k, uint32_t len) {
@@ -43,12 +46,21 @@ __device__ __forceinline__ unsigned long long hash_id(const uint8_t* k, uint32_t
 }
 
 __device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) {
+#ifdef __CUDA_ARCH__
   uint32_t v;
   asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p));
   return v;
+#else
+  return *(const volatile uint32_t*)p;
+#endif
 }
 
 // id -> dense index. Returns 0xffffffff when the dictionary is full (the call then fails as a whole).
+//
+// A new id takes its arena bytes first and a dense index only if the bytes fit, so every index below max_keys is written and
+// none is lost to a claim refused on bytes. ctl[0] and ctl[1] still count refused claims: readers clamp them to max_keys and
+// arena_cap. A refused claim leaves its slot dead (slot_idx 0xffffffff): probes step over it, so an admitted id further along
+// the same chain is still found, and the refused id, arriving again, claims a new slot and is refused again.
 __device__ uint32_t intern(const DgDict& d, const uint8_t* id, uint32_t len) {
   const unsigned long long h = hash_id(id, len);
   uint64_t pos = h & d.slots_mask;
@@ -57,10 +69,10 @@ __device__ uint32_t intern(const DgDict& d, const uint8_t* id, uint32_t len) {
     if (tag == 0ull) {
       tag = atomicCAS(d.tags + pos, 0ull, h);
       if (tag == 0ull) {   // this thread owns the slot: the id is new
-        const unsigned long long idx = atomicAdd(d.ctl + 0, 1ull);
         const unsigned long long need = ((unsigned long long)len + 7) & ~7ull;
         const unsigned long long off = atomicAdd(d.ctl + 1, need);
-        if (idx >= d.max_keys || off + need > d.arena_cap) {
+        const unsigned long long idx = off + need <= d.arena_cap ? atomicAdd(d.ctl + 0, 1ull) : ~0ull;
+        if (idx >= d.max_keys) {
           atomicAdd(d.ctl + 5, 1ull);
           __threadfence();
           atomicExch(d.slot_idx + pos, 0xffffffffu);
@@ -76,7 +88,7 @@ __device__ uint32_t intern(const DgDict& d, const uint8_t* id, uint32_t len) {
     if (tag != h) continue;
     uint32_t v;
     while ((v = ld_volatile_u32(d.slot_idx + pos)) == 0u) __nanosleep(40);   // the owner is still writing the id
-    if (v == 0xffffffffu) return 0xffffffffu;
+    if (v == 0xffffffffu) continue;                                           // a dead slot
     __threadfence();
     // (L2 loads: an L1 line fetched before the owner wrote its part would be stale)
     const uint2 ref = __ldcg(d.key_ref + (v - 1u));
