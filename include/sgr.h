@@ -60,7 +60,9 @@ extern "C" {
  * Fixed record (SGR_REC_FIXED64): 64 bytes, little-endian, 64-byte aligned in the log
  *   +0  u32 type      event type = index into the program's rule table
  *   +4  u32 seq       sequence number (Counter: sequenceNumber)
- *   +8  u64 agg       dense aggregate index (or global index before routing)
+ *   +8  u64 agg       dense aggregate index (or global index before routing). A program may read it like any
+ *                     other bytes, except on a routed engine: there sgr_dist_route_and_fold refuses a program
+ *                     with an op reading any of bytes 8..15 (SGR_ERR_UNSUPPORTED), see the multi-GPU block
  *   +16 u8  payload[48]  program-defined view (Counter: i32 by @16;
  *                        BankAccount: uuid @16, f64 balance @32, owner @40, code @56)
  *
@@ -413,12 +415,19 @@ int32_t sgr_dist_ipc_import(sgr_engine* e, const void* handles64_by_rank);
  *               every rank repeats the exchange in ordered mode (decoupled look-back) — automatically on real ranks, by
  *               SGR_ERR_AGAIN + option "push_ordered" on loopback ranks.
  *   fused == 3  as 2, but only the record words the fold program reads cross NVLink (u32 local index + slot words:
- *               16 bytes per record for the Counter model). */
+ *               16 bytes per record for the Counter model); a program that reads more than 7 record words (event type
+ *               included) is refused with SGR_ERR_UNSUPPORTED, use fused == 2.
+ * On a routed engine (nranks > 1, or option "force_route") what arrives in a record's aggregate field depends on the mode (the
+ * owner's local index, the record's index within its chunk, or the global index), so a program with an op that reads any of
+ * record bytes 8..15 is refused with SGR_ERR_UNSUPPORTED on every rank, before anything is launched or exchanged. */
 int32_t sgr_dist_route_and_fold(sgr_engine* e, const void* d_records, uint64_t n_records, int32_t fused);
 /* Several ranks inside ONE process on one device ("loopback", for single-GPU tests of the multi-rank logic): sgr_dist_init with
  * unique_id128 == NULL and nranks > 1 creates such a rank; the ranks hand each other their receive allocation as plain device
  * pointers (sgr_dist_recv_base -> sgr_dist_set_peers) and the caller runs every rank's sgr_dist_route_and_fold(fused >= 2)
- * concurrently (one host thread per rank), with a barrier of its own between calls. fused <= 1 needs NCCL and is refused. */
+ * concurrently (one host thread per rank), with a barrier of its own between calls. fused <= 1 needs NCCL and is refused.
+ * The ranks' streams share the device's hardware queues, so inside the call each loopback rank enqueues all of its partition
+ * and flag kernels, then waits on the host for its peers to do the same (at most 60 s, else SGR_ERR_DIST), and only then
+ * enqueues the kernels that wait for arrival flags: a waiting kernel never stands in a queue ahead of a flag it waits for. */
 int32_t sgr_dist_recv_base(sgr_engine* e, void** base);
 /* Allocate everything sgr_dist_route_and_fold(fused >= 2) needs for logs of up to max_records records now (after
  * sgr_dist_set_partitions and the "push_chunks" option), so that the call itself allocates nothing. Optional for real ranks;

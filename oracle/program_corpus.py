@@ -48,6 +48,148 @@ def draw_program(rng):
     return state_bytes, rules, f64
 
 
+# ------------------------------------------------------------------ sort-free programs (bulk_fold.cu, route_push.cu)
+# The four bulk entry layouts by (mode of state word 0, mode of state word 1). CREATE and TOMBSTONE reset both words, which
+# makes both set words (fold_rows.cu build_row_program), so tombstones and CREATE come only with ("set", "set").
+LAYOUTS = [("add", "add"), ("add", "set"), ("set", "add"), ("set", "set")]
+# record words a sort-free program may read: the type word, seq, and the payload words 4..15 (bytes 16..63); words 2 and 3
+# hold the aggregate index
+SORT_FREE_SOURCES = [0, 1] + list(range(4, 16))
+
+
+def draw_sort_free_program(rng, layout=None, tombstones=None, n_types=None, n_src=None):
+    """A 16-byte class-0 program in which each state word is add-only or set-only: MATERIALISE / CREATE / TOMBSTONE / THROW
+    rules, 32-bit ops only. layout: one of LAYOUTS; tombstones: only with ("set", "set"); n_types: 1..16 (raised to fit the
+    sources); n_src: distinct record words read, 1..14 (n_slots = 1 + n_src: 2..7 fit a compact exchange record, 8 and more
+    do not). Returns (rules, n_slots)."""
+    layout = tuple(layout) if layout is not None else LAYOUTS[int(rng.integers(0, 4))]
+    both_set = layout == ("set", "set")
+    if tombstones is None:
+        tombstones = both_set and rng.random() < 0.5
+    assert both_set or not tombstones, "a tombstone resets both words: only the (set, set) layout has tombstones"
+    n_src = int(rng.integers(1, 7)) if n_src is None else int(n_src)
+    pool = [int(w) for w in rng.choice(SORT_FREE_SOURCES, size=n_src, replace=False)]
+    todo = list(pool)
+    n_op_rules = -(-n_src // 2)
+    n_types = int(rng.integers(1, 17)) if n_types is None else int(n_types)
+    n_types = min(16, max(n_types, n_op_rules + int(tombstones)))
+    writers = [I.MATERIALISE, I.CREATE] if both_set else [I.MATERIALISE]
+    extra = writers + [I.MATERIALISE, I.THROW] + ([I.TOMBSTONE] if tombstones else [])
+
+    def op(word, ex):
+        src = todo.pop() if todo else int(rng.choice(pool))
+        if layout[word] == "add":
+            opc = int(rng.choice([I.OP_ADD_I32, I.OP_SUB_I32]))
+        else:   # over a reset state (CREATE) an ADD or a SUB is a set too
+            opc = int(rng.choice([I.OP_SET, I.OP_ADD_I32, I.OP_SUB_I32])) if ex == I.CREATE else I.OP_SET
+        return (opc, 4 * int(word), 4 * src, 4)
+
+    rules = []
+    for t in range(n_types):
+        if t < n_op_rules:   # these rules read every source once and write both words, so the layout is what was asked
+            ex = int(rng.choice(writers))
+            ops = [op(w, ex) for w in rng.permutation(2)]
+        else:
+            ex = int(rng.choice(extra))
+            if t == n_op_rules and tombstones:
+                ex = I.TOMBSTONE
+            ops = [] if ex in (I.TOMBSTONE, I.THROW) else [op(int(w), ex) for w in rng.permutation(2)[:int(rng.integers(0, 3))]]
+        rules.append((ex, ops))
+    assert not todo
+    order = rng.permutation(n_types)
+    return [rules[int(i)] for i in order], 1 + n_src
+
+
+def row_slots(rules):
+    """n_slots of fold_rows.cu build_row_program for a program it accepts: slot 0 is the event type, then one slot per
+    distinct record word the ops read (a read of the type word takes a slot of its own)."""
+    words = set()
+    for ex, ops in rules:
+        if ex in (I.TOMBSTONE, I.THROW):
+            continue
+        for _, _, src, ln in ops:
+            words.update(range(src // 4, (src + ln) // 4))
+    return 1 + len(words)
+
+
+def bulk_layout(rules, state_bytes=16):
+    """Twin of bulk_fold.cu bulk_layout_for (after build_row_program): None when the program is outside the sort-free class,
+    else dict(set_only_mask, has_none, entry_shift, word_off, last_needed_mask)."""
+    if state_bytes != 16 or len(rules) > 16 or any(ex == I.IF_EXISTS for ex, _ in rules):
+        return None
+    has_add = has_set = has_none = 0
+    sets_of = {}
+    for t, (ex, ops) in enumerate(rules):
+        if ex == I.THROW:
+            continue
+        reset = ex in (I.CREATE, I.TOMBSTONE)
+        mode = [2, 2] if reset else [0, 0]
+        written = [False, False]
+        for opc, dst, src, ln in ([] if ex == I.TOMBSTONE else ops):
+            if opc > I.OP_SUB_I32 or src + ln > 64:
+                return None
+            for j in range(ln // 4):
+                w = dst // 4 + j
+                if w >= 2 or written[w]:
+                    return None
+                written[w] = True
+                mode[w] = 2 if (opc == I.OP_SET or reset) else 1
+        if row_slots(rules) > 16:
+            return None
+        has_none |= ex == I.TOMBSTONE
+        for w in range(2):
+            has_add |= (mode[w] == 1) << w
+            has_set |= (mode[w] == 2) << w
+        sets_of[t] = 2 in mode
+    if has_add & has_set:
+        return None
+    n_set = bin(has_set & 3).count("1")
+    if n_set == 2:
+        shift, word_off = 5, [8, 16]
+    elif n_set == 1:
+        ws = 0 if has_set & 1 else 1
+        shift, word_off = 4, [0, 0]
+        word_off[ws], word_off[ws ^ 1] = 8, 4
+    else:
+        shift, word_off = 4, [4, 8]
+    last = 0
+    for t, sets in sets_of.items():
+        if has_none or not sets:
+            last |= 1 << t
+    return dict(set_only_mask=has_set, has_none=int(has_none), entry_shift=shift, word_off=word_off, last_needed_mask=last)
+
+
+# MatchError types a routed log carries besides n_types..15: the projected record keeps min(type, 16) in 5 bits, so types of
+# 32 and more are where a missing clamp would wrap into a valid type
+FAR_TYPES = [16, 17, 32, 33, 48, 1 << 31, 0xFFFFFFFF]
+
+
+def draw_sort_free_log(rng, rules, n_agg, n_rec, hot_len, p_throw=0.0, p_empty=0.1, p_zero=0.05):
+    """Fixed records in CSR order over n_agg aggregates (about n_rec records, the aggregate index at +8): random payload
+    words and a random seq (set values are not monotone along an aggregate), a share p_empty of empty aggregates, one hot
+    aggregate of hot_len records, record words 4..15 zero with probability p_zero (ADDs of 0), and with probability p_throw a
+    throwing type: a THROW rule or a MatchError (n_types..15 and FAR_TYPES). Returns (records [n, 64] u8, seg_offsets, hot)."""
+    counts = rng.geometric(1.0 / (n_rec / n_agg + 1), size=n_agg) - 1
+    counts[rng.random(n_agg) < p_empty] = 0
+    hot = int(rng.integers(0, n_agg))
+    counts[hot] = hot_len
+    n = int(counts.sum())
+    rec = rng.integers(0, 256, size=(n, 64), dtype=np.uint8)
+    words = rec.view(np.uint32)
+    zero = rng.random((n, 12)) < p_zero
+    words[:, 4:16][zero] = 0
+    ok = np.array([t for t, (ex, _) in enumerate(rules) if ex != I.THROW], dtype=np.uint32)
+    bad = np.array([t for t, (ex, _) in enumerate(rules) if ex == I.THROW] + list(range(len(rules), 16)) + FAR_TYPES, dtype=np.uint32)
+    types = ok[rng.integers(0, len(ok), size=n)] if len(ok) else bad[rng.integers(0, len(bad), size=n)]
+    hit = rng.random(n) < p_throw
+    types[hit] = bad[rng.integers(0, len(bad), size=int(hit.sum()))]
+    words[:, 0] = types
+    words[:, 2:4] = np.repeat(np.arange(n_agg, dtype=np.uint64), counts).view(np.uint32).reshape(-1, 2)
+    off = np.zeros(n_agg + 1, dtype=np.uint64)
+    np.cumsum(counts * 64, out=off[1:])
+    return rec, off, hot
+
+
 def draw_log(rng, n_types, n_agg, long_len, f64):
     counts = rng.integers(0, 13, size=n_agg)
     counts[rng.integers(0, n_agg)] = long_len

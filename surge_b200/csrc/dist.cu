@@ -24,6 +24,8 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <chrono>
+#include <map>
 #include <string>
 #include <vector>
 
@@ -287,6 +289,29 @@ int dist_ipc_import(DistState* d, const void* handles, std::string* err) {
   return SGR_OK;
 }
 
+bool LoopbackGroup::arrive_and_wait(int seconds) {
+  std::unique_lock<std::mutex> l(mu);
+  const uint64_t gen = generation;
+  if (++arrived == nranks) { arrived = 0; ++generation; cv.notify_all(); return true; }
+  if (cv.wait_for(l, std::chrono::seconds(seconds), [&] { return generation != gen; })) return true;
+  --arrived;
+  return false;
+}
+
+// the group of the loopback ranks whose rank 0 owns receive allocation `key` (one group per live job)
+static std::shared_ptr<LoopbackGroup> loopback_group(const void* key, int nranks) {
+  static std::mutex mu;
+  static std::map<const void*, std::weak_ptr<LoopbackGroup>> groups;
+  std::lock_guard<std::mutex> l(mu);
+  std::shared_ptr<LoopbackGroup> g = groups[key].lock();
+  if (!g || g->nranks != nranks) {
+    g = std::make_shared<LoopbackGroup>();
+    g->nranks = nranks;
+    groups[key] = g;
+  }
+  return g;
+}
+
 // loopback ranks (one process, one device): the other ranks' receive allocations as plain device pointers
 int dist_set_peers(DistState* d, void* const* bases, std::string* err) {
   if (!d->loopback) { *err = "sgr_dist_set_peers is for loopback ranks (sgr_dist_init without a unique id)"; return SGR_ERR_INVALID; }
@@ -296,6 +321,7 @@ int dist_set_peers(DistState* d, void* const* bases, std::string* err) {
     d->peer_base[r] = (uint8_t*)bases[r];
     d->peer_recv[r] = (uint8_t*)bases[r] + kRecvHeaderBytes;
   }
+  d->group = loopback_group(d->peer_base[0], d->nranks);
   d->peers_mapped = true;
   return SGR_OK;
 }

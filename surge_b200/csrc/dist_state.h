@@ -4,6 +4,9 @@
 #include <nccl.h>
 #include <stdint.h>
 
+#include <condition_variable>
+#include <memory>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -32,6 +35,18 @@ struct NcclApi {
 };
 NcclApi& nccl_api();
 
+// Loopback ranks are streams of one process on one device, and streams share the device's hardware queues, each run in order.
+// A fold launch that waits for its rank's spinning wait kernel can stand at the head of a queue and hold back a peer's partition
+// or flag kernel queued behind it, and the wait spins until its limit. So every loopback rank enqueues all its partition and flag
+// kernels, meets its peers here, and only then enqueues its waits and folds: nothing a wait needs is ever queued behind a wait.
+struct LoopbackGroup {
+  std::mutex mu;
+  std::condition_variable cv;
+  int nranks = 0, arrived = 0;
+  uint64_t generation = 0;
+  bool arrive_and_wait(int seconds);   // false: a peer did not arrive in time (it left the barrier as it found it)
+};
+
 struct DistState {
   int rank = 0, nranks = 1;
   bool loopback = false;                 // several ranks inside one process (tests): no NCCL, peers handed over as raw pointers
@@ -53,6 +68,7 @@ struct DistState {
   cudaEvent_t pev[4] = {};
   uint32_t epoch = 0;
   void* h_pinned = nullptr;              // page-locked landing area of the per-call read-backs
+  std::shared_ptr<LoopbackGroup> group;  // loopback ranks: shared by the ranks whose rank 0 has the same receive allocation
 };
 
 }  // namespace sgr

@@ -544,6 +544,25 @@ int dist_push_fold(DistState* d, const uint8_t* d_records, uint64_t n, const Pus
   DTRY(cudaStreamWaitEvent(s1, d->pev[0], 0));
   DTRY(cudaStreamWaitEvent(sp, d->pev[0], 0));
   unsigned long long* my_flags = (unsigned long long*)d->peer_base[d->rank];
+  // receiver side of chunk c: wait for the flags of every source, then the sort-free accumulate over the chunk's regions
+  auto fold_chunk = [&](uint32_t c) -> cudaError_t {
+    push_wait_kernel<<<1, 32, 0, s1>>>(my_flags, c, (uint32_t)R, epoch, status);
+    BulkSrc bs{};
+    bs.n_regions = (uint32_t)R; bs.compact = pf.compact ? 1u : 0u; bs.rec_bytes = out_bytes; bs.rotate = (uint32_t)d->rank; bs.carried = 1;
+    bs.blocks_per_sm = push_tuning().fold_blocks_per_sm > 0 ? (uint32_t)push_tuning().fold_blocks_per_sm : 0xffffffffu;
+    for (int s = 0; s < R; ++s) {
+      // pull: source s keeps what it has for me in ITS buffer, region (me, chunk): the fold reads it over NVLink
+      bs.base[s] = pull ? d->peer_recv[s] + ((uint64_t)d->rank * C + c) * cap_region * out_bytes
+                        : d->peer_recv[d->rank] + ((uint64_t)s * C + c) * cap_region * out_bytes;
+      bs.count_flag[s] = my_flags + (size_t)s * kMaxChunks + c;
+      bs.count[s] = cap_region;
+      // + the index the record carries within ITS SOURCE's chunk c. The sources cut their logs into chunks of different lengths
+      // (each from its own record count), so the base must not depend on any rank's chunk length: a fixed stride that bounds
+      // them all keeps the arrival index monotone along every aggregate's log
+      bs.idx_base[s] = (uint32_t)((uint64_t)c * idx_stride);
+    }
+    return launch_bulk_accumulate(bs, pf.n_slots, pf.scratch, *pf.prog, *pf.lay, pf.counters, pf.num_sms, s1);
+  };
   for (uint32_t c = 0; c < C; ++c) {
     const uint64_t begin = (uint64_t)c * chunk_recs;
     const uint64_t cn = begin >= n ? 0 : (n - begin < chunk_recs ? n - begin : chunk_recs);
@@ -577,23 +596,12 @@ int dist_push_fold(DistState* d, const uint8_t* d_records, uint64_t n, const Pus
     for (int q = 0; q < R; ++q) f.peer_flag[q] = (unsigned long long*)d->peer_base[q] + (size_t)d->rank * kMaxChunks + c;
     f.totals = totals + (size_t)c * kMaxRanks; f.status = status; f.nranks = (uint32_t)R; f.epoch = epoch;
     push_flag_kernel<<<1, 32, 0, sp>>>(f);
-    // ---- receiver side of chunk c
-    push_wait_kernel<<<1, 32, 0, s1>>>(my_flags, c, (uint32_t)R, epoch, status);
-    BulkSrc bs{};
-    bs.n_regions = (uint32_t)R; bs.compact = pf.compact ? 1u : 0u; bs.rec_bytes = out_bytes; bs.rotate = (uint32_t)d->rank; bs.carried = 1;
-    bs.blocks_per_sm = push_tuning().fold_blocks_per_sm > 0 ? (uint32_t)push_tuning().fold_blocks_per_sm : 0xffffffffu;
-    for (int s = 0; s < R; ++s) {
-      // pull: source s keeps what it has for me in ITS buffer, region (me, chunk): the fold reads it over NVLink
-      bs.base[s] = pull ? d->peer_recv[s] + ((uint64_t)d->rank * C + c) * cap_region * out_bytes
-                        : d->peer_recv[d->rank] + ((uint64_t)s * C + c) * cap_region * out_bytes;
-      bs.count_flag[s] = my_flags + (size_t)s * kMaxChunks + c;
-      bs.count[s] = cap_region;
-      // + the index the record carries within ITS SOURCE's chunk c. The sources cut their logs into chunks of different lengths
-      // (each from its own record count), so the base must not depend on any rank's chunk length: a fixed stride that bounds
-      // them all keeps the arrival index monotone along every aggregate's log
-      bs.idx_base[s] = (uint32_t)((uint64_t)c * idx_stride);
-    }
-    DTRY(launch_bulk_accumulate(bs, pf.n_slots, pf.scratch, *pf.prog, *pf.lay, pf.counters, pf.num_sms, s1));
+    if (!d->group) DTRY(fold_chunk(c));
+  }
+  if (d->group) {   // loopback ranks: every rank's partition and flag kernels are queued before any rank queues a wait
+    DTRY(cudaGetLastError());
+    if (!d->group->arrive_and_wait(60)) { *err = "time-out waiting for the other loopback ranks to enter the exchange"; return SGR_ERR_DIST; }
+    for (uint32_t c = 0; c < C; ++c) DTRY(fold_chunk(c));
   }
   DTRY(cudaGetLastError());
   DTRY(cudaEventRecord(d->pev[1], sp));    // all partition kernels done and flagged

@@ -158,3 +158,79 @@ def test_sample_programs_match_the_sample_model_oracle(name, model, make):
     got2, gev2, gerr2 = I.c_fold(rules, sb, rec, off, initial=want, f64_fields=f64)
     same(got2, want2, name + " with prior states")
     assert (gev2, gerr2) == (nev2, nerr2), name
+
+
+# ------------------------------------------------------------------ sort-free programs (the bulk fold and the routed path)
+def draw_sort_free_case(seed):
+    """One drawn sort-free program per seed, cycling through the four layouts, with and without tombstones, and 1..14 sources."""
+    rng = np.random.default_rng(35000 + seed)
+    layout = PC.LAYOUTS[seed % 4]
+    tomb = layout == ("set", "set") and (seed // 4) % 2 == 1
+    n_src = 1 + seed % 6 if seed % 10 else int(rng.integers(7, 15))
+    rules, n_slots = PC.draw_sort_free_program(rng, layout=layout, tombstones=tomb, n_src=n_src)
+    return rng, layout, tomb, rules, n_slots
+
+
+@pytest.mark.parametrize("seed", range(300))
+def test_sort_free_programs_have_their_layout_and_match_the_interpreter(seed):
+    rng, layout, tomb, rules, n_slots = draw_sort_free_case(seed)
+    lay = PC.bulk_layout(rules)
+    what = f"seed {seed} layout {layout} tombstones {tomb} rules {rules}"
+    assert lay is not None, what
+    assert lay["set_only_mask"] == sum(1 << w for w in range(2) if layout[w] == "set"), what
+    assert lay["has_none"] == int(tomb), what
+    assert PC.row_slots(rules) == n_slots, what
+    rec, off, _ = PC.draw_sort_free_log(rng, rules, 60, 400, 150, p_throw=0.02)
+    want = I.fold(rules, 16, rec, off)
+    got, nev, nerr = I.c_fold(rules, 16, rec, off)
+    same(got, want, what)
+    assert (nev, nerr) == implied_stats(want, 16, np.diff(off.astype(np.int64)) // 64), what
+
+
+def test_bulk_layout_twin_on_known_programs():
+    """bulk_fold.cu bulk_layout_for by hand: the Counter (add, set), the snapshot restore (set, set) with tombstones, and
+    programs outside the class (a word both set and added, IF_EXISTS, a 32-byte state, a 64-bit add)."""
+    counter = rules_of(P.counter_program())
+    assert PC.bulk_layout(counter) == dict(set_only_mask=2, has_none=0, entry_shift=4, word_off=[4, 8], last_needed_mask=0b0100)
+    restore = [(I.CREATE, [(I.OP_SET, 0, 16, 4), (I.OP_SET, 4, 20, 4)]), (I.TOMBSTONE, [])]
+    assert PC.bulk_layout(restore) == dict(set_only_mask=3, has_none=1, entry_shift=5, word_off=[8, 16], last_needed_mask=0b11)
+    set_add = [(I.MATERIALISE, [(I.OP_SET, 0, 4, 4), (I.OP_ADD_I32, 4, 16, 4)]), (I.MATERIALISE, []), (I.THROW, [])]
+    assert PC.bulk_layout(set_add) == dict(set_only_mask=1, has_none=0, entry_shift=4, word_off=[8, 4], last_needed_mask=0b10)
+    assert PC.bulk_layout([(I.MATERIALISE, [(I.OP_SET, 0, 16, 4)]), (I.MATERIALISE, [(I.OP_ADD_I32, 0, 20, 4)])]) is None
+    assert PC.bulk_layout([(I.IF_EXISTS, [(I.OP_SET, 0, 16, 4)])]) is None
+    assert PC.bulk_layout([(I.MATERIALISE, [(I.OP_SET, 0, 16, 4)])], state_bytes=32) is None
+    assert PC.bulk_layout([(I.MATERIALISE, [(I.OP_ADD_I64, 0, 16, 8)])]) is None
+    assert PC.bulk_layout([(I.MATERIALISE, [(I.OP_SET, 0, 16, 4), (I.OP_SET, 0, 20, 4)])]) is None   # a word written twice
+
+
+def test_the_sort_free_draws_cover_what_the_routed_tests_claim():
+    """The draws reach every layout with and without tombstones, rules without ops, SUB, 1..16 types, 2..7 slots and 8 or
+    more, and reads of the type word, seq, bytes 16..31 and bytes 32..63; the log carries ADDs of 0 and every MatchError."""
+    seen = set()
+    for seed in range(300):
+        _, layout, tomb, rules, n_slots = draw_sort_free_case(seed)
+        seen.add((layout, tomb))
+        seen.add(("types", len(rules)))
+        seen.add(("slots", min(n_slots, 8)))
+        for ex, ops in rules:
+            if ex in (I.MATERIALISE, I.CREATE) and not ops:
+                seen.add("no ops")
+            for opc, _, src, _ in ops:
+                seen.add("sub" if opc == I.OP_SUB_I32 else "op")
+                seen.add(("read", 0 if src == 0 else 1 if src == 4 else 16 if src < 32 else 32))
+    for layout in PC.LAYOUTS:
+        assert (layout, False) in seen
+    assert (("set", "set"), True) in seen
+    assert {("types", k) for k in range(1, 17)} <= seen, sorted(x for x in seen if x[0] == "types")
+    assert {("slots", k) for k in range(2, 9)} <= seen
+    assert {"no ops", "sub", ("read", 0), ("read", 1), ("read", 16), ("read", 32)} <= seen
+    rng = np.random.default_rng(5)
+    rules, _ = PC.draw_sort_free_program(rng, layout=("add", "add"), n_types=3)
+    rec, off, hot = PC.draw_sort_free_log(rng, rules, 100, 20_000, 4096, p_throw=0.05)
+    types = rec[:, 0:4].copy().view(np.uint32).ravel()
+    assert set(range(3, 16)) | set(PC.FAR_TYPES) <= set(types.tolist())
+    assert (rec[:, 16:20].copy().view(np.uint32) == 0).any()
+    assert int(off[hot + 1] - off[hot]) // 64 == 4096
+    assert (np.diff(off.astype(np.int64)) == 0).any()
+    rec0, _, _ = PC.draw_sort_free_log(rng, rules, 100, 20_000, 10, p_throw=0.0)
+    assert (rec0[:, 0:4].copy().view(np.uint32) < 3).all()
