@@ -266,7 +266,8 @@ int32_t sgr_get_index(sgr_engine* e, uint64_t agg, void* out, uint32_t cap,
  * the engine's operation lock throughout and waits for an sgr_fold_async first: every row of a batch comes from one table
  * generation, and batch readers serialise (one call should carry many ids). SGR_ERR_STATE before any fold; SGR_ERR_INVALID on
  * non-monotone key_offsets or a duplicate id in the key table; SGR_ERR_CAPACITY (nothing written) when
- * cap < n * (state_bytes - 8). n == 0 is a no-op. */
+ * cap < n * (state_bytes - 8); SGR_ERR_UNSUPPORTED on a routed engine without a current rank key table (sgr_dist_load_keys),
+ * whose rows are local slots. n == 0 is a no-op. */
 int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n,
                       void* out, uint64_t cap, uint32_t* flags, int64_t* indices);
 
@@ -288,7 +289,8 @@ int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_of
  * byte states, FIXED64 or VAR16 records: rows are states, not records), and on an engine without a table, which it creates.
  * Key table: one of sgr_load_keys, one built by earlier put batches, or none. SGR_ERR_STATE (nothing applied) when it mirrors
  * an ingest's id dictionary (sgr_fold_ingested, the device ingest, sgr_append_keys), which numbers new ids itself;
- * SGR_ERR_UNSUPPORTED on a routed engine (sgr_dist_init).
+ * SGR_ERR_UNSUPPORTED on a routed engine (sgr_dist_init), with or without a rank key table: a new id would need a global
+ * aggregate index and an owner, which only the partition table can give.
  * All or nothing: SGR_ERR_INVALID on NULL arguments, non-monotone key_offsets or a duplicate id in the key table;
  * SGR_ERR_CAPACITY when the key table would reach 2^32 - 1 ids or pass 4 GiB of id bytes; SGR_ERR_UNSUPPORTED for n >= 2^32;
  * n == 0 is a no-op. Holds the operation lock and waits for an sgr_fold_async, as sgr_get_batch does. */
@@ -312,7 +314,7 @@ int32_t sgr_put_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_of
  * Holds the operation lock and waits for an sgr_fold_async, as sgr_get_batch does. SGR_ERR_STATE before any fold;
  * SGR_ERR_INVALID on NULL arguments, a bad select, max_rows == 0 or cur->next > n_agg; SGR_ERR_CAPACITY (nothing written,
  * the cursor unchanged) when the first selected row's id alone exceeds ids_cap; SGR_ERR_UNSUPPORTED on a routed engine
- * (sgr_dist_init), whose rows are local slots. */
+ * without a current rank key table (sgr_dist_load_keys), whose rows are local slots. */
 typedef struct sgr_changes_cursor {
   uint64_t next;     /* in/out: first dense index not yet reported; 0 starts an export; n_agg when the export is complete */
   uint64_t token;    /* in/out: 0 on the first page; the engine sets it and later pages pass it back */
@@ -345,7 +347,7 @@ int32_t sgr_export_changes(sgr_engine* e, uint32_t select, sgr_changes_cursor* c
  * max_rows + 1 u32, ids ids_cap bytes (NULL when ids_cap == 0).
  * SGR_ERR_STATE before any fold; SGR_ERR_INVALID on NULL buffers, max_rows == 0 or a duplicate id in the key table;
  * SGR_ERR_CAPACITY (nothing written) when the first row's id alone exceeds ids_cap; SGR_ERR_UNSUPPORTED on a routed engine
- * (sgr_dist_init), whose rows are local slots, and for tables of 2^32 - 1 rows or more. */
+ * without a current rank key table (sgr_dist_load_keys), whose rows are local slots, and for tables of 2^32 - 1 rows or more. */
 int32_t sgr_scan(sgr_engine* e, const uint8_t* from, uint32_t from_len, int32_t from_exclusive, const uint8_t* to, uint32_t to_len,
                  uint64_t max_rows, void* rows, uint32_t* flags, int64_t* indices, uint8_t* ids, uint64_t ids_cap,
                  uint32_t* id_offsets, uint64_t* n_rows, int32_t* more);
@@ -441,6 +443,25 @@ int32_t sgr_states_hash(sgr_engine* e, uint64_t* out);
 int32_t sgr_dist_get_stats(sgr_engine* e, sgr_dist_stats* out);
 /* global aggregate index of each local state slot (host copy, n_local u32) */
 int32_t sgr_dist_local_aggregates(sgr_engine* e, uint32_t* out, uint64_t cap, uint64_t* n_local);
+/* The key table of a routed rank: keys[key_offsets[g] .. key_offsets[g+1]) is the id of GLOBAL aggregate g, for every g of the
+ * partition table (n_global == the n_global_agg of sgr_dist_set_partitions). The engine keeps the ids of the aggregates this
+ * rank owns, in local-slot order: id i of the rank's key table is that of global aggregate sgr_dist_local_aggregates()[i].
+ * Each Surge node answers getAggregateBytes, range and all from the KTable partitions it owns; with this table a rank does the
+ * same from its rows. sgr_get, sgr_get_batch(_values), sgr_export_changes(_values), sgr_scan(_values) and sgr_set_state_writer
+ * then serve the rank as they serve one engine, over the rank's rows: a dense index is a local slot (the row order of
+ * sgr_export_states), and an id another rank owns is unknown, as a KTable miss is. After sgr_dist_route_and_fold every row is
+ * flagged, so sgr_export_changes(SGR_ST_CHANGED | SGR_ST_ERROR) pages the rank's share of a republished state topic.
+ * The ids are gathered on the host and installed as sgr_load_keys installs a table: ingest ids are dropped, the key-table
+ * epoch advances (an export in progress ends with SGR_ERR_STATE) and the device id index and id order are rebuilt by the
+ * next read. The table stays current until sgr_dist_init, sgr_dist_set_partitions, sgr_load_keys, sgr_append_keys or an
+ * ingest replaces it; after that the reads are refused again until this call is repeated.
+ * The partition table is the caller's contract: when it disagrees with KafkaPartitionProvider.partitionForKey of the ids, a
+ * rank holds ids the router would never send it.
+ * SGR_ERR_NOT_LOADED before sgr_dist_init and sgr_dist_set_partitions; SGR_ERR_INVALID (the key table unchanged) on NULL
+ * arguments, non-monotone key_offsets, n_global different from the partition table's size, or two equal ids among the ones
+ * this rank owns (as sgr_load_keys). sgr_put_batch and the state-topic mode of the device ingest stay refused on a routed
+ * engine: they number new ids themselves, which a partition table cannot hold. */
+int32_t sgr_dist_load_keys(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n_global);
 
 /* ------------------------------------------------------------------ ingest: Kafka record batches -> packed records (SURVEY §8 f1, f2)
  * What feeds the store today is a Kafka consumer in read_committed mode
@@ -621,7 +642,8 @@ int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, c
  * (SurgeModel.scala:64), value = the serialized state, null deletes, the last write per key wins.
  * When: SGR_ERR_STATE while a poll is pending, after any successful fold since create or sgr_dingest_reset (one dictionary and
  * one set of positions belong to one topic), and once a JSON member table is registered (its offsets mean different things in
- * the two modes: set the mode first). SGR_ERR_UNSUPPORTED on a routed engine (sgr_dist_init), as sgr_put_batch. The mode
+ * the two modes: set the mode first). SGR_ERR_UNSUPPORTED on a routed engine (sgr_dist_init), with or without a rank key
+ * table, as sgr_put_batch: the restore numbers new ids itself. The mode
  * survives sgr_dingest_reset, as the value framing does.
  * Records: everything a read_committed consumer does stays as in events mode (CRC first, control batches, aborted
  * transactions, a trailing partial batch, duplicates below the partition's position, the positions of the lag gate). Then:
@@ -692,7 +714,7 @@ int32_t sgr_dingest_get_stats(sgr_dingest* g, sgr_ingest_stats* out);
  * topic's JSON member table does; at most one SGR_JSON_ID member; names non-empty, well-formed UTF-8 and distinct. The restore's
  * table for the same values is this table without its ID member. n_members == 0 clears the writer. SGR_ERR_NO_PROGRAM before
  * sgr_register_program, and a later sgr_register_program clears the writer; SGR_ERR_INVALID on a bad table (nothing changes);
- * SGR_ERR_UNSUPPORTED on a routed engine (sgr_dist_init). */
+ * SGR_ERR_UNSUPPORTED on a routed engine without a current rank key table (sgr_dist_load_keys). */
 int32_t sgr_set_state_writer(sgr_engine* e, const sgr_json_field* members, uint32_t n_members);
 /* Three reads that return values instead of rows. Each matches its twin (sgr_get_batch, sgr_export_changes, sgr_scan) in
  * locking, table generation, id-index update, paging, cursor / token and error codes, with the rows replaced by values

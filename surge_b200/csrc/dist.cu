@@ -368,6 +368,7 @@ int dist_set_partitions(DistState* d, const uint32_t* partition_of_agg, uint64_t
 }
 
 uint64_t dist_n_local(const DistState* d) { return d->n_local; }
+uint64_t dist_n_global(const DistState* d) { return d->n_global; }
 int dist_nranks(const DistState* d) { return d->nranks; }
 bool dist_is_loopback(const DistState* d) { return d->loopback; }
 void dist_clear_stats(DistState* d, uint64_t n_records) { d->stats = DistStats{}; d->stats.n_sent = n_records; d->stats.n_recv = n_records; }

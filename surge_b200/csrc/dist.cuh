@@ -27,6 +27,7 @@ int dist_set_partitions(DistState* d, const uint32_t* partition_of_agg, uint64_t
 int dist_route(DistState* d, const uint8_t* d_records, uint64_t n, bool fused, unsigned long long* d_counters, cudaStream_t st,
                uint64_t* n_recv_out, std::string* err);
 uint64_t dist_n_local(const DistState* d);
+uint64_t dist_n_global(const DistState* d);   // 0 until a partition table is set
 int dist_nranks(const DistState* d);
 bool dist_is_loopback(const DistState* d);
 void dist_clear_stats(DistState* d, uint64_t n_records);

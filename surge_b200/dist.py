@@ -8,7 +8,8 @@ modules/common/src/main/scala/surge/kafka/KafkaPartitioner.scala:7-9) -> owner =
 from __future__ import annotations
 
 import ctypes as C
-from typing import List, Optional, Sequence, Tuple
+import heapq
+from typing import Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -106,3 +107,39 @@ def exchange_ids(engine, rank: int, nranks: int, recv_capacity_records: int, fus
         handles: List[Optional[bytes]] = [None] * nranks
         dist.all_gather_object(handles, mine)
         engine.dist_ipc_import(handles)
+
+
+def read_routed(engines: Sequence, ids: Sequence[str], num_partitions: int, arrays: bool = False):
+    """getAggregateBytes for many ids over the ranks of one routed table, each rank holding its rank key table
+    (ReplayEngine.dist_load_keys): every id goes to its owner, rank partitionForKey(id) % len(engines), as the Surge router sends
+    a command to the node that owns the id's partition, and the answers come back in query order. For ranks inside one process;
+    a real rank reads its own engine only. Returns what get_many returns: a list of Optional[bytes], or with arrays=True
+    (states u8[n, state_bytes - 8], flags u32[n], indices i64[n]) where an index is a local slot of the owner (-1: unknown)."""
+    R = len(engines)
+    owner = partitions_for_keys(ids, num_partitions) % np.uint32(R)
+    n = len(ids)
+    user = engines[0].state_bytes - 8
+    states = np.zeros((n, user), dtype=np.uint8)
+    flags = np.zeros(n, dtype=np.uint32)
+    indices = np.full(n, -1, dtype=np.int64)
+    for r, e in enumerate(engines):
+        pos = np.nonzero(owner == r)[0]
+        if len(pos):
+            states[pos], flags[pos], indices[pos] = e.get_many([ids[i] for i in pos], arrays=True)
+    if arrays:
+        return states, flags, indices
+    return [states[i].tobytes() if flags[i] & N.ST_EXISTS else None for i in range(n)]
+
+
+def merge_scans(engines: Sequence, frm: Optional[str] = None, to: Optional[str] = None,
+                page_rows: int = 1 << 20) -> Iterator[Tuple[str, int, int, int, bytes]]:
+    """One scan of [frm, to] over the ranks of one routed table: the ranks' ordered pages (ReplayEngine.scan on each rank key
+    table) merged into one stream in Bytes order of the ids, as range / all over every node's KTable would be. Each rank holds
+    distinct ids, so the merge only interleaves. Yields (id, rank, local index, flags, program bytes) per live aggregate."""
+    def rows(r, e):
+        for idx, fl, st, page_ids in e.scan(frm, to, page_rows=page_rows):
+            for i, k in enumerate(page_ids):
+                yield k.encode("utf-8"), k, r, int(idx[i]), int(fl[i]), st[i].tobytes()
+
+    for _, k, r, idx, fl, row in heapq.merge(*(rows(r, e) for r, e in enumerate(engines))):
+        yield k, r, idx, fl, row

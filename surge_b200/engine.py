@@ -488,6 +488,16 @@ class ReplayEngine:
         self._ck(self._lib.sgr_dist_local_aggregates(self._h, out.ctypes.data, len(out), C.byref(n)))
         return out
 
+    def dist_load_keys(self, ids: Sequence) -> None:
+        """The ids of global aggregates 0..n_global - 1 (str or bytes), in the partition table's order (sgr_dist_load_keys):
+        this rank keeps the ones it owns, in local-slot order, and get(), get_many(), export_changes(), scan() and their
+        *_values twins then read its rows by id. An id another rank owns is unknown here."""
+        enc = [k if isinstance(k, bytes) else k.encode("utf-8") for k in ids]
+        offs = np.zeros(len(enc) + 1, dtype=np.uint32)
+        np.cumsum([len(b) for b in enc], out=offs[1:])
+        blob = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8).copy()
+        self._ck(self._lib.sgr_dist_load_keys(self._h, blob.ctypes.data, offs.ctypes.data, len(enc)))
+
     def stats(self) -> N.sgr_stats:
         s = N.sgr_stats()
         self._ck(self._lib.sgr_get_stats(self._h, C.byref(s)))

@@ -151,6 +151,7 @@ ABI = [
     ("sgr_states_hash", C.c_int32, [_P, C.POINTER(C.c_uint64)]),
     ("sgr_dist_get_stats", C.c_int32, [_P, C.POINTER(sgr_dist_stats)]),
     ("sgr_dist_local_aggregates", C.c_int32, [_P, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
+    ("sgr_dist_load_keys", C.c_int32, [_P, _P, _P, C.c_uint64]),
     ("sgr_partitions_for_keys", C.c_int32, [_P, _P, C.c_uint64, C.c_uint32, C.c_int32, _P]),
     ("sgr_string_hash_utf16", C.c_int32, [_P, C.c_uint32]),
     ("sgr_partition_for_key_utf8", C.c_int32, [_P, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(C.c_int32)]),
