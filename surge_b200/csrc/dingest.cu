@@ -23,7 +23,6 @@
 // A compacted STATE topic (sgr_dingest_set_state_topic) takes the same chain; its parse writes rows of program bytes, and the
 // fold applies them last write wins with sgr_put_batch's kernels (put_decoded_poll) instead of folding events.
 #include <cuda_runtime.h>
-#include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -33,29 +32,17 @@
 #include <map>
 #include <string>
 #include <thread>
-#include <unordered_set>
 #include <vector>
 
 #include "../../include/sgr.h"
 #include "devbuf.h"
 #include "dingest_kernels.cuh"
 #include "engine_internal.h"
+#include "record_batch.h"
 
 using namespace sgr;
 
 namespace {
-inline uint16_t be16(const uint8_t* p) { return (uint16_t)((p[0] << 8) | p[1]); }
-inline uint32_t be32(const uint8_t* p) { return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]; }
-inline uint64_t be64(const uint8_t* p) { return ((uint64_t)be32(p) << 32) | be32(p + 4); }
-constexpr uint64_t kBatchHeader = 61;
-
-struct PartState {
-  int64_t decoded_next = 0, folded_next = 0;
-  bool seen = false;
-  std::vector<std::pair<int64_t, int64_t>> aborted;   // (first_offset, producer_id), ascending, not yet reached
-  std::unordered_set<int64_t> aborting;               // producers inside an aborted transaction right now
-};
-
 // growable device buffer that keeps its content (the staged fetches of one poll accumulate in it)
 struct KeepBuf {
   DevBuf b;
@@ -80,8 +67,8 @@ struct sgr_dingest {
   sgr_engine* eng = nullptr;
   cudaStream_t stream = nullptr;
   std::string last_error;
-  std::map<int32_t, PartState> parts;       // committed view (after the last successful fold)
-  std::map<int32_t, PartState> staged;      // view after the submissions of the current poll
+  std::map<int32_t, PartitionState> parts;  // committed view (after the last successful fold)
+  std::map<int32_t, PartitionState> staged; // view after the submissions of the current poll
   int32_t null_value_type = -1;
   int32_t value_framing = SGR_VALUE_PACKED;
   DevBuf json_table;                        // SGR_VALUE_JSON: member table (vf::Class[], vf::Field[], names) on the device
@@ -158,12 +145,7 @@ struct sgr_dingest {
 };
 
 namespace {
-int32_t dfail(sgr_dingest* g, int32_t code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);
-  if (g) g->last_error = buf;
-  return code;
-}
+template <class... A> int32_t dfail(sgr_dingest* g, int32_t code, const char* fmt, A... a) { return g ? set_error(&g->last_error, code, fmt, a...) : code; }
 #define DG_TRY(g, call)                                                                                          \
   do {                                                                                                           \
     cudaError_t _e = (call);                                                                                     \
@@ -422,7 +404,7 @@ int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, c
     if (engine_program_state_bytes(g->eng, &row_limit, &routed) != SGR_OK || !row_limit) return dfail(g, SGR_ERR_NO_PROGRAM, "state topic: register a fold program first");
     row_limit -= 8;
   }
-  // the same checks as sgr_ingest_set_json_packer; the table goes to the device as classes, fields, then the names
+  // the table goes to the device as classes, fields, then the names
   std::vector<vf::Class> classes;
   std::vector<vf::Field> fields;
   std::string names = discriminator;
@@ -433,12 +415,9 @@ int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, c
     names += e.type_name;
     for (uint32_t f = 0; f < e.n_fields; ++f) {
       const sgr_json_field& jf = e.fields[f];
-      const uint32_t size = jf.kind == SGR_JSON_I32 ? 4u : jf.kind == SGR_JSON_UUID ? 16u : jf.kind == SGR_JSON_PSTR ? jf.len : 8u;
-      // a member may land on the sequence number (+4, Int only) or anywhere in the payload (+16 .. +64); never on type or agg.
-      // State topic: anywhere in the row's program bytes.
-      const bool ok = jf.name && jf.kind <= SGR_JSON_PSTR && jf.dst_off % 4 == 0 && size >= 4 && size % 4 == 0 &&
-                      (g->state_topic ? (uint64_t)jf.dst_off + size <= row_limit
-                                      : ((jf.dst_off == 4 && jf.kind == SGR_JSON_I32) || (jf.dst_off >= 16 && jf.dst_off + size <= 64)));
+      // state topic: anywhere in the row's program bytes
+      const uint32_t size = json_member_size(jf);
+      const bool ok = size && (g->state_topic ? (uint64_t)jf.dst_off + size <= row_limit : json_event_slot_ok(jf, size));
       if (!ok) return dfail(g, SGR_ERR_INVALID, "JSON %s %u field %u: bad name, kind, length or %s offset", g->state_topic ? "state" : "event", i, f,
                             g->state_topic ? "program byte" : "record");
       row_end = std::max(row_end, jf.dst_off + size);
@@ -467,9 +446,7 @@ int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, c
 
 int32_t sgr_dingest_set_aborted(sgr_dingest* g, int32_t partition, const int64_t* producer_ids, const int64_t* first_offsets, uint64_t n) {
   if (!g || (n && (!producer_ids || !first_offsets))) return dfail(g, SGR_ERR_INVALID, "null argument");
-  PartState& ps = g->staged[partition];
-  for (uint64_t i = 0; i < n; ++i) ps.aborted.emplace_back(first_offsets[i], producer_ids[i]);
-  std::sort(ps.aborted.begin(), ps.aborted.end());
+  g->staged[partition].announce_aborted(producer_ids, first_offsets, n);
   return SGR_OK;
 }
 
@@ -477,83 +454,58 @@ int32_t sgr_dingest_set_aborted(sgr_dingest* g, int32_t partition, const int64_t
 int32_t sgr_dingest_submit(sgr_dingest* g, int32_t partition, const void* data, uint64_t nbytes, sgr_ingest_stats* stats) {
   if (!g || (!data && nbytes)) return dfail(g, SGR_ERR_INVALID, "null argument");
   const uint8_t* buf = (const uint8_t*)data;
-  PartState ps = g->staged[partition];   // work on a copy: a malformed fetch leaves the staged view untouched
+  PartitionState ps = g->staged[partition];   // work on a copy: a malformed fetch leaves the staged view untouched
   sgr_ingest_stats st{};
   std::vector<DgBatch> add;
   uint64_t slots = 0, pos = 0;
-  while (nbytes - pos >= 12) {
-    const int64_t base_offset = (int64_t)be64(buf + pos);
-    const int32_t batch_length = (int32_t)be32(buf + pos + 8);
-    if (batch_length < (int32_t)(kBatchHeader - 12)) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: batch length %d is smaller than a v2 header", partition, (long long)base_offset, batch_length);
-    const uint64_t total = 12ull + (uint32_t)batch_length;
-    if (nbytes - pos < total) break;   // a trailing partial batch: the next fetch repeats it
-    const uint8_t* b = buf + pos;
-    if ((int8_t)b[16] != 2) return dfail(g, SGR_ERR_UNSUPPORTED, "partition %d offset %lld: message format v%d (only RecordBatch magic 2 is decoded)", partition, (long long)base_offset, (int)(int8_t)b[16]);
-    const uint16_t attrs = be16(b + 21);
-    const int32_t last_offset_delta = (int32_t)be32(b + 23);
-    const int64_t producer_id = (int64_t)be64(b + 43);
-    const int32_t records_count = (int32_t)be32(b + 57);
-    if (last_offset_delta < 0 || records_count < 0) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: negative lastOffsetDelta / recordsCount", partition, (long long)base_offset);
-    const int64_t last_offset = base_offset + last_offset_delta;
-    const int codec = attrs & 7;
-    const bool transactional = attrs & 0x10, control = attrs & 0x20;
+  for (BatchHeader h;; pos += h.total) {
+    if (const int32_t rc = frame_batch(partition, buf, nbytes, pos, &h, &g->last_error)) return rc;
+    if (!h.total) break;   // a trailing partial batch: the next fetch repeats it
+    if (const int32_t rc = read_batch_fields(partition, &h, &g->last_error)) return rc;
     ++st.n_batches;
-    while (!ps.aborted.empty() && ps.aborted.front().first <= last_offset) { ps.aborting.insert(ps.aborted.front().second); ps.aborted.erase(ps.aborted.begin()); }
-    if (control) {
+    const bool aborted_batch = ps.reach(h);
+    if (h.control) {
       // tiny and never compressed by the broker: read on the host (CRC included), it only steers the bookkeeping. Read as the
       // host decoder reads it: a codec other than none / lz4 is refused, an lz4 one is decompressed, the key must fit.
       ++st.n_control_batches;
-      if (sgr_crc32c(b + 21, total - 21) != be32(b + 17)) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: CRC-32C mismatch in a control batch", partition, (long long)base_offset);
-      if (codec != 0 && codec != 3) return dfail(g, SGR_ERR_UNSUPPORTED, "partition %d offset %lld: compression codec %d (none and lz4 are decoded)", partition, (long long)base_offset, codec);
-      const uint8_t* r = b + kBatchHeader; const uint8_t* end = b + total;
+      if (sgr_crc32c(h.b + 21, h.total - 21) != h.stored_crc) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: CRC-32C mismatch in a control batch", partition, (long long)h.base_offset);
+      if (h.codec != 0 && h.codec != 3) return dfail(g, SGR_ERR_UNSUPPORTED, "partition %d offset %lld: compression codec %d (none and lz4 are decoded)", partition, (long long)h.base_offset, h.codec);
+      const uint8_t* r = h.b + kBatchHeader; const uint8_t* end = h.b + h.total;
       std::vector<uint8_t> plain;
-      if (codec == 3) {
+      if (h.codec == 3) {
         uint64_t n = 0;
-        if (sgr_lz4_frame_decode(r, total - kBatchHeader, nullptr, 0, &n) == SGR_ERR_INVALID) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: bad lz4 frame in a control batch", partition, (long long)base_offset);
+        if (sgr_lz4_frame_decode(r, h.total - kBatchHeader, nullptr, 0, &n) == SGR_ERR_INVALID) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: bad lz4 frame in a control batch", partition, (long long)h.base_offset);
         plain.resize(n);
-        if (n && sgr_lz4_frame_decode(r, total - kBatchHeader, plain.data(), n, &n) != SGR_OK) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: bad lz4 frame in a control batch", partition, (long long)base_offset);
-        st.n_compressed_bytes += total - kBatchHeader; st.n_decompressed_bytes += n;
+        if (n && sgr_lz4_frame_decode(r, h.total - kBatchHeader, plain.data(), n, &n) != SGR_OK) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: bad lz4 frame in a control batch", partition, (long long)h.base_offset);
+        st.n_compressed_bytes += h.total - kBatchHeader; st.n_decompressed_bytes += n;
         r = plain.data(); end = r + n;
       }
-      // record: varint length, attributes, varlong ts delta, varint offset delta, varint key length, key = int16 version, int16 type
-      auto varint = [&](int max_bytes, bool* ok) { uint64_t v = 0; int sh = 0; *ok = false;
-        for (int k = 0; k < max_bytes && r < end; ++k) { const uint8_t c = *r++; v |= (uint64_t)(c & 0x7f) << sh; if (!(c & 0x80)) { *ok = true; break; } sh += 7; }
-        return v; };
-      bool ok = true, t;
-      varint(5, &t); ok &= t;
-      if (r < end) ++r; else ok = false;
-      varint(10, &t); ok &= t; varint(5, &t); ok &= t;
-      const uint32_t zk = (uint32_t)varint(5, &t); ok &= t;
-      const int32_t kl = (int32_t)(zk >> 1) ^ -(int32_t)(zk & 1);
-      if (ok && kl >= 4 && (uint64_t)(end - r) >= (uint64_t)kl && be16(r + 2) == 0) ps.aborting.erase(producer_id);   // ABORT marker ends the transaction
-    } else if (transactional && ps.aborting.count(producer_id)) {
+      ps.apply_control(h, r, (uint64_t)(end - r));
+    } else if (aborted_batch) {
       // skipped unread, as Kafka's consumer skips it, but only after its CRC: a damaged batch is refused here as on the host
-      if (sgr_crc32c(b + 21, total - 21) != be32(b + 17)) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: CRC-32C mismatch in an aborted batch", partition, (long long)base_offset);
-      ++st.n_aborted_batches; st.n_aborted_records += (uint64_t)records_count;
+      if (sgr_crc32c(h.b + 21, h.total - 21) != h.stored_crc) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: CRC-32C mismatch in an aborted batch", partition, (long long)h.base_offset);
+      ++st.n_aborted_batches; st.n_aborted_records += (uint64_t)h.records_count;
     } else {
       // A batch entirely below the position (a refetch) is decoded and checked like any other and its records count as
       // duplicates, as the host decoder and Kafka's consumer do: skipping it unread would accept damage the host refuses.
-      if (codec != 0 && codec != 3) {
+      if (h.codec != 0 && h.codec != 3) {
         // the CRC comes first, as on the host and in Kafka's consumer: a damaged batch is invalid whatever its codec says
-        if (sgr_crc32c(b + 21, total - 21) != be32(b + 17)) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: CRC-32C mismatch", partition, (long long)base_offset);
-        return dfail(g, SGR_ERR_UNSUPPORTED, "partition %d offset %lld: compression codec %d (none and lz4 are decoded)", partition, (long long)base_offset, codec);
+        if (sgr_crc32c(h.b + 21, h.total - 21) != h.stored_crc) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: CRC-32C mismatch", partition, (long long)h.base_offset);
+        return dfail(g, SGR_ERR_UNSUPPORTED, "partition %d offset %lld: compression codec %d (none and lz4 are decoded)", partition, (long long)h.base_offset, h.codec);
       }
-      if (total < kBatchHeader) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: batch shorter than its header", partition, (long long)base_offset);
       // Every record is at least 7 bytes and lz4 expands at most 255-fold: a recordsCount beyond that is refused here, before the
       // poll sizes its per-record buffers by it (the decode kernels then check the exact bound, as the host decoder does).
-      const uint64_t max_section = codec == 3 ? (total - kBatchHeader) * 255ull + 64 : total - kBatchHeader;
-      if ((uint64_t)records_count > max_section / 7 + 1) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: recordsCount %d does not fit the batch", partition, (long long)base_offset, records_count);
+      const uint64_t max_section = h.codec == 3 ? (h.total - kBatchHeader) * 255ull + 64 : h.total - kBatchHeader;
+      if ((uint64_t)h.records_count > max_section / 7 + 1) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: recordsCount %d does not fit the batch", partition, (long long)h.base_offset, h.records_count);
       DgBatch d{};
-      d.src_off = g->wire.used + pos; d.base_offset = base_offset; d.min_offset = ps.seen ? ps.decoded_next : INT64_MIN;
-      d.total_len = (uint32_t)total; d.n_records = (uint32_t)records_count; d.codec = (uint16_t)codec; d.stored_crc = be32(b + 17);
+      d.src_off = g->wire.used + pos; d.base_offset = h.base_offset; d.min_offset = ps.seen ? ps.decoded_next : INT64_MIN;
+      d.total_len = (uint32_t)h.total; d.n_records = (uint32_t)h.records_count; d.codec = (uint16_t)h.codec; d.stored_crc = h.stored_crc;
       d.rec_base = (uint32_t)(g->n_record_slots + slots);
-      slots += (uint64_t)records_count;
-      if (codec == 3) st.n_compressed_bytes += total - kBatchHeader;
+      slots += (uint64_t)h.records_count;
+      if (h.codec == 3) st.n_compressed_bytes += h.total - kBatchHeader;
       add.push_back(d);
     }
-    if (!ps.seen || last_offset + 1 > ps.decoded_next) ps.decoded_next = last_offset + 1;
-    ps.seen = true;
-    pos += total;
+    ps.close(h);
   }
   st.n_bytes = pos; st.n_trailing_bytes = nbytes - pos;
   if (g->n_record_slots + slots >= (1ull << 32)) return dfail(g, SGR_ERR_CAPACITY, "more than 2^32 records in one poll");
@@ -591,11 +543,8 @@ int32_t sgr_dingest_submit(sgr_dingest* g, int32_t partition, const void* data, 
   }
   g->n_record_slots += slots;
   g->staged[partition] = ps;
-  sgr_ingest_stats& t = g->poll;
-  t.n_bytes += st.n_bytes; t.n_batches += st.n_batches; t.n_control_batches += st.n_control_batches; t.n_aborted_batches += st.n_aborted_batches;
-  t.n_aborted_records += st.n_aborted_records; t.n_duplicates += st.n_duplicates; t.n_compressed_bytes += st.n_compressed_bytes;
-  t.n_decompressed_bytes += st.n_decompressed_bytes;   // (lz4 control batches; data batches add theirs at the fold)
-  t.n_trailing_bytes = st.n_trailing_bytes;
+  add_stats(&g->poll, st);   // (n_decompressed_bytes: lz4 control batches; data batches add theirs at the fold)
+  g->poll.n_trailing_bytes = st.n_trailing_bytes;
   if (stats) *stats = st;
   return SGR_OK;
 }
@@ -741,10 +690,7 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
   g->folded = true;
   if (nb) DG_TRY(g, reset_poll_counters(g));
   clear_poll(g);
-  sgr_ingest_stats& t = g->total;
-  t.n_bytes += st.n_bytes; t.n_batches += st.n_batches; t.n_records += st.n_records; t.n_markers += st.n_markers; t.n_null_values += st.n_null_values;
-  t.n_control_batches += st.n_control_batches; t.n_aborted_batches += st.n_aborted_batches; t.n_aborted_records += st.n_aborted_records;
-  t.n_duplicates += st.n_duplicates; t.n_new_keys += st.n_new_keys; t.n_compressed_bytes += st.n_compressed_bytes; t.n_decompressed_bytes += st.n_decompressed_bytes;
+  add_stats(&g->total, st);
   if (stats) *stats = st;
   return SGR_OK;
 }
@@ -763,11 +709,7 @@ int32_t sgr_dingest_reset(sgr_dingest* g) {
 }
 
 int32_t sgr_dingest_offsets(sgr_dingest* g, int32_t partition, int64_t* decoded_next, int64_t* folded_next) {
-  if (!g) return SGR_ERR_INVALID;
-  auto it = g->parts.find(partition);
-  if (decoded_next) *decoded_next = it == g->parts.end() ? 0 : it->second.decoded_next;
-  if (folded_next) *folded_next = it == g->parts.end() ? 0 : it->second.folded_next;
-  return SGR_OK;
+  return g ? partition_offsets(g->parts, partition, decoded_next, folded_next) : SGR_ERR_INVALID;
 }
 
 int32_t sgr_dingest_last_timing(sgr_dingest* g, float* ms8) {

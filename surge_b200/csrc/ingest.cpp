@@ -16,7 +16,6 @@
 // Host-only C++: the decode is byte parsing with data-dependent control flow on a few MB per poll; the fold it
 // feeds is the GPU path. Nothing here touches CUDA.
 #include <errno.h>
-#include <stdarg.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -32,10 +31,12 @@
 #include <thread>
 #include <map>
 #include <string>
-#include <unordered_set>
 #include <vector>
 
 #include "../../include/sgr.h"
+#include "record_batch.h"
+
+using namespace sgr;
 
 namespace {
 
@@ -205,54 +206,17 @@ std::string lz4_frame_decode(const uint8_t* src, uint64_t n, std::vector<uint8_t
   return std::string();
 }
 
-// ------------------------------------------------------------------ big-endian fields and zig-zag varints
-inline uint16_t be16(const uint8_t* p) { return (uint16_t)((p[0] << 8) | p[1]); }
-inline uint32_t be32(const uint8_t* p) { return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]; }
-inline uint64_t be64(const uint8_t* p) { return ((uint64_t)be32(p) << 32) | be32(p + 4); }
-
-struct Cursor {
-  const uint8_t* p; uint64_t n; uint64_t pos = 0; bool ok = true;
-  Cursor(const uint8_t* p_, uint64_t n_) : p(p_), n(n_) {}
-  int64_t varlong() {  // ByteUtils.readVarlong: zig-zag, at most 10 bytes
-    if (pos < n && !(p[pos] & 0x80)) { const uint64_t b = p[pos++]; return (int64_t)(b >> 1) ^ -(int64_t)(b & 1); }
-    uint64_t v = 0; int shift = 0;
-    for (int i = 0; i < 10; ++i) {
-      if (pos >= n) { ok = false; return 0; }
-      const uint8_t b = p[pos++];
-      v |= (uint64_t)(b & 0x7f) << shift;
-      if (!(b & 0x80)) return (int64_t)(v >> 1) ^ -(int64_t)(v & 1);
-      shift += 7;
-    }
-    ok = false; return 0;
+uint64_t uvarint(Cursor& c) {   // protobuf base-128 varint (no zig-zag), at most 10 bytes
+  uint64_t v = 0; int shift = 0;
+  for (int i = 0; i < 10; ++i) {
+    if (c.pos >= c.n) { c.ok = false; return 0; }
+    const uint8_t b = c.p[c.pos++];
+    v |= (uint64_t)(b & 0x7f) << shift;
+    if (!(b & 0x80)) return v;
+    shift += 7;
   }
-  int32_t varint() {  // ByteUtils.readVarint: zig-zag, at most 5 bytes
-    if (pos < n && !(p[pos] & 0x80)) { const uint32_t b = p[pos++]; return (int32_t)(b >> 1) ^ -(int32_t)(b & 1); }
-    uint32_t v = 0; int shift = 0;
-    for (int i = 0; i < 5; ++i) {
-      if (pos >= n) { ok = false; return 0; }
-      const uint8_t b = p[pos++];
-      v |= (uint32_t)(b & 0x7f) << shift;
-      if (!(b & 0x80)) return (int32_t)(v >> 1) ^ -(int32_t)(v & 1);
-      shift += 7;
-    }
-    ok = false; return 0;
-  }
-  uint64_t uvarint() {   // protobuf base-128 varint (no zig-zag), at most 10 bytes
-    uint64_t v = 0; int shift = 0;
-    for (int i = 0; i < 10; ++i) {
-      if (pos >= n) { ok = false; return 0; }
-      const uint8_t b = p[pos++];
-      v |= (uint64_t)(b & 0x7f) << shift;
-      if (!(b & 0x80)) return v;
-      shift += 7;
-    }
-    ok = false; return 0;
-  }
-  const uint8_t* bytes(uint64_t k) {
-    if (k > n - pos) { ok = false; return nullptr; }
-    const uint8_t* r = p + pos; pos += k; return r;
-  }
-};
+  c.ok = false; return 0;
+}
 
 // ------------------------------------------------------------------ growable aggregate-id dictionary (first-seen order = dense index)
 inline uint64_t hash_bytes(const uint8_t* k, uint32_t len) {   // 8 bytes at a time, multiply-xorshift mixing
@@ -660,14 +624,6 @@ struct ProbeOut {                 // one worker's probe results: (record positio
   std::vector<size_t> off;        // n_fetches + 1
 };
 
-struct PartitionState {
-  int64_t decoded_next = 0;   // next offset this partition expects (last decoded batch's lastOffset + 1)
-  int64_t folded_next = 0;    // everything below this offset is inside the state table
-  bool seen = false;
-  std::vector<std::pair<int64_t, int64_t>> aborted;  // (first_offset, producer_id), ascending first_offset, not yet reached
-  std::unordered_set<int64_t> aborting;              // producer ids inside an aborted transaction right now
-};
-
 struct KeyRef { uint32_t off, len; uint64_t hash; };
 struct Staged {
   std::vector<uint8_t> recs;      // 64-byte records, agg field still zero
@@ -708,18 +664,12 @@ struct sgr_ingest {
 };
 
 namespace {
-int32_t ifail(sgr_ingest* g, int32_t code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);
-  if (g) g->last_error = buf;
-  return code;
-}
+template <class... A> int32_t ifail(sgr_ingest* g, int32_t code, const char* fmt, A... a) { return g ? set_error(&g->last_error, code, fmt, a...) : code; }
 
 const char* codec_name(int c) {
   switch (c) { case 1: return "gzip"; case 2: return "snappy"; case 4: return "zstd"; default: return "unknown"; }
 }
 
-constexpr uint64_t kBatchHeader = 61;  // baseOffset .. recordsCount
 }  // namespace
 
 extern "C" {
@@ -762,11 +712,8 @@ int32_t sgr_ingest_set_json_packer(sgr_ingest* g, const char* discriminator, con
     JsonEventSpec es{e.type_name, e.event_type, {}};
     for (uint32_t f = 0; f < e.n_fields; ++f) {
       const sgr_json_field& jf = e.fields[f];
-      const uint32_t size = jf.kind == SGR_JSON_I32 ? 4u : jf.kind == SGR_JSON_UUID ? 16u : jf.kind == SGR_JSON_PSTR ? jf.len : 8u;
-      // a member may land on the sequence number (+4, Int only) or anywhere in the payload (+16 .. +64); never on type or agg
-      const bool ok = jf.name && jf.kind <= SGR_JSON_PSTR && jf.dst_off % 4 == 0 && size >= 4 && size % 4 == 0 &&
-                      ((jf.dst_off == 4 && jf.kind == SGR_JSON_I32) || (jf.dst_off >= 16 && jf.dst_off + size <= 64));
-      if (!ok) return ifail(g, SGR_ERR_INVALID, "JSON event %u field %u: bad name, kind, length or record offset", i, f);
+      const uint32_t size = json_member_size(jf);
+      if (!size || !json_event_slot_ok(jf, size)) return ifail(g, SGR_ERR_INVALID, "JSON event %u field %u: bad name, kind, length or record offset", i, f);
       es.fields.push_back(JsonFieldSpec{jf.name, jf.kind, jf.dst_off, size});
     }
     jp.events.push_back(es);
@@ -797,9 +744,7 @@ int32_t sgr_ingest_set_dictionary_limits(sgr_ingest* g, uint64_t max_ids, uint64
 
 int32_t sgr_ingest_set_aborted(sgr_ingest* g, int32_t partition, const int64_t* producer_ids, const int64_t* first_offsets, uint64_t n) {
   if (!g || (n && (!producer_ids || !first_offsets))) return ifail(g, SGR_ERR_INVALID, "null argument");
-  PartitionState& ps = g->parts[partition];
-  for (uint64_t i = 0; i < n; ++i) ps.aborted.emplace_back(first_offsets[i], producer_ids[i]);
-  std::sort(ps.aborted.begin(), ps.aborted.end());
+  g->parts[partition].announce_aborted(producer_ids, first_offsets, n);
   return SGR_OK;
 }
 
@@ -807,87 +752,55 @@ int32_t sgr_ingest_set_aborted(sgr_ingest* g, int32_t partition, const int64_t* 
 
 // ---- phase 1 (any thread, touches nothing shared): one fetch -> staged records + key references
 namespace {
-int32_t sfail(Staged* o, int32_t code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);
-  o->err = buf; o->rc = code;
-  return code;
-}
-
 int32_t decode_fetch(int32_t partition, const uint8_t* buf, uint64_t nbytes, Staged* o) {
   PartitionState& ps = o->ps;
   sgr_ingest_stats& st = o->st;
   o->recs.reserve(nbytes + nbytes / 4);
   uint64_t pos = 0;
-  while (nbytes - pos >= 12) {
-    const int64_t base_offset = (int64_t)be64(buf + pos);
-    const int32_t batch_length = (int32_t)be32(buf + pos + 8);
-    if (batch_length < (int32_t)(kBatchHeader - 12)) return sfail(o, SGR_ERR_INVALID, "partition %d offset %lld: batch length %d is smaller than a v2 header", partition, (long long)base_offset, batch_length);
-    const uint64_t total = 12ull + (uint32_t)batch_length;
-    if (nbytes - pos < total) break;  // a fetch response may end with a partial batch: not an error, the next fetch repeats it
-    const uint8_t* b = buf + pos;
-    const int8_t magic = (int8_t)b[16];
-    if (magic != 2) return sfail(o, SGR_ERR_UNSUPPORTED, "partition %d offset %lld: message format v%d (only RecordBatch magic 2 is decoded)", partition, (long long)base_offset, (int)magic);
-    const uint32_t crc = be32(b + 17);
-    const uint32_t got = crc32c(b + 21, total - 21);
-    if (crc != got) return sfail(o, SGR_ERR_INVALID, "partition %d offset %lld: CRC-32C mismatch (stored %08x, computed %08x)", partition, (long long)base_offset, crc, got);
-    const uint16_t attrs = be16(b + 21);
-    const int32_t last_offset_delta = (int32_t)be32(b + 23);
-    const int64_t producer_id = (int64_t)be64(b + 43);
-    const int32_t records_count = (int32_t)be32(b + 57);
-    if (last_offset_delta < 0 || records_count < 0) return sfail(o, SGR_ERR_INVALID, "partition %d offset %lld: negative lastOffsetDelta / recordsCount", partition, (long long)base_offset);
-    const int64_t last_offset = base_offset + last_offset_delta;
-    const int codec = attrs & 7;
-    const bool transactional = attrs & 0x10, control = attrs & 0x20;
+  for (BatchHeader h;; pos += h.total) {
+    if (const int32_t rc = frame_batch(partition, buf, nbytes, pos, &h, &o->err)) return rc;
+    if (!h.total) break;
+    const uint32_t got = crc32c(h.b + 21, h.total - 21);
+    if (h.stored_crc != got) return set_error(&o->err, SGR_ERR_INVALID, "partition %d offset %lld: CRC-32C mismatch (stored %08x, computed %08x)", partition, (long long)h.base_offset, h.stored_crc, got);
+    if (const int32_t rc = read_batch_fields(partition, &h, &o->err)) return rc;
     ++st.n_batches;
-    pos += total;
-
-    // read_committed bookkeeping, as the Java consumer does it: aborted transactions announced for this fetch become
-    // active once the log reaches their first offset; the producer's ABORT marker ends them
-    while (!ps.aborted.empty() && ps.aborted.front().first <= last_offset) { ps.aborting.insert(ps.aborted.front().second); ps.aborted.erase(ps.aborted.begin()); }
 
     // A batch of an aborted transaction is skipped after its CRC and before anything else, as Kafka's consumer skips it: its
     // codec is not looked at and it is not decompressed.
-    const bool aborted_batch = !control && transactional && ps.aborting.count(producer_id);
-    const uint8_t* recs = b + kBatchHeader;
-    uint64_t recs_len = total - kBatchHeader;
-    if (codec != 0 && !aborted_batch) {
-      if (codec != 3) return sfail(o, SGR_ERR_UNSUPPORTED, "partition %d offset %lld: %s-compressed batch (none and lz4 are decoded)", partition, (long long)base_offset, codec_name(codec));
+    const bool aborted_batch = ps.reach(h);
+    const uint8_t* recs = h.b + kBatchHeader;
+    uint64_t recs_len = h.total - kBatchHeader;
+    if (h.codec != 0 && !aborted_batch) {
+      if (h.codec != 3) return set_error(&o->err, SGR_ERR_UNSUPPORTED, "partition %d offset %lld: %s-compressed batch (none and lz4 are decoded)", partition, (long long)h.base_offset, codec_name(h.codec));
       o->scratch.clear();
       const std::string err = lz4_frame_decode(recs, recs_len, &o->scratch);
-      if (!err.empty()) return sfail(o, SGR_ERR_INVALID, "partition %d offset %lld: %s", partition, (long long)base_offset, err.c_str());
+      if (!err.empty()) return set_error(&o->err, SGR_ERR_INVALID, "partition %d offset %lld: %s", partition, (long long)h.base_offset, err.c_str());
       recs = o->scratch.data(); recs_len = o->scratch.size();
-      st.n_compressed_bytes += total - kBatchHeader; st.n_decompressed_bytes += recs_len;
+      st.n_compressed_bytes += h.total - kBatchHeader; st.n_decompressed_bytes += recs_len;
     }
 
-    if (control) {
+    if (h.control) {
       ++st.n_control_batches;
-      // control record key: int16 version, int16 type (0 = ABORT, 1 = COMMIT)
-      Cursor c(recs, recs_len);
-      c.varint();
-      c.bytes(1); c.varlong(); c.varint();
-      const int32_t kl = c.varint();
-      const uint8_t* k = (c.ok && kl >= 4) ? c.bytes((uint64_t)kl) : nullptr;
-      if (k && c.ok && be16(k + 2) == 0) ps.aborting.erase(producer_id);
+      ps.apply_control(h, recs, recs_len);
     } else if (aborted_batch) {
-      ++st.n_aborted_batches; st.n_aborted_records += (uint64_t)records_count;
+      ++st.n_aborted_batches; st.n_aborted_records += (uint64_t)h.records_count;
     } else {
       Cursor c(recs, recs_len);
       // every record is at least 7 bytes on the wire, so the count cannot lie by much; size the outputs once per batch
-      if ((uint64_t)records_count > recs_len / 7 + 1) return sfail(o, SGR_ERR_INVALID, "partition %d offset %lld: recordsCount %d does not fit %llu bytes", partition, (long long)base_offset, records_count, (unsigned long long)recs_len);
+      if ((uint64_t)h.records_count > recs_len / 7 + 1) return set_error(&o->err, SGR_ERR_INVALID, "partition %d offset %lld: recordsCount %d does not fit %llu bytes", partition, (long long)h.base_offset, h.records_count, (unsigned long long)recs_len);
       const size_t recs_at0 = o->recs.size(), arena_at0 = o->arena.size();
-      o->recs.resize(recs_at0 + 64 * (size_t)records_count);
+      o->recs.resize(recs_at0 + 64 * (size_t)h.records_count);
       o->arena.resize(arena_at0 + recs_len);
       const size_t keys_at0 = o->keys.size();
-      o->keys.resize(keys_at0 + (size_t)records_count);
-      o->shard.resize(keys_at0 + (size_t)records_count);
+      o->keys.resize(keys_at0 + (size_t)h.records_count);
+      o->shard.resize(keys_at0 + (size_t)h.records_count);
       KeyRef* kr = o->keys.data() + keys_at0;
       uint8_t* shp = o->shard.data() + keys_at0;
       uint8_t* rec = o->recs.data() + recs_at0;
       uint8_t* ar = o->arena.data() + arena_at0;
-      for (int32_t r = 0; r < records_count; ++r) {
+      for (int32_t r = 0; r < h.records_count; ++r) {
         const int32_t rec_len = c.varint();
-        if (!c.ok || rec_len < 0 || (uint64_t)rec_len > recs_len - c.pos) return sfail(o, SGR_ERR_INVALID, "partition %d offset %lld: record %d length runs past the batch", partition, (long long)base_offset, r);
+        if (!c.ok || rec_len < 0 || (uint64_t)rec_len > recs_len - c.pos) return set_error(&o->err, SGR_ERR_INVALID, "partition %d offset %lld: record %d length runs past the batch", partition, (long long)h.base_offset, r);
         Cursor q(recs + c.pos, (uint64_t)rec_len);
         c.pos += (uint64_t)rec_len;
         q.bytes(1);             // record attributes (unused in v2)
@@ -902,8 +815,8 @@ int32_t decode_fetch(int32_t partition, const uint8_t* buf, uint64_t nbytes, Sta
           const int32_t hk = q.varint(); if (hk < 0) { q.ok = false; break; } q.bytes((uint64_t)hk);
           const int32_t hv = q.varint(); if (hv > 0) q.bytes((uint64_t)hv);
         }
-        if (!q.ok || q.pos != q.n || n_headers < 0) return sfail(o, SGR_ERR_INVALID, "partition %d offset %lld: record %d is malformed", partition, (long long)base_offset, r);
-        const int64_t offset = base_offset + offset_delta;
+        if (!q.ok || q.pos != q.n || n_headers < 0) return set_error(&o->err, SGR_ERR_INVALID, "partition %d offset %lld: record %d is malformed", partition, (long long)h.base_offset, r);
+        const int64_t offset = h.base_offset + offset_delta;
         if (ps.seen && offset < ps.decoded_next) { ++st.n_duplicates; continue; }  // refetch after a restart: already decoded
         if (key_len <= 0) { ++st.n_markers; continue; }                              // the producer's empty-key flush record
         if (wire_val_len < 0 && o->null_value_type < 0) { ++st.n_null_values; continue; }
@@ -914,14 +827,14 @@ int32_t decode_fetch(int32_t partition, const uint8_t* buf, uint64_t nbytes, Sta
           Cursor pb(val, (uint64_t)val_len);
           const uint8_t* payload = nullptr; uint64_t payload_len = 0;
           while (pb.ok && pb.pos < pb.n) {
-            const uint64_t tag = pb.uvarint();
+            const uint64_t tag = uvarint(pb);
             if (!pb.ok) break;
             switch (tag & 7) {
-              case 0: pb.uvarint(); break;
+              case 0: uvarint(pb); break;
               case 1: pb.bytes(8); break;
               case 5: pb.bytes(4); break;
               case 2: {
-                const uint64_t ln = pb.uvarint();
+                const uint64_t ln = uvarint(pb);
                 const uint8_t* b = pb.ok ? pb.bytes(ln) : nullptr;
                 if (pb.ok && (tag >> 3) == 2) { payload = b; payload_len = ln; }
                 break;
@@ -929,22 +842,22 @@ int32_t decode_fetch(int32_t partition, const uint8_t* buf, uint64_t nbytes, Sta
               default: pb.ok = false;
             }
           }
-          if (!pb.ok) return sfail(o, SGR_ERR_INVALID, "partition %d offset %lld: value is not a protobuf Event", partition, (long long)offset);
+          if (!pb.ok) return set_error(&o->err, SGR_ERR_INVALID, "partition %d offset %lld: value is not a protobuf Event", partition, (long long)offset);
           val = payload; val_len = (int32_t)(payload_len > 0x7fffffff ? 0x7fffffff : payload_len);
         }
         uint8_t json_out[56];
         if (val_len >= 0 && o->value_framing == SGR_VALUE_JSON) {
           const char* why = json_pack(*o->json, val, (uint32_t)val_len, json_out, &o->json_tmp);
-          if (why) return sfail(o, SGR_ERR_INVALID, "partition %d offset %lld: JSON event: %s", partition, (long long)offset, why);
+          if (why) return set_error(&o->err, SGR_ERR_INVALID, "partition %d offset %lld: JSON event: %s", partition, (long long)offset, why);
           val = json_out; val_len = 56;
         }
-        if (val_len >= 0 && (val_len < 8 || val_len > 56)) return sfail(o, SGR_ERR_INVALID, "partition %d offset %lld: packed event value of %d bytes (expected 8..56: u32 type, u32 seq, payload)", partition, (long long)offset, val_len);
+        if (val_len >= 0 && (val_len < 8 || val_len > 56)) return set_error(&o->err, SGR_ERR_INVALID, "partition %d offset %lld: packed event value of %d bytes (expected 8..56: u32 type, u32 seq, payload)", partition, (long long)offset, val_len);
         uint32_t id_len = 0;
         {   // PartitionStringUpToColon (KafkaPartitioner.scala:38-42)
           const void* colon = memchr(key, ':', (size_t)key_len);
           id_len = colon ? (uint32_t)((const uint8_t*)colon - key) : (uint32_t)key_len;
         }
-        if (id_len >= (1u << 24)) return sfail(o, SGR_ERR_INVALID, "partition %d offset %lld: aggregate id of %u bytes", partition, (long long)offset, id_len);
+        if (id_len >= (1u << 24)) return set_error(&o->err, SGR_ERR_INVALID, "partition %d offset %lld: aggregate id of %u bytes", partition, (long long)offset, id_len);
         const uint64_t kh = hash_bytes(key, id_len);
         *kr++ = KeyRef{(uint32_t)(ar - o->arena.data()), id_len, kh};
         *shp++ = (uint8_t)ShardedDict::shard_of(kh);
@@ -965,14 +878,13 @@ int32_t decode_fetch(int32_t partition, const uint8_t* buf, uint64_t nbytes, Sta
       o->arena.resize((size_t)(ar - o->arena.data()));
       o->keys.resize((size_t)(kr - o->keys.data()));
       o->shard.resize((size_t)(shp - o->shard.data()));
-      if (c.pos != recs_len) return sfail(o, SGR_ERR_INVALID, "partition %d offset %lld: %llu stray bytes after the last record", partition, (long long)base_offset, (unsigned long long)(recs_len - c.pos));
+      if (c.pos != recs_len) return set_error(&o->err, SGR_ERR_INVALID, "partition %d offset %lld: %llu stray bytes after the last record", partition, (long long)h.base_offset, (unsigned long long)(recs_len - c.pos));
     }
-    if (!ps.seen || last_offset + 1 > ps.decoded_next) ps.decoded_next = last_offset + 1;
-    ps.seen = true;
+    ps.close(h);
   }
   st.n_trailing_bytes = nbytes - pos;
   st.n_bytes = pos;
-  if (o->arena.size() >= (1ull << 32)) return sfail(o, SGR_ERR_INVALID, "partition %d: more than 4 GiB of aggregate ids in one fetch", partition);
+  if (o->arena.size() >= (1ull << 32)) return set_error(&o->err, SGR_ERR_INVALID, "partition %d: more than 4 GiB of aggregate ids in one fetch", partition);
   return SGR_OK;
 }
 
@@ -1058,12 +970,7 @@ void commit_fetch(sgr_ingest* g, int32_t partition, Staged* o) {
   const int64_t folded = live.folded_next;
   live = std::move(o->ps);
   live.folded_next = folded;
-  sgr_ingest_stats& t = g->total; const sgr_ingest_stats& st = o->st;
-  t.n_batches += st.n_batches; t.n_records += st.n_records; t.n_markers += st.n_markers;
-  t.n_null_values += st.n_null_values; t.n_control_batches += st.n_control_batches;
-  t.n_aborted_batches += st.n_aborted_batches; t.n_aborted_records += st.n_aborted_records;
-  t.n_duplicates += st.n_duplicates; t.n_new_keys += st.n_new_keys; t.n_bytes += st.n_bytes;
-  t.n_compressed_bytes += st.n_compressed_bytes; t.n_decompressed_bytes += st.n_decompressed_bytes;
+  add_stats(&g->total, o->st);
 }
 
 }  // namespace
@@ -1093,7 +1000,7 @@ int32_t sgr_ingest_record_batches_mt(sgr_ingest* g, uint32_t n, const int32_t* p
       staged[i].null_value_type = g->null_value_type;
       staged[i].value_framing = g->value_framing;
       staged[i].json = &g->json;
-      if (decode_fetch(partitions[i], (const uint8_t*)datas[i], nbytes[i], &staged[i]) != SGR_OK) return;
+      if ((staged[i].rc = decode_fetch(partitions[i], (const uint8_t*)datas[i], nbytes[i], &staged[i])) != SGR_OK) return;
       from = &staged[i].ps;
     }
   };
@@ -1177,11 +1084,7 @@ int32_t sgr_ingest_mark_folded(sgr_ingest* g) {
 }
 
 int32_t sgr_ingest_offsets(sgr_ingest* g, int32_t partition, int64_t* decoded_next, int64_t* folded_next) {
-  if (!g) return SGR_ERR_INVALID;
-  auto it = g->parts.find(partition);
-  if (decoded_next) *decoded_next = it == g->parts.end() ? 0 : it->second.decoded_next;
-  if (folded_next) *folded_next = it == g->parts.end() ? 0 : it->second.folded_next;
-  return SGR_OK;
+  return g ? partition_offsets(g->parts, partition, decoded_next, folded_next) : SGR_ERR_INVALID;
 }
 
 int32_t sgr_ingest_get_stats(sgr_ingest* g, sgr_ingest_stats* out) {

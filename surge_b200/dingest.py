@@ -10,10 +10,8 @@ from __future__ import annotations
 import ctypes as C
 from typing import Dict, Sequence, Tuple
 
-import numpy as np
-
 from . import native as N
-from .ingest import IngestError, _as_pointer, json_events
+from .ingest import IngestError, _as_pointer, _offsets, _set_aborted, _stats, json_events
 
 
 class DeviceIngest:
@@ -45,10 +43,6 @@ class DeviceIngest:
             msg = self._lib.sgr_dingest_last_error(self._h)
             raise IngestError(rc, msg.decode("utf-8", "replace") if msg else "")
 
-    @staticmethod
-    def _stats(st) -> Dict[str, int]:
-        return {n: int(getattr(st, n)) for n, _ in N.sgr_ingest_stats._fields_ if n != "reserved"}
-
     def set_null_value_type(self, event_type: int) -> None:
         self._check(self._lib.sgr_dingest_set_null_value_type(self._h, event_type))
 
@@ -67,11 +61,7 @@ class DeviceIngest:
         self._check(self._lib.sgr_dingest_set_state_topic(self._h, 1 if on else 0))
 
     def set_aborted(self, partition: int, aborted: Sequence[Tuple[int, int]]) -> None:
-        if not aborted:
-            return
-        pids = np.asarray([a[0] for a in aborted], dtype=np.int64)
-        offs = np.asarray([a[1] for a in aborted], dtype=np.int64)
-        self._check(self._lib.sgr_dingest_set_aborted(self._h, partition, pids.ctypes.data, offs.ctypes.data, len(aborted)))
+        _set_aborted(self._check, self._lib.sgr_dingest_set_aborted, self._h, partition, aborted)
 
     def submit(self, partition: int, data) -> Dict[str, int]:
         """bytes of one fetch response (bytes, numpy uint8 array, or a pinned torch uint8 tensor): header walk + H2D copy."""
@@ -82,7 +72,7 @@ class DeviceIngest:
             ptr, n = _as_pointer(data), len(data)
         self._keep.append(data)
         self._check(self._lib.sgr_dingest_submit(self._h, partition, ptr, n, C.byref(st)))
-        return self._stats(st)
+        return _stats(st)
 
     def fold(self) -> Dict[str, int]:
         """decode + intern + fold everything submitted since the last fold; returns the poll's statistics."""
@@ -91,7 +81,7 @@ class DeviceIngest:
             self._check(self._lib.sgr_dingest_fold(self._h, C.byref(st)))
         finally:
             self._keep = []
-        return self._stats(st)
+        return _stats(st)
 
     def last_timing(self) -> Dict[str, float]:
         ms = (C.c_float * 8)()
@@ -106,6 +96,4 @@ class DeviceIngest:
         self._check(self._lib.sgr_dingest_reset(self._h))
 
     def offsets(self, partition: int) -> Tuple[int, int]:
-        d, f = C.c_int64(), C.c_int64()
-        self._check(self._lib.sgr_dingest_offsets(self._h, partition, C.byref(d), C.byref(f)))
-        return d.value, f.value
+        return _offsets(self._check, self._lib.sgr_dingest_offsets, self._h, partition)

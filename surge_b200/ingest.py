@@ -46,6 +46,26 @@ def json_events(events: Sequence[Tuple[str, int, Sequence[Tuple]]]):
     return arr
 
 
+def _stats(st) -> Dict[str, int]:
+    return {n: int(getattr(st, n)) for n, _ in N.sgr_ingest_stats._fields_ if n != "reserved"}
+
+
+def _set_aborted(check, fn, handle, partition: int, aborted: Sequence[Tuple[int, int]]) -> None:
+    """fn: sgr_ingest_set_aborted or sgr_dingest_set_aborted; `check` raises on its return code"""
+    if not aborted:
+        return
+    pids = np.asarray([a[0] for a in aborted], dtype=np.int64)
+    offs = np.asarray([a[1] for a in aborted], dtype=np.int64)
+    check(fn(handle, partition, pids.ctypes.data, offs.ctypes.data, len(aborted)))
+
+
+def _offsets(check, fn, handle, partition: int) -> Tuple[int, int]:
+    """(decoded_next, folded_next) through fn = sgr_ingest_offsets or sgr_dingest_offsets"""
+    d, f = C.c_int64(), C.c_int64()
+    check(fn(handle, partition, C.byref(d), C.byref(f)))
+    return d.value, f.value
+
+
 class Ingest:
     def __init__(self):
         self._lib = N.load_library()
@@ -94,16 +114,12 @@ class Ingest:
 
     def set_aborted(self, partition: int, aborted: Sequence[Tuple[int, int]]) -> None:
         """aborted = [(producer_id, first_offset)] from the fetch response."""
-        if not aborted:
-            return
-        pids = np.asarray([a[0] for a in aborted], dtype=np.int64)
-        offs = np.asarray([a[1] for a in aborted], dtype=np.int64)
-        self._check(self._lib.sgr_ingest_set_aborted(self._h, partition, pids.ctypes.data, offs.ctypes.data, len(aborted)))
+        _set_aborted(self._check, self._lib.sgr_ingest_set_aborted, self._h, partition, aborted)
 
     def record_batches(self, partition: int, data: bytes) -> Dict[str, int]:
         st = N.sgr_ingest_stats()
         self._check(self._lib.sgr_ingest_record_batches(self._h, partition, _as_pointer(data), len(data), C.byref(st)))
-        return {n: int(getattr(st, n)) for n, _ in N.sgr_ingest_stats._fields_ if n != "reserved"}
+        return _stats(st)
 
     def record_batches_mt(self, fetches: Sequence[Tuple[int, bytes]], threads: int = 0) -> List[Dict[str, int]]:
         """Several fetches [(partition, bytes)] in one call, decoded on `threads` host threads (0 = one per partition,
@@ -119,7 +135,7 @@ class Ingest:
         st = (N.sgr_ingest_stats * n)()
         thr = threads or min(len({p for p, _ in fetches}), os.cpu_count() or 1)
         self._check(self._lib.sgr_ingest_record_batches_mt(self._h, n, parts, ptrs, lens, thr, st))
-        return [{k: int(getattr(s, k)) for k, _ in N.sgr_ingest_stats._fields_ if k != "reserved"} for s in st]
+        return [_stats(s) for s in st]
 
     def pending(self) -> np.ndarray:
         """Copy of the pending packed records, [n, 64] uint8."""
@@ -145,11 +161,9 @@ class Ingest:
 
     def offsets(self, partition: int) -> Tuple[int, int]:
         """(decoded_next, folded_next): next offset to fetch, and the offset to commit for the lag gate."""
-        d, f = C.c_int64(), C.c_int64()
-        self._check(self._lib.sgr_ingest_offsets(self._h, partition, C.byref(d), C.byref(f)))
-        return d.value, f.value
+        return _offsets(self._check, self._lib.sgr_ingest_offsets, self._h, partition)
 
     def stats(self) -> Dict[str, int]:
         st = N.sgr_ingest_stats()
         self._check(self._lib.sgr_ingest_get_stats(self._h, C.byref(st)))
-        return {n: int(getattr(st, n)) for n, _ in N.sgr_ingest_stats._fields_ if n != "reserved"}
+        return _stats(st)
