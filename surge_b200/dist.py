@@ -14,17 +14,15 @@ from typing import Iterator, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import native as N
+from .engine import _id_batch, _rows_or_none
 
 
 def partitions_for_keys(keys: Sequence[str], num_partitions: int, up_to_colon: bool = True) -> np.ndarray:
     """partition_of[i] = abs(MurmurHash3.stringHash(keys[i].takeWhile(_ != ':')) % num_partitions)."""
     lib = N.load_library()
-    enc = [k.encode("utf-8") for k in keys]
-    offs = np.zeros(len(enc) + 1, dtype=np.uint32)
-    np.cumsum([len(b) for b in enc], out=offs[1:])
-    blob = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8).copy()
-    out = np.zeros(len(enc), dtype=np.uint32)
-    rc = lib.sgr_partitions_for_keys(blob.ctypes.data, offs.ctypes.data, len(enc), num_partitions, 1 if up_to_colon else 0, out.ctypes.data)
+    blob, offs = _id_batch([k.encode("utf-8") for k in keys])
+    out = np.zeros(len(offs) - 1, dtype=np.uint32)
+    rc = lib.sgr_partitions_for_keys(blob.ctypes.data, offs.ctypes.data, len(out), num_partitions, 1 if up_to_colon else 0, out.ctypes.data)
     if rc != 0:
         raise ValueError(f"sgr_partitions_for_keys -> {rc}")
     return out
@@ -126,9 +124,7 @@ def read_routed(engines: Sequence, ids: Sequence[str], num_partitions: int, arra
         pos = np.nonzero(owner == r)[0]
         if len(pos):
             states[pos], flags[pos], indices[pos] = e.get_many([ids[i] for i in pos], arrays=True)
-    if arrays:
-        return states, flags, indices
-    return [states[i].tobytes() if flags[i] & N.ST_EXISTS else None for i in range(n)]
+    return (states, flags, indices) if arrays else _rows_or_none(states, flags)
 
 
 def merge_scans(engines: Sequence, frm: Optional[str] = None, to: Optional[str] = None,

@@ -18,15 +18,68 @@ def _is_cuda_tensor(x) -> bool:
     return hasattr(x, "is_cuda") and bool(getattr(x, "is_cuda"))
 
 
-def _producer_done(*tensors) -> None:
-    """The engine launches on its own non-blocking stream: a tensor torch is still writing on ITS current stream must be complete
-    before the engine borrows it (the `_device` entry points take plain pointers, they cannot order against torch's stream)."""
+def _borrow(t) -> Tuple[object, int]:
+    """A CUDA tensor argument as the `_device` entry points borrow it: flat and contiguous, with its byte count. The engine
+    launches on its own non-blocking stream and those entry points take plain pointers, which cannot order against torch's
+    stream: so what torch is still writing on ITS current stream is waited for first."""
     import torch
 
-    for t in tensors:
-        if _is_cuda_tensor(t):
-            torch.cuda.current_stream(t.device).synchronize()
-            return
+    flat = t.contiguous().view(-1)
+    if _is_cuda_tensor(flat):
+        torch.cuda.current_stream(flat.device).synchronize()
+    return flat, flat.numel() * flat.element_size()
+
+
+def _host_bytes(a) -> np.ndarray:
+    return np.ascontiguousarray(a).view(np.uint8).reshape(-1)
+
+
+def _id_batch(enc: Sequence[bytes]) -> Tuple[np.ndarray, np.ndarray]:
+    """A batch of encoded ids as the C ABI takes it: (blob u8, offsets u32[n + 1]), id i = blob[offsets[i]:offsets[i + 1]].
+    The blob views the joined bytes without copying them (the C side only reads it) and is never empty, so its pointer is
+    never NULL."""
+    offs = np.zeros(len(enc) + 1, dtype=np.uint32)
+    np.cumsum([len(b) for b in enc], out=offs[1:])
+    return np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8), offs
+
+
+def _rows_or_none(states: np.ndarray, flags: np.ndarray) -> List[Optional[bytes]]:
+    """Rows of a batched read as getAggregateBytes answers: the program bytes, or None when the state does not exist."""
+    return [states[i].tobytes() if flags[i] & N.ST_EXISTS else None for i in range(len(flags))]
+
+
+def _split_values(buf: np.ndarray, offs: np.ndarray, n: int) -> List[Optional[bytes]]:
+    raw = buf[:int(offs[n])].tobytes() if n else b""
+    return [raw[offs[i]:offs[i + 1]] if offs[i + 1] > offs[i] else None for i in range(n)]
+
+
+class _Page:
+    """The buffers one page of an export or a scan is written into. Its rows are the program bytes, or with values_cap the JSON
+    values of the *_values twin, whose arguments in their place (values, values_cap, value_offsets) `out` holds."""
+
+    def __init__(self, cap: int, user: int, ids_cap: int, values_cap: Optional[int]):
+        if values_cap is None:
+            self.rows, self.voffs = np.empty((cap, user), dtype=np.uint8), None
+            self.out = (self.rows.ctypes.data,)
+        else:
+            self.rows, self.voffs = np.empty(max(values_cap, 1), dtype=np.uint8), np.empty(cap + 1, dtype=np.uint64)
+            self.out = (self.rows.ctypes.data, values_cap, self.voffs.ctypes.data)
+        self.flags = np.empty(cap, dtype=np.uint32)
+        self.idx = np.empty(cap, dtype=np.int64)
+        self.offs = np.empty(cap + 1, dtype=np.uint32)
+        self.blob = np.empty(max(ids_cap, 1), dtype=np.uint8)
+
+    def data(self, k: int):
+        return self.rows[:k] if self.voffs is None else _split_values(self.rows, self.voffs, k)
+
+    def ids(self, k: int, n_keys: Optional[int] = None) -> List[Optional[str]]:
+        """The page's ids; with n_keys, None for a row at or past the key table (its empty span is told apart from the id "" by its
+        index)."""
+        offs = self.offs
+        raw = self.blob[:int(offs[k])].tobytes() if k else b""
+        if n_keys is None:
+            return [raw[offs[i]:offs[i + 1]].decode("utf-8") for i in range(k)]
+        return [raw[offs[i]:offs[i + 1]].decode("utf-8") if self.idx[i] < n_keys else None for i in range(k)]
 
 
 class _DevView:
@@ -73,6 +126,13 @@ class ReplayEngine:
     def _ck(self, rc: int) -> None:
         N.check(self._lib, self._h, rc)
 
+    def _lend(self, t, *also) -> Tuple[int, int]:
+        """Borrow a CUDA tensor for a load or a rebuild: the engine may read it until the next one, so it and `also` replace
+        the kept tensors. Returns (pointer, bytes)."""
+        flat, nbytes = _borrow(t)
+        self._keep = [flat, *also]
+        return flat.data_ptr(), nbytes
+
     # -- program
     def register_program(self, prog: N.sgr_fold_program) -> None:
         self._ck(self._lib.sgr_register_program(self._h, C.byref(prog)))
@@ -83,27 +143,21 @@ class ReplayEngine:
         """CSR event log. numpy -> copied to HBM; CUDA tensors -> borrowed."""
         if _is_cuda_tensor(events):
             assert _is_cuda_tensor(seg_offsets)
-            ev = events.contiguous().view(-1)
-            nbytes = ev.numel() * ev.element_size()
-            n_agg = seg_offsets.numel() - 1
-            _producer_done(ev)
-            self._keep = [ev, seg_offsets]
-            self._ck(self._lib.sgr_load_events_device(self._h, ev.data_ptr(), nbytes, seg_offsets.data_ptr(), n_agg))
+            ev, nbytes = self._lend(events, seg_offsets)
+            self._ck(self._lib.sgr_load_events_device(self._h, ev, nbytes, seg_offsets.data_ptr(), seg_offsets.numel() - 1))
             return
-        ev = np.ascontiguousarray(events).view(np.uint8).reshape(-1)
+        ev = _host_bytes(events)
         off = np.ascontiguousarray(seg_offsets, dtype=np.uint64)
         self._ck(self._lib.sgr_load_events(self._h, ev.ctypes.data, ev.size, off.ctypes.data, len(off) - 1))
 
     def load_events_indexed(self, events, seg_offsets, rec_offsets) -> None:
         """Variable records + record directory (rec_offsets[n_records+1]): enables the record-parallel kernel."""
         if _is_cuda_tensor(events):
-            ev = events.contiguous().view(-1)
-            _producer_done(ev)
-            self._keep = [ev, seg_offsets, rec_offsets]
-            self._ck(self._lib.sgr_load_events_indexed_device(self._h, ev.data_ptr(), ev.numel() * ev.element_size(), seg_offsets.data_ptr(),
-                                                              seg_offsets.numel() - 1, rec_offsets.data_ptr(), rec_offsets.numel() - 1))
+            ev, nbytes = self._lend(events, seg_offsets, rec_offsets)
+            self._ck(self._lib.sgr_load_events_indexed_device(self._h, ev, nbytes, seg_offsets.data_ptr(), seg_offsets.numel() - 1,
+                                                              rec_offsets.data_ptr(), rec_offsets.numel() - 1))
             return
-        ev = np.ascontiguousarray(events).view(np.uint8).reshape(-1)
+        ev = _host_bytes(events)
         off = np.ascontiguousarray(seg_offsets, dtype=np.uint64)
         ro = np.ascontiguousarray(rec_offsets, dtype=np.uint64)
         self._ck(self._lib.sgr_load_events_indexed(self._h, ev.ctypes.data, ev.size, off.ctypes.data, len(off) - 1, ro.ctypes.data, len(ro) - 1))
@@ -111,24 +165,19 @@ class ReplayEngine:
     def load_unsorted(self, records, n_agg: int) -> None:
         """Fixed 64-byte records in arrival order; grouped stably by aggregate on the device."""
         if _is_cuda_tensor(records):
-            r = records.contiguous().view(-1)
-            n = r.numel() * r.element_size() // 64
-            _producer_done(r)
-            self._keep = [r]
-            self._ck(self._lib.sgr_load_unsorted_device(self._h, r.data_ptr(), n, n_agg))
+            r, nbytes = self._lend(records)
+            self._ck(self._lib.sgr_load_unsorted_device(self._h, r, nbytes // 64, n_agg))
             return
-        r = np.ascontiguousarray(records).view(np.uint8).reshape(-1)
+        r = _host_bytes(records)
         self._ck(self._lib.sgr_load_unsorted(self._h, r.ctypes.data, r.size // 64, n_agg))
 
     def fold_unsorted(self, records, n_agg: int) -> None:
         """Rebuild all states from an arrival-order log (Kafka partition order) in one call."""
         if _is_cuda_tensor(records):
-            r = records.contiguous().view(-1)
-            _producer_done(r)
-            self._keep = [r]
-            self._ck(self._lib.sgr_fold_unsorted_device(self._h, r.data_ptr(), r.numel() * r.element_size() // 64, n_agg))
+            r, nbytes = self._lend(records)
+            self._ck(self._lib.sgr_fold_unsorted_device(self._h, r, nbytes // 64, n_agg))
             return
-        r = np.ascontiguousarray(records).view(np.uint8).reshape(-1)
+        r = _host_bytes(records)
         self._ck(self._lib.sgr_fold_unsorted(self._h, r.ctypes.data, r.size // 64, n_agg))
 
     def set_initial_states(self, states: Optional[np.ndarray]) -> None:
@@ -151,13 +200,13 @@ class ReplayEngine:
 
     def fold_incremental(self, records) -> None:
         if _is_cuda_tensor(records):
-            r = records.contiguous().view(-1)
-            _producer_done(r)
+            # the micro-batch is read only during the call; the loaded log's tensors stay kept
+            r, nbytes = _borrow(records)
             self._keep.append(r)
-            self._ck(self._lib.sgr_fold_incremental_device(self._h, r.data_ptr(), r.numel() * r.element_size() // 64))
+            self._ck(self._lib.sgr_fold_incremental_device(self._h, r.data_ptr(), nbytes // 64))
             self._keep.pop()
             return
-        r = np.ascontiguousarray(records).view(np.uint8).reshape(-1)
+        r = _host_bytes(records)
         self._ck(self._lib.sgr_fold_incremental(self._h, r.ctypes.data, r.size // 64))
 
     def grow_states(self, n_agg: int) -> None:
@@ -169,10 +218,14 @@ class ReplayEngine:
         self._ck(self._lib.sgr_fold_ingested(self._h, ingest.handle))
 
     # -- results
-    def n_aggregates(self) -> int:
+    def _states_device(self) -> Tuple[int, int, int]:
+        """(device pointer, n_agg, state_bytes) of the live state table."""
         p, n, sb = C.c_void_p(), C.c_uint64(), C.c_uint32()
         self._ck(self._lib.sgr_states_device(self._h, C.byref(p), C.byref(n), C.byref(sb)))
-        return int(n.value)
+        return p.value, int(n.value), int(sb.value)
+
+    def n_aggregates(self) -> int:
+        return self._states_device()[1]
 
     def export_states(self, out: Optional[np.ndarray] = None, bitmaps: bool = False):
         n = self.n_aggregates()
@@ -190,10 +243,8 @@ class ReplayEngine:
         """The live device state table as a torch uint8 tensor [n_agg, state_bytes] (borrowed)."""
         import torch
 
-        p, n, sb = C.c_void_p(), C.c_uint64(), C.c_uint32()
-        self._ck(self._lib.sgr_states_device(self._h, C.byref(p), C.byref(n), C.byref(sb)))
-        view = _DevView(p.value, n.value * sb.value, self)
-        return torch.as_tensor(view, device=f"cuda:{self.device}").view(n.value, sb.value)
+        p, n, sb = self._states_device()
+        return torch.as_tensor(_DevView(p, n * sb, self), device=f"cuda:{self.device}").view(n, sb)
 
     def events_tensors(self):
         """(events u8[nbytes], seg_offsets i64[n_agg+1]) device tensors of the engine's CSR log (borrowed)."""
@@ -205,11 +256,8 @@ class ReplayEngine:
         return ev, po.value
 
     def load_keys(self, keys: Sequence[str]) -> None:
-        enc = [k.encode("utf-8") for k in keys]
-        offs = np.zeros(len(enc) + 1, dtype=np.uint32)
-        np.cumsum([len(b) for b in enc], out=offs[1:])
-        blob = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8).copy()
-        self._ck(self._lib.sgr_load_keys(self._h, blob.ctypes.data, offs.ctypes.data, len(enc)))
+        blob, offs = _id_batch([k.encode("utf-8") for k in keys])
+        self._ck(self._lib.sgr_load_keys(self._h, blob.ctypes.data, offs.ctypes.data, len(offs) - 1))
 
     def get(self, key: str) -> Optional[bytes]:
         """getAggregateBytes(aggregateId): Option[Array[Byte]] — None when the state does not exist."""
@@ -225,31 +273,23 @@ class ReplayEngine:
         """getAggregateBytes for many ids in one call, served from the device table (sgr_get_batch): a list of Optional[bytes],
         the same as get() for each id. arrays=True: (states u8[n, state_bytes - 8], flags u32[n], indices i64[n]) instead, with
         zero rows for None states and unknown ids, flags 0 and index -1 for unknown ids."""
-        enc = [k.encode("utf-8") for k in keys]
-        n = len(enc)
-        offs = np.zeros(n + 1, dtype=np.uint32)
-        np.cumsum([len(b) for b in enc], out=offs[1:])
-        blob = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8)
+        blob, offs = _id_batch([k.encode("utf-8") for k in keys])
+        n = len(offs) - 1
         states = np.zeros((n, max(self.state_bytes - 8, 0)), dtype=np.uint8)
         flags = np.zeros(n, dtype=np.uint32)
         indices = np.zeros(n, dtype=np.int64)
         self._ck(self._lib.sgr_get_batch(self._h, blob.ctypes.data, offs.ctypes.data, n, states.ctypes.data, states.nbytes,
                                          flags.ctypes.data, indices.ctypes.data))
-        if arrays:
-            return states, flags, indices
-        return [states[i].tobytes() if flags[i] & N.ST_EXISTS else None for i in range(n)]
+        return (states, flags, indices) if arrays else _rows_or_none(states, flags)
 
     def put_batch(self, ids: Sequence[str], rows, present=None) -> int:
         """Records of a state topic, in arrival order, applied to the table on the device (sgr_put_batch): the last write per id
         wins, a tombstone (present[i] false) leaves None. rows: u8[n, state_bytes - 8] (or n rows of bytes) holding the program
         bytes; present: bool[n], None for all rows present. New ids get the next dense indices in order of first appearance and
         join the key table get() / get_many() / export_changes() / scan() read. Returns the number of new ids."""
-        enc = [k.encode("utf-8") for k in ids]
-        n = len(enc)
+        blob, offs = _id_batch([k.encode("utf-8") for k in ids])
+        n = len(offs) - 1
         user = self.state_bytes - 8
-        offs = np.zeros(n + 1, dtype=np.uint32)
-        np.cumsum([len(b) for b in enc], out=offs[1:])
-        blob = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8)
         if isinstance(rows, np.ndarray):
             r = np.ascontiguousarray(rows, dtype=np.uint8).reshape(n, user)
         else:
@@ -272,24 +312,28 @@ class ReplayEngine:
         state is None. A page holds at most page_rows rows (None: the whole table) and page_id_bytes id bytes. Every page of one
         export reads the same table: a fold, grow, set_initial_states or load_keys between two pages raises
         InvalidStateStoreException (SGR_ERR_STATE) from the next one."""
+        for idx, flags, err, ids, rows in self._export_pages(select, page_rows, page_id_bytes):
+            yield idx, flags, err, rows, ids
+
+    def _export_pages(self, select: int, max_rows: Optional[int], ids_cap: int, values_cap: Optional[int] = None):
+        """The pages of sgr_export_changes, or with values_cap of sgr_export_changes_values: (indices, flags, err_idx, ids, rows
+        or values). The export ends when the cursor reaches the end of the table."""
         n_agg = self.n_aggregates()
-        cap = max(1, n_agg if page_rows is None else min(int(page_rows), max(n_agg, 1)))
-        user = self.state_bytes - 8
+        cap = max(1, n_agg if max_rows is None else min(int(max_rows), max(n_agg, 1)))
+        ids_cap = int(ids_cap)
+        values_cap = None if values_cap is None else int(values_cap)
+        fn = self._lib.sgr_export_changes if values_cap is None else self._lib.sgr_export_changes_values
         cur = N.sgr_changes_cursor()
         n = C.c_uint64()
         while True:
-            rows = np.empty((cap, user), dtype=np.uint8)
-            flags, err = np.empty(cap, dtype=np.uint32), np.empty(cap, dtype=np.uint32)
-            idx = np.empty(cap, dtype=np.int64)
-            offs = np.empty(cap + 1, dtype=np.uint32)
-            blob = np.empty(max(int(page_id_bytes), 1), dtype=np.uint8)
-            self._ck(self._lib.sgr_export_changes(self._h, int(select), C.byref(cur), cap, rows.ctypes.data, flags.ctypes.data, err.ctypes.data,
-                                                  idx.ctypes.data, blob.ctypes.data, int(page_id_bytes), offs.ctypes.data, C.byref(n)))
-            k, n_keys = int(n.value), int(cur.n_keys)
-            raw = blob[:int(offs[k])].tobytes() if k else b""
-            ids = [raw[offs[i]:offs[i + 1]].decode("utf-8") if idx[i] < n_keys else None for i in range(k)]
+            pg = _Page(cap, self.state_bytes - 8, ids_cap, values_cap)
+            err = np.empty(cap, dtype=np.uint32)
+            self._ck(fn(self._h, int(select), C.byref(cur), cap, *pg.out, pg.flags.ctypes.data, err.ctypes.data, pg.idx.ctypes.data,
+                        pg.blob.ctypes.data, ids_cap, pg.offs.ctypes.data, C.byref(n)))
+            k = int(n.value)
+            ids = pg.ids(k, int(cur.n_keys))
             if k:
-                yield idx[:k], flags[:k], err[:k], rows[:k], ids
+                yield pg.idx[:k], pg.flags[:k], err[:k], ids, pg.data(k)
             if cur.next >= n_agg:
                 return
 
@@ -299,29 +343,31 @@ class ReplayEngine:
         that end open. Yields pages of (indices i64[n], flags u32[n], rows u8[n, state_bytes - 8], ids), at most page_rows rows
         and page_id_bytes id bytes each. Each page resumes after the last id of the one before, so folds between pages are
         fine: an id live throughout is reported exactly once."""
+        for idx, flags, ids, rows in self._scan_pages(frm, to, page_rows, page_id_bytes):
+            yield idx, flags, rows, ids
+
+    def _scan_pages(self, frm: Optional[str], to: Optional[str], max_rows: int, ids_cap: int, values_cap: Optional[int] = None):
+        """The pages of sgr_scan, or with values_cap of sgr_scan_values: (indices, flags, ids, rows or values). Each page resumes
+        after the last id of the one before (from_exclusive); the scan ends on a page that left no live row in range out."""
         n_agg = self.n_aggregates()
-        cap = max(1, min(int(page_rows), max(n_agg, 1)))
-        user = self.state_bytes - 8
+        cap = max(1, min(int(max_rows), max(n_agg, 1)))
+        ids_cap = int(ids_cap)
+        values_cap = None if values_cap is None else int(values_cap)
+        fn = self._lib.sgr_scan if values_cap is None else self._lib.sgr_scan_values
         lo = None if frm is None else frm.encode("utf-8")
         hi = None if to is None else to.encode("utf-8")
         hi_buf = None if hi is None else C.create_string_buffer(hi, max(len(hi), 1))
         exclusive = 0
         n, more = C.c_uint64(), C.c_int32()
         while True:
-            rows = np.empty((cap, user), dtype=np.uint8)
-            flags = np.empty(cap, dtype=np.uint32)
-            idx = np.empty(cap, dtype=np.int64)
-            offs = np.empty(cap + 1, dtype=np.uint32)
-            blob = np.empty(max(int(page_id_bytes), 1), dtype=np.uint8)
+            pg = _Page(cap, self.state_bytes - 8, ids_cap, values_cap)
             lo_buf = None if lo is None else C.create_string_buffer(lo, max(len(lo), 1))
-            self._ck(self._lib.sgr_scan(self._h, lo_buf, 0 if lo is None else len(lo), exclusive, hi_buf, 0 if hi is None else len(hi), cap,
-                                        rows.ctypes.data, flags.ctypes.data, idx.ctypes.data, blob.ctypes.data, int(page_id_bytes),
-                                        offs.ctypes.data, C.byref(n), C.byref(more)))
+            self._ck(fn(self._h, lo_buf, 0 if lo is None else len(lo), exclusive, hi_buf, 0 if hi is None else len(hi), cap, *pg.out,
+                        pg.flags.ctypes.data, pg.idx.ctypes.data, pg.blob.ctypes.data, ids_cap, pg.offs.ctypes.data, C.byref(n), C.byref(more)))
             k = int(n.value)
             if k:
-                raw = blob[:int(offs[k])].tobytes()
-                yield idx[:k], flags[:k], rows[:k], [raw[offs[i]:offs[i + 1]].decode("utf-8") for i in range(k)]
-                lo, exclusive = raw[offs[k - 1]:offs[k]], 1
+                yield pg.idx[:k], pg.flags[:k], pg.ids(k), pg.data(k)
+                lo, exclusive = pg.blob[int(pg.offs[k - 1]):int(pg.offs[k])].tobytes(), 1
             if not more.value:
                 return
 
@@ -339,19 +385,11 @@ class ReplayEngine:
                 arr[i].len = m[3] if len(m) > 3 else 0
         self._ck(self._lib.sgr_set_state_writer(self._h, arr, len(members)))
 
-    @staticmethod
-    def _split_values(buf: np.ndarray, offs: np.ndarray, n: int) -> List[Optional[bytes]]:
-        raw = buf[:int(offs[n])].tobytes() if n else b""
-        return [raw[offs[i]:offs[i + 1]] if offs[i + 1] > offs[i] else None for i in range(n)]
-
     def get_many_values(self, keys: Sequence[str], values_cap: Optional[int] = None) -> List[Optional[bytes]]:
         """The JSON state value of each id (sgr_get_batch_values), None for a None state or an unknown id. values_cap: the byte
         budget of one call (None: sized from the first attempt)."""
-        enc = [k.encode("utf-8") for k in keys]
-        n = len(enc)
-        offs = np.zeros(n + 1, dtype=np.uint32)
-        np.cumsum([len(b) for b in enc], out=offs[1:])
-        blob = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8)
+        blob, offs = _id_batch([k.encode("utf-8") for k in keys])
+        n = len(offs) - 1
         flags = np.zeros(max(n, 1), dtype=np.uint32)
         voffs = np.zeros(n + 1, dtype=np.uint64)
         need = C.c_uint64()
@@ -364,63 +402,19 @@ class ReplayEngine:
                 cap = int(need.value)
                 continue
             self._ck(rc)
-            return self._split_values(buf, voffs, n)
+            return _split_values(buf, voffs, n)
 
     def export_changes_values(self, select: int = N.ST_CHANGED, max_rows: Optional[int] = 1 << 20, values_cap: int = 64 << 20,
                               page_id_bytes: int = 64 << 20) -> Iterator[Tuple[np.ndarray, np.ndarray, np.ndarray, List[Optional[str]], List[Optional[bytes]]]]:
         """export_changes with JSON values in place of rows (sgr_export_changes_values). Yields pages of (indices i64[n], flags
         u32[n], err_idx u32[n], ids, values): values[i] is the row's JSON state, or None for a None state (the tombstone: the
         (id, null) record of a republish). A page also ends before a value that does not fit in values_cap bytes."""
-        n_agg = self.n_aggregates()
-        cap = max(1, n_agg if max_rows is None else min(int(max_rows), max(n_agg, 1)))
-        cur = N.sgr_changes_cursor()
-        n = C.c_uint64()
-        while True:
-            buf = np.empty(max(int(values_cap), 1), dtype=np.uint8)
-            voffs = np.empty(cap + 1, dtype=np.uint64)
-            flags, err = np.empty(cap, dtype=np.uint32), np.empty(cap, dtype=np.uint32)
-            idx = np.empty(cap, dtype=np.int64)
-            offs = np.empty(cap + 1, dtype=np.uint32)
-            blob = np.empty(max(int(page_id_bytes), 1), dtype=np.uint8)
-            self._ck(self._lib.sgr_export_changes_values(self._h, int(select), C.byref(cur), cap, buf.ctypes.data, int(values_cap), voffs.ctypes.data,
-                                                         flags.ctypes.data, err.ctypes.data, idx.ctypes.data, blob.ctypes.data, int(page_id_bytes),
-                                                         offs.ctypes.data, C.byref(n)))
-            k, n_keys = int(n.value), int(cur.n_keys)
-            raw = blob[:int(offs[k])].tobytes() if k else b""
-            ids = [raw[offs[i]:offs[i + 1]].decode("utf-8") if idx[i] < n_keys else None for i in range(k)]
-            if k:
-                yield idx[:k], flags[:k], err[:k], ids, self._split_values(buf, voffs, k)
-            if cur.next >= n_agg:
-                return
+        yield from self._export_pages(select, max_rows, page_id_bytes, values_cap)
 
     def scan_values(self, frm: Optional[str] = None, to: Optional[str] = None, max_rows: int = 1 << 20, values_cap: int = 64 << 20,
                     page_id_bytes: int = 64 << 20) -> Iterator[Tuple[np.ndarray, np.ndarray, List[str], List[bytes]]]:
         """scan with JSON values in place of rows (sgr_scan_values). Yields pages of (indices i64[n], flags u32[n], ids, values)."""
-        n_agg = self.n_aggregates()
-        cap = max(1, min(int(max_rows), max(n_agg, 1)))
-        lo = None if frm is None else frm.encode("utf-8")
-        hi = None if to is None else to.encode("utf-8")
-        hi_buf = None if hi is None else C.create_string_buffer(hi, max(len(hi), 1))
-        exclusive = 0
-        n, more = C.c_uint64(), C.c_int32()
-        while True:
-            buf = np.empty(max(int(values_cap), 1), dtype=np.uint8)
-            voffs = np.empty(cap + 1, dtype=np.uint64)
-            flags = np.empty(cap, dtype=np.uint32)
-            idx = np.empty(cap, dtype=np.int64)
-            offs = np.empty(cap + 1, dtype=np.uint32)
-            blob = np.empty(max(int(page_id_bytes), 1), dtype=np.uint8)
-            lo_buf = None if lo is None else C.create_string_buffer(lo, max(len(lo), 1))
-            self._ck(self._lib.sgr_scan_values(self._h, lo_buf, 0 if lo is None else len(lo), exclusive, hi_buf, 0 if hi is None else len(hi), cap,
-                                               buf.ctypes.data, int(values_cap), voffs.ctypes.data, flags.ctypes.data, idx.ctypes.data,
-                                               blob.ctypes.data, int(page_id_bytes), offs.ctypes.data, C.byref(n), C.byref(more)))
-            k = int(n.value)
-            if k:
-                raw = blob[:int(offs[k])].tobytes()
-                yield idx[:k], flags[:k], [raw[offs[i]:offs[i + 1]].decode("utf-8") for i in range(k)], self._split_values(buf, voffs, k)
-                lo, exclusive = raw[offs[k - 1]:offs[k]], 1
-            if not more.value:
-                return
+        yield from self._scan_pages(frm, to, max_rows, page_id_bytes, values_cap)
 
     def get_index(self, agg: int) -> Tuple[Optional[bytes], int, int]:
         """(program bytes or None, flags, err_idx) of one dense aggregate index."""
@@ -451,10 +445,8 @@ class ReplayEngine:
     def dist_route_and_fold(self, records, fused) -> None:
         """records: CUDA tensor of fixed 64-byte records in arrival order carrying GLOBAL aggregate indices.
         fused: 0 NCCL all-to-all, 1 peer scatter, 2 pipelined push + fold, 3 the same with projected records (see sgr.h)."""
-        r = records.contiguous().view(-1)
-        _producer_done(r)
-        self._keep = [r]
-        self._ck(self._lib.sgr_dist_route_and_fold(self._h, r.data_ptr(), r.numel() * r.element_size() // 64, int(fused)))
+        r, nbytes = self._lend(records)
+        self._ck(self._lib.sgr_dist_route_and_fold(self._h, r, nbytes // 64, int(fused)))
 
     def dist_recv_base(self) -> int:
         p = C.c_void_p()
@@ -492,11 +484,8 @@ class ReplayEngine:
         """The ids of global aggregates 0..n_global - 1 (str or bytes), in the partition table's order (sgr_dist_load_keys):
         this rank keeps the ones it owns, in local-slot order, and get(), get_many(), export_changes(), scan() and their
         *_values twins then read its rows by id. An id another rank owns is unknown here."""
-        enc = [k if isinstance(k, bytes) else k.encode("utf-8") for k in ids]
-        offs = np.zeros(len(enc) + 1, dtype=np.uint32)
-        np.cumsum([len(b) for b in enc], out=offs[1:])
-        blob = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8).copy()
-        self._ck(self._lib.sgr_dist_load_keys(self._h, blob.ctypes.data, offs.ctypes.data, len(enc)))
+        blob, offs = _id_batch([k if isinstance(k, bytes) else k.encode("utf-8") for k in ids])
+        self._ck(self._lib.sgr_dist_load_keys(self._h, blob.ctypes.data, offs.ctypes.data, len(offs) - 1))
 
     def stats(self) -> N.sgr_stats:
         s = N.sgr_stats()
