@@ -15,7 +15,6 @@ import json
 import os
 import subprocess
 import sys
-import threading
 import time
 
 import numpy as np
@@ -64,26 +63,19 @@ def rebuild(n: int, part: np.ndarray):
     src = (arrival["agg"] % 64).astype(np.int64) % R
     feeds = [torch.from_numpy(arrival[src == r].view(np.uint8).reshape(-1).copy()).to("cuda:0") for r in range(R)]
     cap = int(len(rec) / R * 1.5) + 64 * 1024 * R
-    ranks = []
-    for r in range(R):
+
+    def engine():
         e = ReplayEngine(0)
         e.register_program(P.counter_program())
-        e.dist_init(r, R, None, cap)
-        e.dist_set_partitions(part)
-        ranks.append(e)
-    bases = [e.dist_recv_base() for e in ranks]
-    for r, e in enumerate(ranks):
-        e.dist_set_peers(bases)
-        e.dist_reserve(feeds[r].numel() // 64)
-    th = [threading.Thread(target=ranks[r].dist_route_and_fold, args=(feeds[r], 2)) for r in range(R)]
-    for t in th:
-        t.start()
-    for t in th:
-        t.join()
+        return e
+
+    ranks = D.LoopbackRanks(engine, part, feeds, cap)
+    errors, _, _ = ranks.run(2)
+    assert not any(errors), errors
     one = ReplayEngine(0)
     one.register_program(P.counter_program())
     one.fold_unsorted(arrival, n)
-    return ranks, one
+    return ranks.engines, one
 
 
 def main() -> None:

@@ -332,7 +332,6 @@ cudaError_t exclusive_scan_u32_public(const uint32_t* in, uint32_t* out, uint32_
 int dist_set_partitions(DistState* d, const uint32_t* partition_of_agg, uint64_t n_global, cudaStream_t st, std::string* err) {
   if (n_global >= (1ull << 32)) { *err = "at most 2^32 global aggregates"; return SGR_ERR_UNSUPPORTED; }
   cudaError_t ce;
-#define DTRY(x) if ((ce = (x)) != cudaSuccess) { *err = std::string(#x ": ") + cudaGetErrorString(ce); return SGR_ERR_CUDA; }
   DTRY(d->part_tmp.reserve(n_global * 4)); DTRY(d->owner_of.reserve(n_global)); DTRY(d->local_of.reserve(n_global * 4));
   DTRY(d->flags.reserve(n_global * 4)); DTRY(d->pos.reserve(n_global * 4));
   DTRY(d->scan_tmp.reserve((2 * (n_global / 4096 + 2) + 4 * 4096) * 4));
@@ -363,7 +362,6 @@ int dist_set_partitions(DistState* d, const uint32_t* partition_of_agg, uint64_t
   route_table_kernel<<<nb, 256, 0, st>>>((const uint8_t*)d->owner_of.p, (const uint32_t*)d->local_of.p, n_global, (uint32_t*)d->route_of.p);
   DTRY(cudaStreamSynchronize(st));
   d->n_global = n_global; d->n_local = n_local;
-#undef DTRY
   return SGR_OK;
 }
 
@@ -381,8 +379,6 @@ const uint8_t* dist_recv_buffer(const DistState* d) { return d->peer_recv[d->ran
 int dist_route(DistState* d, const uint8_t* d_records, uint64_t n, bool fused, unsigned long long* d_counters, cudaStream_t st,
                uint64_t* n_recv_out, std::string* err) {
   cudaError_t ce;
-#define DTRY(x) if ((ce = (x)) != cudaSuccess) { *err = std::string(#x ": ") + cudaGetErrorString(ce); return SGR_ERR_CUDA; }
-#define NTRY(x) { ncclResult_t _r = (x); if (_r != ncclSuccess) { *err = std::string(#x ": ") + g_nccl.GetErrorString(_r); return SGR_ERR_DIST; } }
   if (!d->n_global) { *err = "no partition table: call sgr_dist_set_partitions first"; return SGR_ERR_NOT_LOADED; }
   if (d->loopback) { *err = "loopback ranks have no NCCL communicator: use fused >= 2 with a sort-free program"; return SGR_ERR_UNSUPPORTED; }
   if (n >= (1ull << 32)) { *err = "at most 2^32 records per rank per exchange"; return SGR_ERR_UNSUPPORTED; }
@@ -492,8 +488,6 @@ int dist_route(DistState* d, const uint8_t* d_records, uint64_t n, bool fused, u
   uint64_t remote = 0;
   for (int q = 0; q < R; ++q) if (q != d->rank) remote += send_cnt[q];
   d->stats.n_sent_remote = remote;
-#undef DTRY
-#undef NTRY
   return SGR_OK;
 }
 

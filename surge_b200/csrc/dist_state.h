@@ -35,6 +35,11 @@ struct NcclApi {
 };
 NcclApi& nccl_api();
 
+// The exchange code's error path: a failed CUDA (DTRY) or NCCL (NTRY) call puts its source text and the library's reason into
+// *err and returns SGR_ERR_CUDA / SGR_ERR_DIST. DTRY needs `cudaError_t ce` and both need `std::string* err` in scope.
+#define DTRY(x) if ((ce = (x)) != cudaSuccess) { *err = std::string(#x ": ") + cudaGetErrorString(ce); return SGR_ERR_CUDA; }
+#define NTRY(x) { ncclResult_t _r = (x); if (_r != ncclSuccess) { *err = std::string(#x ": ") + nccl_api().GetErrorString(_r); return SGR_ERR_DIST; } }
+
 // Loopback ranks are streams of one process on one device, and streams share the device's hardware queues, each run in order.
 // A fold launch that waits for its rank's spinning wait kernel can stand at the head of a queue and hold back a peer's partition
 // or flag kernel queued behind it, and the wait spins until its limit. So every loopback rank enqueues all its partition and flag

@@ -462,9 +462,17 @@ PushTuning& push_tuning() { static PushTuning t; return t; }
 
 static int tile_recs() { const int t = push_tuning().tile; return t == 256 || t == 1024 ? t : 512; }
 // chunks are whole multiples of 1024 records (the largest tile), so the chunk boundaries do not depend on the tile size
+// (surge_b200/dist.py chunk_records is the Python twin)
 static uint64_t chunk_records(uint64_t n, uint32_t n_chunks) {
   const uint64_t c = (n + n_chunks - 1) / n_chunks;
   return (c + 1023) / 1024 * 1024;
+}
+
+// One arrival-flag word, (epoch << 32) | count + 1: false when it is not this epoch's or the source failed (count 0xffffffff).
+static bool arrived_count(unsigned long long v, uint32_t epoch, uint32_t* count) {
+  if ((uint32_t)(v >> 32) != epoch || (uint32_t)v == 0xffffffffu) return false;
+  *count = (uint32_t)v - 1u;
+  return true;
 }
 
 // CUDA loads a kernel lazily at its first launch, and that load can wait for the kernels already running on the device — such as
@@ -505,8 +513,6 @@ int dist_push_reserve(DistState* d, uint64_t n, uint32_t n_chunks, std::string* 
 int dist_push_fold(DistState* d, const uint8_t* d_records, uint64_t n, const PushFoldArgs& pf, cudaStream_t st, PushFoldResult* out,
                    std::string* err) {
   cudaError_t ce;
-#define DTRY(x) if ((ce = (x)) != cudaSuccess) { *err = std::string(#x ": ") + cudaGetErrorString(ce); return SGR_ERR_CUDA; }
-#define NTRY(x) { ncclResult_t _r = (x); if (_r != ncclSuccess) { *err = std::string(#x ": ") + nccl_api().GetErrorString(_r); return SGR_ERR_DIST; } }
   const int R = d->nranks;
   if (!d->n_global) { *err = "no partition table: call sgr_dist_set_partitions first"; return SGR_ERR_NOT_LOADED; }
   if (R > 1 && !d->peers_mapped) { *err = "the push path needs the peers' receive buffers (sgr_dist_ipc_import / sgr_dist_set_peers)"; return SGR_ERR_NOT_LOADED; }
@@ -544,6 +550,12 @@ int dist_push_fold(DistState* d, const uint8_t* d_records, uint64_t n, const Pus
   DTRY(cudaStreamWaitEvent(s1, d->pev[0], 0));
   DTRY(cudaStreamWaitEvent(sp, d->pev[0], 0));
   unsigned long long* my_flags = (unsigned long long*)d->peer_base[d->rank];
+  // region (source s, owner q, chunk c): push, the source stores it into the owner's buffer at [s][c]; pull, the source keeps
+  // it in its own buffer at [q][c] and the owner's fold reads it over NVLink
+  auto region = [&](int s, int q, uint32_t c) -> uint8_t* {
+    return pull ? d->peer_recv[s] + ((uint64_t)q * C + c) * cap_region * out_bytes
+                : d->peer_recv[q] + ((uint64_t)s * C + c) * cap_region * out_bytes;
+  };
   // receiver side of chunk c: wait for the flags of every source, then the sort-free accumulate over the chunk's regions
   auto fold_chunk = [&](uint32_t c) -> cudaError_t {
     push_wait_kernel<<<1, 32, 0, s1>>>(my_flags, c, (uint32_t)R, epoch, status);
@@ -551,9 +563,7 @@ int dist_push_fold(DistState* d, const uint8_t* d_records, uint64_t n, const Pus
     bs.n_regions = (uint32_t)R; bs.compact = pf.compact ? 1u : 0u; bs.rec_bytes = out_bytes; bs.rotate = (uint32_t)d->rank; bs.carried = 1;
     bs.blocks_per_sm = push_tuning().fold_blocks_per_sm > 0 ? (uint32_t)push_tuning().fold_blocks_per_sm : 0xffffffffu;
     for (int s = 0; s < R; ++s) {
-      // pull: source s keeps what it has for me in ITS buffer, region (me, chunk): the fold reads it over NVLink
-      bs.base[s] = pull ? d->peer_recv[s] + ((uint64_t)d->rank * C + c) * cap_region * out_bytes
-                        : d->peer_recv[d->rank] + ((uint64_t)s * C + c) * cap_region * out_bytes;
+      bs.base[s] = region(s, d->rank, c);
       bs.count_flag[s] = my_flags + (size_t)s * kMaxChunks + c;
       bs.count[s] = cap_region;
       // + the index the record carries within ITS SOURCE's chunk c. The sources cut their logs into chunks of different lengths
@@ -570,10 +580,7 @@ int dist_push_fold(DistState* d, const uint8_t* d_records, uint64_t n, const Pus
       PushArgs a{};
       a.rec = d_records + begin * 64; a.n = (uint32_t)cn; a.nranks = (uint32_t)R; a.n_global = d->n_global;
       a.route_of = (const uint32_t*)d->route_of.p;
-      // push: region (me, chunk) inside every owner's buffer (remote stores); pull: region (owner, chunk) inside MY buffer
-      for (int q = 0; q < R; ++q)
-        a.dst[q] = pull ? d->peer_recv[d->rank] + ((uint64_t)q * C + c) * cap_region * out_bytes
-                        : d->peer_recv[q] + ((uint64_t)d->rank * C + c) * cap_region * out_bytes;
+      for (int q = 0; q < R; ++q) a.dst[q] = region(d->rank, q, c);
       a.cap_region = (uint32_t)cap_region; a.out_bytes = out_bytes;
       a.lb = (unsigned long long*)d->lb.p + (size_t)c * ctas_per_chunk * kMaxRanks; a.n_ctas = (uint32_t)ctas_per_chunk;
       a.ticket = tickets + c; a.totals = totals + (size_t)c * kMaxRanks; a.status = status;
@@ -623,16 +630,16 @@ int dist_push_fold(DistState* d, const uint8_t* d_records, uint64_t n, const Pus
   float ms_push = 0, ms_total = 0;
   cudaEventElapsedTime(&ms_push, d->pev[0], d->pev[1]);
   cudaEventElapsedTime(&ms_total, d->pev[0], d->pev[3]);
-  uint64_t n_recv = 0; bool remote_err = false;
+  // what arrived, and what stayed local: region (me, *)
+  uint64_t n_recv = 0, kept = 0; bool remote_err = false;
   out->regions.clear();
   for (int s = 0; s < R; ++s)
     for (uint32_t c = 0; c < C; ++c) {
-      const unsigned long long v = h_flags[(size_t)s * kMaxChunks + c];
-      if ((uint32_t)(v >> 32) != epoch || (uint32_t)v == 0xffffffffu) { remote_err = true; continue; }
-      const uint32_t cnt = (uint32_t)v - 1u;
+      uint32_t cnt;
+      if (!arrived_count(h_flags[(size_t)s * kMaxChunks + c], epoch, &cnt)) { remote_err = true; continue; }
       n_recv += cnt;
-      out->regions.push_back({pull ? d->peer_recv[s] + ((uint64_t)d->rank * C + c) * cap_region * out_bytes
-                                   : d->peer_recv[d->rank] + ((uint64_t)s * C + c) * cap_region * out_bytes, cnt});
+      if (s == d->rank) kept += cnt;
+      out->regions.push_back({region(s, d->rank, c), cnt});
     }
   int my_err = SGR_OK;
   if (h_status[0]) { *err = std::to_string(h_status[0]) + " records carry a global aggregate index >= n_global"; my_err = SGR_ERR_INVALID; }
@@ -660,15 +667,8 @@ int dist_push_fold(DistState* d, const uint8_t* d_records, uint64_t n, const Pus
   d->stats = DistStats{};
   d->stats.n_sent = n; d->stats.n_recv = n_recv;
   d->stats.ms_scatter = ms_push; d->stats.ms_exchange = 0;
-  uint64_t kept = 0;
-  {
-    // what stayed local: region (me, *) — read back from my own flags
-    for (uint32_t c = 0; c < C; ++c) { const unsigned long long v = h_flags[(size_t)d->rank * kMaxChunks + c]; if ((uint32_t)(v >> 32) == epoch && (uint32_t)v != 0xffffffffu) kept += (uint32_t)v - 1u; }
-  }
   d->stats.n_sent_remote = n >= kept ? n - kept : 0;
   return my_err;
-#undef DTRY
-#undef NTRY
 }
 
 // contiguous 64-byte copy of everything that arrived, regions in (source, chunk) order: an aggregate's events keep their order

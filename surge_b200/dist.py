@@ -9,7 +9,9 @@ from __future__ import annotations
 
 import ctypes as C
 import heapq
-from typing import Iterator, List, Optional, Sequence, Tuple
+import threading
+import time
+from typing import Callable, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -105,6 +107,93 @@ def exchange_ids(engine, rank: int, nranks: int, recv_capacity_records: int, fus
         handles: List[Optional[bytes]] = [None] * nranks
         dist.all_gather_object(handles, mine)
         engine.dist_ipc_import(handles)
+
+
+def chunk_records(n: int, chunks: int) -> int:
+    """A rank's chunk length on the push path (csrc/route_push.cu chunk_records) for a log of n records cut into `chunks`
+    chunks: whole multiples of 1024 records."""
+    c = -(-n // chunks)
+    return -(-c // 1024) * 1024
+
+
+class LoopbackRanks:
+    """The ranks of one routed job inside this process, every one an engine on the same device (sgr_dist_init without a unique
+    id), set up as include/sgr.h asks: every rank learns every rank's receive base, and reserves the push path's buffers for
+    its feed up front, because nothing may allocate while a peer's wait kernel spins. new_engine() returns a new engine with
+    its program registered and its options set; feeds[r] is rank r's device tensor of 64-byte records in arrival order, with
+    the global aggregate index at +8. The engines are the caller's to read and are closed with the ranks."""
+
+    def __init__(self, new_engine: Callable[[], object], part: np.ndarray, feeds: Sequence, capacity: int):
+        R = len(feeds)
+        self.engines: List = []
+        self.feeds = list(feeds)
+        try:
+            for r in range(R):
+                e = new_engine()
+                self.engines.append(e)
+                e.dist_init(r, R, None, capacity)
+                e.dist_set_partitions(part)
+            if R > 1:
+                bases = [e.dist_recv_base() for e in self.engines]
+                for e in self.engines:
+                    e.dist_set_peers(bases)
+            for e, f in zip(self.engines, self.feeds):
+                e.dist_reserve(f.nbytes // 64)
+        except BaseException:
+            self.close()
+            raise
+
+    def close(self) -> None:
+        for e in self.engines:
+            e.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def run(self, fused: int, timeout: float = 120.0):
+        """Every rank's dist_route_and_fold(feed, fused) on a thread of its own. A rank that meets a throwing aggregate
+        returns SGR_ERR_AGAIN: real ranks agree over NCCL to repeat the exchange in log order, loopback ranks leave that to
+        their caller, so when every rank returned either nothing or SGR_ERR_AGAIN, every rank repeats the call once with
+        option push_ordered = 1. push_ordered is 0 again on return, whatever happened. A rank still inside its call after
+        `timeout` seconds fails an assertion, and so does SGR_ERR_AGAIN next to another error.
+
+        Returns (errors, repeated, times) of the last attempt: each rank's exception or None, whether the ordered repeat ran,
+        and when each rank entered and left its call, in seconds after the threads were started."""
+        R = len(self.engines)
+        repeated = False
+        try:
+            for _attempt in range(2):
+                errors, times = [None] * R, [None] * R
+                t0 = time.monotonic()
+
+                def one(r):
+                    start = time.monotonic()
+                    try:
+                        self.engines[r].dist_route_and_fold(self.feeds[r], fused)
+                    except Exception as ex:  # noqa: BLE001 — reported to the caller with the rank's other outcomes
+                        errors[r] = ex
+                    times[r] = (round(start - t0, 4), round(time.monotonic() - t0, 4))
+
+                th = [threading.Thread(target=one, args=(r,)) for r in range(R)]
+                for t in th:
+                    t.start()
+                for t in th:
+                    t.join(timeout=timeout)
+                assert not any(t.is_alive() for t in th), ("a loopback rank hung", "entered, returned:", times)
+                again = [getattr(x, "code", None) == N.SGR_ERR_AGAIN for x in errors]
+                if not any(again):
+                    break
+                assert all(x is None or a for x, a in zip(errors, again)), (errors, "entered, returned:", times)
+                repeated = True
+                for e in self.engines:
+                    e.set_option("push_ordered", 1)
+        finally:
+            for e in self.engines:
+                e.set_option("push_ordered", 0)
+        return errors, repeated, times
 
 
 def read_routed(engines: Sequence, ids: Sequence[str], num_partitions: int, arrays: bool = False):

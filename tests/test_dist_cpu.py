@@ -4,8 +4,10 @@ The device kernels (csrc/dist.cu) mirror surge_b200.dist.route_on_host; here the
 import os
 import socket
 import sys
+import threading
 
 import numpy as np
+import pytest
 import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
@@ -103,3 +105,117 @@ def test_topic_partitions_split_over_ranks_need_no_exchange():
     assert len(owners) == len(keys)
     owner, _, _ = D.owner_and_local_index(part, nranks)          # the routed path's owner table says the same
     assert [owners[k] for k in keys] == owner.tolist()
+
+
+# ------------------------------------------------------------------ the loopback-ranks driver, on fake engines
+class _FakeRank:
+    """One rank for surge_b200.dist.LoopbackRanks, without a library or a GPU: it records the calls the driver makes, and its
+    dist_route_and_fold returns or raises what answer(rank, push_ordered) says (None, or an exception to raise)."""
+
+    def __init__(self, answer):
+        self.answer, self.rank, self.log, self.push_ordered, self.calls, self.closed = answer, None, [], 0, [], False
+
+    def dist_init(self, rank, nranks, unique_id, capacity):
+        self.rank = rank
+        self.log.append(("init", rank, nranks, unique_id, capacity))
+
+    def dist_set_partitions(self, part):
+        self.log.append(("partitions", len(part)))
+
+    def dist_recv_base(self):
+        return 0x1000 * (self.rank + 1)
+
+    def dist_set_peers(self, bases):
+        self.log.append(("peers", list(bases)))
+
+    def dist_reserve(self, n):
+        self.log.append(("reserve", n))
+
+    def set_option(self, name, value):
+        assert name == "push_ordered"
+        self.push_ordered = value
+
+    def dist_route_and_fold(self, feed, fused):
+        self.calls.append((fused, self.push_ordered))
+        ex = self.answer(self.rank, self.push_ordered)
+        if ex is not None:
+            raise ex
+
+    def close(self):
+        self.closed = True
+
+
+def _fake_ranks(answer, R=3):
+    from surge_b200 import dist as D
+
+    feeds = [np.zeros(64 * (r + 1), np.uint8) for r in range(R)]
+    return D.LoopbackRanks(lambda: _FakeRank(answer), np.zeros(10, np.uint32), feeds, 4096)
+
+
+def _again():
+    from surge_b200 import native as N
+
+    return N.SgrError(N.SGR_ERR_AGAIN, "throwing aggregates")
+
+
+def test_loopback_ranks_set_up_and_run_without_a_repeat():
+    with _fake_ranks(lambda r, ordered: None) as ranks:
+        bases = [0x1000, 0x2000, 0x3000]
+        for r, e in enumerate(ranks.engines):
+            assert e.log == [("init", r, 3, None, 4096), ("partitions", 10), ("peers", bases), ("reserve", r + 1)]
+        errors, repeated, times = ranks.run(2)
+        assert errors == [None] * 3 and not repeated
+        assert all(e.calls == [(2, 0)] and e.push_ordered == 0 for e in ranks.engines)
+        assert all(0 <= t[0] <= t[1] for t in times)
+    assert all(e.closed for e in ranks.engines)
+
+
+def test_loopback_ranks_repeat_in_order_when_every_rank_says_again():
+    with _fake_ranks(lambda r, ordered: None if ordered else _again()) as ranks:
+        errors, repeated, _ = ranks.run(3)
+        assert errors == [None] * 3 and repeated
+        assert all(e.calls == [(3, 0), (3, 1)] and e.push_ordered == 0 for e in ranks.engines)
+
+
+def test_loopback_ranks_refuse_again_next_to_another_error():
+    from surge_b200 import native as N
+
+    other = N.SgrError(N.SGR_ERR_CAPACITY, "a source rank reported a full receive region")
+    with _fake_ranks(lambda r, ordered: _again() if r == 0 else other if r == 1 else None) as ranks:
+        with pytest.raises(AssertionError) as info:
+            ranks.run(2)
+        assert "SGR_ERR_AGAIN" in str(info.value) and "SGR_ERR_CAPACITY" in str(info.value)
+        assert all(len(e.calls) == 1 and e.push_ordered == 0 for e in ranks.engines)
+
+
+def test_loopback_ranks_report_a_rank_that_hangs():
+    release, threads = threading.Event(), []
+
+    def answer(r, ordered):
+        if r == 2:
+            threads.append(threading.current_thread())
+            release.wait()
+        return None
+
+    try:
+        with _fake_ranks(answer) as ranks:
+            with pytest.raises(AssertionError, match="hung"):
+                ranks.run(2, timeout=0.2)
+            assert all(e.push_ordered == 0 for e in ranks.engines)
+    finally:
+        release.set()
+        for t in threads:
+            t.join(timeout=10)
+    assert len(threads) == 1 and not threads[0].is_alive()
+
+
+def test_loopback_ranks_reset_push_ordered_when_a_rank_raises():
+    def answer(r, ordered):
+        if not ordered:
+            return _again()
+        return RuntimeError("lost rank") if r == 1 else None
+
+    with _fake_ranks(answer) as ranks:
+        errors, repeated, _ = ranks.run(2)
+        assert repeated and errors[0] is None and errors[2] is None and str(errors[1]) == "lost rank"
+        assert all(e.calls == [(2, 0), (2, 1)] and e.push_ordered == 0 for e in ranks.engines)

@@ -10,7 +10,6 @@ Three layers:
 import os
 import subprocess
 import sys
-import threading
 
 import numpy as np
 import pytest
@@ -168,52 +167,23 @@ def _loopback_job(R, n_global, rec_all, part, fused, chunks, capacity, prog=None
     torch = _torch()
     arrival = S.interleave_arrival(rec_all, seed=seed)
     src = (arrival["agg"] % 64).astype(np.int64) % R
-    engines, feeds = [], []
-    for r in range(R):
+    feeds = [torch.from_numpy(arrival[src == r].view(np.uint8).reshape(-1).copy()).to("cuda:0") for r in range(R)]
+
+    def engine():
         e = ReplayEngine(0)
         e.register_program(prog or P.counter_program())
         e.set_option("push_chunks", chunks)
-        e.dist_init(r, R, None, capacity)           # no unique id: loopback
-        e.dist_set_partitions(part)
-        engines.append(e)
-        mine = arrival[src == r]
-        feeds.append(torch.from_numpy(mine.view(np.uint8).reshape(-1).copy()).to("cuda:0"))
-    bases = [e.dist_recv_base() for e in engines]
-    for r, e in enumerate(engines):
-        e.dist_set_peers(bases)
-        e.dist_reserve(feeds[r].numel() // 64)   # ranks share one device here: nothing may allocate while a peer's wait kernel spins
-    errors = [None] * R
+        return e
 
-    def run(r):
-        try:
-            engines[r].dist_route_and_fold(feeds[r], fused)
-        except SgrError as ex:  # noqa: PERF203
-            errors[r] = ex
-
+    ranks = D.LoopbackRanks(engine, part, feeds, capacity)
     again_rounds = 0
     for _round in range(2):       # twice: epochs, scratch hygiene, region reuse
-        for _attempt in range(2):
-            errors = [None] * R
-            th = [threading.Thread(target=run, args=(r,)) for r in range(R)]
-            for t in th:
-                t.start()
-            for t in th:
-                t.join(timeout=120)
-            assert not any(t.is_alive() for t in th), "a loopback rank hung"
-            if not any(isinstance(x, SgrError) and x.code == N.SGR_ERR_AGAIN for x in errors):
-                break
-            # a rank met a throwing aggregate: what real ranks agree on over NCCL, loopback ranks leave to the caller —
-            # EVERY rank repeats the call in ordered mode
-            again_rounds += 1
-            assert all(x is None or x.code == N.SGR_ERR_AGAIN for x in errors), errors
-            for e in engines:
-                e.set_option("push_ordered", 1)
-        for e in engines:
-            e.set_option("push_ordered", 0)
+        errors, repeated, _ = ranks.run(fused)
+        again_rounds += repeated
         if any(errors):
             break
-    engines[0].again_rounds = again_rounds
-    return engines, errors
+    ranks.engines[0].again_rounds = again_rounds
+    return ranks.engines, errors
 
 
 def _check_loopback(engines, want, R):

@@ -59,82 +59,25 @@ def split_feeds(rng, rec, R):
     return arrival, [arrival[src == r] for r in range(R)]
 
 
-def chunk_records(n, chunks):
-    c = -(-n // chunks)
-    return -(-c // 1024) * 1024
-
-
-class Ranks:
+def Ranks(prog, part, feeds, chunks=4):
     """R loopback ranks on cuda:0 holding `prog`, partition table `part`, feeds[r] in arrival order (global index at +8)."""
+    torch = _torch()
+    cap = len(feeds) * chunks * max(D.chunk_records(len(f), chunks) for f in feeds) + 1024
 
-    def __init__(self, prog, part, feeds, chunks=4, force_route=False):
-        torch = _torch()
-        R = len(feeds)
-        cap = R * chunks * max(chunk_records(len(f), chunks) for f in feeds) + 1024
-        self.engines, self.feeds = [], []
-        try:
-            for r in range(R):
-                e = ReplayEngine(0)
-                self.engines.append(e)
-                e.register_program(prog)
-                e.set_option("push_chunks", chunks)
-                if force_route:
-                    e.set_option("force_route", 1)
-                e.dist_init(r, R, None, cap)
-                e.dist_set_partitions(part)
-                self.feeds.append(torch.from_numpy(np.ascontiguousarray(feeds[r]).reshape(-1)).to("cuda:0"))
-            if R > 1:
-                bases = [e.dist_recv_base() for e in self.engines]
-                for e in self.engines:
-                    e.dist_set_peers(bases)
-            for r, e in enumerate(self.engines):
-                e.dist_reserve(len(feeds[r]))   # ranks share one device: nothing may allocate while a peer's wait kernel spins
-        except BaseException:
-            self.close()
-            raise
+    def engine():
+        e = ReplayEngine(0)
+        e.register_program(prog)
+        e.set_option("push_chunks", chunks)
+        return e
 
-    def close(self):
-        for e in self.engines:
-            e.close()
+    return D.LoopbackRanks(engine, part, [torch.from_numpy(np.ascontiguousarray(f).reshape(-1)).to("cuda:0") for f in feeds], cap)
 
-    def __enter__(self):
-        return self
 
-    def __exit__(self, *a):
-        self.close()
-
-    def run(self, fused):
-        """Every rank's route_and_fold on a thread of its own; after SGR_ERR_AGAIN every rank repeats with push_ordered = 1.
-        Returns whether the ordered repeat ran."""
-        R = len(self.engines)
-        repeated = False
-        try:
-            for _attempt in range(2):
-                errors = [None] * R
-
-                def one(r):
-                    try:
-                        self.engines[r].dist_route_and_fold(self.feeds[r], fused)
-                    except SgrError as ex:
-                        errors[r] = ex
-
-                th = [threading.Thread(target=one, args=(r,)) for r in range(R)]
-                for t in th:
-                    t.start()
-                for t in th:
-                    t.join(timeout=120)
-                assert not any(t.is_alive() for t in th), "a loopback rank hung"
-                if not any(x is not None and x.code == N.SGR_ERR_AGAIN for x in errors):
-                    break
-                assert all(x is None or x.code == N.SGR_ERR_AGAIN for x in errors), errors
-                repeated = True
-                for e in self.engines:
-                    e.set_option("push_ordered", 1)
-        finally:
-            for e in self.engines:
-                e.set_option("push_ordered", 0)
-        assert not any(errors), errors
-        return repeated
+def fold(ranks, fused):
+    """Every rank's route_and_fold, which must succeed; returns whether the ordered repeat ran."""
+    errors, repeated, _ = ranks.run(fused)
+    assert not any(errors), errors
+    return repeated
 
 
 def single_engine(prog, arrival, n_global, ids):
@@ -283,7 +226,7 @@ def test_loopback_ranks_serve_their_rows_by_id(name, throws):
                 for e in ranks.engines:
                     e.dist_load_keys(ids)
                 for fused in (2, 3):
-                    assert ranks.run(fused) == throws
+                    assert fold(ranks, fused) == throws
                     check_rank_reads(ranks.engines, single, ids, want, rng, f"{name} R={R} fused={fused}")
         finally:
             single.close()
@@ -549,7 +492,7 @@ def test_four_million_aggregates_on_four_ranks():
 
     try:
         with Ranks(P.counter_program(), part, feeds) as ranks:
-            ranks.run(2)
+            fold(ranks, 2)
             th = threading.Thread(target=sample)
             th.start()
             try:

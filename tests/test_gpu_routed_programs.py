@@ -12,9 +12,6 @@ and error counts with oracle/program_interp.py c_fold over the global CSR log.
 Part B folds the same kind of programs on one engine over logs of 2 M records: fold_unsorted on the bulk kernels and on
 the micro-batch kernel, and three micro-batches onto the live table, against c_fold_arrival_order.
 """
-import threading
-import time
-
 import numpy as np
 import pytest
 
@@ -40,97 +37,29 @@ def same(got, want, what):
         raise AssertionError(f"{what}: {len(bad)} of {len(want)} states differ; first {bad[:6]}\n got {got[bad[:3]].tolist()}\nwant {want[bad[:3]].tolist()}")
 
 
-def chunk_records(n, chunks):
-    """route_push.cu chunk_records: a rank's chunk length, whole multiples of 1024 records."""
-    c = -(-n // chunks)
-    return -(-c // 1024) * 1024
-
-
 # ------------------------------------------------------------------ loopback ranks
-class Ranks:
+def Ranks(rules, part, feeds, chunks, force_route=False):
     """R loopback ranks on cuda:0. feeds[r]: rank r's records in arrival order (global aggregate index at +8). The receive
     capacity is R x chunks x the longest chunk of any rank, so no region can overflow whatever the partition table."""
+    torch = _torch()
+    cap = len(feeds) * chunks * max(D.chunk_records(len(f), chunks) for f in feeds) + 1024
 
-    def __init__(self, rules, part, feeds, chunks, force_route=False):
-        torch = _torch()
-        R = len(feeds)
-        self.chunks = chunks
-        cap = R * chunks * max(chunk_records(len(f), chunks) for f in feeds) + 1024
-        self.engines, self.feeds = [], []
-        try:
-            for r in range(R):
-                e = ReplayEngine(0)
-                self.engines.append(e)
-                e.register_program(P.make_program(16, N.REC_FIXED64, rules))
-                e.set_option("push_chunks", chunks)
-                if force_route:
-                    e.set_option("force_route", 1)
-                e.dist_init(r, R, None, cap)
-                e.dist_set_partitions(part)
-                self.feeds.append(torch.from_numpy(np.ascontiguousarray(feeds[r]).reshape(-1)).to("cuda:0"))
-            if R > 1:
-                bases = [e.dist_recv_base() for e in self.engines]
-                for e in self.engines:
-                    e.dist_set_peers(bases)
-            for r, e in enumerate(self.engines):
-                e.dist_reserve(len(feeds[r]))   # ranks share one device: nothing may allocate while a peer's wait kernel spins
-        except BaseException:
-            self.close()
-            raise
+    def engine():
+        e = ReplayEngine(0)
+        e.register_program(P.make_program(16, N.REC_FIXED64, rules))
+        e.set_option("push_chunks", chunks)
+        if force_route:
+            e.set_option("force_route", 1)
+        return e
 
-    def close(self):
-        for e in self.engines:
-            e.close()
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
-
-    def run(self, fused):
-        """Every rank's route_and_fold on a thread of its own. After SGR_ERR_AGAIN (a rank met a throwing aggregate) every
-        rank repeats the call with push_ordered = 1, which real ranks agree on over NCCL. Returns (errors, repeated); when
-        each rank entered and left its call, in seconds after the threads were started, is kept in last_times."""
-        R = len(self.engines)
-        repeated = False
-        try:
-            for _attempt in range(2):
-                errors, times = [None] * R, [None] * R
-                t0 = time.monotonic()
-
-                def one(r):
-                    start = time.monotonic()
-                    try:
-                        self.engines[r].dist_route_and_fold(self.feeds[r], fused)
-                    except SgrError as ex:
-                        errors[r] = ex
-                    times[r] = (round(start - t0, 4), round(time.monotonic() - t0, 4))
-
-                th = [threading.Thread(target=one, args=(r,)) for r in range(R)]
-                for t in th:
-                    t.start()
-                for t in th:
-                    t.join(timeout=120)
-                assert not any(t.is_alive() for t in th), "a loopback rank hung"
-                self.last_times = times
-                if not any(x is not None and x.code == N.SGR_ERR_AGAIN for x in errors):
-                    break
-                assert all(x is None or x.code == N.SGR_ERR_AGAIN for x in errors), (errors, "entered, returned:", times)
-                repeated = True
-                for e in self.engines:
-                    e.set_option("push_ordered", 1)
-        finally:
-            for e in self.engines:
-                e.set_option("push_ordered", 0)
-        return errors, repeated
+    return D.LoopbackRanks(engine, part, [torch.from_numpy(np.ascontiguousarray(f).reshape(-1)).to("cuda:0") for f in feeds], cap)
 
 
 def exchange_bytes(fused, n_slots):
     return 64 if fused == 2 else 16 if (1 + n_slots) * 4 <= 16 else 32
 
 
-def check_ranks(ranks, want, nev, nerr, fused, n_slots, what):
+def check_ranks(ranks, chunks, want, nev, nerr, fused, n_slots, what):
     total, n_seen = 0, 0
     for r, e in enumerate(ranks.engines):
         gl = e.dist_local_aggregates().astype(np.int64)
@@ -140,7 +69,7 @@ def check_ranks(ranks, want, nev, nerr, fused, n_slots, what):
             assert h == 0, f"{what}, rank {r} owns nothing"
         total = (total + h) % (1 << 64)
         n_seen += len(gl)
-        assert e.stats().fold_launches == 2 * ranks.chunks + 1, f"{what}, rank {r}: the push path did not run"
+        assert e.stats().fold_launches == 2 * chunks + 1, f"{what}, rank {r}: the push path did not run"
         assert e.dist_stats().exchange_record_bytes == exchange_bytes(fused, n_slots), what
     assert n_seen == len(want), what
     assert total == D.states_hash(want), what
@@ -177,9 +106,9 @@ def run_and_check(rng, rules, n_slots, rec, off, want, nev, nerr, R, fused_modes
     with Ranks(rules, part, feeds, chunks) as ranks:
         for fused in fused_modes:
             for rnd in range(2):                     # twice: epochs, scratch hygiene, region reuse
-                errors, repeated = ranks.run(fused)
-                assert not any(errors), (what, errors, "entered, returned:", ranks.last_times)
-                check_ranks(ranks, want, nev, nerr, fused, n_slots, f"{what} fused={fused} round {rnd}")
+                errors, repeated, times = ranks.run(fused)
+                assert not any(errors), (what, errors, "entered, returned:", times)
+                check_ranks(ranks, chunks, want, nev, nerr, fused, n_slots, f"{what} fused={fused} round {rnd}")
                 if expect_repeat is not None:
                     assert repeated == expect_repeat, f"{what}: ordered repeat {repeated}"
 
@@ -270,7 +199,7 @@ def test_exchange_variants_with_a_seven_slot_tombstone_program(pull, staged, til
 
 
 def refused_everywhere(ranks, fused, what):
-    errors, _ = ranks.run(fused)
+    errors, _, _ = ranks.run(fused)
     assert all(isinstance(x, SgrError) and x.code == N.SGR_ERR_UNSUPPORTED for x in errors), (what, errors)
     return errors
 
@@ -284,9 +213,9 @@ def test_compact_exchange_refuses_eight_slots():
     with Ranks(rules, rng.integers(0, 32, size=len(off) - 1).astype(np.uint32), feeds, 4) as ranks:
         refused_everywhere(ranks, 3, "8 slots, fused 3")
         for _ in range(2):
-            errors, _ = ranks.run(2)
+            errors, _, _ = ranks.run(2)
             assert not any(errors), errors
-            check_ranks(ranks, want, nev, nerr, 2, n_slots, "8 slots, fused 2")
+            check_ranks(ranks, 4, want, nev, nerr, 2, n_slots, "8 slots, fused 2")
 
 
 OUTSIDE_SORT_FREE = {
