@@ -119,26 +119,26 @@ __device__ __forceinline__ void apply_rec(const RecView& r, uint32_t idx1, uint3
   if (slot >= a.n_slots) { atomicAdd(a.counters + 4, 1ull); return; }
   uint8_t* entry = a.scr + (slot << a.lay.entry_shift);
   const uint32_t fl = type < 16u ? tab[type * kTabStride] : 0u;
-  if (!(fl & 1u)) {   // handler exception / MatchError: sticky mark, the slot is replayed exactly afterwards
+  if (!(fl & kRuleValid)) {   // handler exception / MatchError: sticky mark, the slot is replayed exactly afterwards
     atomicOr(a.throw_bits + (slot >> 5), 1u << (slot & 31u));
     return;
   }
 #pragma unroll
   for (int w = 0; w < 2; ++w) {
     const uint32_t spec = tab[type * kTabStride + 1 + w];
-    const uint32_t mode = spec & 3u, s = spec >> 3;
+    const uint32_t mode = spec_mode(spec), s = spec_slot(spec);
     if (!mode) continue;
     uint32_t v = 0;
     if (s) {
       const uint32_t rw = COMPACT ? 1u + s : pg.slot_word[s];
       v = rw < 8u ? pick8(r.q0, r.q1, rw) : __ldg(reinterpret_cast<const uint32_t*>(r.p) + rw);
     }
-    if (spec & 4u) v = 0u - v;
-    if (mode == 1u) { if (v) red_add_u32<HINTS>(reinterpret_cast<uint32_t*>(entry + a.lay.word_off[w]), v, pol_last); }
+    if (spec_neg(spec)) v = 0u - v;
+    if (mode == kModeAdd) { if (v) red_add_u32<HINTS>(reinterpret_cast<uint32_t*>(entry + a.lay.word_off[w]), v, pol_last); }
     else red_max_u64<HINTS>(reinterpret_cast<unsigned long long*>(entry + a.lay.word_off[w]), ((unsigned long long)idx1 << 32) | v, pol_last);
   }
   if ((a.lay.last_needed_mask >> type) & 1u)
-    red_max_u32<HINTS>(reinterpret_cast<uint32_t*>(entry), (idx1 << 2) | ((fl & 2u) ? 2u : 1u), pol_last);
+    red_max_u32<HINTS>(reinterpret_cast<uint32_t*>(entry), (idx1 << 2) | rule_ex(fl), pol_last);
 }
 
 template <bool COMPACT, bool HINTS, int kUnroll>
@@ -225,7 +225,7 @@ __global__ void __launch_bounds__(kThreads) bulk_finish_kernel(const __grid_cons
     uint4* st = reinterpret_cast<uint4*>(a.states + slot * 16);
     const uint4 old = *st;
     const uint32_t ex0 = old.z & SGR_ST_EXISTS;
-    const uint32_t exn = (a.lay.has_none && (e0.x & 3u) == 2u) ? 0u : SGR_ST_EXISTS;
+    const uint32_t exn = (a.lay.has_none && (e0.x & 3u) == EX_NONE) ? 0u : SGR_ST_EXISTS;
     const uint32_t b[2] = {ex0 ? old.x : 0u, ex0 ? old.y : 0u};
     uint32_t nv[2];
 #pragma unroll
@@ -236,10 +236,7 @@ __global__ void __launch_bounds__(kThreads) bulk_finish_kernel(const __grid_cons
       for (int k = 1; k < 8; ++k) { if ((uint32_t)k == c) lo = ew[k]; if ((uint32_t)k == c + 1u) hi = ew[k]; }
       nv[w] = ((a.lay.set_only_mask >> w) & 1u) ? (hi ? lo : b[w]) : b[w] + lo;
     }
-    if (!exn) { nv[0] = 0; nv[1] = 0; }
-    uint32_t changed = exn != ex0;
-    if (exn && ex0) changed |= (nv[0] != old.x) | (nv[1] != old.y);
-    *st = make_uint4(nv[0], nv[1], exn | (changed ? SGR_ST_CHANGED : 0u), 0u);
+    finish_row16(st, old, ex0, nv[0], nv[1], exn);
   }
 }
 
@@ -290,34 +287,23 @@ cudaError_t bulk_preload_kernels() {
 
 bool bulk_layout_for(const RowProgram& prog, BulkLayout* out) {
   if (prog.user_words != 2 || prog.cls != 0 || prog.f64_mask || prog.slot_word[0] != 0) return false;
-  uint32_t has_add = 0, has_set = 0, has_none = 0;
-  for (int t = 0; t < 16; ++t) {
-    const uint32_t fl = prog.tab[t * kTabStride];
-    if (!(fl & 1u)) continue;
-    if (fl & 2u) has_none = 1;
-    for (int w = 0; w < 2; ++w) {
-      const uint32_t mode = prog.tab[t * kTabStride + 1 + w] & 3u;
-      if (mode == 1u) has_add |= 1u << w;
-      if (mode == 2u) has_set |= 1u << w;
-    }
-  }
-  if (has_add & has_set) return false;
+  const WordModes wm = word_modes(prog);
+  if (wm.add & wm.set) return false;
   BulkLayout l{};
-  l.set_only_mask = has_set; l.has_none = has_none;
+  l.set_only_mask = wm.set; l.has_none = wm.none;
   // cells: `last` at +0; add-only words take 4 bytes, set-only words 8 (8-byte aligned)
-  const int n_set = __builtin_popcount(has_set & 3u);
+  const int n_set = __builtin_popcount(wm.set & 3u);
   if (n_set == 2) { l.entry_shift = 5; l.word_off[0] = 8; l.word_off[1] = 16; }
   else if (n_set == 1) {
     l.entry_shift = 4;
-    const int ws = (has_set & 1u) ? 0 : 1;
+    const int ws = (wm.set & 1u) ? 0 : 1;
     l.word_off[ws] = 8; l.word_off[ws ^ 1] = 4;
   } else { l.entry_shift = 4; l.word_off[0] = 4; l.word_off[1] = 8; }
   for (int t = 0; t < 16; ++t) {
-    const uint32_t fl = prog.tab[t * kTabStride];
-    if (!(fl & 1u)) continue;
+    if (!(prog.tab[t * kTabStride] & kRuleValid)) continue;
     bool sets = false;
-    for (int w = 0; w < 2; ++w) sets |= (prog.tab[t * kTabStride + 1 + w] & 3u) == 2u;
-    if (has_none || !sets) l.last_needed_mask |= 1u << t;
+    for (int w = 0; w < 2; ++w) sets |= spec_mode(prog.tab[t * kTabStride + 1 + w]) == kModeSet;
+    if (wm.none || !sets) l.last_needed_mask |= 1u << t;
   }
   *out = l;
   return true;

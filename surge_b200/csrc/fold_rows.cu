@@ -36,9 +36,6 @@
 namespace sgr {
 namespace {
 
-constexpr uint32_t M_ERR = 0x80000000u;   // some event in the range threw
-constexpr uint32_t EX_SOME = 1u, EX_NONE = 2u;
-
 template <int W>
 struct Xf {
   uint32_t m;      // bits [2w+1:2w]: mode of word w (bit0 ADD, bit1 SET; OR-composable), bit31 error
@@ -71,12 +68,6 @@ __device__ __forceinline__ uint4 ldg_stream(const uint4* p) {
                : "l"(p));
   return v;
 }
-__device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) {
-  uint32_t v;
-  asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p));
-  return v;
-}
-
 
 // select one of four registers by a 2-bit lane-dependent index (3 SEL)
 __device__ __forceinline__ uint32_t sel4(uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, int i) {
@@ -106,29 +97,14 @@ __device__ __forceinline__ void finish_segment(const RowArgs& a, uint64_t seg, b
   if (nonempty) {
     exn = (tex == EX_NONE) ? 0u : SGR_ST_EXISTS;
 #pragma unroll
-    for (int w = 0; w < W; ++w) {
-      nw[w] = (ts.m & (2u << (2 * w))) ? ts.v[w] : old[w] + ts.v[w];
-      if (!exn) nw[w] = 0u;
-    }
+    for (int w = 0; w < W; ++w) nw[w] = (ts.m & (2u << (2 * w))) ? ts.v[w] : old[w] + ts.v[w];
   }
-  uint32_t changed = exn != ex0;
-  if (exn && ex0) {
-#pragma unroll
-    for (int w = 0; w < W; ++w) changed |= (nw[w] != old[w]);
-  }
-  uint32_t outw[W + 2];
-#pragma unroll
-  for (int w = 0; w < W; ++w) outw[w] = nw[w];
-  outw[W] = exn | (changed ? SGR_ST_CHANGED : 0u);
-  outw[W + 1] = 0u;
-  uint4* dp = reinterpret_cast<uint4*>(a.states_out + slot * (uint64_t)(W + 2) * 4);
-#pragma unroll
-  for (int q = 0; q < (W + 2) / 4; ++q) dp[q] = make_uint4(outw[4 * q], outw[4 * q + 1], outw[4 * q + 2], outw[4 * q + 3]);
+  finish_row<W>(a.states_out + slot * (uint64_t)(W + 2) * 4, old, ex0, nw, exn);
 }
 
 template <int W, int NS>
 __global__ void __launch_bounds__(kRowThreads, 3) fold_rows_kernel(const __grid_constant__ RowArgs a, const __grid_constant__ RowProgram pg) {
-  // per type, one uint4-aligned entry: [0] flags (bit0 valid, bit1 result is None), [1+w] mode | neg<<2 | slot<<3
+  // per type, one uint4-aligned entry of RowProgram::tab
   __shared__ __align__(16) uint32_t tab[16 * kTabStride];
   for (int i = threadIdx.x; i < 16 * kTabStride; i += kRowThreads) tab[i] = pg.tab[i];
   __syncthreads();
@@ -248,10 +224,10 @@ __global__ void __launch_bounds__(kRowThreads, 3) fold_rows_kernel(const __grid_
       const uint32_t type = sv[0];
       uint4 e0 = make_uint4(0, 0, 0, 0);
       if (type < 16u) e0 = *reinterpret_cast<const uint4*>(tab + type * kTabStride);
-      if (!(e0.x & 1u)) {
+      if (!(e0.x & kRuleValid)) {
         t.m = M_ERR;  // THROW rule or scala.MatchError: replayed exactly by the sequential kernel
       } else {
-        ex = (e0.x & 2u) ? EX_NONE : EX_SOME;
+        ex = rule_ex(e0.x);
         uint32_t spec[W];
         spec[0] = e0.y;
         if (W > 1) spec[1] = e0.z;
@@ -262,9 +238,9 @@ __global__ void __launch_bounds__(kRowThreads, 3) fold_rows_kernel(const __grid_
         for (int w = 0; w < W; ++w) {
           uint32_t val = 0;
 #pragma unroll
-          for (int s = 1; s < NS; ++s) val = ((int)(spec[w] >> 3) == s) ? sv[s] : val;
-          if (spec[w] & 4u) val = 0u - val;
-          const uint32_t mode = spec[w] & 3u;
+          for (int s = 1; s < NS; ++s) val = ((int)spec_slot(spec[w]) == s) ? sv[s] : val;
+          if (spec_neg(spec[w])) val = 0u - val;
+          const uint32_t mode = spec_mode(spec[w]);
           t.v[w] = mode ? val : 0u;
           t.m |= mode << (2 * w);
         }
@@ -367,7 +343,7 @@ __global__ void __launch_bounds__(kRowThreads, 3) fold_rows_kernel(const __grid_
       for (int w = 0; w < W; ++w) part_data[1 + w] = carry.v[w];
       part_data[W + 1] = carry_ex | (span_has_head ? 4u : 0u);
       __threadfence();
-      asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(a.part_flags + gw), "r"(a.epoch) : "memory");
+      st_volatile_u32(a.part_flags + gw, a.epoch);
     }
     if (inh_pending && lane == 0) {
       // decoupled look-back: compose predecessors' open transformers until one that contains a head
@@ -453,7 +429,7 @@ bool build_row_program(const DevProgram& dp, RowProgram* out) {
     if (r.exists_rule == SGR_THROW) { e[0] = 0; continue; }
     uint32_t mode[kMaxRowWords] = {0}, slot[kMaxRowWords] = {0}, neg[kMaxRowWords] = {0};
     const bool reset = r.exists_rule == SGR_CREATE || r.exists_rule == SGR_TOMBSTONE;
-    if (reset) for (uint32_t w = 0; w < dp.user_words; ++w) mode[w] = 2;  // SET 0
+    if (reset) for (uint32_t w = 0; w < dp.user_words; ++w) mode[w] = kModeSet;  // SET 0
     for (uint32_t i = 0; i < r.n_ops; ++i) {
       const uint32_t op = r.ops[i];
       const uint32_t opcode = op & 15u, nwords = (op >> 4) & 63u, dw = (op >> 10) & 63u, sw = op >> 16;
@@ -472,15 +448,29 @@ bool build_row_program(const DevProgram& dp, RowProgram* out) {
         }
         slot[w] = s;
         neg[w] = opcode == SGR_OP_SUB_I32;
-        mode[w] = (opcode == SGR_OP_SET || reset) ? 2u : 1u;  // over a reset state ADD v == SET v and SUB v == SET -v
+        mode[w] = (opcode == SGR_OP_SET || reset) ? kModeSet : kModeAdd;  // over a reset state ADD v == SET v and SUB v == SET -v
       }
     }
-    // 8u: the rule builds a new state instance (Scala constructor or copy): CREATE, or any field op
-    e[0] = 1u | (r.exists_rule == SGR_TOMBSTONE ? 2u : 0u) | (r.exists_rule == SGR_IF_EXISTS ? 4u : 0u) |
-           ((r.exists_rule == SGR_CREATE || r.n_ops > 0) ? 8u : 0u);
-    for (uint32_t w = 0; w < dp.user_words; ++w) e[1 + w] = mode[w] | (neg[w] << 2) | (slot[w] << 3);
+    e[0] = kRuleValid | (r.exists_rule == SGR_TOMBSTONE ? kRuleNone : 0u) | (r.exists_rule == SGR_IF_EXISTS ? kRuleIfExists : 0u) |
+           ((r.exists_rule == SGR_CREATE || r.n_ops > 0) ? kRuleNew : 0u);
+    for (uint32_t w = 0; w < dp.user_words; ++w) e[1 + w] = spec_encode(mode[w], neg[w], slot[w]);
   }
   return true;
+}
+
+WordModes word_modes(const RowProgram& prog) {
+  WordModes m{0u, 0u, false};
+  for (int t = 0; t < 16; ++t) {
+    const uint32_t fl = prog.tab[t * kTabStride];
+    if (!(fl & kRuleValid)) continue;
+    if (fl & kRuleNone) m.none = true;
+    for (int w = 0; w < 2; ++w) {
+      const uint32_t mode = spec_mode(prog.tab[t * kTabStride + 1 + w]);
+      if (mode == kModeAdd) m.add |= 1u << w;
+      if (mode == kModeSet) m.set |= 1u << w;
+    }
+  }
+  return m;
 }
 
 namespace {

@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <string.h>
 
+#include "../../include/sgr.h"
 #include "sgr_device.cuh"
 
 namespace sgr {
@@ -12,6 +13,28 @@ constexpr int kRowThreads = 256;
 constexpr int kMaxSlots = 16;   // distinct record words a program may read (slot 0 = event type)
 constexpr int kMaxRowWords = 14;  // widest state in transformer form: 64-byte struct
 constexpr int kTabStride = 16;   // words per type in RowProgram::tab
+
+// ---- RowProgram::tab, the only place that knows its encoding. Per type, word 0 holds the rule flags:
+constexpr uint32_t kRuleValid = 1u;     // the rule does not throw (THROW rules and unknown types read as 0)
+constexpr uint32_t kRuleNone = 2u;      // the result is None (TOMBSTONE)
+constexpr uint32_t kRuleIfExists = 4u;  // IF_EXISTS: the ops apply only to an existing state
+constexpr uint32_t kRuleNew = 8u;       // the rule builds a new state instance (Scala constructor or copy): CREATE, or any field op
+// and word 1+w the spec of state word w: mode | neg << 2 | slot << 3 (mode 0 keeps the word; slot 0 reads no record word)
+constexpr uint32_t kModeAdd = 1u, kModeSet = 2u;
+
+__host__ __device__ __forceinline__ uint32_t spec_encode(uint32_t mode, uint32_t neg, uint32_t slot) { return mode | (neg << 2) | (slot << 3); }
+__host__ __device__ __forceinline__ uint32_t spec_mode(uint32_t spec) { return spec & 3u; }
+__host__ __device__ __forceinline__ uint32_t spec_slot(uint32_t spec) { return spec >> 3; }
+// the op subtracts: the word takes -v from the record word v
+__host__ __device__ __forceinline__ bool spec_neg(uint32_t spec) { return (spec & 4u) != 0u; }
+
+// ---- transformer form shared by the fold kernels: mode word bits and the exists-op of an event
+constexpr uint32_t M_ERR = 0x80000000u;   // some event in the range threw
+constexpr uint32_t M_COPY = 0x40000000u;  // some applied event built a new state instance (fold_runs.cu finish_segment)
+static_assert((kRuleNew << 27) == M_COPY, "rule_copy_bit moves the new-instance flag onto M_COPY");
+__host__ __device__ __forceinline__ uint32_t rule_copy_bit(uint32_t flags) { return (flags & kRuleNew) << 27; }
+constexpr uint32_t EX_SOME = 1u, EX_NONE = 2u;
+__host__ __device__ __forceinline__ uint32_t rule_ex(uint32_t flags) { return (flags & kRuleNone) ? EX_NONE : EX_SOME; }
 
 // Program in transformer form: per event type, how each state word is produced.
 // Two closed classes of programs (build_row_program decides):
@@ -26,7 +49,7 @@ struct RowProgram {
   uint32_t cls;                   // 0 / 1, see above
   uint32_t f64_mask;              // bit w: state words w, w+1 form a JVM Double (numeric == for the publish rule)
   uint32_t slot_word[kMaxSlots];  // record word index of each slot
-  uint32_t tab[16 * kTabStride];  // per type: [0] bit0 valid, bit1 result is None, bit2 IF_EXISTS rule; [1+w] mode | neg<<2 | slot<<3
+  uint32_t tab[16 * kTabStride];  // per type: [0] kRule* flags, [1+w] spec of state word w (see above)
 };
 
 struct RowArgs {
@@ -54,6 +77,37 @@ struct RowArgs {
 // false if the program is outside the transformer algebra (IF_EXISTS rules, 64-bit adds, f64 fields,
 // unsupported state width): the caller then uses the lane-sequential kernel.
 bool build_row_program(const DevProgram& dp, RowProgram* out);
+// over the valid types: which of state words 0, 1 some type ADDs to (bit w of add) or SETs (set), and whether one makes None
+struct WordModes {
+  uint32_t add, set;
+  bool none;
+};
+WordModes word_modes(const RowProgram& prog);
+
+// The publish rule for an integer row of W state words, then the row itself (W + 2 words, 16-byte aligned): the words
+// (zeroed when the result is None), exn | CHANGED, a zero err word. CHANGED when existence flips, or when the state
+// exists before and after and a word differs. old/ex0: the prior state (words zero when it was None); nw/exn the new one.
+template <int W>
+__device__ __forceinline__ void finish_row(uint8_t* row, const uint32_t (&old)[W], uint32_t ex0, const uint32_t (&nw)[W], uint32_t exn) {
+  uint32_t outw[W + 2], changed = exn != ex0;
+#pragma unroll
+  for (int w = 0; w < W; ++w) {
+    outw[w] = exn ? nw[w] : 0u;
+    if (exn && ex0) changed |= (outw[w] != old[w]);
+  }
+  outw[W] = exn | (changed ? SGR_ST_CHANGED : 0u);
+  outw[W + 1] = 0u;
+  uint4* dp = reinterpret_cast<uint4*>(row);
+#pragma unroll
+  for (int q = 0; q < (W + 2) / 4; ++q) dp[q] = make_uint4(outw[4 * q], outw[4 * q + 1], outw[4 * q + 2], outw[4 * q + 3]);
+}
+// the same for a 16-byte row, against the row as it was read (old.x, old.y are compared only when ex0 is set)
+__device__ __forceinline__ void finish_row16(uint4* row, const uint4& old, uint32_t ex0, uint32_t n0, uint32_t n1, uint32_t exn) {
+  if (!exn) { n0 = 0; n1 = 0; }
+  uint32_t changed = exn != ex0;
+  if (exn && ex0) changed |= (n0 != old.x) | (n1 != old.y);
+  *row = make_uint4(n0, n1, exn | (changed ? SGR_ST_CHANGED : 0u), 0u);
+}
 // one pass over the CSR offsets at load time: are all segments 64-byte aligned relative to the first, and
 // where does the log begin/end (device offsets are opaque to the host otherwise)
 cudaError_t inspect_offsets(const uint64_t* d_off, uint64_t n_seg, unsigned long long* d_scratch, cudaStream_t st,

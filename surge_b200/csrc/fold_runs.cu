@@ -45,9 +45,6 @@
 namespace sgr {
 namespace {
 
-constexpr uint32_t M_ERR = 0x80000000u;  // some event in the range threw
-constexpr uint32_t M_COPY = 0x40000000u; // some applied event built a new state instance (tab flag 8u << 27), see finish_segment
-constexpr uint32_t EX_SOME = 1u, EX_NONE = 2u;
 constexpr int kRunThreads = 128;
 constexpr int kRunWarps = kRunThreads / 32;
 
@@ -91,22 +88,6 @@ __device__ __forceinline__ Xf<W> shfl_xf(const Xf<W>& t, int src) {
   return r;
 }
 
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ unsigned long long ld_volatile_u64(const unsigned long long* p) {
-  unsigned long long v;
-  asm volatile("ld.volatile.global.u64 %0, [%1];" : "=l"(v) : "l"(p));
-  return v;
-}
-__device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) {
-  uint32_t v;
-  asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p));
-  return v;
-}
 // programmatic dependent launch: no-ops when the grid was launched without the attribute
 __device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -460,12 +441,12 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
           const uint32_t type = sv[0];
           uint4 e0 = make_uint4(0, 0, 0, 0);
           if (type < 16u) e0 = *reinterpret_cast<const uint4*>(tab + type * kTabStride);
-          if (!(e0.x & 1u)) {
+          if (!(e0.x & kRuleValid)) {
             cur.m |= M_ERR;  // THROW rule or scala.MatchError
-          } else if (CLS == 1 && (e0.x & 4u) && cur.ex == EX_NONE) {
+          } else if (CLS == 1 && (e0.x & kRuleIfExists) && cur.ex == EX_NONE) {
             // IF_EXISTS event after a tombstone in this run: the state does not exist, the event is a no-op
           } else {
-            if (CLS == 0 || !(e0.x & 4u)) cur.ex = (e0.x & 2u) ? EX_NONE : EX_SOME;  // an IF_EXISTS event leaves the exists-op as it is
+            if (CLS == 0 || !(e0.x & kRuleIfExists)) cur.ex = rule_ex(e0.x);  // an IF_EXISTS event leaves the exists-op as it is
             uint32_t spec[W];
             spec[0] = e0.y;
             if (W > 1) spec[1] = e0.z;
@@ -476,19 +457,19 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
             for (int w = 0; w < W; ++w) {
               uint32_t val = 0;
               if (DIRECT) {
-                const uint32_t sl = spec[w] >> 3;
+                const uint32_t sl = spec_slot(spec[w]);
                 if (sl) { const uint32_t sw = pg.slot_word[sl]; val = lds32(rec + ((((par4 + (sw >> 2)) ^ lane7) << 4) | ((sw & 3u) << 2))); }
               } else {
 #pragma unroll
-                for (int s = 1; s < NS; ++s) val = ((spec[w] >> 3) == (uint32_t)s) ? sv[s] : val;
+                for (int s = 1; s < NS; ++s) val = (spec_slot(spec[w]) == (uint32_t)s) ? sv[s] : val;
               }
-              if (spec[w] & 4u) val = 0u - val;
-              const uint32_t mode = spec[w] & 3u;
-              if (mode == 2u) cur.v[w] = val;
-              else if (mode == 1u) cur.v[w] += val;
+              if (spec_neg(spec[w])) val = 0u - val;
+              const uint32_t mode = spec_mode(spec[w]);
+              if (mode == kModeSet) cur.v[w] = val;
+              else if (mode == kModeAdd) cur.v[w] += val;
               cur.m |= mode << (2 * w);
             }
-            cur.m |= (e0.x & 8u) << 27;   // M_COPY: this rule builds a new instance (CREATE, or any field op)
+            cur.m |= rule_copy_bit(e0.x);
           }
         }
       }
@@ -553,7 +534,7 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
         for (int w = 0; w < W; ++w) part_data[1 + w] = carry.v[w];
         part_data[W + 1] = carry.ex | (span_has_head ? 4u : 0u);
         __threadfence();
-        asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(a.part_flags + chunk), "r"(a.epoch) : "memory");
+        st_volatile_u32(a.part_flags + chunk, a.epoch);
       }
       if (lane == 0) {
         // the previous chunk's look-back, left until now: its predecessors were folded while this chunk was
@@ -639,22 +620,23 @@ __device__ __noinline__ void replay_segments(const RowArgs& a, const RowProgram&
       const uint32_t* rec = reinterpret_cast<const uint32_t*>(a.events + pos);
       const uint32_t type = rec[pg.slot_word[0]];
       const uint32_t fl = type < 16u ? tab[type * kTabStride] : 0u;
-      if (!(fl & 1u)) { threw = true; break; }
-      if (fl & 2u) { exn = 0u; for (int w = 0; w < W; ++w) st[w] = 0u; continue; }  // tombstone
-      if ((fl & 4u) && !exn) continue;                                                // IF_EXISTS on None: no-op
+      if (!(fl & kRuleValid)) { threw = true; break; }
+      if (fl & kRuleNone) { exn = 0u; for (int w = 0; w < W; ++w) st[w] = 0u; continue; }  // tombstone
+      if ((fl & kRuleIfExists) && !exn) continue;                                          // IF_EXISTS on None: no-op
 #pragma unroll
       for (int w = 0; w < W; ++w) {
         const uint32_t spec = tab[type * kTabStride + 1 + w];
-        const uint32_t mode = spec & 3u;
-        uint32_t val = (spec >> 3) ? rec[pg.slot_word[spec >> 3]] : 0u;
-        if (spec & 4u) val = 0u - val;
-        if (mode == 2u) st[w] = val; else if (mode == 1u) st[w] = (exn ? st[w] : 0u) + val;
+        const uint32_t mode = spec_mode(spec);
+        uint32_t val = spec_slot(spec) ? rec[pg.slot_word[spec_slot(spec)]] : 0u;
+        if (spec_neg(spec)) val = 0u - val;
+        if (mode == kModeSet) st[w] = val; else if (mode == kModeAdd) st[w] = (exn ? st[w] : 0u) + val;
         else if (!exn) st[w] = 0u;
       }
       exn = SGR_ST_EXISTS;
     }
-    uint32_t* dp = reinterpret_cast<uint32_t*>(a.states_out + slot * (uint64_t)(W + 2) * 4);
+    uint8_t* row = a.states_out + slot * (uint64_t)(W + 2) * 4;
     if (threw) {
+      uint32_t* dp = reinterpret_cast<uint32_t*>(row);
 #pragma unroll
       for (int w = 0; w < W; ++w) dp[w] = old[w];
       dp[W] = ex0 | SGR_ST_ERROR;
@@ -662,11 +644,7 @@ __device__ __noinline__ void replay_segments(const RowArgs& a, const RowProgram&
       ++n_err;
       n_dropped += ((e - b) >> 6) - k;
     } else {
-      uint32_t changed = exn != ex0;
-#pragma unroll
-      for (int w = 0; w < W; ++w) { if (!exn) st[w] = 0u; if (exn && ex0) changed |= st[w] != old[w]; dp[w] = st[w]; }  // (a replayed segment that did not throw cannot occur)
-      dp[W] = exn | (changed ? SGR_ST_CHANGED : 0u);
-      dp[W + 1] = 0u;
+      finish_row<W>(row, old, ex0, st, exn);  // (a replayed segment that did not throw cannot occur)
     }
   }
   for (int o = 16; o > 0; o >>= 1) {

@@ -25,8 +25,6 @@
 namespace sgr {
 namespace {
 
-constexpr uint32_t M_ERR = 0x80000000u;
-constexpr uint32_t EX_SOME = 1u, EX_NONE = 2u;
 constexpr int W = 2;
 
 struct Xv {
@@ -47,13 +45,6 @@ __device__ __forceinline__ Xv xv_shfl(const Xv& t, int src) {
   r.v[0] = __shfl_sync(0xffffffffu, t.v[0], src); r.v[1] = __shfl_sync(0xffffffffu, t.v[1], src);
   return r;
 }
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ uint32_t ldv32(const uint32_t* p) { uint32_t v; asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p)); return v; }
 
 // full rebuild only: prior state is None (the table is zeroed before the launch, empty aggregates stay None)
 __device__ __forceinline__ void finish_var(const VarArgs& a, uint32_t seg, const Xv& ts) {
@@ -65,9 +56,8 @@ __device__ __forceinline__ void finish_var(const VarArgs& a, uint32_t seg, const
   }
   if (!ts.ex) return;
   const uint32_t exn = (ts.ex == EX_NONE) ? 0u : SGR_ST_EXISTS;
-  uint32_t n0 = ts.v[0], n1 = ts.v[1];  // old state is zero: SET v -> v, ADD v -> 0 + v
-  if (!exn) { n0 = 0; n1 = 0; }
-  *reinterpret_cast<uint4*>(a.states_out + (uint64_t)seg * 16) = make_uint4(n0, n1, exn | (exn ? SGR_ST_CHANGED : 0u), 0u);
+  // old state is zero: SET v -> v, ADD v -> 0 + v
+  finish_row16(reinterpret_cast<uint4*>(a.states_out + (uint64_t)seg * 16), make_uint4(0, 0, 0, 0), 0u, ts.v[0], ts.v[1], exn);
 }
 
 template <int NSTAGE>
@@ -152,24 +142,24 @@ __global__ void __launch_bounds__(512) fold_vruns_kernel(const __grid_constant__
       ok = ok && hdr.z <= 0x10000u && ((rec_bytes + 15u) & ~15u) == len;          // directory and header agree on the length
       uint32_t fl = 0;
       if (ok && hdr.x < 16u) fl = tab[hdr.x * kTabStride];
-      if (!(fl & 1u)) ok = false;
+      if (!(fl & kRuleValid)) ok = false;
       if (ok) {
         uint32_t mode[W], val[W];
 #pragma unroll
         for (int w = 0; w < W; ++w) {
           const uint32_t spec = tab[hdr.x * kTabStride + 1 + w];
-          mode[w] = spec & 3u;
+          mode[w] = spec_mode(spec);
           uint32_t v = 0;
-          if (spec >> 3) {
-            const uint32_t wo = pg.slot_word[spec >> 3] * 4;
+          if (spec_slot(spec)) {
+            const uint32_t wo = pg.slot_word[spec_slot(spec)] * 4;
             if (wo + 4 > rec_bytes) ok = false;                                          // the event class needs a word the record does not have
             else v = in_stage ? lds32(base + wo) : *reinterpret_cast<const uint32_t*>(grec + wo);
           }
-          if (spec & 4u) v = 0u - v;
+          if (spec_neg(spec)) v = 0u - v;
           val[w] = mode[w] ? v : 0u;
         }
         if (ok) {
-          t.ex = (fl & 2u) ? EX_NONE : EX_SOME;
+          t.ex = rule_ex(fl);
           t.m = mode[0] | (mode[1] << 2);
           t.v[0] = val[0]; t.v[1] = val[1];
         }
@@ -234,20 +224,20 @@ __global__ void __launch_bounds__(512) fold_vruns_kernel(const __grid_constant__
     if (lane == 0) {
       pd[0] = carry.m; pd[1] = carry.v[0]; pd[2] = carry.v[1]; pd[3] = carry.ex | (span_has_head ? 4u : 0u); pd[4] = carry.cnt;
       __threadfence();
-      asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(a.part_flags + gw), "r"(a.epoch) : "memory");
+      st_volatile_u32(a.part_flags + gw, a.epoch);
     }
     if (lane == 0 && (inh_pending || end_needs_lookback)) {
       Xv pre = xv_identity();
       uint64_t p = gw;
       while (p > 0) {
         --p;
-        while (ldv32(a.part_flags + p) != a.epoch) { __nanosleep(64); }
+        while (ld_volatile_u32(a.part_flags + p) != a.epoch) { __nanosleep(64); }
         __threadfence();
         const uint32_t* q = a.part_data + p * 8;
         Xv e;
-        e.m = ldv32(q); e.v[0] = ldv32(q + 1); e.v[1] = ldv32(q + 2);
-        const uint32_t tw = ldv32(q + 3);
-        e.ex = tw & 3u; e.cnt = ldv32(q + 4);
+        e.m = ld_volatile_u32(q); e.v[0] = ld_volatile_u32(q + 1); e.v[1] = ld_volatile_u32(q + 2);
+        const uint32_t tw = ld_volatile_u32(q + 3);
+        e.ex = tw & 3u; e.cnt = ld_volatile_u32(q + 4);
         pre = xv_compose(e, pre);
         if (tw & 4u) break;
       }

@@ -120,6 +120,29 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
   asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
   return v;
 }
+
+// ---------------------------------------------------------------- PTX wrappers: cp.async staging, volatile flags
+// 16 bytes global -> shared (dst a shared-window address), L1 bypassed; completion by commit / wait groups
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+// look-back flags and counters another CTA publishes while this one spins
+__device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ unsigned long long ld_volatile_u64(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("ld.volatile.global.u64 %0, [%1];" : "=l"(v) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ void st_volatile_u32(uint32_t* p, uint32_t v) {
+  asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
 #endif  // __CUDACC__
 
 }  // namespace sgr
