@@ -117,7 +117,7 @@ struct sgr_dingest {
   KeepBuf arena, d_batches;
   KeepBuf rec_off, rec_batch, out;          // per record slot; they keep their content when a later group needs them larger
   KeepBuf st_idx, st_present;               // ... state mode: the slot's dense index (~0u: hole) and 0 / 1 (tombstone / row)
-  DevBuf key_offs_dev, key_bytes_dev;
+  DevBuf key_offs_dev, key_bytes_dev, key_scan_tmp;
   // chains of launches per group of batches
   uint64_t launched_batches = 0;            // batches of this poll whose chain has been launched
   uint32_t group_batches = 8192;            // SGR_DINGEST_GROUP
@@ -353,7 +353,7 @@ int32_t sgr_dingest_destroy(sgr_dingest* g) {
   g->batches.release();
   g->wire.b.release(); g->d_batches.b.release(); g->arena.b.release(); g->rec_off.b.release(); g->rec_batch.b.release(); g->out.b.release();
   g->st_idx.b.release(); g->st_present.b.release();
-  g->key_offs_dev.release(); g->key_bytes_dev.release(); g->json_table.release();
+  g->key_offs_dev.release(); g->key_bytes_dev.release(); g->key_scan_tmp.release(); g->json_table.release();
   g->tags.release(); g->slot_idx.release(); g->key_ref.release(); g->id_arena.release(); g->ctl.release();
   if (g->h_ctl) cudaFreeHost(g->h_ctl);
   delete g;
@@ -646,11 +646,10 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
     if (n_keys > g->keys_on_host) {
       const uint64_t add = n_keys - g->keys_on_host;
       const uint64_t id_bytes_max = id_bytes - g->id_bytes_on_host;   // (an upper bound: arena entries are padded to 8 bytes)
-      DG_TRY(g, g->key_offs_dev.reserve((add + 2) * 4 + (2 * (add / 4096 + 2) + 4 * 4096) * 4));
+      DG_TRY(g, g->key_offs_dev.reserve((add + 2) * 4));
       DG_TRY(g, g->key_bytes_dev.reserve(id_bytes_max + 64));
       uint32_t* d_offs = (uint32_t*)g->key_offs_dev.p;
-      uint32_t* d_tmp = d_offs + add + 2;
-      DG_TRY(g, dg_gather_keys(p.dict, g->keys_on_host, (uint32_t)add, d_offs, (uint8_t*)g->key_bytes_dev.p, d_tmp, g->stream));
+      DG_TRY(g, dg_gather_keys(p.dict, g->keys_on_host, (uint32_t)add, d_offs, (uint8_t*)g->key_bytes_dev.p, g->key_scan_tmp, g->stream));
       if (g->h_keys_cap < (add + 2) * 4 + id_bytes_max + 64) {
         if (g->h_keys) cudaFreeHost(g->h_keys);
         g->h_keys = nullptr; g->h_keys_cap = 0;

@@ -28,6 +28,7 @@
 // per lz4 sequence, where bytes walked straight from global memory cost ~10, and in a warp of 32 independent batches some lane
 // misses at every step.
 #include "dingest_kernels.cuh"
+#include "group_kernels.cuh"
 #include "lz4_fast.h"
 
 namespace sgr {
@@ -451,14 +452,12 @@ cudaError_t dg_launch_decode_walk_fast(const uint8_t* wire, uint8_t* arena, DgBa
   return cudaGetLastError();
 }
 
-cudaError_t exclusive_scan_u32_public(const uint32_t* in, uint32_t* out, uint32_t n, uint32_t* tmp, cudaStream_t st);
-
 // ids [from, from + n) of the dictionary as contiguous bytes in dense-index order: d_offs[n + 1] (exclusive prefix of the lengths),
-// d_bytes. d_tmp: scratch of at least 2 * (n / 4096 + 2) + 4 * 4096 u32.
-cudaError_t dg_gather_keys(const DgDict& d, uint64_t from, uint32_t n, uint32_t* d_offs, uint8_t* d_bytes, uint32_t* d_tmp, cudaStream_t st) {
+// d_bytes. scan_tmp: the scan's temp storage.
+cudaError_t dg_gather_keys(const DgDict& d, uint64_t from, uint32_t n, uint32_t* d_offs, uint8_t* d_bytes, DevBuf& scan_tmp, cudaStream_t st) {
   if (!n) return cudaSuccess;
   dg_key_lens_kernel<<<(n + 1 + 255) / 256, 256, 0, st>>>(d.key_ref, from, n, d_offs);
-  cudaError_t e = exclusive_scan_u32_public(d_offs, d_offs, n + 1, d_tmp, st);
+  cudaError_t e = exclusive_sum_u32(d_offs, d_offs, n + 1, scan_tmp, st);
   if (e != cudaSuccess) return e;
   dg_key_copy_kernel<<<(uint32_t)(((uint64_t)n * 8 + 255) / 256), 256, 0, st>>>(d.key_ref, d.arena, from, n, d_offs, d_bytes);
   return cudaGetLastError();

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "devbuf.h"
 #include "id_dict.cuh"
 #include "value_framing.h"
 
@@ -73,6 +74,6 @@ cudaError_t dg_launch_crc_size_fast(const uint8_t* wire, DgBatch* batches, uint3
 // arena_ctl as given to dg_launch_crc_size_fast for the same batches (nullptr: dsize is exact, not a slot capacity)
 cudaError_t dg_launch_decode_walk_fast(const uint8_t* wire, uint8_t* arena, DgBatch* batches, uint32_t n, uint32_t index_base, uint32_t* rec_off, uint32_t* rec_batch,
                                        unsigned long long* arena_ctl, cudaStream_t st);
-cudaError_t dg_gather_keys(const DgDict& d, uint64_t from, uint32_t n, uint32_t* d_offs, uint8_t* d_bytes, uint32_t* d_tmp, cudaStream_t st);
+cudaError_t dg_gather_keys(const DgDict& d, uint64_t from, uint32_t n, uint32_t* d_offs, uint8_t* d_bytes, DevBuf& scan_tmp, cudaStream_t st);
 
 }  // namespace sgr

@@ -3,33 +3,30 @@
 // A Kafka partition log interleaves aggregates; the fold wants each aggregate's events
 // contiguous and in log order. The reference gets that from the broker + KTable keyed store
 // (modules/common/src/main/scala/surge/kafka/streams/SurgeStateStoreConsumer.scala:57-76);
-// here it is a stable LSD radix sort of (aggregate index, arrival index) pairs — 8 bytes per
+// here it is a stable radix sort of (aggregate index, arrival index) pairs — 8 bytes per
 // record instead of 64 — followed by ONE gather of the 64-byte records into CSR order:
-//   extract keys -> [hist -> scan -> stable scatter] x ceil(bits/8) -> offsets -> gather
-// Stability of every pass keeps per-aggregate arrival order, which is the only order the
+//   extract keys -> cub::DeviceRadixSort::SortPairs over bits [0, bits) -> offsets -> gather
+// The sort's stability keeps per-aggregate arrival order, which is the only order the
 // fold depends on. All kernels are plain HBM-bound integer kernels (no tensor cores).
 #include "group_kernels.cuh"
 
 #include <stdio.h>
+
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 #include "../../include/sgr.h"
 
 namespace sgr {
 namespace {
 
-constexpr int kThreads = 256;
-constexpr int kItems = 16;
-constexpr int kTile = kThreads * kItems;  // 4096 keys per block
-constexpr int kWarps = kThreads / 32;
-constexpr int kPerWarp = kTile / kWarps;  // 512 keys per warp
-constexpr int kRounds = kPerWarp / 32;    // 16
-
 // ---------------------------------------------------------------- keys
 // kHoles: a hole (agg == ~0, a record the device decode dropped) gets the key n_agg, one past the table, so that every hole
 // sorts behind every live record; holes are counted in bad[2] (one atomic per warp), apart from the bad records in bad[0].
+// idx[i] = i: the sort's values are the arrival indices.
 template <bool kHoles>
 __global__ void extract_keys_kernel(const uint8_t* __restrict__ rec, uint32_t n, uint64_t n_agg,
-                                    uint32_t* __restrict__ keys, unsigned long long* __restrict__ bad) {
+                                    uint32_t* __restrict__ keys, uint32_t* __restrict__ idx, unsigned long long* __restrict__ bad) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   unsigned long long agg = *reinterpret_cast<const unsigned long long*>(rec + (size_t)i * 64 + 8);
@@ -46,162 +43,7 @@ __global__ void extract_keys_kernel(const uint8_t* __restrict__ rec, uint32_t n,
     atomicAdd(bad, 1ull);
   }
   keys[i] = (uint32_t)agg;
-}
-
-// ---------------------------------------------------------------- exclusive scan (u32), three-kernel, recursive on block sums
-__device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t* total, uint32_t* smem /*[kWarps]*/) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint32_t x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) smem[warp] = x;
-  __syncthreads();
-  uint32_t base = 0, tot = 0;
-#pragma unroll
-  for (int w = 0; w < kWarps; ++w) {
-    const uint32_t s = smem[w];
-    if (w < warp) base += s;
-    tot += s;
-  }
-  __syncthreads();
-  *total = tot;
-  return base + x - v;
-}
-
-__global__ void __launch_bounds__(kThreads) scan_reduce_kernel(const uint32_t* __restrict__ in, uint32_t n, uint32_t* __restrict__ sums) {
-  __shared__ uint32_t sm[kWarps];
-  const uint32_t base = blockIdx.x * kTile + threadIdx.x * kItems;
-  uint32_t s = 0;
-#pragma unroll
-  for (int j = 0; j < kItems; ++j) s += (base + j < n) ? in[base + j] : 0u;
-  uint32_t total;
-  block_exclusive_scan(s, &total, sm);
-  if (threadIdx.x == 0) sums[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(kThreads) scan_down_kernel(const uint32_t* __restrict__ in, uint32_t n, const uint32_t* __restrict__ sums_ex,
-                                                             uint32_t* __restrict__ out) {
-  __shared__ uint32_t sm[kWarps];
-  const uint32_t base = blockIdx.x * kTile + threadIdx.x * kItems;
-  uint32_t v[kItems];
-  uint32_t s = 0;
-#pragma unroll
-  for (int j = 0; j < kItems; ++j) { v[j] = (base + j < n) ? in[base + j] : 0u; s += v[j]; }
-  uint32_t total;
-  uint32_t run = block_exclusive_scan(s, &total, sm) + (sums_ex ? sums_ex[blockIdx.x] : 0u);
-#pragma unroll
-  for (int j = 0; j < kItems; ++j) { if (base + j < n) out[base + j] = run; run += v[j]; }
-}
-
-// exclusive scan of in[0..n) into out (may alias in). tmp must hold >= 2*ceil(n/kTile)+ 2*kTile u32.
-cudaError_t exclusive_scan_u32(const uint32_t* in, uint32_t* out, uint32_t n, uint32_t* tmp, cudaStream_t st) {
-  if (n == 0) return cudaSuccess;
-  const uint32_t nb = (n + kTile - 1) / kTile;
-  if (nb == 1) {
-    scan_down_kernel<<<1, kThreads, 0, st>>>(in, n, nullptr, out);
-    return cudaGetLastError();
-  }
-  scan_reduce_kernel<<<nb, kThreads, 0, st>>>(in, n, tmp);
-  cudaError_t e = exclusive_scan_u32(tmp, tmp, nb, tmp + nb, st);
-  if (e != cudaSuccess) return e;
-  scan_down_kernel<<<nb, kThreads, 0, st>>>(in, n, tmp, out);
-  return cudaGetLastError();
-}
-
-// lanes holding the same 8-bit digit; invalid lanes match nobody. (One MATCH.ANY in place of eight ballots, one per bit.)
-__device__ __forceinline__ uint32_t match_digit(uint32_t d, bool valid) {
-  const uint32_t m = __match_any_sync(0xffffffffu, valid ? d : (256u + (threadIdx.x & 31)));
-  return valid ? m : 0u;
-}
-
-// ---------------------------------------------------------------- radix pass
-// Per-block digit histogram: hist[digit * nblocks + block]
-__global__ void __launch_bounds__(kThreads) radix_hist_kernel(const uint32_t* __restrict__ keys, uint32_t n, int shift,
-                                                              uint32_t* __restrict__ hist, uint32_t nblocks) {
-  __shared__ uint32_t h[256];
-  h[threadIdx.x] = 0;
-  __syncthreads();
-  const uint32_t base = blockIdx.x * kTile;
-#pragma unroll
-  for (int j = 0; j < kItems; ++j) {
-    const uint32_t i = base + j * kThreads + threadIdx.x;
-    if (i < n) atomicAdd(&h[(keys[i] >> shift) & 255u], 1u);
-  }
-  __syncthreads();
-  hist[threadIdx.x * nblocks + blockIdx.x] = h[threadIdx.x];
-}
-
-// Stable scatter. Warp w of the block owns keys [w*512, (w+1)*512) of the tile, in 16 rounds of 32.
-// A key's place inside the tile's digit-sorted order = (keys of smaller digits in the tile) + keys with the same
-// digit in earlier warps + in this warp's earlier rounds + in lower lanes of this round. The (key, index) pairs are
-// first reordered in shared memory and then written out in that order, so every digit's run of the tile goes to
-// consecutive global addresses (coalesced) instead of 32 scattered 4-byte stores per warp instruction.
-__global__ void __launch_bounds__(kThreads) radix_scatter_kernel(const uint32_t* __restrict__ keys_in, const uint32_t* __restrict__ idx_in,
-                                                                 uint32_t* __restrict__ keys_out, uint32_t* __restrict__ idx_out, uint32_t n,
-                                                                 int shift, const uint32_t* __restrict__ base, uint32_t nblocks) {
-  __shared__ uint32_t wh[kWarps][256];
-  __shared__ uint32_t skey[kTile];
-  __shared__ uint32_t sidx[kTile];
-  __shared__ uint32_t gbase[256];
-  __shared__ uint32_t scan_sm[kWarps];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int i = threadIdx.x; i < kWarps * 256; i += kThreads) (&wh[0][0])[i] = 0;
-  __syncthreads();
-  const uint32_t tile0 = blockIdx.x * kTile;
-  const uint32_t start = tile0 + warp * kPerWarp;
-  uint32_t key[kRounds];
-  uint16_t pre[kRounds];   // keys with the same digit in this warp's earlier rounds + in lower lanes of this round
-  const uint32_t lt = (1u << lane) - 1u;
-  // phase 1: this warp's digit counts, and every key's rank among the warp's keys of its digit — ONE match per key: the second
-  // MATCH.ANY of the placement phase (r01: 32 per warp and tile, the kernel's main cost) is replaced by a register
-#pragma unroll
-  for (int r = 0; r < kRounds; ++r) {
-    const uint32_t i = start + r * 32 + lane;
-    const bool valid = i < n;
-    key[r] = valid ? keys_in[i] : 0u;
-    const uint32_t d = (key[r] >> shift) & 255u;
-    const uint32_t m = match_digit(d, valid);
-    const uint32_t earlier = valid ? wh[warp][d] : 0u;    // read by every lane of the digit before its leader adds this round
-    pre[r] = (uint16_t)(earlier + __popc(m & lt));
-    __syncwarp();
-    if (valid && (m & lt) == 0) wh[warp][d] = earlier + __popc(m);
-    __syncwarp();
-  }
-  __syncthreads();
-  // phase 2: per digit, exclusive prefix over warps; then exclusive scan over digits = start of the digit's run in the tile
-  {
-    const uint32_t d = threadIdx.x;
-    uint32_t off = 0;
-#pragma unroll
-    for (int w = 0; w < kWarps; ++w) { const uint32_t c = wh[w][d]; wh[w][d] = off; off += c; }
-    uint32_t total;
-    const uint32_t tile_start = block_exclusive_scan(off, &total, scan_sm);
-#pragma unroll
-    for (int w = 0; w < kWarps; ++w) wh[w][d] += tile_start;
-    gbase[d] = base[d * nblocks + blockIdx.x] - tile_start;  // global position = gbase[digit] + place in tile
-  }
-  __syncthreads();
-  // phase 3: place every pair at its digit-sorted position in shared memory
-#pragma unroll
-  for (int r = 0; r < kRounds; ++r) {
-    const uint32_t i = start + r * 32 + lane;
-    if (i < n) {
-      const uint32_t pos = wh[warp][(key[r] >> shift) & 255u] + pre[r];
-      skey[pos] = key[r]; sidx[pos] = idx_in ? idx_in[i] : i;
-    }
-  }
-  __syncthreads();
-  // phase 4: write the tile out in sorted order
-  const uint32_t tile_n = n - tile0 < (uint32_t)kTile ? n - tile0 : (uint32_t)kTile;
-  for (uint32_t j = threadIdx.x; j < tile_n; j += kThreads) {
-    const uint32_t k = skey[j];
-    const uint32_t pos = gbase[(k >> shift) & 255u] + j;
-    keys_out[pos] = k;
-    idx_out[pos] = sidx[j];
-  }
+  idx[i] = i;
 }
 
 // ---------------------------------------------------------------- CSR offsets from sorted keys
@@ -270,8 +112,12 @@ inline uint32_t cdiv(uint64_t a, uint32_t b) { return (uint32_t)((a + b - 1) / b
 
 }  // namespace
 
-cudaError_t exclusive_scan_u32_public(const uint32_t* in, uint32_t* out, uint32_t n, uint32_t* tmp, cudaStream_t st) {
-  return exclusive_scan_u32(in, out, n, tmp, st);
+cudaError_t exclusive_sum_u32(const uint32_t* in, uint32_t* out, uint32_t n, DevBuf& tmp, cudaStream_t st) {
+  if (n == 0) return cudaSuccess;
+  size_t bytes = 0;
+  cudaError_t e;
+  if ((e = cub::DeviceScan::ExclusiveSum(nullptr, bytes, in, out, n, st)) != cudaSuccess || (e = tmp.reserve(bytes)) != cudaSuccess) return e;
+  return cub::DeviceScan::ExclusiveSum(tmp.p, bytes, in, out, n, st);
 }
 
 void clear_batch_flags(uint8_t* d_states, uint32_t state_bytes, const uint32_t* d_ids, uint64_t n, cudaStream_t stream) {
@@ -295,49 +141,41 @@ cudaError_t group_by_agg_stable(GroupScratch& sc, const uint8_t* d_records, uint
     } else if ((e = cudaMemsetAsync(d_out_offsets, 0, 8, st)) != cudaSuccess) return e;
     return cudaStreamSynchronize(st);
   }
-  const uint32_t nblocks = cdiv(n, kTile);
   if ((e = sc.keys_a.reserve((size_t)n * 4)) != cudaSuccess || (e = sc.keys_b.reserve((size_t)n * 4)) != cudaSuccess ||
-      (e = sc.idx_a.reserve((size_t)n * 4)) != cudaSuccess || (e = sc.idx_b.reserve((size_t)n * 4)) != cudaSuccess ||
-      (e = sc.hist.reserve((size_t)256 * nblocks * 4)) != cudaSuccess ||
-      (e = sc.scan_tmp.reserve(((size_t)2 * cdiv((uint64_t)256 * nblocks > n ? (uint64_t)256 * nblocks : n, kTile) + 4 * kTile) * 4)) != cudaSuccess)
+      (e = sc.idx_a.reserve((size_t)n * 4)) != cudaSuccess || (e = sc.idx_b.reserve((size_t)n * 4)) != cudaSuccess)
     return e;
-  uint32_t *ka = (uint32_t*)sc.keys_a.p, *kb = (uint32_t*)sc.keys_b.p, *ia = (uint32_t*)sc.idx_a.p, *ib = (uint32_t*)sc.idx_b.p;
-  uint32_t* hist = (uint32_t*)sc.hist.p;
-  uint32_t* tmp = (uint32_t*)sc.scan_tmp.p;
-
-  if ((e = cudaMemsetAsync(d_counters, 0, 64, st)) != cudaSuccess) return e;
-  if (holes_out) extract_keys_kernel<true><<<cdiv(n, 256), 256, 0, st>>>(d_records, n, n_agg, ka, d_counters + 4);
-  else extract_keys_kernel<false><<<cdiv(n, 256), 256, 0, st>>>(d_records, n, n_agg, ka, d_counters + 4);
-
+  cub::DoubleBuffer<uint32_t> keys((uint32_t*)sc.keys_a.p, (uint32_t*)sc.keys_b.p), idx((uint32_t*)sc.idx_a.p, (uint32_t*)sc.idx_b.p);
   // the keys run up to n_agg - 1, or up to n_agg with holes
   const uint64_t key_end = holes_out ? n_agg + 1 : n_agg;
   int bits = 1;
   while (bits < 32 && (1ull << bits) < key_end) ++bits;
-  for (int shift = 0; shift < bits; shift += 8) {
-    radix_hist_kernel<<<nblocks, kThreads, 0, st>>>(ka, n, shift, hist, nblocks);
-    if ((e = exclusive_scan_u32(hist, hist, 256 * nblocks, tmp, st)) != cudaSuccess) return e;
-    // first pass: the arrival index is the position itself
-    radix_scatter_kernel<<<nblocks, kThreads, 0, st>>>(ka, shift == 0 ? nullptr : ia, kb, ib, n, shift, hist, nblocks);
-    uint32_t* t;
-    t = ka; ka = kb; kb = t;
-    t = ia; ia = ib; ib = t;
-  }
-  // ka/ia now hold the sorted keys and the arrival indices in CSR order, holes last (the full-mode lower bound of n_agg is
-  // the first hole, so offsets[n_agg] ends the CSR before them)
+  size_t sort_bytes = 0;
+  if ((e = cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys, idx, n, 0, bits, st)) != cudaSuccess ||
+      (e = sc.cub_tmp.reserve(sort_bytes)) != cudaSuccess)
+    return e;
+
+  if ((e = cudaMemsetAsync(d_counters, 0, 64, st)) != cudaSuccess) return e;
+  if (holes_out) extract_keys_kernel<true><<<cdiv(n, 256), 256, 0, st>>>(d_records, n, n_agg, keys.Current(), idx.Current(), d_counters + 4);
+  else extract_keys_kernel<false><<<cdiv(n, 256), 256, 0, st>>>(d_records, n, n_agg, keys.Current(), idx.Current(), d_counters + 4);
+  if ((e = cub::DeviceRadixSort::SortPairs(sc.cub_tmp.p, sort_bytes, keys, idx, n, 0, bits, st)) != cudaSuccess) return e;
+  // sorted keys and the arrival indices in CSR order, holes last (the full-mode lower bound of n_agg is the first hole, so
+  // offsets[n_agg] ends the CSR before them)
+  const uint32_t* sorted = keys.Current();
+  const uint32_t* order = idx.Current();
   const unsigned long long* d_holes = d_counters + 6;
   if (!d_touched_ids) {
-    offsets_full_kernel<<<cdiv(n_agg + 1, 256), 256, 0, st>>>(ka, n, n_agg, d_out_offsets);
+    offsets_full_kernel<<<cdiv(n_agg + 1, 256), 256, 0, st>>>(sorted, n, n_agg, d_out_offsets);
   } else {
     if ((e = sc.flags.reserve((size_t)n * 8)) != cudaSuccess) return e;
     uint32_t* heads = (uint32_t*)sc.flags.p;
     uint32_t* pos = heads + n;
-    heads_kernel<<<cdiv(n, 256), 256, 0, st>>>(ka, n, heads);
-    if ((e = exclusive_scan_u32(heads, pos, n, tmp, st)) != cudaSuccess) return e;
-    if (holes_out) compact_kernel<true><<<cdiv(n, 256), 256, 0, st>>>(ka, n, heads, pos, d_touched_ids, d_out_offsets, d_counters + 5, d_holes);
-    else compact_kernel<false><<<cdiv(n, 256), 256, 0, st>>>(ka, n, heads, pos, d_touched_ids, d_out_offsets, d_counters + 5, nullptr);
+    heads_kernel<<<cdiv(n, 256), 256, 0, st>>>(sorted, n, heads);
+    if ((e = exclusive_sum_u32(heads, pos, n, sc.cub_tmp, st)) != cudaSuccess) return e;
+    if (holes_out) compact_kernel<true><<<cdiv(n, 256), 256, 0, st>>>(sorted, n, heads, pos, d_touched_ids, d_out_offsets, d_counters + 5, d_holes);
+    else compact_kernel<false><<<cdiv(n, 256), 256, 0, st>>>(sorted, n, heads, pos, d_touched_ids, d_out_offsets, d_counters + 5, nullptr);
   }
-  if (holes_out) gather_records_kernel<true><<<cdiv((uint64_t)n * 4, 256), 256, 0, st>>>(d_records, ia, n, d_out_records, d_holes);
-  else gather_records_kernel<false><<<cdiv((uint64_t)n * 4, 256), 256, 0, st>>>(d_records, ia, n, d_out_records, nullptr);
+  if (holes_out) gather_records_kernel<true><<<cdiv((uint64_t)n * 4, 256), 256, 0, st>>>(d_records, order, n, d_out_records, d_holes);
+  else gather_records_kernel<false><<<cdiv((uint64_t)n * 4, 256), 256, 0, st>>>(d_records, order, n, d_out_records, nullptr);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   unsigned long long h[3];
   if ((e = cudaMemcpyAsync(h, d_counters + 4, holes_out ? 24 : 16, cudaMemcpyDeviceToHost, st)) != cudaSuccess) return e;

@@ -8,16 +8,19 @@
 namespace sgr {
 
 struct GroupScratch {
-  DevBuf keys_a, keys_b, idx_a, idx_b;  // radix-sort ping-pong buffers (u32 each)
-  DevBuf hist;                          // per-(digit, block) counts
-  DevBuf scan_tmp;                      // block sums of the scans (all levels)
+  DevBuf keys_a, keys_b, idx_a, idx_b;  // radix-sort double buffers (u32 each)
+  DevBuf cub_tmp;                       // CUB temp storage of the sort and of the compact mode's scan
   DevBuf flags;                         // segment-head flags / positions (compact mode)
   DevBuf batch_records;                 // grouped records of an incremental batch
   void release() {
-    keys_a.release(); keys_b.release(); idx_a.release(); idx_b.release(); hist.release(); scan_tmp.release();
+    keys_a.release(); keys_b.release(); idx_a.release(); idx_b.release(); cub_tmp.release();
     flags.release(); batch_records.release();
   }
 };
+
+// out[i] = in[0] + ... + in[i - 1] for i < n, by cub::DeviceScan::ExclusiveSum; out == in scans in place.
+// tmp is CUB's temp storage, grown to the size CUB asks for.
+cudaError_t exclusive_sum_u32(const uint32_t* in, uint32_t* out, uint32_t n, DevBuf& tmp, cudaStream_t stream);
 
 // Stable group-by of n fixed 64-byte records by their aggregate index (u64 at +8, < n_agg).
 // Replaces what the Kafka broker + KTable do in the reference: per-key log order is kept
