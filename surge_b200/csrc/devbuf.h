@@ -1,21 +1,96 @@
-// devbuf.h — growable device buffer owned by the engine.
+// devbuf.h — owners of the host code's CUDA resources: device buffers, page-locked host buffers, streams and events. Each frees
+// what it holds when it is destroyed or assigned over; none is copyable, so a block has one owner. Never make one a static or
+// namespace-scope object: its destructor would run after the CUDA runtime is torn down.
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
 
+#include <type_traits>
+#include <utility>
+
 namespace sgr {
-struct DevBuf {
+
+// One block of memory, released by Free.
+template <cudaError_t (*Free)(void*)>
+struct OwnedBlock {
   void* p = nullptr;
   size_t cap = 0;
+
+  OwnedBlock() = default;
+  OwnedBlock(OwnedBlock&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+  OwnedBlock& operator=(OwnedBlock&& o) noexcept {
+    if (this != &o) { free(); p = std::exchange(o.p, nullptr); cap = std::exchange(o.cap, 0); }
+    return *this;
+  }
+  ~OwnedBlock() { free(); }
+
+ protected:
+  void free() { if (p) Free(p); p = nullptr; cap = 0; }
+};
+
+// Growable device buffer.
+struct DevBuf : OwnedBlock<cudaFree> {
+  // At least n bytes (at least 256), content not kept. The old block is freed before the new one is allocated, so a large
+  // buffer never exists twice.
   cudaError_t reserve(size_t n) {
     if (n <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr; cap = 0;
+    free();
     if (n < 256) n = 256;
     cudaError_t e = cudaMalloc(&p, n);
-    if (e == cudaSuccess) cap = n;
+    if (e == cudaSuccess) cap = n; else p = nullptr;
     return e;
   }
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+
+  // Exactly new_cap bytes (at least 256) when that is more than cap, keeping the first `keep` bytes: they are copied on st, st is
+  // synchronised (kernels before this point are done with the old block), then the old block is freed. On failure nothing moves.
+  cudaError_t grow_keep(size_t new_cap, size_t keep, cudaStream_t st) {
+    if (new_cap <= cap) return cudaSuccess;
+    DevBuf nb;
+    cudaError_t e = nb.reserve(new_cap);
+    if (e == cudaSuccess && keep) e = cudaMemcpyAsync(nb.p, p, keep, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) *this = std::move(nb);
+    return e;
+  }
 };
+static_assert(!std::is_copy_constructible_v<DevBuf>, "a device block has one owner");
+
+// Page-locked host buffer.
+struct HostBuf : OwnedBlock<cudaFreeHost> {
+  // Exactly n bytes by cudaHostAlloc(flags), content not kept. The old block is freed first: no stream may still be copying
+  // from or into it.
+  cudaError_t alloc(size_t n, unsigned flags) {
+    free();
+    cudaError_t e = cudaHostAlloc(&p, n, flags);
+    if (e == cudaSuccess) cap = n; else p = nullptr;
+    return e;
+  }
+};
+static_assert(!std::is_copy_constructible_v<HostBuf>, "a page-locked block has one owner");
+
+// One handle (a stream, an event, ...) released by Destroy. It converts to the raw handle, so launch sites read as they would
+// with the raw handle.
+template <class H, auto Destroy>
+class Owned {
+ public:
+  Owned() = default;
+  Owned(Owned&& o) noexcept : h_(std::exchange(o.h_, nullptr)) {}
+  Owned& operator=(Owned&& o) noexcept {
+    if (this != &o) { reset(); h_ = std::exchange(o.h_, nullptr); }
+    return *this;
+  }
+  ~Owned() { reset(); }
+
+  operator H() const { return h_; }
+  // Where a create call writes the new handle; the one held so far is released first.
+  H* put() { reset(); return &h_; }
+  void reset() { if (h_) Destroy(h_); h_ = nullptr; }
+
+ private:
+  H h_ = nullptr;
+};
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+static_assert(!std::is_copy_constructible_v<Event>, "a handle has one owner");
+
 }  // namespace sgr

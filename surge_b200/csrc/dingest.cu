@@ -30,6 +30,7 @@
 #include <algorithm>
 #include <chrono>
 #include <map>
+#include <memory>
 #include <string>
 #include <thread>
 #include <vector>
@@ -41,27 +42,6 @@
 #include "record_batch.h"
 
 using namespace sgr;
-
-namespace {
-// growable device buffer that keeps its content (the staged fetches of one poll accumulate in it)
-struct KeepBuf {
-  DevBuf b;
-  uint64_t used = 0;
-  cudaError_t ensure(uint64_t extra, cudaStream_t st) {
-    if (used + extra <= b.cap) return cudaSuccess;
-    DevBuf nb;
-    uint64_t cap = b.cap ? b.cap : (1ull << 20);
-    while (cap < used + extra) cap *= 2;
-    cudaError_t e = nb.reserve(cap);
-    if (e != cudaSuccess) return e;
-    if (used) { e = cudaMemcpyAsync(nb.p, b.p, used, cudaMemcpyDeviceToDevice, st); if (e == cudaSuccess) e = cudaStreamSynchronize(st); }
-    if (e != cudaSuccess) { nb.release(); return e; }
-    b.release();
-    b = nb;
-    return cudaSuccess;
-  }
-};
-}  // namespace
 
 struct sgr_dingest {
   sgr_engine* eng = nullptr;
@@ -82,63 +62,64 @@ struct sgr_dingest {
   bool folded = false;                      // a fold succeeded since create / sgr_dingest_reset
   uint32_t row_bytes = 0;                   // state mode: program bytes of a row (state_bytes - 8), read when a poll's first group launches
   uint32_t json_row_end = 0;                // state mode: end of the registered JSON members in the row
-  // staged submissions
-  KeepBuf wire;
+  // staged submissions: the fetches of one poll accumulate in `wire`, whose first wire_used bytes are taken
+  DevBuf wire;
+  uint64_t wire_used = 0;
   // descriptors of the poll's data batches, in PAGE-LOCKED memory: every copy of them is a true asynchronous DMA (a copy from
   // pageable memory makes the host wait for the stream, which serialised the submissions behind each other's CRC kernels)
   struct PinnedBatches {
-    DgBatch* p = nullptr; size_t n = 0, cap = 0;
-    bool reserve(size_t want) {
+    HostBuf buf;
+    size_t n = 0, cap = 0;
+    bool reserve(size_t want) {   // (keeps the first n descriptors)
       if (want <= cap) return true;
       size_t c = cap ? cap : 4096;
       while (c < want) c *= 2;
-      DgBatch* np = nullptr;
-      if (cudaHostAlloc((void**)&np, c * sizeof(DgBatch), cudaHostAllocMapped) != cudaSuccess) return false;
-      if (n) memcpy(np, p, n * sizeof(DgBatch));
-      if (p) cudaFreeHost(p);
-      p = np; cap = c;
+      HostBuf nb;
+      if (nb.alloc(c * sizeof(DgBatch), cudaHostAllocMapped) != cudaSuccess) return false;
+      if (n) memcpy(nb.p, buf.p, n * sizeof(DgBatch));
+      buf = std::move(nb);
+      cap = c;
       return true;
     }
     size_t size() const { return n; }
     bool empty() const { return n == 0; }
     void clear() { n = 0; }
-    DgBatch* data() { return p; }
-    DgBatch& operator[](size_t i) { return p[i]; }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; n = cap = 0; }
+    DgBatch* data() { return (DgBatch*)buf.p; }
+    DgBatch& operator[](size_t i) { return data()[i]; }
   } batches;
   uint64_t n_record_slots = 0;
   sgr_ingest_stats poll{};                  // statistics of the current poll (host-side parts)
   sgr_ingest_stats total{};
   struct Sub { uint32_t batch_begin, batch_end; uint64_t nbytes; cudaEvent_t copied; };
   std::vector<Sub> subs;                    // the submissions of the current poll, in order
-  std::vector<cudaEvent_t> event_pool;
-  cudaStream_t copy_stream = nullptr;       // H2D copies of the wire bytes: they overlap the decode of earlier submissions
+  std::vector<Event> event_pool;
+  Stream copy_stream;                       // H2D copies of the wire bytes: they overlap the decode of earlier submissions
   // device scratch
-  KeepBuf arena, d_batches;
-  KeepBuf rec_off, rec_batch, out;          // per record slot; they keep their content when a later group needs them larger
-  KeepBuf st_idx, st_present;               // ... state mode: the slot's dense index (~0u: hole) and 0 / 1 (tombstone / row)
+  DevBuf arena, d_batches;
+  DevBuf rec_off, rec_batch, out;           // per record slot; they keep their content when a later group needs them larger
+  DevBuf st_idx, st_present;                // ... state mode: the slot's dense index (~0u: hole) and 0 / 1 (tombstone / row)
   DevBuf key_offs_dev, key_bytes_dev, key_scan_tmp;
   // chains of launches per group of batches
   uint64_t launched_batches = 0;            // batches of this poll whose chain has been launched
   uint32_t group_batches = 8192;            // SGR_DINGEST_GROUP
   static constexpr int kGroupStreams = 8;
-  cudaStream_t gstream[kGroupStreams] = {};
-  std::vector<cudaEvent_t> group_events;    // pool; the first n_groups are this poll's "group done" events
+  Stream gstream[kGroupStreams];
+  std::vector<Event> group_events;          // pool; the first n_groups are this poll's "group done" events
   uint32_t n_groups = 0;
   uint64_t launched_records = 0;            // record slots covered by the launched chains
   // SGR_DINGEST_TIMING: per group the device times (ms since the poll's first copy was queued) at which its bytes had landed,
   // its CRC + size pass, its decode and its parse ended; printed to stderr by sgr_dingest_fold
-  std::vector<cudaEvent_t> tl_events;       // 4 per group, + [last] the poll's origin
-  cudaEvent_t tl_origin = nullptr;
-  void* h_keys = nullptr; uint64_t h_keys_cap = 0;   // page-locked landing area of the new ids
+  std::vector<Event> tl_events;             // 4 per group
+  Event tl_origin;                          // the poll's origin
+  HostBuf h_keys;                           // page-locked landing area of the new ids
   // device dictionary
   DevBuf tags, slot_idx, key_ref, id_arena, ctl;
   uint64_t slots = 0, max_keys = 0, arena_cap = 0;
   uint64_t keys_on_host = 0;                // ids already appended to the engine's key table
   uint64_t id_bytes_on_host = 0;            // ... and the id-arena bytes they occupy
-  cudaEvent_t keys_landed = nullptr;
+  Event keys_landed;
   uint64_t generation = 0;                  // bumped by sgr_dingest_reset: a new dictionary is a new owner of the engine's key table
-  void* h_ctl = nullptr;                    // page-locked landing area
+  HostBuf h_ctl;                            // page-locked landing area
   bool timing_syncs = false;                // SGR_DINGEST_TIMING=1: record the per-group device timeline (tl_events)
   float ms[8] = {};                         // last fold: [0] wait for the copies and every chain [1] exact-layout repeat [2] unused
                                             //            [3] keys to host [4] table growth + fold [5] total
@@ -152,6 +133,16 @@ template <class... A> int32_t dfail(sgr_dingest* g, int32_t code, const char* fm
     if (_e == cudaErrorMemoryAllocation) (void)cudaGetLastError();   /* not sticky: the engine's next launch check must not see it */ \
     if (_e != cudaSuccess) return dfail((g), _e == cudaErrorMemoryAllocation ? SGR_ERR_OOM : SGR_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(_e)); \
   } while (0)
+
+// grow an event pool to n events
+cudaError_t grow_pool(std::vector<Event>& pool, size_t n, unsigned flags) {
+  while (pool.size() < n) {
+    Event ev;
+    if (const cudaError_t e = cudaEventCreateWithFlags(ev.put(), flags)) return e;
+    pool.push_back(std::move(ev));
+  }
+  return cudaSuccess;
+}
 
 std::string dg_err_text(const sgr_dingest* g, uint32_t e) {
   if ((e & 0xffu) == DG_VALUE_FRAMING) {   // the host decoder's text: JSON reasons follow "JSON event: "
@@ -201,7 +192,7 @@ cudaError_t reset_poll_counters(sgr_dingest* g) {
 }
 
 void clear_poll(sgr_dingest* g) {
-  g->wire.used = 0; g->batches.clear(); g->n_record_slots = 0; g->poll = sgr_ingest_stats{}; g->subs.clear();
+  g->wire_used = 0; g->batches.clear(); g->n_record_slots = 0; g->poll = sgr_ingest_stats{}; g->subs.clear();
   g->launched_batches = 0; g->n_groups = 0; g->launched_records = 0;
 }
 
@@ -214,29 +205,31 @@ void discard_poll(sgr_dingest* g) {
 
 DgParse parse_args(sgr_dingest* g) {
   DgParse p{};
-  p.wire = (const uint8_t*)g->wire.b.p; p.arena = (const uint8_t*)g->arena.b.p;
-  p.batches = (DgBatch*)g->d_batches.b.p;
-  p.rec_off = (const uint32_t*)g->rec_off.b.p; p.rec_batch = (const uint32_t*)g->rec_batch.b.p; p.out = (uint8_t*)g->out.b.p; p.null_value_type = g->null_value_type;
+  p.wire = (const uint8_t*)g->wire.p; p.arena = (const uint8_t*)g->arena.p;
+  p.batches = (DgBatch*)g->d_batches.p;
+  p.rec_off = (const uint32_t*)g->rec_off.p; p.rec_batch = (const uint32_t*)g->rec_batch.p; p.out = (uint8_t*)g->out.p; p.null_value_type = g->null_value_type;
   p.value_framing = g->value_framing; p.json = g->json;
   p.dict.tags = (unsigned long long*)g->tags.p; p.dict.slot_idx = (uint32_t*)g->slot_idx.p; p.dict.key_ref = (uint2*)g->key_ref.p;
   p.dict.arena = (uint8_t*)g->id_arena.p; p.dict.ctl = (unsigned long long*)g->ctl.p; p.dict.slots_mask = g->slots - 1;
   p.dict.max_keys = g->max_keys; p.dict.arena_cap = g->arena_cap;
   p.state_topic = g->state_topic; p.row_bytes = g->row_bytes;
-  p.idx = (uint32_t*)g->st_idx.b.p; p.present = (uint8_t*)g->st_present.b.p;
+  p.idx = (uint32_t*)g->st_idx.p; p.present = (uint8_t*)g->st_present.p;
   return p;
 }
 
-// grow a content-keeping buffer; anything that moves waits for every stream first (kernels in flight hold the old address)
-cudaError_t grow_keeping(sgr_dingest* g, KeepBuf& kb, uint64_t keep_bytes, uint64_t want_bytes) {
-  if (want_bytes <= kb.b.cap) return cudaSuccess;
+// Grow a buffer to at least want_bytes, doubling from 1 MiB, keeping its first keep_bytes. Anything that moves waits for every
+// stream first (kernels in flight hold the old address).
+cudaError_t grow_keeping(sgr_dingest* g, DevBuf& b, uint64_t keep_bytes, uint64_t want_bytes) {
+  if (want_bytes <= b.cap) return cudaSuccess;
   cudaError_t e = sync_all(g);
   if (e != cudaSuccess) return e;
-  kb.used = keep_bytes;
-  return kb.ensure(want_bytes - keep_bytes, g->stream);   // (ensure doubles, copies `used` bytes and synchronises)
+  uint64_t cap = b.cap ? b.cap : (1ull << 20);
+  while (cap < want_bytes) cap *= 2;
+  return b.grow_keep(cap, keep_bytes, g->stream);
 }
 
 cudaError_t set_arena_capacity(sgr_dingest* g) {
-  const unsigned long long cap = g->arena.b.cap >= 512 ? g->arena.b.cap - 512 : 0;   // (the walk's ring reads 256 bytes past a slot)
+  const unsigned long long cap = g->arena.cap >= 512 ? g->arena.cap - 512 : 0;   // (the walk's ring reads 256 bytes past a slot)
   return cudaMemcpy((unsigned long long*)g->ctl.p + 9, &cap, 8, cudaMemcpyHostToDevice);
 }
 
@@ -267,34 +260,30 @@ int32_t launch_group(sgr_dingest* g, uint64_t batch_end, uint64_t rec_end, cudaE
     DG_TRY(g, grow_keeping(g, g->st_idx, r0 * 4, rec_end * 4 + 64));
     DG_TRY(g, grow_keeping(g, g->st_present, r0, rec_end + 64));
   }
-  const uint64_t arena_want = (uint64_t)claim_multiple(g) * g->wire.b.cap + 512;
-  if (g->arena.b.cap < arena_want) {
-    DG_TRY(g, grow_keeping(g, g->arena, b0 ? g->arena.b.cap : 0, arena_want));
+  const uint64_t arena_want = (uint64_t)claim_multiple(g) * g->wire.cap + 512;
+  if (g->arena.cap < arena_want) {
+    DG_TRY(g, grow_keeping(g, g->arena, b0 ? g->arena.cap : 0, arena_want));
     DG_TRY(g, set_arena_capacity(g));
   }
-  if (g->n_groups >= g->group_events.size()) {
-    cudaEvent_t ev;
-    DG_TRY(g, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    g->group_events.push_back(ev);
-  }
+  DG_TRY(g, grow_pool(g->group_events, g->n_groups + 1, cudaEventDisableTiming));
   cudaStream_t s = g->gstream[g->n_groups % sgr_dingest::kGroupStreams];
   DG_TRY(g, cudaStreamWaitEvent(s, landed, 0));
-  cudaEvent_t* tl = nullptr;
+  const Event* tl = nullptr;
   if (g->timing_syncs) {
-    while (g->tl_events.size() < 4 * (size_t)(g->n_groups + 1)) { cudaEvent_t ev; DG_TRY(g, cudaEventCreate(&ev)); g->tl_events.push_back(ev); }
+    DG_TRY(g, grow_pool(g->tl_events, 4 * (size_t)(g->n_groups + 1), cudaEventDefault));
     tl = g->tl_events.data() + 4 * (size_t)g->n_groups;
     DG_TRY(g, cudaEventRecord(tl[0], s));
   }
-  DgBatch* db = (DgBatch*)g->d_batches.b.p + b0;
+  DgBatch* db = (DgBatch*)g->d_batches.p + b0;
   {
     void* mapped = nullptr;   // the descriptors go up by a kernel: a copy-engine transfer would queue behind every fetch of the poll
-    DG_TRY(g, cudaHostGetDevicePointer(&mapped, g->batches.p + b0, 0));
+    DG_TRY(g, cudaHostGetDevicePointer(&mapped, g->batches.data() + b0, 0));
     DG_TRY(g, dg_copy_from_mapped_host(mapped, db, nb * sizeof(DgBatch), s));
   }
-  if (rec_end > r0) DG_TRY(g, cudaMemsetAsync((uint32_t*)g->rec_batch.b.p + r0, 0xff, (rec_end - r0) * 4, s));
-  DG_TRY(g, dg_launch_crc_size_fast((const uint8_t*)g->wire.b.p, db, (uint32_t)nb, (unsigned long long*)g->ctl.p + 8, claim_multiple(g), s));
+  if (rec_end > r0) DG_TRY(g, cudaMemsetAsync((uint32_t*)g->rec_batch.p + r0, 0xff, (rec_end - r0) * 4, s));
+  DG_TRY(g, dg_launch_crc_size_fast((const uint8_t*)g->wire.p, db, (uint32_t)nb, (unsigned long long*)g->ctl.p + 8, claim_multiple(g), s));
   if (tl) DG_TRY(g, cudaEventRecord(tl[1], s));
-  DG_TRY(g, dg_launch_decode_walk_fast((const uint8_t*)g->wire.b.p, (uint8_t*)g->arena.b.p, db, (uint32_t)nb, (uint32_t)b0, (uint32_t*)g->rec_off.b.p, (uint32_t*)g->rec_batch.b.p, (unsigned long long*)g->ctl.p + 8, s));
+  DG_TRY(g, dg_launch_decode_walk_fast((const uint8_t*)g->wire.p, (uint8_t*)g->arena.p, db, (uint32_t)nb, (uint32_t)b0, (uint32_t*)g->rec_off.p, (uint32_t*)g->rec_batch.p, (unsigned long long*)g->ctl.p + 8, s));
   if (tl) DG_TRY(g, cudaEventRecord(tl[2], s));
   DgParse p = parse_args(g);
   p.n_batches = (uint32_t)batch_end; p.rec_begin = (uint32_t)r0; p.n_records = (uint32_t)rec_end;
@@ -314,14 +303,14 @@ int32_t sgr_dingest_create(sgr_engine* e, uint64_t max_keys, uint64_t max_id_byt
   *out = nullptr;
   void* st = nullptr;
   if (sgr_stream(e, &st) != SGR_OK) return SGR_ERR_INVALID;
-  sgr_dingest* g = new sgr_dingest();
+  std::unique_ptr<sgr_dingest> g(new sgr_dingest());   // (a failure below frees whatever was made)
   g->eng = e; g->stream = (cudaStream_t)st;
   g->timing_syncs = getenv("SGR_DINGEST_TIMING") != nullptr;
   if (const char* gb = getenv("SGR_DINGEST_GROUP")) { const long v = atol(gb); if (v >= 64 && v <= (1l << 24)) g->group_batches = (uint32_t)v; }
-  if (dg_prepare() != cudaSuccess) { delete g; return SGR_ERR_CUDA; }
-  if (cudaStreamCreateWithFlags(&g->copy_stream, cudaStreamNonBlocking) != cudaSuccess) { delete g; return SGR_ERR_CUDA; }
-  for (cudaStream_t& s : g->gstream)
-    if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) { sgr_dingest_destroy(g); return SGR_ERR_CUDA; }
+  if (dg_prepare() != cudaSuccess) return SGR_ERR_CUDA;
+  if (cudaStreamCreateWithFlags(g->copy_stream.put(), cudaStreamNonBlocking) != cudaSuccess) return SGR_ERR_CUDA;
+  for (Stream& s : g->gstream)
+    if (cudaStreamCreateWithFlags(s.put(), cudaStreamNonBlocking) != cudaSuccess) return SGR_ERR_CUDA;
   g->max_keys = max_keys;
   g->slots = 1024;
   while (g->slots < 2 * max_keys) g->slots *= 2;          // load factor <= 0.5
@@ -329,33 +318,17 @@ int32_t sgr_dingest_create(sgr_engine* e, uint64_t max_keys, uint64_t max_id_byt
   cudaError_t ce;
   if ((ce = g->tags.reserve(g->slots * 8)) != cudaSuccess || (ce = g->slot_idx.reserve(g->slots * 4)) != cudaSuccess ||
       (ce = g->key_ref.reserve(max_keys * 8)) != cudaSuccess || (ce = g->id_arena.reserve(g->arena_cap + 64)) != cudaSuccess ||
-      (ce = g->ctl.reserve(128)) != cudaSuccess || (ce = cudaHostAlloc(&g->h_ctl, 256, cudaHostAllocDefault)) != cudaSuccess ||
+      (ce = g->ctl.reserve(128)) != cudaSuccess || (ce = g->h_ctl.alloc(256, cudaHostAllocDefault)) != cudaSuccess ||
       (ce = cudaMemsetAsync(g->tags.p, 0, g->slots * 8, g->stream)) != cudaSuccess || (ce = cudaMemsetAsync(g->slot_idx.p, 0, g->slots * 4, g->stream)) != cudaSuccess ||
-      (ce = cudaMemsetAsync(g->ctl.p, 0, 128, g->stream)) != cudaSuccess || (ce = cudaStreamSynchronize(g->stream)) != cudaSuccess) {
-    sgr_dingest_destroy(g);
+      (ce = cudaMemsetAsync(g->ctl.p, 0, 128, g->stream)) != cudaSuccess || (ce = cudaStreamSynchronize(g->stream)) != cudaSuccess)
     return ce == cudaErrorMemoryAllocation ? SGR_ERR_OOM : SGR_ERR_CUDA;
-  }
-  *out = g;
+  *out = g.release();
   return SGR_OK;
 }
 
 int32_t sgr_dingest_destroy(sgr_dingest* g) {
   if (!g) return SGR_OK;
   sync_all(g);
-  if (g->copy_stream) cudaStreamDestroy(g->copy_stream);
-  for (cudaStream_t s : g->gstream) if (s) cudaStreamDestroy(s);
-  for (cudaEvent_t ev : g->event_pool) cudaEventDestroy(ev);
-  for (cudaEvent_t ev : g->group_events) cudaEventDestroy(ev);
-  for (cudaEvent_t ev : g->tl_events) cudaEventDestroy(ev);
-  if (g->tl_origin) cudaEventDestroy(g->tl_origin);
-  if (g->keys_landed) cudaEventDestroy(g->keys_landed);
-  if (g->h_keys) cudaFreeHost(g->h_keys);
-  g->batches.release();
-  g->wire.b.release(); g->d_batches.b.release(); g->arena.b.release(); g->rec_off.b.release(); g->rec_batch.b.release(); g->out.b.release();
-  g->st_idx.b.release(); g->st_present.b.release();
-  g->key_offs_dev.release(); g->key_bytes_dev.release(); g->key_scan_tmp.release(); g->json_table.release();
-  g->tags.release(); g->slot_idx.release(); g->key_ref.release(); g->id_arena.release(); g->ctl.release();
-  if (g->h_ctl) cudaFreeHost(g->h_ctl);
   delete g;
   return SGR_OK;
 }
@@ -433,11 +406,9 @@ int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, c
   DG_TRY(g, sync_all(g));   // (no kernel of an earlier poll may still read the old table)
   DevBuf nb;
   DG_TRY(g, nb.reserve(blob.size()));
-  const cudaError_t ce = cudaMemcpy(nb.p, blob.data(), blob.size(), cudaMemcpyHostToDevice);
-  if (ce != cudaSuccess) { nb.release(); DG_TRY(g, ce); }
-  g->json_table.release();
-  g->json_table = nb;
-  const uint8_t* base = (const uint8_t*)nb.p;
+  DG_TRY(g, cudaMemcpy(nb.p, blob.data(), blob.size(), cudaMemcpyHostToDevice));
+  g->json_table = std::move(nb);
+  const uint8_t* base = (const uint8_t*)g->json_table.p;
   g->json = vf::Table{base + cls_bytes + fld_bytes, (const vf::Class*)base, (const vf::Field*)(base + cls_bytes), (uint32_t)classes.size(), 0,
                       (uint32_t)strlen(discriminator), unknown_type < 0 ? -1 : unknown_type};
   g->json_row_end = row_end;
@@ -498,7 +469,7 @@ int32_t sgr_dingest_submit(sgr_dingest* g, int32_t partition, const void* data, 
       const uint64_t max_section = h.codec == 3 ? (h.total - kBatchHeader) * 255ull + 64 : h.total - kBatchHeader;
       if ((uint64_t)h.records_count > max_section / 7 + 1) return dfail(g, SGR_ERR_INVALID, "partition %d offset %lld: recordsCount %d does not fit the batch", partition, (long long)h.base_offset, h.records_count);
       DgBatch d{};
-      d.src_off = g->wire.used + pos; d.base_offset = h.base_offset; d.min_offset = ps.seen ? ps.decoded_next : INT64_MIN;
+      d.src_off = g->wire_used + pos; d.base_offset = h.base_offset; d.min_offset = ps.seen ? ps.decoded_next : INT64_MIN;
       d.total_len = (uint32_t)h.total; d.n_records = (uint32_t)h.records_count; d.codec = (uint16_t)h.codec; d.stored_crc = h.stored_crc;
       d.rec_base = (uint32_t)(g->n_record_slots + slots);
       slots += (uint64_t)h.records_count;
@@ -511,21 +482,16 @@ int32_t sgr_dingest_submit(sgr_dingest* g, int32_t partition, const void* data, 
   if (g->n_record_slots + slots >= (1ull << 32)) return dfail(g, SGR_ERR_CAPACITY, "more than 2^32 records in one poll");
   sgr_dingest::Sub sub{};
   sub.batch_begin = (uint32_t)g->batches.size(); sub.batch_end = sub.batch_begin + (uint32_t)add.size(); sub.nbytes = pos;
-  if (g->subs.size() >= g->event_pool.size()) {
-    cudaEvent_t ev;
-    DG_TRY(g, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    g->event_pool.push_back(ev);
-  }
+  DG_TRY(g, grow_pool(g->event_pool, g->subs.size() + 1, cudaEventDisableTiming));
   sub.copied = g->event_pool[g->subs.size()];
   if (g->timing_syncs && g->subs.empty()) {
-    if (!g->tl_origin) DG_TRY(g, cudaEventCreate(&g->tl_origin));
+    if (!g->tl_origin) DG_TRY(g, cudaEventCreate(g->tl_origin.put()));
     DG_TRY(g, cudaEventRecord(g->tl_origin, g->copy_stream));
   }
   if (pos) {
-    if (g->wire.used + pos + 272 > g->wire.b.cap) DG_TRY(g, sync_all(g));   // the buffer moves: no copy in flight, no kernel reading it
-    DG_TRY(g, g->wire.ensure(pos + 272, g->copy_stream));                     // (the input ring reads up to 256 bytes past a batch)
-    DG_TRY(g, cudaMemcpyAsync((uint8_t*)g->wire.b.p + g->wire.used, buf, pos, cudaMemcpyHostToDevice, g->copy_stream));
-    g->wire.used += (pos + 15) & ~15ull;
+    DG_TRY(g, grow_keeping(g, g->wire, g->wire_used, g->wire_used + pos + 272));   // (the input ring reads up to 256 bytes past a batch)
+    DG_TRY(g, cudaMemcpyAsync((uint8_t*)g->wire.p + g->wire_used, buf, pos, cudaMemcpyHostToDevice, g->copy_stream));
+    g->wire_used += (pos + 15) & ~15ull;
   }
   DG_TRY(g, cudaEventRecord(sub.copied, g->copy_stream));
   g->subs.push_back(sub);
@@ -534,7 +500,7 @@ int32_t sgr_dingest_submit(sgr_dingest* g, int32_t partition, const void* data, 
       DG_TRY(g, sync_all(g));
       if (!g->batches.reserve(g->batches.n + add.size())) return dfail(g, SGR_ERR_OOM, "page-locked descriptor array");
     }
-    memcpy(g->batches.p + g->batches.n, add.data(), add.size() * sizeof(DgBatch));
+    memcpy(g->batches.data() + g->batches.n, add.data(), add.size() * sizeof(DgBatch));
     g->batches.n += add.size();
     if (g->batches.n - g->launched_batches >= g->group_batches) {
       const int32_t rc = launch_group(g, g->batches.n, g->n_record_slots + slots, sub.copied);
@@ -554,7 +520,7 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
   const uint32_t nb = (uint32_t)g->batches.size();
   const uint32_t nrec = (uint32_t)g->n_record_slots;
   sgr_ingest_stats st = g->poll;
-  unsigned long long* h = (unsigned long long*)g->h_ctl;
+  unsigned long long* h = (unsigned long long*)g->h_ctl.p;
   typedef std::chrono::steady_clock Clk;
   const Clk::time_point t_begin = Clk::now();
   Clk::time_point t_last = t_begin;
@@ -565,7 +531,7 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
     // ---- chains: launch the remainder, wait for every group, bring the verdicts back
     { const int32_t rc = launch_group(g, nb, nrec, g->subs.back().copied); if (rc) { discard_poll(g); return rc; } }
     for (uint32_t k = 0; k < g->n_groups; ++k) DG_TRY(g, cudaStreamWaitEvent(g->stream, g->group_events[k], 0));
-    DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.b.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
+    DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
     DG_TRY(g, cudaMemcpyAsync(h, g->ctl.p, 128, cudaMemcpyDeviceToHost, g->stream));
     DG_TRY(g, cudaStreamSynchronize(g->stream));
     lap(0);
@@ -580,8 +546,8 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
       // the arena claims overflowed (the poll compresses better than 3x): lay the arena out exactly and decode + parse again.
       // Ids the first attempt interned stay (an id is an id); its records are overwritten slot for slot.
       // (exact sizes first: the claim mode never measured them)
-      DG_TRY(g, dg_launch_crc_size_fast((const uint8_t*)g->wire.b.p, (DgBatch*)g->d_batches.b.p, nb, nullptr, 0, g->stream));
-      DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.b.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
+      DG_TRY(g, dg_launch_crc_size_fast((const uint8_t*)g->wire.p, (DgBatch*)g->d_batches.p, nb, nullptr, 0, g->stream));
+      DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
       DG_TRY(g, cudaStreamSynchronize(g->stream));
       uint64_t need = 0;
       double ratio = 0;
@@ -597,20 +563,19 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
       }
       if (g->value_framing != SGR_VALUE_PACKED || g->state_topic)
         while (g->claim_mult < 16 && (double)g->claim_mult < ratio) g->claim_mult = g->claim_mult < 4 ? 4 : 2 * g->claim_mult;
-      g->arena.used = 0;
-      DG_TRY(g, g->arena.ensure(need + 512, g->stream));
+      DG_TRY(g, grow_keeping(g, g->arena, 0, need + 512));
       DG_TRY(g, set_arena_capacity(g));
       p = parse_args(g);
       h[2] = h[3] = h[4] = h[5] = h[6] = 0; h[8] = need; h[10] = 0;
       DG_TRY(g, cudaMemcpyAsync((unsigned long long*)g->ctl.p + 2, h + 2, 5 * 8, cudaMemcpyHostToDevice, g->stream));
       DG_TRY(g, cudaMemcpyAsync((unsigned long long*)g->ctl.p + 8, h + 8, 8, cudaMemcpyHostToDevice, g->stream));
       DG_TRY(g, cudaMemcpyAsync((unsigned long long*)g->ctl.p + 10, h + 10, 8, cudaMemcpyHostToDevice, g->stream));
-      DG_TRY(g, cudaMemsetAsync(g->rec_batch.b.p, 0xff, (size_t)nrec * 4 + 4, g->stream));
-      DG_TRY(g, cudaMemcpyAsync(g->d_batches.b.p, g->batches.data(), (size_t)nb * sizeof(DgBatch), cudaMemcpyHostToDevice, g->stream));
-      DG_TRY(g, dg_launch_decode_walk_fast((const uint8_t*)g->wire.b.p, (uint8_t*)g->arena.b.p, (DgBatch*)g->d_batches.b.p, nb, 0, (uint32_t*)g->rec_off.b.p, (uint32_t*)g->rec_batch.b.p, nullptr, g->stream));
+      DG_TRY(g, cudaMemsetAsync(g->rec_batch.p, 0xff, (size_t)nrec * 4 + 4, g->stream));
+      DG_TRY(g, cudaMemcpyAsync(g->d_batches.p, g->batches.data(), (size_t)nb * sizeof(DgBatch), cudaMemcpyHostToDevice, g->stream));
+      DG_TRY(g, dg_launch_decode_walk_fast((const uint8_t*)g->wire.p, (uint8_t*)g->arena.p, (DgBatch*)g->d_batches.p, nb, 0, (uint32_t*)g->rec_off.p, (uint32_t*)g->rec_batch.p, nullptr, g->stream));
       p.n_batches = nb; p.rec_begin = 0; p.n_records = nrec;
       DG_TRY(g, dg_launch_parse(p, g->stream));
-      DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.b.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
+      DG_TRY(g, cudaMemcpyAsync(g->batches.data(), g->d_batches.p, (size_t)nb * sizeof(DgBatch), cudaMemcpyDeviceToHost, g->stream));
       DG_TRY(g, cudaMemcpyAsync(h, g->ctl.p, 128, cudaMemcpyDeviceToHost, g->stream));
       DG_TRY(g, cudaStreamSynchronize(g->stream));
       lap(1);
@@ -650,18 +615,13 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
       DG_TRY(g, g->key_bytes_dev.reserve(id_bytes_max + 64));
       uint32_t* d_offs = (uint32_t*)g->key_offs_dev.p;
       DG_TRY(g, dg_gather_keys(p.dict, g->keys_on_host, (uint32_t)add, d_offs, (uint8_t*)g->key_bytes_dev.p, g->key_scan_tmp, g->stream));
-      if (g->h_keys_cap < (add + 2) * 4 + id_bytes_max + 64) {
-        if (g->h_keys) cudaFreeHost(g->h_keys);
-        g->h_keys = nullptr; g->h_keys_cap = 0;
-        const uint64_t want = 2 * ((add + 2) * 4 + id_bytes_max + 64);
-        DG_TRY(g, cudaHostAlloc(&g->h_keys, want, cudaHostAllocDefault));
-        g->h_keys_cap = want;
-      }
-      uint32_t* h_offs = (uint32_t*)g->h_keys;
-      uint8_t* h_bytes = (uint8_t*)g->h_keys + (add + 2) * 4;
+      const uint64_t h_need = (add + 2) * 4 + id_bytes_max + 64;
+      if (g->h_keys.cap < h_need) DG_TRY(g, g->h_keys.alloc(2 * h_need, cudaHostAllocDefault));
+      uint32_t* h_offs = (uint32_t*)g->h_keys.p;
+      uint8_t* h_bytes = (uint8_t*)g->h_keys.p + (add + 2) * 4;
       DG_TRY(g, cudaMemcpyAsync(h_offs, d_offs, (add + 1) * 4, cudaMemcpyDeviceToHost, g->stream));
       if (id_bytes_max) DG_TRY(g, cudaMemcpyAsync(h_bytes, g->key_bytes_dev.p, id_bytes_max, cudaMemcpyDeviceToHost, g->stream));
-      if (!g->keys_landed) DG_TRY(g, cudaEventCreateWithFlags(&g->keys_landed, cudaEventDisableTiming));
+      if (!g->keys_landed) DG_TRY(g, cudaEventCreateWithFlags(g->keys_landed.put(), cudaEventDisableTiming));
       DG_TRY(g, cudaEventRecord(g->keys_landed, g->stream));
       int dev = 0;
       cudaGetDevice(&dev);
@@ -674,8 +634,8 @@ int32_t sgr_dingest_fold(sgr_dingest* g, sgr_ingest_stats* stats) {
     }
     lap(3);
     int32_t rc_fold = SGR_OK;
-    if (nrec && g->state_topic) rc_fold = put_decoded_poll(g->eng, g->out.b.p, (const uint32_t*)g->st_idx.b.p, (const uint8_t*)g->st_present.b.p, nrec, st.n_records);
-    else if (nrec) rc_fold = fold_decoded_poll(g->eng, g->out.b.p, nrec, st.n_records);
+    if (nrec && g->state_topic) rc_fold = put_decoded_poll(g->eng, g->out.p, (const uint32_t*)g->st_idx.p, (const uint8_t*)g->st_present.p, nrec, st.n_records);
+    else if (nrec) rc_fold = fold_decoded_poll(g->eng, g->out.p, nrec, st.n_records);
     if (appender.joinable()) appender.join();
     if (rc_fold) { dfail(g, rc_fold, "engine: %s", sgr_last_error(g->eng)); discard_poll(g); return rc_fold; }
     if (rc_append) { dfail(g, rc_append, "engine: %s", sgr_last_error(g->eng)); discard_poll(g); return rc_append; }

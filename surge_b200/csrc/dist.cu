@@ -210,21 +210,12 @@ NcclApi& nccl_api() { static NcclApi api; return api; }
 
 DistState* dist_create() { return new DistState(); }
 
-void dist_destroy(DistState* d) {
-  if (!d) return;
-  for (void* p : d->opened) cudaIpcCloseMemHandle(p);
-  if (d->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(d->comm);
-  d->owner_of.release(); d->local_of.release(); d->global_of_local.release(); d->part_tmp.release(); d->flags.release();
-  d->pos.release(); d->scan_tmp.release(); d->hist.release(); d->owner_total.release(); d->counts_all.release();
-  d->send_buf.release(); d->recv_buf.release();
-  d->route_of.release(); d->lb.release(); d->push_ctl.release(); d->gather_buf.release();
-  if (d->stream2) cudaStreamDestroy(d->stream2);
-  if (d->stream_hi) cudaStreamDestroy(d->stream_hi);
-  if (d->h_pinned) cudaFreeHost(d->h_pinned);
-  for (auto& e : d->pev) if (e) cudaEventDestroy(e);
-  for (auto& e : d->ev) if (e) cudaEventDestroy(e);
-  delete d;
+DistState::~DistState() {
+  for (void* p : opened) cudaIpcCloseMemHandle(p);
+  if (comm && g_nccl.CommDestroy) g_nccl.CommDestroy(comm);
 }
+
+void dist_destroy(DistState* d) { delete d; }
 
 int dist_unique_id(void* out128, std::string* err) {
   if (!g_nccl.load(err)) return SGR_ERR_DIST;
@@ -240,13 +231,13 @@ int dist_init(DistState* d, int rank, int nranks, const void* unique_id, uint64_
   if (nranks < 1 || nranks > kMaxRanks || rank < 0 || rank >= nranks) { *err = "rank/nranks out of range"; return SGR_ERR_INVALID; }
   d->rank = rank; d->nranks = nranks; d->recv_capacity = recv_capacity_records;
   d->loopback = nranks > 1 && !unique_id;   // ranks of one process (tests): peers arrive through dist_set_peers, barriers are the caller's
-  for (auto& e : d->ev) if (!e && cudaEventCreate(&e) != cudaSuccess) { *err = "cudaEventCreate"; return SGR_ERR_CUDA; }
-  for (auto& e : d->pev) if (!e && cudaEventCreate(&e) != cudaSuccess) { *err = "cudaEventCreate"; return SGR_ERR_CUDA; }
+  for (Event& e : d->ev) if (!e && cudaEventCreate(e.put()) != cudaSuccess) { *err = "cudaEventCreate"; return SGR_ERR_CUDA; }
+  for (Event& e : d->pev) if (!e && cudaEventCreate(e.put()) != cudaSuccess) { *err = "cudaEventCreate"; return SGR_ERR_CUDA; }
   if (!d->stream2) {
     int lo = 0, hi = 0;
     cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    if (cudaStreamCreateWithPriority(&d->stream2, cudaStreamNonBlocking, lo) != cudaSuccess ||
-        cudaStreamCreateWithPriority(&d->stream_hi, cudaStreamNonBlocking, hi) != cudaSuccess) { *err = "cudaStreamCreate"; return SGR_ERR_CUDA; }
+    if (cudaStreamCreateWithPriority(d->stream2.put(), cudaStreamNonBlocking, lo) != cudaSuccess ||
+        cudaStreamCreateWithPriority(d->stream_hi.put(), cudaStreamNonBlocking, hi) != cudaSuccess) { *err = "cudaStreamCreate"; return SGR_ERR_CUDA; }
   }
   if (nranks > 1 && !d->loopback) {
     if (!g_nccl.load(err)) return SGR_ERR_DIST;

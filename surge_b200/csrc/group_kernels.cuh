@@ -12,10 +12,6 @@ struct GroupScratch {
   DevBuf cub_tmp;                       // CUB temp storage of the sort and of the compact mode's scan
   DevBuf flags;                         // segment-head flags / positions (compact mode)
   DevBuf batch_records;                 // grouped records of an incremental batch
-  void release() {
-    keys_a.release(); keys_b.release(); idx_a.release(); idx_b.release(); cub_tmp.release();
-    flags.release(); batch_records.release();
-  }
 };
 
 // out[i] = in[0] + ... + in[i - 1] for i < n, by cub::DeviceScan::ExclusiveSum; out == in scans in place.

@@ -56,21 +56,12 @@ __global__ void __launch_bounds__(kThreads) gb_gather_kernel(const uint8_t* __re
 
 uint32_t blocks_for(uint64_t n) { return (uint32_t)((n + kThreads - 1) / kThreads); }
 
-// grow a device buffer to at least `need` bytes, keeping its first `keep` bytes
-cudaError_t grow_keep(DevBuf& b, size_t need, size_t keep, cudaStream_t st) {
+// grow a device buffer to at least `need` bytes, doubling from 4096, keeping its first `keep` bytes
+cudaError_t grow_doubling(DevBuf& b, size_t need, size_t keep, cudaStream_t st) {
   if (need <= b.cap) return cudaSuccess;
   size_t cap = b.cap ? b.cap : 4096;
   while (cap < need) cap *= 2;
-  DevBuf nb;
-  cudaError_t e = nb.reserve(cap);
-  if (e != cudaSuccess) return e;
-  if (keep) {
-    if ((e = cudaMemcpyAsync(nb.p, b.p, keep, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) { nb.release(); return e; }
-    if ((e = cudaStreamSynchronize(st)) != cudaSuccess) { nb.release(); return e; }
-  }
-  b.release();
-  b = nb;
-  return cudaSuccess;
+  return b.grow_keep(cap, keep, st);
 }
 
 }  // namespace
@@ -109,8 +100,8 @@ cudaError_t id_index_append(IdIndex& x, const uint8_t* bytes, const uint32_t* of
 }
 
 cudaError_t id_index_reserve(IdIndex& x, uint64_t ids, uint64_t arena_bytes, cudaStream_t st) {
-  cudaError_t e = grow_keep(x.key_ref, ids * sizeof(uint2), x.n * sizeof(uint2), st);
-  return e != cudaSuccess ? e : grow_keep(x.arena, arena_bytes, x.arena_used, st);
+  cudaError_t e = grow_doubling(x.key_ref, ids * sizeof(uint2), x.n * sizeof(uint2), st);
+  return e != cudaSuccess ? e : grow_doubling(x.arena, arena_bytes, x.arena_used, st);
 }
 
 cudaError_t id_index_insert(IdIndex& x, uint64_t to, unsigned long long* d_ctl, cudaStream_t st) {

@@ -27,7 +27,6 @@ struct IdIndex {
     d.ctl = ctl; d.slots_mask = slots ? slots - 1 : 0; d.max_keys = n; d.arena_cap = arena.cap;
     return d;
   }
-  void release() { tags.release(); slot_idx.release(); key_ref.release(); arena.release(); slots = n = arena_used = 0; valid = false; }
 };
 
 // Host bytes ids [from, to) of a key table take in the staging buffer of id_index_append (their refs and 8-byte aligned bytes).

@@ -17,8 +17,6 @@ struct IdOrder {
   DevBuf order;                // u32[n]
   uint64_t n = 0;              // ids [0, n) of the index are ordered
   uint64_t builds = ~0ull;     // the IdIndex::builds the order was made for (another value: order again from id 0)
-
-  void release() { order.release(); n = 0; builds = ~0ull; }
 };
 
 // Bring the order up to ids [0, to) of the index: from id 0 when o.n == 0, else sort ids [o.n, to) and merge them with the

@@ -494,7 +494,7 @@ int dist_push_reserve(DistState* d, uint64_t n, uint32_t n_chunks, std::string* 
   const uint64_t chunk_recs = chunk_records(n, n_chunks);
   const uint64_t ctas_per_chunk = chunk_recs / 256;   // sized for the smallest tile
   cudaError_t ce;
-  if (!d->h_pinned && (ce = cudaHostAlloc(&d->h_pinned, 128 + (size_t)kMaxRanks * kMaxChunks * 8 + 256, cudaHostAllocDefault)) != cudaSuccess) {
+  if (!d->h_pinned.p && (ce = d->h_pinned.alloc(128 + (size_t)kMaxRanks * kMaxChunks * 8 + 256, cudaHostAllocDefault)) != cudaSuccess) {
     *err = std::string("page-locked read-back buffer: ") + cudaGetErrorString(ce);
     return SGR_ERR_OOM;
   }
@@ -620,7 +620,7 @@ int dist_push_fold(DistState* d, const uint8_t* d_records, uint64_t n, const Pus
   // ---- results
   // page-locked landing area: a copy into pageable memory blocks inside the driver, which stalls the launches of the other
   // ranks of a loopback job (one process, one context) and with them the flags this rank is waiting for
-  unsigned long long* h_status = (unsigned long long*)d->h_pinned;
+  unsigned long long* h_status = (unsigned long long*)d->h_pinned.p;
   unsigned long long* h_cnt = h_status + 8;
   unsigned long long* h_flags = h_status + 16;
   DTRY(cudaMemcpyAsync(h_status, status, 64, cudaMemcpyDeviceToHost, s0));
@@ -651,7 +651,7 @@ int dist_push_fold(DistState* d, const uint8_t* d_records, uint64_t n, const Pus
   // ANY rank saw a throwing slot (then every rank repeats the call in ordered mode, see engine.cu)
   out->any_err_slots = h_cnt[3] != 0;
   if (R > 1 && !d->loopback) {
-    uint32_t* all = (uint32_t*)((uint8_t*)d->h_pinned + 128 + (size_t)kMaxRanks * kMaxChunks * 8);
+    uint32_t* all = (uint32_t*)((uint8_t*)d->h_pinned.p + 128 + (size_t)kMaxRanks * kMaxChunks * 8);
     uint32_t* mine = all + 2 * kMaxRanks;   // behind the gathered verdicts
     mine[0] = my_err ? 1u : 0u; mine[1] = h_cnt[3] ? 1u : 0u;
     DTRY(cudaMemcpyAsync((uint8_t*)d->push_ctl.p + off_proj, mine, 8, cudaMemcpyHostToDevice, s0));
