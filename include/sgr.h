@@ -69,6 +69,8 @@ extern "C" {
  * Variable record (SGR_REC_VAR16): 16-byte header + payload padded to 16 bytes
  *   +0  u32 type   +4 u32 seq   +8 u32 payload_len (unpadded)   +12 u32 agg
  *   +16 payload, padded with zeros up to a multiple of 16
+ *   A record is at most 528 bytes (16 + payload_len, before padding) unless option "max_record_bytes" (16..2064,
+ *   set before the load) says otherwise; a longer record is a malformed event: the handler throws at it.
  *
  * CSR: u64 seg_offsets[n_agg+1], BYTE offsets into the event log; segment i is
  *   [seg_offsets[i], seg_offsets[i+1]); every offset is a multiple of 16 so that
@@ -170,7 +172,7 @@ typedef struct sgr_stats {
   uint64_t event_bytes;     /* stored event-record bytes read by the last fold */
   uint64_t algorithmic_bytes;/* event_bytes + 8*(n_agg+1) + state_bytes*n_agg (+ prior states read) */
   uint64_t n_errors;        /* aggregates whose handler threw */
-  uint64_t n_long_segments; /* aggregates taken by the split (long-segment) path */
+  uint64_t n_long_segments; /* always 0 (kept for ABI layout; no fold skips long segments) */
   float    ms_h2d;          /* host->device copy of the last load (0 for _device loads) */
   float    ms_group;        /* stable group-by of the last unsorted load */
   float    ms_fold;         /* device time of the last fold (all its kernels); a record-parallel fold queued behind a

@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE — random fold programs and logs for the program tests (tests/test_gpu_program_fuzz.py,
-tests/test_gpu_program_scale.py, tests/test_program_oracle_cpu.py).
+tests/test_gpu_program_scale.py, tests/test_gpu_var_limits.py, tests/test_program_oracle_cpu.py).
 
 draw_program / draw_log / interleave / draw_var_program / draw_var_log are the small-case drawers of the fuzz test, moved
 here unchanged: the same seeds give byte-identical programs and logs. The scale drawers below build logs of millions of
@@ -272,6 +272,104 @@ def draw_var_log(rng, n_types, n_agg, long_len):
     big = int(rng.integers(0, n))
     buf[int(rec_off[big]) + 8:int(rec_off[big]) + 12] = np.frombuffer(np.uint32(0x7FFFFFF0).tobytes(), np.uint8)
     return buf, seg, rec_off
+
+
+VAR_CAPS = [64, 100, 520, 528, 529, 600, 1040, 1041, 1500, 2064]   # max_record_bytes values the variable-record tests use
+
+
+def draw_var_program_wide(rng, cap, state_bytes=None):
+    """A variable-record program over the whole language at record cap `cap` (max_record_bytes): every state width
+    16..128, class 0 / class 1 / mixed rules, 1..16 types of 0..8 ops, SETs of any multiple of 4 that fits, 64-bit adds
+    and subtracts at any 4-aligned destination, 0..2 Double fields (sometimes the last 8 bytes of the program area), and
+    sources anywhere in [0, cap - len], a fifth of them within 16 bytes of the cap. cap = 64 draws a fixed-record program.
+    Returns (state_bytes, rules, f64_fields)."""
+    state_bytes = 16 * int(rng.integers(1, 9)) if state_bytes is None else int(state_bytes)
+    user = state_bytes - 8
+    family = ["class0", "class1", "mixed"][int(rng.integers(0, 3))]
+    pool = {"class0": [I.MATERIALISE, I.CREATE, I.TOMBSTONE, I.THROW], "class1": [I.IF_EXISTS, I.CREATE, I.TOMBSTONE, I.THROW],
+            "mixed": [I.IF_EXISTS, I.MATERIALISE, I.CREATE, I.TOMBSTONE, I.THROW]}[family]
+    weights = {4: [0.55, 0.25, 0.1, 0.1], 5: [0.3, 0.3, 0.2, 0.1, 0.1]}[len(pool)]
+    n_types = int(rng.integers(1, 17))
+    rules = []
+    for t in range(n_types):
+        if t == 0:      # type 0 builds a state
+            ex = I.CREATE if family == "class1" else [I.MATERIALISE, I.CREATE][int(rng.integers(0, 2))]
+        elif family == "mixed" and t == 1:
+            ex = I.IF_EXISTS
+        else:
+            ex = int(rng.choice(pool, p=weights))
+        ops = []
+        for _ in range(int(rng.integers(0, 9)) if ex not in (I.TOMBSTONE, I.THROW) else 0):
+            opc = int(rng.choice([I.OP_SET, I.OP_ADD_I32, I.OP_SUB_I32, I.OP_ADD_I64, I.OP_SUB_I64], p=[0.4, 0.15, 0.15, 0.15, 0.15]))
+            if opc >= I.OP_ADD_I64 and user < 8:
+                opc = I.OP_SET
+            if opc == I.OP_SET:
+                ln = 4 * int(rng.integers(1, min(user, cap) // 4 + 1)) if rng.random() < 0.5 else 4 * int(rng.integers(1, 3))
+            else:
+                ln = 4 if opc <= I.OP_SUB_I32 else 8
+            dst = 4 * int(rng.integers(0, (user - ln) // 4 + 1))
+            top = (cap - ln) // 4                      # the last 4-aligned source that fits below the cap
+            r = rng.random()
+            if r < 0.2:
+                src = 4 * int(rng.integers(max(0, top - 3), top + 1))
+            elif r < 0.3:
+                src = 4 * int(rng.integers(0, min(4, top + 1)))   # header words
+            else:
+                src = 4 * int(rng.integers(min(4, top), min(top, 4 + 24) + 1))
+            ops.append((opc, dst, src, ln))
+        rules.append((ex, ops))
+    f64 = []
+    if user >= 8 and rng.random() < 0.45:
+        f64 = [user - 8] if rng.random() < 0.4 else [4 * int(rng.integers(0, (user - 8) // 4 + 1))]
+        if user >= 24 and rng.random() < 0.5:
+            other = [o for o in range(0, user - 7, 4) if abs(o - f64[0]) >= 8]
+            f64.append(int(rng.choice(other)))
+        t = int(rng.integers(0, n_types))               # some rule copies a Double into the first field
+        if rules[t][0] not in (I.TOMBSTONE, I.THROW) and len(rules[t][1]) < 8:
+            rules[t] = (rules[t][0], list(rules[t][1]) + [(I.OP_SET, f64[0], 16 + 8 * int(rng.integers(0, 3)), 8)])
+    return state_bytes, rules, f64
+
+
+def cap_lengths(rng, n, cap, ring=2064):
+    """n record lengths (16 + payload_len, before padding) around the cap: a third anywhere in [16, cap], a third within
+    16 bytes of the cap on either side, a third past it, up to 32 bytes past `ring` (a kernel's ring capacity)."""
+    pick = rng.random(n)
+    below = rng.integers(16, cap + 1, size=n)
+    near = rng.integers(max(16, cap - 16), cap + 17, size=n)
+    past = rng.integers(cap + 1, max(cap + 2, ring + 33), size=n)
+    return np.where(pick < 1 / 3, below, np.where(pick < 2 / 3, near, past))
+
+
+def var_log_of(rng, rules, counts, rec_bytes, p_throw=2e-4, f64_srcs=(), f64_values=SPECIAL_F64):
+    """Variable records in CSR order with the given lengths (rec_bytes[i] = 16 + payload_len of record i, every record
+    well formed and inside its segment), random payloads, types from type_mix, seq = position, the aggregate at +12.
+    f64_srcs: record byte offsets that get values drawn from f64_values where the record holds them.
+    Returns (log u8, seg_offsets u64, rec_offsets u64)."""
+    n = int(counts.sum())
+    plen = np.asarray(rec_bytes, dtype=np.int64) - 16
+    assert len(plen) == n and (plen >= 0).all()
+    rlen = 16 + ((plen + 15) // 16) * 16
+    rec_off = np.zeros(n + 1, dtype=np.uint64)
+    np.cumsum(rlen, out=rec_off[1:])
+    buf = rng.integers(0, 256, size=int(rec_off[-1]), dtype=np.uint8)
+    hdr = np.zeros((n, 4), dtype=np.uint32)
+    hdr[:, 0] = type_mix(rules, n, rng, p_throw)
+    hdr[:, 1] = np.arange(1, n + 1, dtype=np.uint32)
+    hdr[:, 2] = plen.astype(np.uint32)
+    hdr[:, 3] = np.repeat(np.arange(len(counts), dtype=np.uint32), counts)
+    hb = hdr.view(np.uint8).reshape(n, 16)
+    starts = rec_off[:-1].astype(np.int64)
+    for j in range(16):
+        buf[starts + j] = hb[:, j]
+    vals = np.asarray(f64_values, dtype=np.float64)
+    for src in f64_srcs:
+        hit = np.nonzero(16 + plen >= src + 8)[0]
+        vb = vals[rng.integers(0, len(vals), size=len(hit))].view(np.uint8).reshape(-1, 8)
+        for j in range(8):
+            buf[starts[hit] + src + j] = vb[:, j]
+    first = np.zeros(len(counts) + 1, dtype=np.int64)
+    np.cumsum(counts, out=first[1:])
+    return buf, rec_off[first].astype(np.uint64), rec_off
 
 
 # ------------------------------------------------------------------ scale: programs whose kernel instantiation is known

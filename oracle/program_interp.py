@@ -141,9 +141,8 @@ def fold_var(rules: Sequence[Rule], state_bytes: int, log: np.ndarray, seg_offse
              f64_fields: Sequence[int] = (), max_record_bytes: int = MAX_VAR_RECORD) -> np.ndarray:
     """Variable records (SGR_REC_VAR16): 16-byte header {type, seq, payload_len, agg} + payload padded to 16 bytes. A record
     that does not fit its segment, or is longer than the format allows (max_record_bytes, header included, before padding),
-    or is too short for the ops of its event class, is a malformed event: the handler throws at that record. (Do not feed
-    records between the cap and 64 KiB: how far past the cap a kernel still parses is an implementation detail the tests
-    stay away from.)"""
+    or is too short for the ops of its event class, is a malformed event: the handler throws at that record, however much
+    room a kernel's ring or stage would have had for it (tests/test_gpu_var_limits.py)."""
     user = state_bytes - 8
     buf = np.ascontiguousarray(log).view(np.uint8).reshape(-1).tobytes()
     n_agg = len(seg_offsets) - 1

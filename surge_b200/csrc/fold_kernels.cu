@@ -30,7 +30,6 @@ namespace sgr {
 namespace {
 
 constexpr uint32_t DESC_LAST = 0x80000000u;
-constexpr uint32_t DESC_SKIP = 0x40000000u;
 constexpr uint32_t DESC_BYTES = 0x3fffffffu;
 
 template <int THREADS, int CH, int NST, int LAG, int KIND>
@@ -112,19 +111,12 @@ fold_stream_kernel(const __grid_constant__ FoldArgs a, const __grid_constant__ D
       nxt_e = a.seg_offsets[sn + 1];
     }
   }
-  bool p_fresh = true;  // at the first chunk of a segment
 
   auto produce = [&](int s) {
     const uint32_t bar = bars + s * 8;
     uint32_t d = 0;
     if (p_has) {
-      uint64_t rem = p_end - p_pos;
-      if (p_fresh && a.long_threshold && rem > a.long_threshold) {
-        // left to the split (long-segment) path
-        d = DESC_LAST | DESC_SKIP;
-        rem = 0;
-        p_pos = p_end;
-      }
+      const uint64_t rem = p_end - p_pos;
       const uint32_t bytes = rem < (uint64_t)CH ? (uint32_t)rem : (uint32_t)CH;
       if (bytes) {
         mbar_arrive_expect_tx(bar, bytes);
@@ -134,14 +126,12 @@ fold_stream_kernel(const __grid_constant__ FoldArgs a, const __grid_constant__ D
       }
       p_pos += bytes;
       d |= bytes;
-      p_fresh = false;
       if (p_pos == p_end) {
         d |= DESC_LAST;
         p_seg += stride;
         p_has = p_seg < n_seg;
         p_pos = nxt_b;
         p_end = nxt_e;
-        p_fresh = true;
         if (p_seg + stride < n_seg) {
           const uint64_t sn = seg_of(p_seg + stride);
           nxt_b = a.seg_offsets[sn];
@@ -160,7 +150,7 @@ fold_stream_kernel(const __grid_constant__ FoldArgs a, const __grid_constant__ D
   bool c_fresh = true;
   uint32_t rp = 0, avail = 0, k = 0, exists = 0, exists0 = 0, err = 0, err_idx = 0;
   uint32_t copied = 0;  // some event of this segment produced a NEW state instance (Scala copy / constructor), see end_segment
-  unsigned long long n_applied = 0, n_err = 0, n_skipped = 0, n_dropped = 0;
+  unsigned long long n_applied = 0, n_err = 0, n_dropped = 0;
   uint32_t c_total = 0;  // bytes of the current segment received so far
 
   auto zero_state = [&]() {
@@ -292,8 +282,9 @@ fold_stream_kernel(const __grid_constant__ FoldArgs a, const __grid_constant__ D
         hdr = lds128(ring + rp);
         rec_bytes = 16 + (hdr.z > 0x10000u ? 0x10000u : hdr.z);  // clamp: anything this long is rejected below
         rec_len = (rec_bytes + 15u) & ~15u;
-        if (rec_len > (uint32_t)(LAG * CH + 16)) {
-          // longer than the ring can hold behind the refill point: a malformed event, never mis-parsed
+        if (rec_bytes > a.max_record_bytes || rec_len > (uint32_t)(LAG * CH + 16)) {
+          // longer than the format allows, or than the ring can hold behind the refill point: a malformed event,
+          // never mis-parsed (the launch keeps max_record_bytes within the ring, the second test is a guard)
           err = 1; err_idx = k; avail = 0;
           break;
         }
@@ -310,7 +301,7 @@ fold_stream_kernel(const __grid_constant__ FoldArgs a, const __grid_constant__ D
     }
     if (d & DESC_LAST) {
       if (avail != 0 && !err) { err = 1; err_idx = k; }  // trailing partial record
-      if (d & DESC_SKIP) ++n_skipped; else end_segment();
+      end_segment();
       c_seg += stride;
       c_has = c_seg < n_seg;
       c_fresh = true;
@@ -338,7 +329,6 @@ fold_stream_kernel(const __grid_constant__ FoldArgs a, const __grid_constant__ D
   for (int o = 16; o > 0; o >>= 1) {
     n_applied += __shfl_xor_sync(0xffffffffu, n_applied, o);
     n_err += __shfl_xor_sync(0xffffffffu, n_err, o);
-    n_skipped += __shfl_xor_sync(0xffffffffu, n_skipped, o);
     n_dropped += __shfl_xor_sync(0xffffffffu, n_dropped, o);
   }
   if ((tid & 31) == 0 && a.counters) {
@@ -346,7 +336,6 @@ fold_stream_kernel(const __grid_constant__ FoldArgs a, const __grid_constant__ D
     if (n_applied) atomicAdd(a.counters + (a.n_seg_dev ? 5 : 0), n_applied);
     if (n_dropped) atomicAdd(a.counters + 4, n_dropped);
     if (n_err) atomicAdd(a.counters + 1, n_err);
-    if (n_skipped) atomicAdd(a.counters + 2, n_skipped);
   }
 }
 
@@ -411,13 +400,15 @@ static cudaError_t launch_variant(int variant, const FoldArgs& args, const DevPr
   return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_fold_stream(const FoldArgs& args, const DevProgram& prog, int variant, int num_sms,
+cudaError_t launch_fold_stream(const FoldArgs& fold_args, const DevProgram& prog, int variant, int num_sms,
                                uint32_t max_record_bytes, cudaStream_t stream, FoldLaunchInfo* info) {
+  FoldArgs args = fold_args;
+  args.max_record_bytes = max_record_bytes;
   const bool explicit_variant = variant >= 0 && variant < kNumVariants && kVariants[variant].kind == (int)prog.record_kind;
   if (prog.record_kind == SGR_REC_VAR16) {
     if (!explicit_variant) variant = max_record_bytes <= 512 + 16 ? 6 : (max_record_bytes <= 1024 + 16 ? 7 : 8);
     // a variable record must fit in LAG*CH+16 bytes of ring behind the slot being refilled
-    if (max_record_bytes > (uint32_t)kVariants[variant].chunk * kVariants[variant].lag + 16) return cudaErrorInvalidValue;
+    if (max_record_bytes > (uint32_t)kVariants[variant].chunk * kVariants[variant].lag + 16) return cudaErrorNotSupported;
     return launch_variant(variant, args, prog, num_sms, stream, info);
   }
   if (explicit_variant) return launch_variant(variant, args, prog, num_sms, stream, info);

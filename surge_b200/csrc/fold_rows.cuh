@@ -128,6 +128,7 @@ struct VarArgs {
   uint32_t* redo_ids; uint64_t redo_cap;
   uint32_t* part_flags; uint32_t* part_data; uint32_t epoch;   // part_data: 8 words per warp
   uint32_t stage_bytes;
+  uint32_t max_record_bytes;      // a longer record (header included, before padding) is malformed: its segment is replayed
 };
 int vruns_config(int num_sms, uint32_t max_record_bytes, uint32_t stage_hint, int nstage, int* threads, size_t* smem, uint32_t* stage_bytes);  // returns max grid, 0 if impossible
 cudaError_t launch_fold_vruns(const VarArgs& args, const RowProgram& prog, int nstage, int grid, int threads, size_t smem, cudaStream_t stream);

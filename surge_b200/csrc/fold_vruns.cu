@@ -140,6 +140,7 @@ __global__ void __launch_bounds__(512) fold_vruns_kernel(const __grid_constant__
       agg = hdr.w;
       const uint32_t rec_bytes = 16 + hdr.z;
       ok = ok && hdr.z <= 0x10000u && ((rec_bytes + 15u) & ~15u) == len;          // directory and header agree on the length
+      ok = ok && rec_bytes <= a.max_record_bytes;                                  // longer than the format allows: malformed
       uint32_t fl = 0;
       if (ok && hdr.x < 16u) fl = tab[hdr.x * kTabStride];
       if (!(fl & kRuleValid)) ok = false;

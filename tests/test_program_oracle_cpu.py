@@ -119,6 +119,68 @@ def test_the_draws_cover_what_the_pin_claims():
     assert f64s >= 20
 
 
+def draw_wide_case(seed):
+    """One wide variable-record program per seed (oracle/program_corpus.py draw_var_program_wide), the caps in turn, and
+    a log whose record lengths sit around the cap (tests/test_gpu_var_limits.py folds the same kind of case)."""
+    rng = np.random.default_rng(36000 + seed)
+    cap = PC.VAR_CAPS[seed % len(PC.VAR_CAPS)]
+    state_bytes, rules, f64 = PC.draw_var_program_wide(rng, cap)
+    counts = rng.integers(0, 7, size=50)
+    counts[int(rng.integers(0, 50))] = 60
+    buf, seg, _ = PC.var_log_of(rng, rules, counts, PC.cap_lengths(rng, int(counts.sum()), cap), p_throw=0.01,
+                                f64_srcs=(16, 24, 32))
+    return rng, cap, state_bytes, rules, f64, counts, buf, seg
+
+
+@pytest.mark.parametrize("seed", range(240))
+def test_wide_variable_programs_match_the_interpreter(seed):
+    """Every state width, 64-bit ops at 4-aligned destinations, long SETs, Double fields, sources up to the cap, records
+    on both sides of it: the compiled oracle equals the interpreter, from None and on top of the first table."""
+    rng, cap, state_bytes, rules, f64, counts, buf, seg = draw_wide_case(seed)
+    what = f"seed {seed} cap {cap} state_bytes {state_bytes} rules {rules} f64 {f64}"
+    want = I.fold_var(rules, state_bytes, buf, seg, f64_fields=f64, max_record_bytes=cap)
+    got, nev, nerr = I.c_fold_var(rules, state_bytes, buf, seg, f64_fields=f64, max_record_bytes=cap)
+    same(got, want, what)
+    assert (nev, nerr) == implied_stats(want, state_bytes, counts), what
+    want2 = I.fold_var(rules, state_bytes, buf, seg, initial=want, f64_fields=f64, max_record_bytes=cap)
+    got2, nev2, nerr2 = I.c_fold_var(rules, state_bytes, buf, seg, initial=want, f64_fields=f64, max_record_bytes=cap)
+    same(got2, want2, what + " with prior states")
+    assert (nev2, nerr2) == implied_stats(want2, state_bytes, counts), what
+
+
+def test_the_wide_draws_cover_what_the_pin_claims():
+    """The wide draws reach every state width 16..128, class 0 / class 1 / mixed programs, 16 types, 8 ops, SETs of 48
+    bytes and more, 64-bit ops at destinations = 4 (mod 8), a Double in the last 8 bytes of the program area, sources
+    within 16 bytes of the cap, and records one byte under, at and one byte over the cap."""
+    seen = set()
+    for seed in range(240):
+        _, cap, state_bytes, rules, f64, _, _, _ = draw_wide_case(seed)
+        seen.add(("width", state_bytes))
+        kinds = {ex for ex, _ in rules}
+        seen.add("class1" if I.MATERIALISE not in kinds and I.IF_EXISTS in kinds else "mixed" if {I.MATERIALISE, I.IF_EXISTS} <= kinds
+                 else "class0" if I.IF_EXISTS not in kinds else None)
+        seen.add(("types", len(rules)))
+        if state_bytes - 16 in f64:                       # user - 8: the last 8 bytes of the program area
+            seen.add("f64 last")
+        for _, ops in rules:
+            seen.add(("ops", len(ops)))
+            for opc, dst, src, ln in ops:
+                if opc == I.OP_SET and ln >= 48:
+                    seen.add("set48")
+                if opc >= I.OP_ADD_I64 and dst % 8 == 4:
+                    seen.add("i64 at 4 mod 8")
+                if src + ln > cap - 16:
+                    seen.add("src near cap")
+    assert {("width", w) for w in range(16, 129, 16)} <= seen, sorted(x for x in seen if isinstance(x, tuple) and x[0] == "width")
+    assert {"class0", "class1", "mixed"} <= seen
+    assert ("types", 16) in seen and ("ops", 8) in seen
+    assert {"set48", "i64 at 4 mod 8", "f64 last", "src near cap"} <= seen
+    rng = np.random.default_rng(7)
+    for cap in PC.VAR_CAPS:
+        lens = PC.cap_lengths(rng, 4000, cap)
+        assert {cap - 1, cap, cap + 1} <= set(lens.tolist()) and lens.max() > 2064, cap
+
+
 SAMPLE_MODELS = [("counter", O.MODEL_COUNTER, P.counter_program), ("ml_counter", O.MODEL_ML_COUNTER, P.ml_counter_program),
                  ("int_balance", O.MODEL_INT_BALANCE, P.int_balance_program), ("bank_account", O.MODEL_BANK_ACCOUNT, P.bank_account_program)]
 
