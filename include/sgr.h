@@ -57,7 +57,7 @@ extern "C" {
 
 /* ------------------------------------------------------------------ packed formats
  *
- * Fixed record (SGR_REC_FIXED64): 64 bytes, little-endian, 64-byte aligned in the log
+ * Fixed record (SGR_REC_FIXED64): 64 bytes, little-endian, 16-byte aligned in the log
  *   +0  u32 type      event type = index into the program's rule table
  *   +4  u32 seq       sequence number (Counter: sequenceNumber)
  *   +8  u64 agg       dense aggregate index (or global index before routing). A program may read it like any
@@ -75,6 +75,14 @@ extern "C" {
  * CSR: u64 seg_offsets[n_agg+1], BYTE offsets into the event log; segment i is
  *   [seg_offsets[i], seg_offsets[i+1]); every offset is a multiple of 16 so that
  *   each segment is a legal source for a 1-D TMA bulk copy.
+ *   Fixed records: a segment may start at any multiple of 16, and its whole records fold at their
+ *   actual byte positions (seg_offsets[i] + 64*k), whatever the log start or the device address.
+ *   A segment whose length is not a multiple of 64 ends in a trailing partial record of 16, 32 or
+ *   48 bytes: a malformed event, at which the handler throws — SGR_ST_ERROR, err_idx = the number
+ *   of whole records before it, the prior state kept. As for any other throw, n_events counts the
+ *   records applied and n_errors counts the aggregate. Option "kernel" 2 and 3 (the record-parallel
+ *   kernels) take only logs whose every offset is seg_offsets[0] (mod 64); they refuse any other
+ *   with SGR_ERR_UNSUPPORTED, and automatic selection folds it on the lane-sequential kernel.
  *
  * State table: n_agg structs of state_bytes (multiple of 16, <= SGR_MAX_STATE_BYTES).
  *   The program owns bytes [0, state_bytes-8); the engine owns the trailing 8:

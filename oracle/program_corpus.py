@@ -1,5 +1,6 @@
 """TEST INFRASTRUCTURE — random fold programs and logs for the program tests (tests/test_gpu_program_fuzz.py,
-tests/test_gpu_program_scale.py, tests/test_gpu_var_limits.py, tests/test_program_oracle_cpu.py).
+tests/test_gpu_program_scale.py, tests/test_gpu_var_limits.py, tests/test_gpu_fixed_alignment.py,
+tests/test_program_oracle_cpu.py).
 
 draw_program / draw_log / interleave / draw_var_program / draw_var_log are the small-case drawers of the fuzz test, moved
 here unchanged: the same seeds give byte-identical programs and logs. The scale drawers below build logs of millions of
@@ -406,6 +407,34 @@ def row_program(rng, user_words, cls, n_src):
     return rules
 
 
+# ------------------------------------------------------------------ named programs the fixed-record GPU tests share
+def w14_double_program():
+    """64-byte states, class 1, a JVM Double at +8 (record +24): CREATE builds, IF_EXISTS copies the Double alone, adds,
+    or hands the instance back."""
+    rules = [
+        (I.CREATE, [(I.OP_SET, 0, 16, 8), (I.OP_SET, 8, 24, 8), (I.OP_SET, 16, 32, 16), (I.OP_ADD_I32, 40, 4, 4)]),
+        (I.IF_EXISTS, [(I.OP_SET, 8, 24, 8)]),
+        (I.IF_EXISTS, []),
+        (I.IF_EXISTS, [(I.OP_ADD_I32, 16, 48, 4), (I.OP_SUB_I32, 44, 52, 4), (I.OP_SET, 48, 56, 8)]),
+        (I.TOMBSTONE, []),
+        (I.THROW, []),
+    ]
+    return rules, [8]
+
+
+# outside the transformer algebra: the lane-sequential kernel folds them
+OUTSIDE = {
+    "i64_adds_16B": (16, [(I.MATERIALISE, [(I.OP_ADD_I64, 0, 16, 8)]), (I.MATERIALISE, [(I.OP_SUB_I64, 0, 24, 8)]),
+                          (I.CREATE, [(I.OP_SET, 0, 4, 4)]), (I.THROW, [])]),
+    "materialise_and_if_exists_32B": (32, [(I.CREATE, [(I.OP_SET, 0, 16, 8)]), (I.MATERIALISE, [(I.OP_ADD_I32, 8, 20, 4)]),
+                                           (I.IF_EXISTS, [(I.OP_SET, 12, 4, 4)]), (I.TOMBSTONE, []), (I.THROW, [])]),
+    "state_48B": (48, [(I.MATERIALISE, [(I.OP_ADD_I32, 0, 16, 4), (I.OP_SET, 4, 4, 4), (I.OP_SET, 24, 32, 16)]),
+                       (I.CREATE, [(I.OP_SET, 8, 20, 16)]), (I.TOMBSTONE, []), (I.THROW, [])]),
+    "state_128B": (128, [(I.CREATE, [(I.OP_SET, 0, 16, 48), (I.OP_SET, 64, 16, 48)]), (I.IF_EXISTS, [(I.OP_ADD_I64, 112, 24, 8)]),
+                         (I.IF_EXISTS, []), (I.THROW, [])]),
+}
+
+
 def type_mix(rules, n, rng, p_throw=2e-4):
     """Event types for n records: throwing types (THROW rules, MatchErrors at n_types .. 16, 255, 2^32 - 1) with
     probability p_throw, every other rule uniformly."""
@@ -460,6 +489,31 @@ def fixed_log(rng, rules, counts, f64_offsets=(), f64_values=SPECIAL_F64, pad_re
     np.cumsum(counts * 64, out=seg[1:])
     seg += pad_records * 64
     return buf, seg, aggs
+
+
+def granular_log(rng, records, counts, tails, start):
+    """Fixed records laid out at 16-byte granularity: `start` random bytes (a multiple of 16) in front of the first segment,
+    then per aggregate counts[i] whole 64-byte records (records [n, 64] in CSR order) followed by tails[i] bytes (0, 16, 32
+    or 48) of a trailing partial record whose first word is the valid type 0. Segment starts fall wherever the tails before
+    them put them. Returns (log u8 flat, seg_offsets u64 byte offsets into the log)."""
+    counts = np.asarray(counts, dtype=np.int64)
+    tails = np.asarray(tails, dtype=np.int64)
+    assert start % 16 == 0 and np.isin(tails, [0, 16, 32, 48]).all()
+    rec = np.ascontiguousarray(records, dtype=np.uint8).reshape(-1, 64)
+    n = int(counts.sum())
+    assert len(rec) == n
+    seg = np.zeros(len(counts) + 1, dtype=np.uint64)
+    seg[0] = start
+    seg[1:] = start + np.cumsum(64 * counts + tails)
+    buf = rng.integers(0, 256, size=int(seg[-1]), dtype=np.uint8)
+    units = buf.reshape(-1, 16)
+    first = np.zeros(len(counts), dtype=np.int64)
+    np.cumsum(counts[:-1], out=first[1:])
+    at = np.repeat(seg[:-1].astype(np.int64) // 16 - 4 * first, counts) + 4 * np.arange(n, dtype=np.int64)
+    units[at[:, None] + np.arange(4)] = rec.reshape(n, 4, 16)
+    part = np.nonzero(tails)[0]
+    buf[(seg[1:][part].astype(np.int64) - tails[part])[:, None] + np.arange(4)] = 0
+    return buf, seg
 
 
 def set_type(buf, seg, agg, k, etype):

@@ -84,9 +84,11 @@ def _equal(a: Optional[bytearray], b: Optional[bytearray], f64_fields: Sequence[
 
 def fold(rules: Sequence[Rule], state_bytes: int, records: np.ndarray, seg_offsets: Sequence[int], initial: Optional[np.ndarray] = None,
          f64_fields: Sequence[int] = ()) -> np.ndarray:
-    """records: [n, 64] uint8 in CSR order; seg_offsets: byte offsets (n_agg + 1). Returns the state table [n_agg, state_bytes]."""
+    """records: the log's bytes from seg_offsets[0] on ([n, 64] or flat uint8), in CSR order; seg_offsets: byte offsets
+    (n_agg + 1), multiples of 16 apart. A segment's whole records fold at their own byte positions; a trailing 16, 32 or
+    48 bytes is a malformed event, the handler throws there (include/sgr.h). Returns the state table [n_agg, state_bytes]."""
     user = state_bytes - 8
-    recs = np.ascontiguousarray(records).view(np.uint8).reshape(-1, 64)
+    buf = np.ascontiguousarray(records).view(np.uint8).reshape(-1).tobytes()
     n_agg = len(seg_offsets) - 1
     base = int(seg_offsets[0])
     out = np.zeros((n_agg, state_bytes), dtype=np.uint8)
@@ -97,14 +99,18 @@ def fold(rules: Sequence[Rule], state_bytes: int, records: np.ndarray, seg_offse
             if struct.unpack_from("<I", row.tobytes(), user)[0] & ST_EXISTS:
                 old = bytearray(row[:user].tobytes())
         cur = old                           # the actor's own instance
-        lo, hi = (int(seg_offsets[i]) - base) // 64, (int(seg_offsets[i + 1]) - base) // 64
-        threw_at = -1
-        for k in range(lo, hi):
+        pos, end, k, threw_at = int(seg_offsets[i]) - base, int(seg_offsets[i + 1]) - base, 0, -1
+        assert pos % 16 == 0 and end % 16 == 0 and end >= pos, "segment offsets are 16-byte granular and monotone"
+        while pos < end:
             try:
-                cur = _handle(rules, user, cur, recs[k].tobytes())
+                if end - pos < 64:
+                    raise _Throw()          # a trailing partial record
+                cur = _handle(rules, user, cur, buf[pos:pos + 64])
             except _Throw:
-                threw_at = k - lo
+                threw_at = k
                 break
+            pos += 64
+            k += 1
         if threw_at >= 0:
             final, flags, err = old, ST_ERROR, threw_at
         else:

@@ -129,7 +129,9 @@ static int check_program(const orc_program* p) {
   return 0;
 }
 
-/* fold: fixed 64-byte records in CSR order; seg_offsets are byte offsets (n_agg + 1), the first one need not be 0.
+/* fold: fixed 64-byte records in CSR order; seg_offsets are byte offsets (n_agg + 1), multiples of 16 apart, the first
+ * one need not be 0. Each segment's whole records fold at their own byte positions; a trailing 16, 32 or 48 bytes is a
+ * malformed event: the handler throws there, at err_idx = the number of whole records (include/sgr.h).
  * initial: prior table or NULL (None everywhere). n_events counts the events applied (those after a throw are dropped). */
 int orc_prog_fold(const orc_program* p, const uint8_t* records, const uint64_t* seg_offsets, uint64_t n_agg,
                   const uint8_t* initial, uint8_t* out, uint64_t* n_events, uint64_t* n_errors) {
@@ -141,14 +143,14 @@ int orc_prog_fold(const orc_program* p, const uint8_t* records, const uint64_t* 
   uint64_t nev = 0, nerr = 0;
   for (uint64_t i = 0; i < n_agg; i++) {
     const uint64_t lo = seg_offsets[i], hi = seg_offsets[i + 1];
-    if (hi < lo || (lo - base) % 64 || (hi - base) % 64) return -1;
+    if (hi < lo || (lo - base) % 16 || (hi - base) % 16) return -1;
     opt_state old, cur;
     load_prior(sb, initial ? initial + i * sb : NULL, &old);
     cur = old;
     int threw = 0;
     uint64_t k = 0;
     for (uint64_t pos = lo - base; pos < hi - base; pos += 64, k++)
-      if (handle(p, sb - 8, &cur, records + pos, 64)) { threw = 1; break; }
+      if (hi - base - pos < 64 || handle(p, sb - 8, &cur, records + pos, 64)) { threw = 1; break; }
     store(p, &old, &cur, threw, k, out + i * sb);
     nev += k; nerr += (uint64_t)threw;
   }

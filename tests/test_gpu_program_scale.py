@@ -19,6 +19,7 @@ import pytest
 
 from oracle import program_corpus as PC
 from oracle import program_interp as I
+from oracle.program_corpus import OUTSIDE, w14_double_program
 from surge_b200 import ReplayEngine, SgrError
 from surge_b200 import native as N
 from surge_b200 import programs as P
@@ -117,20 +118,6 @@ def test_row_program_family_at_scale(name, W, cls, n_src, variants):
             check(e, want2, nev2, nerr2, f"{what} kernel {kernel} with prior states")
 
 
-def w14_double_program():
-    """64-byte states, class 1, a JVM Double at +8 (record +24): CREATE builds, IF_EXISTS copies the Double alone, adds,
-    or hands the instance back."""
-    rules = [
-        (I.CREATE, [(I.OP_SET, 0, 16, 8), (I.OP_SET, 8, 24, 8), (I.OP_SET, 16, 32, 16), (I.OP_ADD_I32, 40, 4, 4)]),
-        (I.IF_EXISTS, [(I.OP_SET, 8, 24, 8)]),
-        (I.IF_EXISTS, []),
-        (I.IF_EXISTS, [(I.OP_ADD_I32, 16, 48, 4), (I.OP_SUB_I32, 44, 52, 4), (I.OP_SET, 48, 56, 8)]),
-        (I.TOMBSTONE, []),
-        (I.THROW, []),
-    ]
-    return rules, [8]
-
-
 def test_w14_class1_double_field_at_scale():
     """NaN, -0.0 and the instance rule: a segment that only copies the same NaN bits over a NaN state builds a new
     instance (published: NaN != NaN); one that only hands the instance back is not published."""
@@ -167,18 +154,6 @@ def test_w14_class1_double_field_at_scale():
 
 
 # ------------------------------------------------------------------ outside the algebra: the lane-sequential kernel
-OUTSIDE = {
-    "i64_adds_16B": (16, [(I.MATERIALISE, [(I.OP_ADD_I64, 0, 16, 8)]), (I.MATERIALISE, [(I.OP_SUB_I64, 0, 24, 8)]),
-                          (I.CREATE, [(I.OP_SET, 0, 4, 4)]), (I.THROW, [])]),
-    "materialise_and_if_exists_32B": (32, [(I.CREATE, [(I.OP_SET, 0, 16, 8)]), (I.MATERIALISE, [(I.OP_ADD_I32, 8, 20, 4)]),
-                                           (I.IF_EXISTS, [(I.OP_SET, 12, 4, 4)]), (I.TOMBSTONE, []), (I.THROW, [])]),
-    "state_48B": (48, [(I.MATERIALISE, [(I.OP_ADD_I32, 0, 16, 4), (I.OP_SET, 4, 4, 4), (I.OP_SET, 24, 32, 16)]),
-                       (I.CREATE, [(I.OP_SET, 8, 20, 16)]), (I.TOMBSTONE, []), (I.THROW, [])]),
-    "state_128B": (128, [(I.CREATE, [(I.OP_SET, 0, 16, 48), (I.OP_SET, 64, 16, 48)]), (I.IF_EXISTS, [(I.OP_ADD_I64, 112, 24, 8)]),
-                         (I.IF_EXISTS, []), (I.THROW, [])]),
-}
-
-
 @pytest.mark.parametrize("name", list(OUTSIDE))
 def test_program_outside_the_algebra_at_scale(name):
     sb, rules = OUTSIDE[name]

@@ -56,6 +56,137 @@ def test_fixed_records_match_the_interpreter(seed):
     assert (nev2, nerr2) == implied_stats(want2, state_bytes, np.diff(off2.astype(np.int64)) // 64), what
 
 
+def draw_granular_case(seed):
+    """A random program on a CSR log at 16-byte granularity (oracle/program_corpus.py granular_log): the log starts at
+    0, 16, 32 or 48 (mod 64), random segments end in a 16-, 32- or 48-byte partial record, and by seed the first, a middle
+    and the last segment, the long segment and a segment of exactly 16 bytes do too. Returns (rng, state_bytes, rules,
+    f64, log, seg_offsets, whole-record counts, tails)."""
+    rng = np.random.default_rng(37000 + seed)
+    state_bytes, rules, f64 = PC.draw_program(rng)
+    rec, off, _ = PC.draw_log(rng, len(rules), 60, 100, f64)
+    counts = np.diff(off.astype(np.int64)) // 64
+    n_agg = len(counts)
+    tails = np.where(rng.random(n_agg) < 0.2, 16 * rng.integers(1, 4, size=n_agg), 0)
+    if seed % 7 == 6:
+        tails[:] = 0                                       # whole records only, off the 64-byte grid by the start alone
+    else:
+        for i in ([0] if seed % 3 == 0 else []) + [n_agg // 2] + ([n_agg - 1] if seed % 3 == 1 else []):
+            tails[i] = 16 * (1 + seed % 3)
+        if seed % 4 == 1:
+            tails[int(np.argmax(counts))] = 48            # a long segment that ends in a partial record
+        if seed % 5 == 0:
+            z = int(rng.integers(0, n_agg))
+            rec = np.delete(rec, np.s_[int(counts[:z].sum()):int(counts[:z + 1].sum())], axis=0)
+            counts[z], tails[z] = 0, 16                   # exactly 16 bytes: throws at err_idx 0
+    start = 16 * (seed % 4) + 64 * int(rng.integers(0, 3))
+    log, seg = PC.granular_log(rng, rec, counts, tails, start)
+    return rng, state_bytes, rules, f64, log, seg, counts, tails
+
+
+@pytest.mark.parametrize("seed", range(300))
+def test_granular_fixed_logs_match_the_interpreter(seed):
+    """Fixed records at 16-byte granularity (include/sgr.h): whole records fold at their byte positions, a trailing
+    partial record throws at err_idx = the whole records before it, and the segments after it start off the 64-byte grid.
+    The compiled oracle equals the interpreter from None and on top of the first table."""
+    _, state_bytes, rules, f64, log, seg, counts, _ = draw_granular_case(seed)
+    what = f"seed {seed} state_bytes {state_bytes} rules {rules} f64 {f64} start {int(seg[0])}"
+    recs = log[int(seg[0]):]
+    want = I.fold(rules, state_bytes, recs, seg, f64_fields=f64)
+    got, nev, nerr = I.c_fold(rules, state_bytes, recs, seg, f64_fields=f64)
+    same(got, want, what)
+    assert (nev, nerr) == implied_stats(want, state_bytes, counts), what
+    want2 = I.fold(rules, state_bytes, recs, seg, initial=want, f64_fields=f64)
+    got2, nev2, nerr2 = I.c_fold(rules, state_bytes, recs, seg, initial=want, f64_fields=f64)
+    same(got2, want2, what + " with prior states")
+    assert (nev2, nerr2) == implied_stats(want2, state_bytes, counts), what
+
+
+def test_granular_partial_records_throw_where_the_rule_says():
+    """The rule itself, not only agreement between the two restatements: every segment that ends in a partial record is an
+    error row at err_idx = its whole records unless an earlier record threw, its prior state kept; every 64-aligned log
+    folds exactly as the same records packed from offset 0."""
+    for seed in range(300):
+        _, state_bytes, rules, f64, log, seg, counts, tails = draw_granular_case(seed)
+        got, _, _ = I.c_fold(rules, state_bytes, log[int(seg[0]):], seg, f64_fields=f64)
+        flags = got[:, state_bytes - 8:state_bytes - 4].copy().view(np.uint32).ravel()
+        err = got[:, state_bytes - 4:].copy().view(np.uint32).ravel()
+        part = tails > 0
+        assert ((flags[part] & I.ST_ERROR) != 0).all(), f"seed {seed}"
+        assert (err[part] <= counts[part]).all() and ((flags[part] & I.ST_EXISTS) == 0).all(), f"seed {seed}"
+        if not part.any():
+            starts = seg[:-1].astype(np.int64)
+            packed = np.concatenate([log[s:s + 64 * c] for s, c in zip(starts, counts)] + [np.zeros(0, np.uint8)])
+            off0 = np.zeros(len(counts) + 1, np.uint64)
+            np.cumsum(64 * counts, out=off0[1:])
+            want, _, _ = I.c_fold(rules, state_bytes, packed, off0, f64_fields=f64)
+            same(got, want, f"seed {seed}: 16-byte start {int(seg[0])} against the packed log")
+
+
+def test_the_granular_draws_cover_what_the_pin_claims():
+    """Every log start mod 64, every tail length, partial records in the first, a middle and the last segment and at the
+    end of the long one, a 16-byte segment, empty segments that start off the 64-byte grid, a partial record after a
+    throw in the same segment, and logs of whole records at each unaligned start."""
+    seen = set()
+    for seed in range(300):
+        _, state_bytes, rules, f64, log, seg, counts, tails = draw_granular_case(seed)
+        rel = seg.astype(np.int64) - int(seg[0])
+        seen.add(("start", int(seg[0]) % 64))
+        seen.update(("tail", int(t)) for t in tails if t)
+        if tails[0]:
+            seen.add("first")
+        if tails[-1]:
+            seen.add("last")
+        if tails[1:-1].any():
+            seen.add("middle")
+        if tails[int(np.argmax(counts))] and counts.max() >= 90:
+            seen.add("long")
+        if ((counts == 0) & (tails == 16)).any():
+            seen.add("16 bytes")
+        if ((np.diff(rel) == 0) & (rel[:-1] % 64 != 0)).any():
+            seen.add("empty off grid")
+        if not tails.any() and int(seg[0]) % 64:
+            seen.add(("whole", int(seg[0]) % 64))
+        got, _, _ = I.c_fold(rules, state_bytes, log[int(seg[0]):], seg, f64_fields=f64)
+        err = got[:, state_bytes - 4:].copy().view(np.uint32).ravel()
+        if ((tails > 0) & (err < counts)).any():
+            seen.add("throw before a partial")
+    assert {("start", s) for s in (0, 16, 32, 48)} <= seen
+    assert {("tail", t) for t in (16, 32, 48)} <= seen
+    assert {("whole", s) for s in (16, 32, 48)} <= seen
+    assert {"first", "middle", "last", "long", "16 bytes", "empty off grid", "throw before a partial"} <= seen, seen
+
+
+@pytest.mark.parametrize("model", [O.MODEL_COUNTER, O.MODEL_BANK_ACCOUNT], ids=["counter", "bank_account"])
+def test_granular_logs_match_the_sample_model_oracle(model):
+    """A third witness: the port of the reference fold walks each segment by byte offset and throws on a short tail
+    (decode_event), so on 16-byte-granular logs it equals the program oracle for the Counter and BankAccount."""
+    rng = np.random.default_rng(38000 + model)
+    prog = P.counter_program() if model == O.MODEL_COUNTER else P.bank_account_program()
+    rules, sb = rules_of(prog), int(prog.state_bytes)
+    f64 = [int(prog.f64_field_off[i]) for i in range(prog.n_f64_fields)]
+    counts = rng.integers(0, 10, size=40_000)
+    counts[17] = 3000
+    n = int(counts.sum())
+    rec = rng.integers(0, 256, size=(n, 64), dtype=np.uint8)
+    types = rng.integers(0, 2, size=n).astype(np.uint32)
+    types[rng.random(n) < 0.001] = 2 if model == O.MODEL_BANK_ACCOUNT else 7   # scala.MatchError
+    rec[:, 0:4] = types.view(np.uint8).reshape(-1, 4)
+    if model == O.MODEL_BANK_ACCOUNT:
+        rec[:, 32:40] = np.asarray(PC.SPECIAL_F64)[rng.integers(0, len(PC.SPECIAL_F64), size=n)].view(np.uint8).reshape(-1, 8)
+    tails = np.where(rng.random(len(counts)) < 0.05, 16 * rng.integers(1, 4, size=len(counts)), 0)
+    tails[[0, 17, len(counts) - 1]] = [16, 32, 48]
+    for start in (16, 32, 48, 64 + 16):
+        log, seg = PC.granular_log(rng, rec, counts, tails, start)
+        want, nev, nerr = O.fold_packed(model, O.REC_FIXED64, log, seg)
+        got, gev, gerr = I.c_fold(rules, sb, log[start:], seg, f64_fields=f64)
+        same(got, want, f"model {model} start {start}")
+        assert (gev, gerr) == (nev, nerr) and nerr > int((tails > 0).sum()) // 2, f"model {model} start {start}"
+        want2, nev2, nerr2 = O.fold_packed(model, O.REC_FIXED64, log, seg, want)
+        got2, gev2, gerr2 = I.c_fold(rules, sb, log[start:], seg, initial=want, f64_fields=f64)
+        same(got2, want2, f"model {model} start {start} with prior states")
+        assert (gev2, gerr2) == (nev2, nerr2)
+
+
 @pytest.mark.parametrize("seed", range(60))
 def test_arrival_order_matches_the_interpreter(seed):
     """Micro-batches onto a live table (per-batch flags cleared, untouched slots kept), and the from-None form."""
