@@ -188,7 +188,8 @@ typedef struct sgr_stats {
                                to its last warp's exit by %globaltimer, every other fold by CUDA events around it */
   float    ms_d2h;          /* device->host copy of the last export */
   uint32_t fold_launches;   /* kernels launched by the last fold */
-  uint32_t reserved[7];
+  uint32_t head_plane;      /* 1: the last fold read each record's 32-byte head from the head plane, not the log */
+  uint32_t reserved[6];
 } sgr_stats;
 
 int32_t sgr_abi_version(void);
@@ -209,6 +210,14 @@ int32_t sgr_register_program(sgr_engine* e, const sgr_fold_program* prog);
  * (SDSL/common/AggregateRefBaseTrait.scala:23-28). */
 int32_t sgr_load_events(sgr_engine* e, const void* events, uint64_t nbytes,
                         const uint64_t* seg_offsets, uint64_t n_agg);
+/* The device log and offsets are borrowed: they must stay allocated and unmodified while they are loaded (until the next
+ * load or sgr_destroy). The engine may keep derived copies of them, such as the head plane below, that a change would
+ * leave stale; to fold changed records, load them again.
+ * Head plane: for a fixed-record log whose segments are 64-byte aligned and a program that reads no record word past
+ * word 7, the engine keeps bytes 0..31 of every record in a dense plane of half the log's size, and the record-parallel
+ * fold reads that instead of the log. A host load builds it behind the copy; a borrowed log gets it from the first fold
+ * that uses it. Every load and sgr_register_program drops it; if it cannot be allocated the fold reads the log.
+ * sgr_set_option("head_plane", 0) keeps every fold on the log. */
 int32_t sgr_load_events_device(sgr_engine* e, const void* d_events, uint64_t nbytes,
                                const uint64_t* d_seg_offsets, uint64_t n_agg);
 

@@ -5,10 +5,14 @@ On the log bench.py folds (synth.counter_csr_device(2^20, 32, seed=2): 2^20 aggr
   (b) the same probe with warps taking chunks by ticket;
   (c) the fold itself: one synchronous fold alone (CUDA events around it, and the kernel's own stats().ms_fold), and
       K back-to-back fold_async calls (ms per fold), as bench.py's `value` times them;
-and reports each as GB/s over the log's bytes and the fold as a share of (a). Prints one JSON document and writes it to
+  (d) the read probe over a dense buffer of half the log's bytes: the head plane the Counter fold stages instead of the
+      log (32 bytes per record), and the fold from the head plane under each --head-variants entry, against (c) on the log
+      ("head_plane" 0);
+  (e) a load of the borrowed log followed by one fold, which builds the head plane, against the same with "head_plane" 0;
+and reports each as GB/s over the log's bytes and the fold as a share of (a) (the head-plane folds: of (d)). Prints one JSON document and writes it to
 OUT/fold_ceiling.json. The card's name and power limit are part of the numbers and are recorded with them.
 
-    python scripts/fold_ceiling.py --out DIR [--reps 30] [--steps 200]
+    python scripts/fold_ceiling.py --out DIR [--reps 30] [--steps 200] [--head-variants 0,1,2,3,4]
 """
 from __future__ import annotations
 
@@ -45,6 +49,8 @@ def main() -> None:
     ap.add_argument("--chunk-bytes", type=int, default=131072, help="chunk of the ticketed read probe (the fold's default)")
     ap.add_argument("--fold-chunk-bytes", type=lambda s: [int(x) for x in s.split(",")], default=[0],
                     help="comma list of the fold's run_chunk_bytes to measure (0: the engine's default)")
+    ap.add_argument("--head-variants", type=lambda s: [int(x) for x in s.split(",")], default=[0],
+                    help="comma list of head_variant values of the head-plane fold to measure")
     args = ap.parse_args()
 
     import torch
@@ -61,13 +67,13 @@ def main() -> None:
     ctl = torch.zeros(2, dtype=torch.int64, device=dev)
     stream = torch.cuda.current_stream()
 
-    def probe(ticketed: int) -> list:
+    def probe(ticketed: int, buf=log) -> list:
         ms = []
         for _ in range(args.reps + 2):
             ctl.zero_()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record(stream)
-            rc = lib.sgr_probe_read(C.c_void_p(log.data_ptr()), nbytes, ticketed, args.chunk_bytes, C.c_void_p(ctl.data_ptr()),
+            rc = lib.sgr_probe_read(C.c_void_p(buf.data_ptr()), buf.numel(), ticketed, args.chunk_bytes, C.c_void_p(ctl.data_ptr()),
                                     C.c_void_p(stream.cuda_stream))
             e1.record(stream)
             if rc != 0:
@@ -81,10 +87,22 @@ def main() -> None:
     out["b_read_probe_ticketed"] = summary(probe(1), nbytes)
 
     for cb in args.fold_chunk_bytes:
-        out.update(measure_fold(log, off, dev, cb, args.reps, args.steps, "" if cb == 0 else f"_chunk{cb}"))
+        out.update(measure_fold(log, off, dev, cb, args.reps, args.steps, "" if cb == 0 else f"_chunk{cb}", {"head_plane": 0}))
+    plane = torch.empty(nbytes // 2, dtype=torch.uint8, device=dev)
+    plane.copy_(log.view(-1, 64)[:, :32].reshape(-1))
+    out["d_read_probe_dense_plane_fixed_spans"] = summary(probe(0, plane), nbytes)
+    out["d_read_probe_dense_plane_ticketed"] = summary(probe(1, plane), nbytes)
+    del plane
+    for hv in args.head_variants:
+        out.update(measure_fold(log, off, dev, 0, args.reps, args.steps, f"_head_variant{hv}", {"head_variant": hv}))
+    out.update(measure_load_then_fold(log, off, dev, args.reps))
 
     a = out["a_read_probe_fixed_spans"]["ms_min"]
-    out["fold_share_of_read_probe"] = {k: a / v["ms_min"] for k, v in out.items() if k.startswith(("b_", "c_fold_alone_events", "c_fold_back"))}
+    out["fold_share_of_read_probe"] = {k: a / v["ms_min"] for k, v in out.items()
+                                       if k.startswith(("b_", "c_fold_alone_events", "c_fold_back")) and "head_variant" not in k}
+    d = out["d_read_probe_dense_plane_fixed_spans"]["ms_min"]
+    out["head_fold_share_of_dense_probe"] = {k: d / v["ms_min"] for k, v in out.items()
+                                             if k.startswith(("c_fold_alone_events", "c_fold_back")) and "head_variant" in k}
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, "fold_ceiling.json"), "w") as f:
         json.dump(out, f, indent=1)
@@ -97,7 +115,7 @@ def summary(ms: list, nbytes: int) -> dict:
     return {"ms_min": best, "ms_median": med, "gb_per_s_at_min": nbytes / best / 1e6, "gb_per_s_at_median": nbytes / med / 1e6}
 
 
-def measure_fold(log, off, dev: str, chunk_bytes: int, reps: int, steps: int, suffix: str) -> dict:
+def measure_fold(log, off, dev: str, chunk_bytes: int, reps: int, steps: int, suffix: str, options: dict) -> dict:
     """The fold alone (CUDA events around it, and stats().ms_fold) and `steps` back-to-back fold_async calls."""
     import torch
 
@@ -110,6 +128,8 @@ def measure_fold(log, off, dev: str, chunk_bytes: int, reps: int, steps: int, su
     eng.register_program(P.counter_program())
     if chunk_bytes:
         eng.set_option("run_chunk_bytes", chunk_bytes)
+    for k, v in options.items():
+        eng.set_option(k, v)
     eng.load_events(log, off)
     s = torch.cuda.ExternalStream(eng.stream_ptr(), device=dev)
     alone, kernel_ms = [], []
@@ -136,8 +156,38 @@ def measure_fold(log, off, dev: str, chunk_bytes: int, reps: int, steps: int, su
         e1.record(s)
         eng.wait()
         runs.append(e0.elapsed_time(e1) / steps)
-    out["c_fold_back_to_back" + suffix] = dict(summary(runs, nbytes), steps=steps)
+    out["c_fold_back_to_back" + suffix] = dict(summary(runs, nbytes), steps=steps, head_plane=int(eng.stats().head_plane))
     eng.close()
+    return out
+
+
+def measure_load_then_fold(log, off, dev: str, reps: int) -> dict:
+    """A borrowed log's load and one fold, host clock around both (the load synchronises first): with the head plane the
+    fold builds it (one pass reading the log, writing half its bytes), without it the fold reads the log."""
+    import time
+
+    import torch
+
+    from surge_b200 import ReplayEngine
+    from surge_b200 import programs as P
+
+    out = {}
+    for plane in (1, 0):
+        eng = ReplayEngine(0)
+        eng.register_program(P.counter_program())
+        eng.set_option("head_plane", plane)
+        ms, fold_ms = [], []
+        for _ in range(reps + 2):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            eng.load_events(log, off)
+            eng.set_initial_states(None)
+            eng.fold()
+            ms.append((time.perf_counter() - t0) * 1e3)
+            fold_ms.append(float(eng.stats().ms_fold))
+        out[f"e_load_then_fold_head_plane{plane}"] = dict(summary(ms[2:], log.numel()), fold_ms_min=min(fold_ms[2:]),
+                                                          head_plane=int(eng.stats().head_plane))
+        eng.close()
     return out
 
 

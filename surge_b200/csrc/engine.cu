@@ -77,6 +77,7 @@ struct PendingFold {
   uint64_t n_seg = 0, event_bytes = 0;
   const uint8_t* events = nullptr; const uint64_t* offsets = nullptr; const uint32_t* ids = nullptr;
   const void* counters = nullptr;
+  bool heads = false;     // the runs fold staged the head plane
 };
 }  // namespace
 
@@ -116,8 +117,8 @@ struct sgr_engine {
   bool row_ok = false;            // program is inside the transformer algebra
   RowProgram row_prog{};
   int row_max_grid = 0;
-  int run_max_grid = 0, run_max_grid_variant = -1;
-  int64_t opt_run_variant = 0;
+  int run_max_grid = 0, run_max_grid_variant = -2, run_max_grid_head = -2;  // -2: not yet sized
+  int64_t opt_run_variant = -1;   // -1: automatic (run variant 0, or the head plane); >= 0 forces that variant on the log
   DevBuf part_flags, part_data, redo_ids;
   DevBuf run_counters;            // 2 x 16 u64, ping-pong; the runs kernel zeroes the other block itself
   int run_counter_idx = 0;
@@ -127,6 +128,16 @@ struct sgr_engine {
   size_t part_flags_cap_seen = 0;
   bool offsets_aligned64 = false; // every segment offset == log_begin (mod 64)
   uint64_t log_begin = 0, log_end = 0, max_seg_bytes = 0;
+  // The head plane (fold_runs.cu): bytes 0..31 of every record of the loaded log, 32 bytes apart, for programs that read no
+  // record word past 7 (RowProgram::head_only). A derived copy: every load and program registration drops it, the first runs
+  // fold that can read it builds it from the log (a host load builds it behind its copy), and a borrowed log must not change
+  // while it is loaded. If its memory cannot be had, the fold reads the log.
+  DevBuf head_plane;
+  enum PlaneState { kPlaneNone, kPlaneValid, kPlaneNoMemory } plane_state = kPlaneNone;
+  int64_t opt_head_plane = 1;     // 0: the runs fold always reads the log
+  int64_t opt_head_variant = 0;
+  Stream side_stream;             // a host load builds the plane here, chunk by chunk behind the copy
+  Event ev_copied, ev_split;
   bool fold_pending = false;      // a fold was enqueued and not yet finished (it is `pending`)
   PendingFold pending;
   Event ev2, ev3;
@@ -333,6 +344,31 @@ int32_t launch_replay(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_
   return SGR_OK;
 }
 
+// The fold of the loaded log may stage the head plane: a runs fold of a head-only program, with no kernel or run variant
+// forced (those keep the fold on the log, so an A/B is one option away).
+bool plane_wanted(const sgr_engine* e) {
+  return e->row_ok && e->row_prog.head_only && e->opt_head_plane && e->opt_kernel == 0 && e->opt_run_variant < 0 &&
+         e->program.record_kind == SGR_REC_FIXED64 && e->offsets_aligned64 && e->log_end > e->log_begin;
+}
+
+// Build the head plane of the loaded log on the stream unless it is there. *ok: the plane is (or will be, in stream order)
+// valid; false when its memory cannot be had, once per load.
+int32_t ensure_plane(sgr_engine* e, bool* ok, bool* built) {
+  *ok = e->plane_state == sgr_engine::kPlaneValid; *built = false;
+  if (e->plane_state != sgr_engine::kPlaneNone) return SGR_OK;
+  const uint64_t n_rec = (e->log_end - e->log_begin) / 64;
+  if (e->head_plane.reserve(n_rec * 32) != cudaSuccess) {
+    (void)cudaGetLastError();   // a failed allocation is not sticky; the fold reads the log instead
+    e->plane_state = sgr_engine::kPlaneNoMemory;
+    return SGR_OK;
+  }
+  cudaError_t le = launch_build_heads(e->d_events + e->log_begin, (uint8_t*)e->head_plane.p, 0, n_rec, e->num_sms, e->stream);
+  if (le != cudaSuccess) return fail(e, SGR_ERR_CUDA, "head plane build: %s", cudaGetErrorString(le));
+  e->plane_state = sgr_engine::kPlaneValid;
+  *ok = *built = true;
+  return SGR_OK;
+}
+
 // Enqueue one fold on the engine's stream (no host synchronisation).
 int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_offsets, const uint32_t* d_ids,
                      uint64_t n_seg, bool use_prior, uint64_t event_bytes, bool aligned64, uint64_t log_begin, uint64_t log_end) {
@@ -347,6 +383,10 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
   if (use_rows && e->opt_kernel == 3 && (e->row_prog.user_words != 2 || e->row_prog.cls != 0 || e->row_prog.n_slots > 6 || e->row_prog.f64_mask))
     return fail(e, SGR_ERR_UNSUPPORTED, "the record-per-lane kernel takes 16-byte class-0 programs only");
   const bool runs = use_rows && e->opt_kernel != 3;
+  bool heads = false, plane_built = false;
+  if (runs && plane_wanted(e) && d_events == e->d_events && d_offsets == e->d_offsets && !d_ids) {
+    int32_t rc = ensure_plane(e, &heads, &plane_built); if (rc) return rc;
+  }
   unsigned long long* counters = (unsigned long long*)e->counters.p;
   if (runs) {
     if (!e->run_counters.p) {
@@ -358,10 +398,11 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
     CUDA_TRY(e, cudaMemsetAsync(e->counters.p, 0, 64, e->stream));
   }
   // A runs fold queued right behind a runs fold of the same log overlaps it (programmatic dependent launch): before its
-  // griddepcontrol.wait it reads only the log, the offsets and the program, which the fold before it does not write. Behind
-  // anything else (a group-by or decode kernel that writes the log, a copy) it is launched plainly.
-  const bool overlap = runs && e->fold_pending && e->pending.kernel == PendingFold::kRuns && e->pending.events == d_events &&
-                       e->pending.offsets == d_offsets && e->pending.ids == d_ids;
+  // griddepcontrol.wait it reads only the log (or its head plane), the offsets and the program, which the fold before it does
+  // not write. Behind anything else (a group-by or decode kernel that writes the log, a plane build, a copy) it is launched
+  // plainly.
+  const bool overlap = runs && !plane_built && e->fold_pending && e->pending.kernel == PendingFold::kRuns && e->pending.events == d_events &&
+                       e->pending.offsets == d_offsets && e->pending.ids == d_ids && e->pending.heads == heads;
   // an overlapping fold stamps its own start and end (counters[8], [9]): an event between two folds would keep the next
   // one from starting while this one drains. Every other fold is timed by CUDA events around its launch.
   if (!overlap) CUDA_TRY(e, cudaEventRecord(e->ev0, e->stream));
@@ -394,20 +435,23 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
     if (use_rows) {
       const bool v1 = e->opt_kernel == 3;
       const int rv = (int)e->opt_run_variant;
+      const int hv = heads ? (int)e->opt_head_variant : -1;
       if (v1 && !e->row_max_grid) e->row_max_grid = row_kernel_max_grid(e->num_sms, e->row_prog);
-      if (!v1 && e->run_max_grid_variant != rv) { e->run_max_grid = run_kernel_max_grid(e->num_sms, rv, e->row_prog); e->run_max_grid_variant = rv; }
+      if (!v1 && (e->run_max_grid_variant != rv || e->run_max_grid_head != hv)) {
+        e->run_max_grid = run_kernel_max_grid(e->num_sms, rv, hv, e->row_prog); e->run_max_grid_variant = rv; e->run_max_grid_head = hv;
+      }
       const int max_grid = v1 ? e->row_max_grid : e->run_max_grid;
       const int wpc = v1 ? kRowThreads / 32 : run_warps_per_cta();
-      const uint64_t step_bytes = v1 ? 2048 : (uint64_t)run_variant_step_bytes(rv, e->row_prog);
+      const uint64_t step_bytes = v1 ? 2048 : (uint64_t)run_variant_step_bytes(rv, hv, e->row_prog);
       const uint64_t steps = (log_end - log_begin + step_bytes - 1) / step_bytes;
       // the runs kernel publishes a look-back partial per chunk of chunk_steps steps, the rows kernel one per warp; a
       // small log is cut into smaller chunks, so that every resident warp gets one
-      const uint64_t chunk_steps = v1 ? 1 : run_variant_chunk_steps(rv, e->row_prog, (uint64_t)e->opt_run_chunk_bytes, steps, (uint64_t)max_grid * wpc);
+      const uint64_t chunk_steps = v1 ? 1 : run_variant_chunk_steps(rv, hv, e->row_prog, (uint64_t)e->opt_run_chunk_bytes, steps, (uint64_t)max_grid * wpc);
       const uint64_t n_chunks = (steps + chunk_steps - 1) / chunk_steps;
       const uint64_t n_parts = v1 ? (uint64_t)max_grid * wpc : n_chunks;
       int32_t rc = begin_lookback(e, n_parts, e->row_prog.user_words + 2); if (rc) return rc;
       RowArgs r{};
-      r.events = d_events; r.seg_offsets = d_offsets; r.seg_ids = d_ids; r.n_seg = n_seg;
+      r.events = d_events; r.heads = heads ? (const uint8_t*)e->head_plane.p : nullptr; r.seg_offsets = d_offsets; r.seg_ids = d_ids; r.n_seg = n_seg;
       r.log_begin = log_begin; r.log_end = log_end;
       r.states_in = states_in; r.states_out = (uint8_t*)e->states.p;
       r.counters = counters;
@@ -418,7 +462,7 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
       uint64_t want = (n_chunks + wpc - 1) / wpc;
       if (want == 0) want = 1;  // all segments empty: one CTA still writes every (None) state
       const int grid = (int)(want < (uint64_t)max_grid ? want : (uint64_t)max_grid);
-      cudaError_t le = v1 ? launch_fold_rows(r, e->row_prog, grid, e->stream) : launch_fold_runs(r, e->row_prog, rv, grid, overlap, e->stream);
+      cudaError_t le = v1 ? launch_fold_rows(r, e->row_prog, grid, e->stream) : launch_fold_runs(r, e->row_prog, rv, hv, grid, overlap, e->stream);
       if (le != cudaSuccess) return fail(e, SGR_ERR_CUDA, "fold launch: %s", cudaGetErrorString(le));
       if (runs) {
         e->run_counter_idx ^= 1;  // the kernel replays throwing segments itself and cleans the other block
@@ -444,8 +488,9 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
   }
   if (!overlap) CUDA_TRY(e, cudaEventRecord(e->ev1, e->stream));
   e->fold_pending = true;
-  e->pending = PendingFold{kernel, overlap, use_prior, n_seg, event_bytes, d_events, d_offsets, d_ids, counters};
+  e->pending = PendingFold{kernel, overlap, use_prior, n_seg, event_bytes, d_events, d_offsets, d_ids, counters, heads};
   e->stats.fold_launches = launches;
+  e->stats.head_plane = heads ? 1u : 0u;
   return SGR_OK;
 }
 
@@ -560,7 +605,8 @@ int32_t sgr_register_program(sgr_engine* e, const sgr_fold_program* prog) {
   e->row_ok = build_row_program(d, &e->row_prog);
   e->bulk_ok = e->row_ok && prog->record_kind == SGR_REC_FIXED64 && bulk_layout_for(e->row_prog, &e->bulk_lay);
   e->bulk_scratch_slots = 0;
-  e->row_max_grid = 0; e->run_max_grid_variant = -1;
+  e->row_max_grid = 0; e->run_max_grid_variant = -2;
+  e->plane_state = sgr_engine::kPlaneNone;
   e->states_valid = false; e->states_n = 0;
   e->writer.n = 0;   // its offsets belonged to the old program
   mark_dirty(e);
@@ -591,6 +637,7 @@ static int32_t after_load(sgr_engine* e, const uint8_t* d_events, const uint64_t
   // the load; a longer record (header included, before padding) is a malformed event in every kernel, never mis-parsed
   e->max_record_bytes = e->program.record_kind == SGR_REC_VAR16 ? (uint32_t)e->opt_max_record_bytes : 64u;
   e->offsets_aligned64 = false; e->log_begin = 0; e->log_end = nbytes;
+  e->plane_state = sgr_engine::kPlaneNone;
   if (e->program.record_kind == SGR_REC_FIXED64) {
     cudaError_t ce = inspect_offsets(d_offsets, n_agg, (unsigned long long*)e->counters.p, e->stream, &e->offsets_aligned64,
                                      &e->log_begin, &e->log_end, &e->max_seg_bytes);
@@ -612,10 +659,47 @@ int32_t sgr_load_events(sgr_engine* e, const void* events, uint64_t nbytes, cons
   int32_t rc = before_load(e); if (rc) return rc;
   CUDA_TRY(e, e->own_events.reserve(nbytes));
   CUDA_TRY(e, e->own_offsets.reserve((n_agg + 1) * 8));
-  rc = upload_timed(e, e->ev0, e->ev1, {{e->own_events.p, events, nbytes}, {e->own_offsets.p, seg_offsets, (n_agg + 1) * 8}});
-  if (rc) return rc;
+  const uint64_t begin = seg_offsets[0], end = seg_offsets[n_agg];
+  bool aligned64 = true;
+  for (uint64_t i = 1; i <= n_agg && aligned64; ++i) aligned64 = (seg_offsets[i] - begin) % 64 == 0;
+  // a head-only program's plane is built on a second stream, each chunk right behind its copy, so it costs no time of its own
+  // (the copy is PCIe-bound, the split an HBM pass over the chunk)
+  bool split = e->row_ok && e->row_prog.head_only && e->opt_head_plane && e->opt_kernel == 0 && e->opt_run_variant < 0 &&
+               e->program.record_kind == SGR_REC_FIXED64 && e->row_prog.user_words != 14 && aligned64 && end > begin;
+  if (split && e->head_plane.reserve((end - begin) / 2) != cudaSuccess) { (void)cudaGetLastError(); split = false; }
+  if (!split) {
+    rc = upload_timed(e, e->ev0, e->ev1, {{e->own_events.p, events, nbytes}, {e->own_offsets.p, seg_offsets, (n_agg + 1) * 8}});
+    if (rc) return rc;
+  } else {
+    if (!e->side_stream) CUDA_TRY(e, cudaStreamCreateWithFlags(e->side_stream.put(), cudaStreamNonBlocking));
+    if (!e->ev_copied) CUDA_TRY(e, cudaEventCreateWithFlags(e->ev_copied.put(), cudaEventDisableTiming));
+    if (!e->ev_split) CUDA_TRY(e, cudaEventCreateWithFlags(e->ev_split.put(), cudaEventDisableTiming));
+    uint8_t* dst = (uint8_t*)e->own_events.p;
+    const uint8_t* src = (const uint8_t*)events;
+    constexpr uint64_t kChunkRecs = 1ull << 20;  // 64 MiB of log per copy
+    const uint64_t n_rec = (end - begin) / 64;
+    CUDA_TRY(e, cudaEventRecord(e->ev0, e->stream));
+    CUDA_TRY(e, cudaMemcpyAsync(e->own_offsets.p, seg_offsets, (n_agg + 1) * 8, cudaMemcpyHostToDevice, e->stream));
+    if (begin) CUDA_TRY(e, cudaMemcpyAsync(dst, src, begin, cudaMemcpyHostToDevice, e->stream));
+    for (uint64_t r0 = 0; r0 < n_rec; r0 += kChunkRecs) {
+      const uint64_t r1 = r0 + kChunkRecs < n_rec ? r0 + kChunkRecs : n_rec;
+      CUDA_TRY(e, cudaMemcpyAsync(dst + begin + r0 * 64, src + begin + r0 * 64, (r1 - r0) * 64, cudaMemcpyHostToDevice, e->stream));
+      CUDA_TRY(e, cudaEventRecord(e->ev_copied, e->stream));
+      CUDA_TRY(e, cudaStreamWaitEvent(e->side_stream, e->ev_copied, 0));   // waits for this record of the event
+      cudaError_t le = launch_build_heads(dst + begin, (uint8_t*)e->head_plane.p, r0, r1, e->num_sms, e->side_stream);
+      if (le != cudaSuccess) return fail(e, SGR_ERR_CUDA, "head plane build: %s", cudaGetErrorString(le));
+    }
+    if (nbytes > end) CUDA_TRY(e, cudaMemcpyAsync(dst + end, src + end, nbytes - end, cudaMemcpyHostToDevice, e->stream));
+    CUDA_TRY(e, cudaEventRecord(e->ev_split, e->side_stream));
+    CUDA_TRY(e, cudaStreamWaitEvent(e->stream, e->ev_split, 0));
+    CUDA_TRY(e, cudaEventRecord(e->ev1, e->stream));
+    CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+    CUDA_TRY(e, cudaEventElapsedTime(&e->stats.ms_h2d, e->ev0, e->ev1));
+  }
   e->stats.ms_group = 0;
-  return after_load(e, (const uint8_t*)e->own_events.p, (const uint64_t*)e->own_offsets.p, nbytes, n_agg);
+  rc = after_load(e, (const uint8_t*)e->own_events.p, (const uint64_t*)e->own_offsets.p, nbytes, n_agg);
+  if (rc == SGR_OK && split && e->offsets_aligned64 && e->log_begin == begin && e->log_end == end) e->plane_state = sgr_engine::kPlaneValid;
+  return rc;
 }
 
 int32_t sgr_load_events_device(sgr_engine* e, const void* d_events, uint64_t nbytes, const uint64_t* d_seg_offsets, uint64_t n_agg) {
@@ -2099,6 +2183,11 @@ int32_t sgr_set_option(sgr_engine* e, const char* name, int64_t value) {
   }
   // test aid: the look-back epoch the next record-parallel fold moves on from (a value near 2^32 makes a few folds wrap it)
   if (!strcmp(name, "lookback_epoch")) { e->epoch = (uint32_t)value; return SGR_OK; }
+  if (!strcmp(name, "head_plane")) { e->opt_head_plane = value ? 1 : 0; return SGR_OK; }
+  if (!strcmp(name, "head_variant")) {
+    if (value < 0 || value >= head_variant_count()) return fail(e, SGR_ERR_INVALID, "head_variant out of range");
+    e->opt_head_variant = value; return SGR_OK;
+  }
   if (!strcmp(name, "run_chunk_bytes")) {
     if (value < 2048 || value > (1ll << 30)) return fail(e, SGR_ERR_INVALID, "run_chunk_bytes must be in [2048, 2^30]");
     e->opt_run_chunk_bytes = value; return SGR_OK;

@@ -455,6 +455,9 @@ bool build_row_program(const DevProgram& dp, RowProgram* out) {
            ((r.exists_rule == SGR_CREATE || r.n_ops > 0) ? kRuleNew : 0u);
     for (uint32_t w = 0; w < dp.user_words; ++w) e[1 + w] = spec_encode(mode[w], neg[w], slot[w]);
   }
+  // slot 0 is the type word; the fold, its look-back and its replay read no record word but the slots
+  out->head_only = 1;
+  for (uint32_t q = 0; q < out->n_slots; ++q) if (out->slot_word[q] >= 8) out->head_only = 0;
   return true;
 }
 

@@ -174,9 +174,10 @@ __device__ __forceinline__ void finish_empty(const RowArgs& a, uint32_t seg) {
   }
 }
 
-template <int R, int NSTAGE>
+// REC: bytes staged per record, 64 (the log itself) or 32 (the head plane: each record's bytes 0..31)
+template <int R, int NSTAGE, int REC = 64>
 __host__ __device__ constexpr int warp_smem_bytes() {
-  return NSTAGE * 2048 * R   // staged steps
+  return NSTAGE * 32 * REC * R  // staged steps
          + 2 * 32 * R * 4    // segment ids at head positions: starting segment, ending segment
          + 32 * 4;           // head bitmap (R words used) + pad
 }
@@ -209,11 +210,16 @@ __device__ __forceinline__ Xf<W> look_back_chunks(const RowArgs& a, uint64_t c) 
 
 // DIRECT: programs with many source words read each state word's source straight from the staged record instead of
 // pre-fetching NS slots and selecting (NS is then unused)
-template <int W, int R, int NSTAGE, int NS, int MINB, bool DIRECT, int CLS>
+// REC == 32: the records are staged from the head plane (RowArgs::heads) rather than the log; offsets still count log bytes.
+template <int W, int R, int NSTAGE, int NS, int MINB, bool DIRECT, int CLS, int REC = 64>
 __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __grid_constant__ RowArgs a, const __grid_constant__ RowProgram pg) {
   static_assert(R % 2 == 0 && 8 % R == 0, "R in {2,4,8}");
-  constexpr int STEP_BYTES = 2048 * R;
+  static_assert(REC == 64 || (REC == 32 && R >= 4), "a lane's run starts on a 128-byte line: R >= 128 / REC");
+  constexpr int STEP_BYTES = 2048 * R;          // log bytes per step
   constexpr int STEP_RECS = 32 * R;
+  constexpr int STAGE_BYTES = STEP_RECS * REC;  // staged bytes per step
+  constexpr int RPL = 128 / REC;                // records per 128-byte shared-memory line
+  constexpr int CPR = REC / 16;                 // 16-byte chunks per record
   extern __shared__ __align__(128) uint8_t smem_raw[];
   __shared__ __align__(16) uint32_t tab[16 * kTabStride];
   // the next fold may be scheduled now: it waits for this grid to complete before it touches anything this one writes
@@ -224,9 +230,9 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
   __syncthreads();
 
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint8_t* wsm = smem_raw + (size_t)warp * warp_smem_bytes<R, NSTAGE>();
+  uint8_t* wsm = smem_raw + (size_t)warp * warp_smem_bytes<R, NSTAGE, REC>();
   const uint32_t stage0 = smem_u32(wsm);
-  uint32_t* hs_start = reinterpret_cast<uint32_t*>(wsm + NSTAGE * STEP_BYTES);  // segment starting at a head
+  uint32_t* hs_start = reinterpret_cast<uint32_t*>(wsm + NSTAGE * STAGE_BYTES);  // segment starting at a head
   uint32_t* hs_end = hs_start + STEP_RECS;                                       // segment ending at a head (0xffffffff: none)
   uint32_t* hmask = hs_end + STEP_RECS;                                          // head bitmap, R words
 
@@ -262,25 +268,27 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
   };
 
   // ---- staging: lane l, copy q of a step moves the 16-byte chunk g = q*32 + l (source order) to its
-  //      swizzled place: record j = g>>2, chunk c = g&3 -> line j>>1, position (4*(j&1)+c) ^ ((j/R)&7)
-  const uint8_t* src_lane = a.events + base + (uint64_t)lane * 16;
-  const uint32_t low_pos = (uint32_t)(4 * ((lane >> 2) & 1) + (lane & 3));
-  const uint32_t lane_jr = (uint32_t)(lane >> 2) / R;
-  uint32_t dst_q[4 * R];  // smem offset (within a stage) of copy q
+  //      swizzled place: record j = g/CPR, chunk c = g%CPR -> line j/RPL, position (CPR*(j%RPL)+c) ^ ((j/R)&7).
+  //      A 512-byte copy holds whole lines, so CPR*(j%RPL)+c == l&7 and the line is q*4 + l/8.
+  constexpr int QPS = STAGE_BYTES / 512;  // copies per step
+  const uint8_t* src_lane = (REC == 64 ? a.events + base : a.heads) + (uint64_t)lane * 16;
+  const uint64_t total_staged = total_bytes / 64 * REC;
+  const uint32_t lane_jr = (uint32_t)(lane / CPR) / R;
+  uint32_t dst_q[QPS];  // smem offset (within a stage) of copy q
 #pragma unroll
-  for (int q = 0; q < 4 * R; ++q)
-    dst_q[q] = (uint32_t)q * 512u + (uint32_t)(lane >> 3) * 128u + ((low_pos ^ (((uint32_t)(q * 8) / R + lane_jr) & 7u)) << 4);
+  for (int q = 0; q < QPS; ++q)
+    dst_q[q] = (uint32_t)q * 512u + (uint32_t)(lane >> 3) * 128u + (((uint32_t)(lane & 7) ^ (((uint32_t)(q * (512 / REC)) / R + lane_jr) & 7u)) << 4);
   auto issue_step = [&](uint64_t s, int stage) {
-    const uint64_t sbyte = s * (uint64_t)STEP_BYTES;
+    const uint64_t sbyte = s * (uint64_t)STAGE_BYTES;
     const uint8_t* src = src_lane + sbyte;
-    const uint32_t dst = stage0 + (uint32_t)stage * STEP_BYTES;
-    if (sbyte + STEP_BYTES <= total_bytes) {  // uniform: the whole step lies inside the log
+    const uint32_t dst = stage0 + (uint32_t)stage * STAGE_BYTES;
+    if (sbyte + STAGE_BYTES <= total_staged) {  // uniform: the whole step lies inside the log
 #pragma unroll
-      for (int q = 0; q < 4 * R; ++q) cp_async16(dst + dst_q[q], src + q * 512);
+      for (int q = 0; q < QPS; ++q) cp_async16(dst + dst_q[q], src + q * 512);
     } else {
 #pragma unroll
-      for (int q = 0; q < 4 * R; ++q)
-        if (sbyte + (uint64_t)q * 512 + (uint64_t)lane * 16 < total_bytes) cp_async16(dst + dst_q[q], src + q * 512);
+      for (int q = 0; q < QPS; ++q)
+        if (sbyte + (uint64_t)q * 512 + (uint64_t)lane * 16 < total_staged) cp_async16(dst + dst_q[q], src + q * 512);
     }
   };
   // ---- issue side: steps are staged in the warp's own order, the current chunk's and then the next one's, so the pipeline
@@ -320,14 +328,15 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
   }
   uint64_t kc = (chunk != kNone && chunk != 0) ? first_boundary(base + chunk * cs * STEP_BYTES) : 0;
 
-  // where lane i finds word (c,k) of a record of parity par: byte (((4*par + c) ^ (i&7)) << 4) + 4k of its 128-byte line
+  // where lane i finds word (c,k) of the record at place rl of its line: byte (((CPR*rl + c) ^ (i&7)) << 4) + 4k of the line
+  // (rl == t % RPL for the t-th record of the run: a run starts on a line)
   constexpr int NSOFF = DIRECT ? 1 : NS;
-  uint32_t soff[2][NSOFF];
+  uint32_t soff[RPL][NSOFF];
 #pragma unroll
   for (int s = 0; s < NSOFF; ++s) {
     const uint32_t c = pg.slot_word[s] >> 2, k = pg.slot_word[s] & 3u;
-    soff[0][s] = ((c ^ (uint32_t)(lane & 7)) << 4) + (k << 2);
-    soff[1][s] = (((4u + c) ^ (uint32_t)(lane & 7)) << 4) + (k << 2);
+#pragma unroll
+    for (int rl = 0; rl < RPL; ++rl) soff[rl][s] = ((((uint32_t)(CPR * rl) + c) ^ (uint32_t)(lane & 7)) << 4) + (k << 2);
   }
   // boundary window: lane j holds off[kc+j] and off[kc+j+1]; reloaded right after boundaries are consumed,
   // so the values a step needs were requested one step earlier
@@ -411,7 +420,7 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
       __syncwarp();
 
       // ---- lane run: R consecutive records, left to right -------------------------------------------------
-      const uint32_t sbase = stage0 + (uint32_t)stage * STEP_BYTES;
+      const uint32_t sbase = stage0 + (uint32_t)stage * STAGE_BYTES;
       uint32_t hbits;
       if (R >= 32) hbits = hmask[lane];
       else hbits = (hmask[(lane * R) >> 5] >> ((lane * R) & 31)) & ((R >= 32) ? 0xffffffffu : ((1u << R) - 1u));
@@ -429,14 +438,14 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
           cur = identity<W>();
         }
         if (p < nvalid) {
-          const uint32_t rec = sbase + (uint32_t)(p >> 1) * 128u;
-          const uint32_t lane7 = (uint32_t)(lane & 7), par4 = (uint32_t)(t & 1) * 4u;  // p&1 == t&1: R is even
+          const uint32_t rec = sbase + (uint32_t)(p / RPL) * 128u;
+          const uint32_t lane7 = (uint32_t)(lane & 7), parc = (uint32_t)(t % RPL) * CPR;  // p%RPL == t%RPL: RPL divides R
           uint32_t sv[DIRECT ? 1 : NS];
           if (DIRECT) {
-            sv[0] = lds32(rec + soff[t & 1][0]);
+            sv[0] = lds32(rec + soff[t % RPL][0]);
           } else {
 #pragma unroll
-            for (int s = 0; s < NS; ++s) sv[s] = lds32(rec + soff[t & 1][s]);
+            for (int s = 0; s < NS; ++s) sv[s] = lds32(rec + soff[t % RPL][s]);
           }
           const uint32_t type = sv[0];
           uint4 e0 = make_uint4(0, 0, 0, 0);
@@ -458,7 +467,7 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
               uint32_t val = 0;
               if (DIRECT) {
                 const uint32_t sl = spec_slot(spec[w]);
-                if (sl) { const uint32_t sw = pg.slot_word[sl]; val = lds32(rec + ((((par4 + (sw >> 2)) ^ lane7) << 4) | ((sw & 3u) << 2))); }
+                if (sl) { const uint32_t sw = pg.slot_word[sl]; val = lds32(rec + ((((parc + (sw >> 2)) ^ lane7) << 4) | ((sw & 3u) << 2))); }
               } else {
 #pragma unroll
                 for (int s = 1; s < NS; ++s) val = (spec_slot(spec[w]) == (uint32_t)s) ? sv[s] : val;
@@ -666,58 +675,71 @@ const RunVariant kRunVariants[] = {
     RUN_VARIANT(4, 2, 3), RUN_VARIANT(4, 1, 5), RUN_VARIANT(2, 2, 5), RUN_VARIANT(2, 1, 5), RUN_VARIANT(4, 3, 2), RUN_VARIANT(8, 1, 3), RUN_VARIANT(2, 3, 4),
 };
 constexpr int kNumRunVariants = sizeof(kRunVariants) / sizeof(kRunVariants[0]);
+// the same staging from the head plane (32 bytes per record): a step stages half the bytes, so deeper pipelines fit. The
+// first is the default: the fastest on the configs[1] log (scripts/fold_ceiling.py --head-variants, DESIGN.md section 4)
+#define HEAD_VARIANT(R, ST, MINB) {{fold_runs_kernel<2, R, ST, 2, MINB, false, 0, 32>, fold_runs_kernel<2, R, ST, 3, MINB, false, 0, 32>, fold_runs_kernel<2, R, ST, 6, MINB, false, 0, 32>}, R, ST, "heads W2 R" #R " st" #ST}
+const RunVariant kHeadVariants[] = {
+    HEAD_VARIANT(8, 2, 3), HEAD_VARIANT(4, 3, 4), HEAD_VARIANT(4, 2, 4), HEAD_VARIANT(4, 4, 3), HEAD_VARIANT(8, 3, 2),
+};
+constexpr int kNumHeadVariants = sizeof(kHeadVariants) / sizeof(kHeadVariants[0]);
 // wider states / many source words: one configuration each (R = 4, 2 stages, direct word reads)
 constexpr int kWideR = 4, kWideStages = 2;
 
-size_t variant_smem(int v, const RowProgram& prog) {
-  const bool wide = prog.user_words != 2 || prog.n_slots > 6 || prog.cls != 0;
-  const int r = wide ? kWideR : kRunVariants[v].r, ns = wide ? kWideStages : kRunVariants[v].nstage;
-  return (size_t)kRunWarps * ((size_t)ns * 2048 * r + 2 * 32 * r * 4 + 32 * 4);
+bool is_wide(const RowProgram& prog) { return prog.user_words != 2 || prog.n_slots > 6 || prog.cls != 0; }
+// head < 0: the row layout, run variant v; head >= 0: the head plane, head variant `head`
+const RunVariant& pick_variant(int v, int head) {
+  if (head >= 0) return kHeadVariants[head < kNumHeadVariants ? head : 0];
+  return kRunVariants[(v >= 0 && v < kNumRunVariants) ? v : 0];
 }
-RunKernel variant_kernel(int v, const RowProgram& prog) {
-  if (prog.user_words == 14) return fold_runs_kernel<14, kWideR, kWideStages, 1, 1, true, 1>;
-  if (prog.user_words == 6) return fold_runs_kernel<6, kWideR, kWideStages, 1, 2, true, 1>;
-  if (prog.n_slots > 6 || prog.cls != 0) return fold_runs_kernel<2, kWideR, kWideStages, 1, 3, true, 1>;
-  return kRunVariants[v].k[prog.n_slots <= 2 ? 0 : (prog.n_slots <= 3 ? 1 : 2)];
+int variant_r(int v, int head, const RowProgram& prog) { return is_wide(prog) ? kWideR : pick_variant(v, head).r; }
+int variant_nstage(int v, int head, const RowProgram& prog) { return is_wide(prog) ? kWideStages : pick_variant(v, head).nstage; }
+size_t variant_smem(int v, int head, const RowProgram& prog) {
+  const size_t r = (size_t)variant_r(v, head, prog), ns = (size_t)variant_nstage(v, head, prog), rec = head >= 0 ? 32 : 64;
+  return (size_t)kRunWarps * (ns * 32 * rec * r + 2 * 32 * r * 4 + 32 * 4);
+}
+RunKernel variant_kernel(int v, int head, const RowProgram& prog) {
+  if (head >= 0) {
+    if (prog.user_words == 14) return fold_runs_kernel<14, kWideR, kWideStages, 1, 1, true, 1, 32>;
+    if (prog.user_words == 6) return fold_runs_kernel<6, kWideR, kWideStages, 1, 2, true, 1, 32>;
+    if (is_wide(prog)) return fold_runs_kernel<2, kWideR, kWideStages, 1, 3, true, 1, 32>;
+  } else {
+    if (prog.user_words == 14) return fold_runs_kernel<14, kWideR, kWideStages, 1, 1, true, 1>;
+    if (prog.user_words == 6) return fold_runs_kernel<6, kWideR, kWideStages, 1, 2, true, 1>;
+    if (is_wide(prog)) return fold_runs_kernel<2, kWideR, kWideStages, 1, 3, true, 1>;
+  }
+  return pick_variant(v, head).k[prog.n_slots <= 2 ? 0 : (prog.n_slots <= 3 ? 1 : 2)];
 }
 
 }  // namespace
 
 int run_variant_count() { return kNumRunVariants; }
 const char* run_variant_name(int v) { return (v >= 0 && v < kNumRunVariants) ? kRunVariants[v].name : "?"; }
+int head_variant_count() { return kNumHeadVariants; }
 
-int run_kernel_max_grid(int num_sms, int variant, const RowProgram& prog) {
-  if (variant < 0 || variant >= kNumRunVariants) variant = 0;
-  const size_t smem = variant_smem(variant, prog);
-  RunKernel k = variant_kernel(variant, prog);
+int run_kernel_max_grid(int num_sms, int variant, int head, const RowProgram& prog) {
+  const size_t smem = variant_smem(variant, head, prog);
+  RunKernel k = variant_kernel(variant, head, prog);
   cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   int per_sm = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kRunThreads, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
   return per_sm * num_sms;
 }
 
-int run_variant_step_bytes(int variant, const RowProgram& prog) {
-  if (variant < 0 || variant >= kNumRunVariants) variant = 0;
-  const bool wide = prog.user_words != 2 || prog.n_slots > 6 || prog.cls != 0;
-  return 2048 * (wide ? kWideR : kRunVariants[variant].r);
-}
+int run_variant_step_bytes(int variant, int head, const RowProgram& prog) { return 2048 * variant_r(variant, head, prog); }
 int run_warps_per_cta() { return kRunWarps; }
 
-uint64_t run_variant_chunk_steps(int variant, const RowProgram& prog, uint64_t chunk_bytes, uint64_t steps, uint64_t n_warps) {
-  if (variant < 0 || variant >= kNumRunVariants) variant = 0;
-  const bool wide = prog.user_words != 2 || prog.n_slots > 6 || prog.cls != 0;
-  const uint64_t ns = (uint64_t)(wide ? kWideStages : kRunVariants[variant].nstage);
+uint64_t run_variant_chunk_steps(int variant, int head, const RowProgram& prog, uint64_t chunk_bytes, uint64_t steps, uint64_t n_warps) {
+  const uint64_t ns = (uint64_t)variant_nstage(variant, head, prog);
   const uint64_t lo = ns > 1 ? ns - 1 : 1;  // what is staged ahead stays inside the next chunk
-  uint64_t hi = chunk_bytes / (uint64_t)run_variant_step_bytes(variant, prog);
+  uint64_t hi = chunk_bytes / (uint64_t)run_variant_step_bytes(variant, head, prog);
   if (hi < lo) hi = lo;
   const uint64_t fair = n_warps ? steps / n_warps : hi;  // a chunk for every warp on a small log
   return fair < lo ? lo : (fair > hi ? hi : fair);
 }
 
-cudaError_t launch_fold_runs(const RowArgs& args, const RowProgram& prog, int variant, int grid, bool overlap, cudaStream_t stream) {
-  if (variant < 0 || variant >= kNumRunVariants) variant = 0;
-  const size_t smem = variant_smem(variant, prog);
-  RunKernel k = variant_kernel(variant, prog);  // its smem attribute was set by run_kernel_max_grid
+cudaError_t launch_fold_runs(const RowArgs& args, const RowProgram& prog, int variant, int head, int grid, bool overlap, cudaStream_t stream) {
+  const size_t smem = variant_smem(variant, head, prog);
+  RunKernel k = variant_kernel(variant, head, prog);  // its smem attribute was set by run_kernel_max_grid
   // overlap: the launch may begin while the fold before it drains (programmatic dependent launch); the kernel waits on the
   // device for its predecessor before it touches anything that predecessor writes
   cudaLaunchAttribute attr[1];
@@ -727,6 +749,26 @@ cudaError_t launch_fold_runs(const RowArgs& args, const RowProgram& prog, int va
   cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(kRunThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
   cfg.attrs = attr; cfg.numAttrs = overlap ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, k, args, prog);
+}
+
+// ---- the head plane: bytes 0..31 of every record of the log, densely --------------------------------------------------
+// One warp moves 16 records per pass: lane l reads the 16-byte chunk l&1 of record l/2, so a warp's reads are the 32-byte
+// halves of 16 consecutive records (sixteen 64-byte blocks, the first of each read) and its 512-byte write is contiguous.
+__global__ void __launch_bounds__(256) build_heads_kernel(const uint8_t* log, uint8_t* heads, uint64_t rec0, uint64_t rec1) {
+  const uint64_t n_chunks = (rec1 - rec0) * 2;
+  for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n_chunks; g += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t r = rec0 + (g >> 1), c = g & 1;
+    const uint4 v = __ldcs(reinterpret_cast<const uint4*>(log + r * 64) + c);
+    reinterpret_cast<uint4*>(heads + r * 32)[c] = v;
+  }
+}
+
+cudaError_t launch_build_heads(const uint8_t* log, uint8_t* heads, uint64_t rec0, uint64_t rec1, int num_sms, cudaStream_t stream) {
+  if (rec1 <= rec0) return cudaSuccess;
+  const uint64_t want = ((rec1 - rec0) * 2 + 255) / 256;
+  const uint64_t cap = (uint64_t)num_sms * 16;
+  build_heads_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, stream>>>(log, heads, rec0, rec1);
+  return cudaGetLastError();
 }
 
 namespace {

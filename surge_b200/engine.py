@@ -140,7 +140,8 @@ class ReplayEngine:
 
     # -- loads
     def load_events(self, events, seg_offsets) -> None:
-        """CSR event log. numpy -> copied to HBM; CUDA tensors -> borrowed."""
+        """CSR event log. numpy -> copied to HBM; CUDA tensors -> borrowed, and must not be modified while loaded: the engine
+        may fold from a copy of their record heads (include/sgr.h, head plane). Load again to fold changed records."""
         if _is_cuda_tensor(events):
             assert _is_cuda_tensor(seg_offsets)
             ev, nbytes = self._lend(events, seg_offsets)
