@@ -532,10 +532,19 @@ const char* sgr_ingest_last_error(const sgr_ingest* g);
  * SGR_VALUE_PROTOBUF_EVENT: the value is the multilanguage module's protobuf `Event { string aggregateId = 1; bytes payload = 2; }`
  * (modules/multilanguage-protocol/src/main/protobuf/multilanguage-protocol.proto:17-20, written by
  * modules/multilanguage/src/main/scala/com/ukg/surge/multilanguage/GenericSurgeCommandBusinessLogic.scala:30-33) and the packed
- * event is its payload. The framing is pinned against the protobuf runtime in tests/test_ingest_cpu.py. */
+ * event is its payload. The framing is pinned against the protobuf runtime in tests/test_ingest_cpu.py.
+ * SGR_VALUE_JSON: the value is a flat JSON object (below).
+ * SGR_VALUE_PROTOBUF_JSON: what the multilanguage gateway writes for a business app that serializes its events as JSON (every
+ * sample app of the reference does): the protobuf Event as under SGR_VALUE_PROTOBUF_EVENT, whose payload is a flat JSON object
+ * read through the registered member table as under SGR_VALUE_JSON. The message is unwrapped first (the last field 2 of wire
+ * type 2 wins, unknown fields are skipped, a malformed message is "value is not a protobuf Event"), then the payload is packed
+ * ("JSON event: <reason>"; a message without field 2 has an empty payload: "JSON event: the value is not a JSON object").
+ * Event.aggregateId (field 1) is not read and not compared with the record key: the key is the id, as under the other
+ * framings. SGR_VALUE_JSON and SGR_VALUE_PROTOBUF_JSON need a JSON packer first, else SGR_ERR_INVALID. */
 #define SGR_VALUE_PACKED          0
 #define SGR_VALUE_PROTOBUF_EVENT  1
 #define SGR_VALUE_JSON            2
+#define SGR_VALUE_PROTOBUF_JSON   3
 int32_t sgr_ingest_set_value_framing(sgr_ingest* g, int32_t framing);
 
 /* SGR_VALUE_JSON: the value is a flat JSON object as the reference's sample models write their events with play-json,
@@ -608,10 +617,11 @@ int32_t sgr_append_keys(sgr_engine* e, const void* owner, const uint8_t* keys, c
  * read_committed bookkeeping (control batches, aborted transactions, partition positions). csrc/ingest.cpp is its checker
  * (tests/test_gpu_dingest.py: identical states, ids, offsets and statistics on the same bytes).
  *   - value framing: as the host ingest's (sgr_dingest_set_value_framing, sgr_dingest_set_json_packer): the packed event, the
- *     protobuf Event's payload or a flat JSON object through a registered member table, converted inside the parse kernel with
+ *     protobuf Event's payload, a flat JSON object through a registered member table, or the protobuf Event whose payload is
+ *     such a JSON object (SGR_VALUE_PROTOBUF_JSON), converted inside the parse kernel with
  *     the host decoder's results and refusal texts ("offset N, record r: JSON event: unknown event class"). Both settings survive
  *     sgr_dingest_reset and are refused with SGR_ERR_STATE between a submit and its fold. JSON compresses better than packed
- *     values: under protobuf / JSON framing a poll that needed the exact-layout repeat raises the arena claim for the next polls
+ *     values: under any framing but SGR_VALUE_PACKED a poll that needed the exact-layout repeat raises the arena claim for the next polls
  *     (to the power of two at or above the ratio it showed, at most 16x the wire bytes);
  *   - every fixed-record program is accepted. Dropped records (flush markers, duplicates, null values without a tombstone type)
  *     stay in place as holes. Sort-free programs skip the holes in the atomic fold; the others group the live records on the
@@ -653,7 +663,7 @@ int32_t sgr_dingest_destroy(sgr_dingest* g);
 const char* sgr_dingest_last_error(const sgr_dingest* g);
 int32_t sgr_dingest_set_null_value_type(sgr_dingest* g, int32_t event_type);
 /* as sgr_ingest_set_value_framing / sgr_ingest_set_json_packer, validated alike; SGR_ERR_STATE while a poll is pending */
-int32_t sgr_dingest_set_value_framing(sgr_dingest* g, int32_t framing);          /* SGR_VALUE_PACKED | _PROTOBUF_EVENT | _JSON */
+int32_t sgr_dingest_set_value_framing(sgr_dingest* g, int32_t framing);   /* SGR_VALUE_PACKED | _PROTOBUF_EVENT | _JSON | _PROTOBUF_JSON */
 int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, const sgr_json_event* events,
                                     uint32_t n_events, int32_t unknown_type);
 /* Decode a compacted STATE topic instead of an events topic (on != 0; 0 goes back to events). The reference recovers by having
@@ -674,7 +684,9 @@ int32_t sgr_dingest_set_json_packer(sgr_dingest* g, const char* discriminator, c
  *   - any other value, after its framing, gives the row's program bytes: SGR_VALUE_PACKED, the value itself, 0 to
  *     state_bytes - 8 bytes, zero-padded; SGR_VALUE_PROTOBUF_EVENT, the payload of the multilanguage
  *     `State { string aggregateId = 1; bytes payload = 2; }` (Event's field numbers); SGR_VALUE_JSON, the members of the
- *     registered table at PROGRAM byte offsets;
+ *     registered table at PROGRAM byte offsets; SGR_VALUE_PROTOBUF_JSON, the members of the State's JSON payload, likewise
+ *     (what a multilanguage store keeps: getAggregateBytes hands the gateway `protobuf.State`, whose payload is the business
+ *     app's JSON state; State.aggregateId is not read, the key is the id);
  *   - a framed value longer than state_bytes - 8 is refused: "offset N, record r: state value of L bytes is longer than the
  *     P program bytes of a row (state_bytes - 8)";
  *   - n_records counts the live records: rows plus tombstones.
@@ -735,6 +747,17 @@ int32_t sgr_dingest_get_stats(sgr_dingest* g, sgr_ingest_stats* out);
  * sgr_register_program, and a later sgr_register_program clears the writer; SGR_ERR_INVALID on a bad table (nothing changes);
  * SGR_ERR_UNSUPPORTED on a routed engine without a current rank key table (sgr_dist_load_keys). */
 int32_t sgr_set_state_writer(sgr_engine* e, const sgr_json_field* members, uint32_t n_members);
+/* How the three reads below wrap the JSON value. SGR_VALUE_JSON (the default): the JSON value as it is. SGR_VALUE_PROTOBUF_JSON:
+ * the multilanguage `State { string aggregateId = 1; bytes payload = 2; }` that a multilanguage store hands the gateway
+ * (getAggregateBytes) and republishes, as ScalaPB's toByteArray writes it: `0x0A varint(len(id)) id`, left out for an empty id
+ * (proto3 omits a default string), then `0x12 varint(len(json)) json`, where json is byte-identical to what SGR_VALUE_JSON gives
+ * for the same row. The id is the row's aggregate id from the key table, as the SGR_JSON_ID member reads it: a row without an
+ * id, or whose id is not well-formed UTF-8, cannot be written, and the message names the State.aggregateId field. None rows keep
+ * their empty span; capacity, values_len, paging and cursors count the wrapped bytes. The value written parses back to its row
+ * through the state-topic restore under SGR_VALUE_PROTOBUF_JSON.
+ * SGR_ERR_INVALID for any other framing; SGR_ERR_NO_PROGRAM before sgr_register_program. The framing survives
+ * sgr_set_state_writer; sgr_register_program, which clears the writer, sets it back to SGR_VALUE_JSON. */
+int32_t sgr_set_state_writer_framing(sgr_engine* e, int32_t framing);
 /* Three reads that return values instead of rows. Each matches its twin (sgr_get_batch, sgr_export_changes, sgr_scan) in
  * locking, table generation, id-index update, paging, cursor / token and error codes, with the rows replaced by values
  * (values_cap bytes) and value_offsets (rows + 1 u64): row i's value is values[value_offsets[i] .. value_offsets[i + 1]). A

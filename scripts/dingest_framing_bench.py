@@ -7,6 +7,10 @@ every step a rebuild from offset 0 into an empty table. Keys are "<uuid>:<seq>".
   json_counter   play-json Counter events (TestBoundedContext), compact separators
   json_bank_money      BankAccount events, balances with two decimals
   json_bank_precise    BankAccount events, balances the repr of random doubles (the exact slow path of the double parse)
+  protobuf_json        the multilanguage Counter's events as its gateway writes them: Event { aggregateId, payload = the
+                       play-json event (the multilanguage TestBoundedContext) }, SGR_VALUE_PROTOBUF_JSON
+  protobuf_json_state  a state-topic restore of the same aggregates: one State { aggregateId, payload = the play-json
+                       AggregateState } per aggregate, keyed by the id (device only: the host decoder has no state-topic mode)
 Per workload: wire bytes per event, device ms/step and events/s, timing slots [0] (copies + decode chains), [1] (the repeat
 from an exact arena layout) and [4] (growth + fold) of sgr_dingest_last_timing, and the host decoder (sgr_ingest_record_batches_mt
 + sgr_fold_ingested) on the same bytes. The first device step is a warm-up: it also raises the arena claim for the framing.
@@ -35,8 +39,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 EPA, N_PART, RPB = 32, 32, 512
-WORKLOADS = ["packed", "protobuf", "json_counter", "json_bank_money", "json_bank_precise"]
+WORKLOADS = ["packed", "protobuf", "json_counter", "json_bank_money", "json_bank_precise", "protobuf_json", "protobuf_json_state"]
 CLS = "surge.core.TestBoundedContext."
+ML_CLS = "com.ukg.surge.multilanguage.TestBoundedContext."
 _lib = None
 
 
@@ -62,14 +67,24 @@ def _ids(aggs):
     return [str(uuid.UUID(int=(a * 0x9E3779B97F4A7C15F39CC0605CEDC835 + 0x1234) & ((1 << 128) - 1))) for a in aggs]
 
 
+def _pb(aid, payload):
+    """the multilanguage Event / State { aggregateId = 1, payload = 2 }"""
+    a = aid.encode()
+    return b"\x0a" + _pb_varint(len(a)) + a + b"\x12" + _pb_varint(len(payload)) + payload
+
+
 def _value(workload, aid, k, kind, by, dbl):
     seq = k + 1
+    if workload == "protobuf_json":
+        name, member = (("CountIncremented", "incrementBy"), ("CountDecremented", "decrementBy"))[kind % 2]
+        return _pb(aid, ('{"_type":"%s%s","aggregateId":"%s","%s":%d,"sequenceNumber":%d}' % (ML_CLS, name, aid, member, by, seq)).encode())
+    if workload == "protobuf_json_state":
+        return _pb(aid, ('{"aggregateId":"%s","count":%d,"version":%d}' % (aid, by, EPA)).encode())
     if workload in ("packed", "protobuf"):
         packed = struct.pack("<IIi", kind, seq, by)
         if workload == "packed":
             return packed
-        a = aid.encode()
-        return b"\x0a" + _pb_varint(len(a)) + a + b"\x12" + _pb_varint(len(packed)) + packed
+        return _pb(aid, packed)
     if workload == "json_counter":
         name = ("CountIncremented", "CountDecremented", "NoOpEvent")[kind]
         member = ('"incrementBy":%d,' % by, '"decrementBy":%d,' % by, "")[kind]
@@ -95,9 +110,9 @@ def encode_partition(args):
     dbls = rng.integers(0, 2**64, (EPA, len(aggs)), dtype=np.uint64).view("<f8")   # random bits: every exponent
     dbls[~np.isfinite(dbls)] = 0.1
     keys, vals = [], []
-    for k in range(EPA):
+    for k in range(1 if workload == "protobuf_json_state" else EPA):   # (a state topic: one record per aggregate, keyed by the id)
         for j, aid in enumerate(ids):
-            keys.append(b"%s:%d" % (aid.encode(), k + 1))
+            keys.append(aid.encode() if workload == "protobuf_json_state" else b"%s:%d" % (aid.encode(), k + 1))
             vals.append(_value(workload, aid, k, int(kinds[k, j]), int(bys[k, j]), float(dbls[k, j])))
     n = len(keys)
     key_offs = np.zeros(n + 1, np.uint64)
@@ -144,11 +159,21 @@ def setup(g, workload):
                                                                              ("accountOwner", N.JSON_PSTR, 40, 16), ("securityCode", N.JSON_PSTR, 56, 8)]),
                                     ("docs.command.BankAccountUpdated", 1, [("accountNumber", N.JSON_UUID, 16), ("newBalance", N.JSON_F64, 32)])])
         g.set_value_framing(N.VALUE_JSON)
+    elif workload == "protobuf_json":
+        g.set_json_packer("_type", [(ML_CLS + "CountIncremented", 0, [("incrementBy", N.JSON_I32, 16), ("sequenceNumber", N.JSON_I32, 4)]),
+                                    (ML_CLS + "CountDecremented", 1, [("decrementBy", N.JSON_I32, 16), ("sequenceNumber", N.JSON_I32, 4)])])
+        g.set_value_framing(N.VALUE_PROTOBUF_JSON)
+    elif workload == "protobuf_json_state":
+        g.set_state_topic(True)
+        g.set_json_packer("", [("AggregateState", 0, [("count", N.JSON_I32, 0), ("version", N.JSON_I32, 4)])])
+        g.set_value_framing(N.VALUE_PROTOBUF_JSON)
 
 
 def program(workload):
     from surge_b200 import programs as P
 
+    if workload.startswith("protobuf_json"):
+        return P.ml_counter_program()
     return P.bank_account_program() if workload.startswith("json_bank") else P.counter_program()
 
 
@@ -218,9 +243,10 @@ def main():
         for w in args.workloads.split(","):
             pinned, wire_bytes = encode(w, args.aggregates, libdir, 2026)
             ms, st, slots = run_device(w, pinned, args.aggregates, args.steps, args.warmup)
-            hms, hst = run_host(w, pinned, args.host_steps)
+            state_topic = w == "protobuf_json_state"
+            hms, hst = run_host(w, pinned, args.host_steps) if not state_topic else ([float("nan")], None)
             n = int(st["n_records"])
-            assert int(hst["n_records"]) == n, (hst, st)
+            assert state_topic or int(hst["n_records"]) == n, (hst, st)
             med, hmed = float(np.median(ms)), float(np.median(hms))
             s = np.median(np.asarray(slots), axis=0)
             print(json.dumps({"workload": w, "events": n, "wire_bytes_per_event": wire_bytes / n, "device_ms_per_step": ms, "device_median_ms": med,

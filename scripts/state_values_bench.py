@@ -5,6 +5,8 @@ row-returning twin:
   get_many_values   100 batches of 100 k ids, and one batch of 10 M ids       (twin: get_many(arrays=True))
   export            a full export_changes_values of the table                  (twin: export_changes)
   scan              a full scan_values                                          (twin: scan)
+the same three reads again with each value wrapped in the multilanguage protobuf State (sgr_set_state_writer_framing
+SGR_VALUE_PROTOBUF_JSON: what a multilanguage store hands its gateway), reported under "protobuf_json" beside the JSON arms,
 and a CPU restatement: the same csrc/state_writer.h compiled for the host (g++ -O3, one thread per core) writing the values
 of the rows get_many returned. This is NOT the JVM's writeState: it says what the same code costs on the host's cores.
 Reported per call: rows/s, value bytes/s, pages, with the card's name and power limit. The host build goes to a temporary
@@ -150,6 +152,20 @@ def run(name, n, host, threads):
             t_vals, pages = timed(vf)
             vb = sum(len(v) for p in pages for v in p[-1] if v)
             out[what] = {"rows_per_s": n / t_vals, "value_bytes_per_s": vb / t_vals, "pages": len(pages), "twin_rows_per_s": n / t_rows}
+        # the same reads under the protobuf wrapping (one length pass and one write pass, as the JSON arms)
+        e.set_state_writer_framing(N.VALUE_PROTOBUF_JSON)
+        e.get_many_values(ids[:1000])
+        pb = {}
+        t_vals, pvals = timed(lambda: [e.get_many_values(ids[i:i + batch]) for i in range(0, nb, batch)])
+        pb["get_100k"] = {"rows_per_s": nb / t_vals, "value_bytes_per_s": sum(len(v) for page in pvals for v in page if v) / t_vals}
+        t_vals, pvals = timed(lambda: e.get_many_values(ids))
+        pb["get_all"] = {"rows_per_s": n / t_vals, "value_bytes_per_s": sum(len(v) for v in pvals if v) / t_vals}
+        for what, vf in (("export", lambda: list(e.export_changes_values(N.ST_CHANGED, max_rows=1 << 20, values_cap=256 << 20))),
+                         ("scan", lambda: list(e.scan_values(max_rows=1 << 20, values_cap=256 << 20)))):
+            t_vals, pages = timed(vf)
+            pb[what] = {"rows_per_s": n / t_vals, "value_bytes_per_s": sum(len(v) for p in pages for v in p[-1] if v) / t_vals, "pages": len(pages)}
+        out["protobuf_json"] = pb
+        e.set_state_writer_framing(N.VALUE_JSON)
         # CPU restatement over the rows get_many returned
         states = np.ascontiguousarray(got[0])
         m3 = np.array([[m[1], m[2] if len(m) > 2 else 0, m[3] if len(m) > 3 else 0] for m in members], np.uint32)

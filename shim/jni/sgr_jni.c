@@ -7,6 +7,7 @@
 #if __has_include(<jni.h>)
 #include <jni.h>
 #include <stdint.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include "sgr.h"
@@ -200,6 +201,12 @@ JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_setStateWriter(JNIEnv* env, j
   if (rc != SGR_OK) throw_for(env, H(h), rc);
   return rc;
 }
+/* sgr_set_state_writer_framing: SGR_VALUE_JSON (2) or SGR_VALUE_PROTOBUF_JSON (3, the multilanguage State around each value). */
+JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_setStateWriterFraming(JNIEnv* env, jobject o, jlong h, jint framing) {
+  int32_t rc = sgr_set_state_writer_framing(H(h), framing);
+  if (rc != SGR_OK) throw_for(env, H(h), rc);
+  return rc;
+}
 /* One sgr_get_batch_values. keys / keyOffsets as for getBatch; values: a direct buffer whose capacity is the byte budget;
  * valueOffsets: n + 1 u64; flags: n u32. Returns the value bytes written, or -(bytes needed) when values is too small (nothing
  * written); throws on every other failure (a row the writer refuses, no writer: InvalidStateStoreException). */
@@ -295,7 +302,71 @@ JNIEXPORT jlong JNICALL Java_surge_gpu_Native_00024_ingestCreate(JNIEnv* env, jo
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_ingestDestroy(JNIEnv* env, jobject o, jlong g) { return sgr_ingest_destroy(G(g)); }
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_ingestSetValueFraming(JNIEnv* env, jobject o, jlong g, jint framing) { return sgr_ingest_set_value_framing(G(g), framing); }
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_ingestSetNullValueType(JNIEnv* env, jobject o, jlong g, jint event_type) { return sgr_ingest_set_null_value_type(G(g), event_type); }
-/* sgr_ingest_set_json_packer takes an array of structs with strings: bind it with a small marshaller (or JNA) on the maintainer's side. */
+/* A JSON member table (sgr_ingest_set_json_packer, sgr_dingest_set_json_packer) from one direct buffer of tableBytes bytes, little
+ * endian as setStateWriter's table: i32 unknown_type, u32 discriminator length + its UTF-8 bytes, u32 n_events, then per event
+ * u32 class-name length + its bytes, u32 event_type, u32 n_fields (at most 8), and per field u32 kind (SGR_JSON_*), u32 offset
+ * (a record offset, or a program byte offset in state-topic mode), u32 PSTR slot bytes, u32 name length + its bytes. Every
+ * string is copied out NUL-terminated; a name holding a NUL byte, a count out of range or a string past tableBytes throws
+ * IllegalArgumentException. Returns the setter's code. */
+#define JP_MAX_EVENTS 64
+typedef int32_t (*packer_fn)(void* g, const char* disc, const sgr_json_event* events, uint32_t n_events, int32_t unknown_type);
+typedef struct { const uint8_t* t; jlong n, at; char* arena; size_t used; const char* err; } TableReader;
+static uint32_t tr_u32(TableReader* r) {
+  uint32_t v = 0;
+  if (r->err) return 0;
+  if (r->n - r->at < 4) { r->err = "table: a field runs past tableBytes"; return 0; }
+  memcpy(&v, r->t + r->at, 4);
+  r->at += 4;
+  return v;
+}
+static const char* tr_str(TableReader* r) {
+  const uint32_t len = tr_u32(r);
+  if (r->err) return "";
+  if ((jlong)len > r->n - r->at) { r->err = "table: a string runs past tableBytes"; return ""; }
+  char* s = r->arena + r->used;
+  memcpy(s, r->t + r->at, len);
+  s[len] = 0;
+  if (strlen(s) != len) r->err = "table: a string holds a NUL byte";
+  r->used += len + 1; r->at += len;
+  return s;
+}
+static int32_t set_json_packer(JNIEnv* env, void* g, packer_fn set, jobject table, jlong table_bytes) {
+  int ok = 1;
+  if (table_bytes < 12) return bad_arg(env, "table: shorter than its header");
+  const uint8_t* t = (const uint8_t*)direct(env, table, table_bytes, "table: direct buffer shorter than tableBytes", &ok);
+  if (!ok) return SGR_ERR_INVALID;
+  /* the strings, NUL-terminated: at most table_bytes bytes of text and one NUL per string (each string has a 4-byte length) */
+  TableReader r = {t, table_bytes, 0, (char*)malloc((size_t)table_bytes + (size_t)table_bytes / 4 + 1), 0, 0};
+  sgr_json_event* ev = (sgr_json_event*)calloc(JP_MAX_EVENTS, sizeof(sgr_json_event));
+  if (!r.arena || !ev) { free(r.arena); free(ev); return bad_arg(env, "table: out of memory"); }
+  const int32_t unknown_type = (int32_t)tr_u32(&r);
+  const char* disc = tr_str(&r);
+  const uint32_t n_events = tr_u32(&r);
+  if (!r.err && n_events > JP_MAX_EVENTS) r.err = "table: more than 64 classes";
+  for (uint32_t i = 0; !r.err && i < n_events; ++i) {
+    ev[i].type_name = tr_str(&r);
+    ev[i].event_type = tr_u32(&r);
+    ev[i].n_fields = tr_u32(&r);
+    if (!r.err && ev[i].n_fields > SGR_JSON_MAX_FIELDS) r.err = "table: more than 8 members in a class";
+    for (uint32_t f = 0; !r.err && f < ev[i].n_fields; ++f) {
+      const uint32_t kind = tr_u32(&r), off = tr_u32(&r);
+      ev[i].fields[f].len = tr_u32(&r);
+      ev[i].fields[f].name = tr_str(&r);
+      if (!r.err && (kind > 255 || off > 0xffff)) r.err = "table: member kind or offset out of range";
+      ev[i].fields[f].kind = (uint8_t)kind;
+      ev[i].fields[f].dst_off = (uint16_t)off;
+    }
+  }
+  const int32_t rc = r.err ? bad_arg(env, r.err) : set(g, disc, ev, n_events, unknown_type);
+  free(r.arena);
+  free(ev);
+  return rc;
+}
+static int32_t ingest_packer(void* g, const char* d, const sgr_json_event* e, uint32_t n, int32_t u) { return sgr_ingest_set_json_packer((sgr_ingest*)g, d, e, n, u); }
+static int32_t dingest_packer(void* g, const char* d, const sgr_json_event* e, uint32_t n, int32_t u) { return sgr_dingest_set_json_packer((sgr_dingest*)g, d, e, n, u); }
+JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_ingestSetJsonPacker(JNIEnv* env, jobject o, jlong g, jobject table, jlong table_bytes) {
+  return set_json_packer(env, G(g), ingest_packer, table, table_bytes);
+}
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_ingestSetAborted(JNIEnv* env, jobject o, jlong g, jint partition, jlongArray pids, jlongArray firsts) {
   jsize n = (*env)->GetArrayLength(env, pids);
   if ((*env)->GetArrayLength(env, firsts) != n) return bad_arg(env, "producerIds and firstOffsets differ in length");
@@ -339,6 +410,9 @@ JNIEXPORT jlong JNICALL Java_surge_gpu_Native_00024_dingestCreate(JNIEnv* env, j
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_dingestDestroy(JNIEnv* env, jobject o, jlong g) { return sgr_dingest_destroy(DG(g)); }
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_dingestSetNullValueType(JNIEnv* env, jobject o, jlong g, jint event_type) { return sgr_dingest_set_null_value_type(DG(g), event_type); }
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_dingestSetValueFraming(JNIEnv* env, jobject o, jlong g, jint framing) { return sgr_dingest_set_value_framing(DG(g), framing); }
+JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_dingestSetJsonPacker(JNIEnv* env, jobject o, jlong g, jobject table, jlong table_bytes) {
+  return set_json_packer(env, DG(g), dingest_packer, table, table_bytes);
+}
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_dingestSetStateTopic(JNIEnv* env, jobject o, jlong g, jint on) { return sgr_dingest_set_state_topic(DG(g), on); }
 JNIEXPORT jint JNICALL Java_surge_gpu_Native_00024_dingestSetAborted(JNIEnv* env, jobject o, jlong g, jint partition, jlongArray pids, jlongArray firsts) {
   jsize n = (*env)->GetArrayLength(env, pids);

@@ -47,6 +47,9 @@ object Native {
   /** the JSON state writer (sgr_set_state_writer): per member (little endian) u32 SGR_JSON_* kind (5 = the aggregate id), u32
    *  program byte offset, u32 PSTR slot bytes, u32 name length, the UTF-8 name; nMembers == 0 clears it */
   @native def setStateWriter(handle: Long, table: ByteBuffer, tableBytes: Long, nMembers: Int): Int // sgr_set_state_writer
+  /** how the value reads wrap the JSON value: 2 = the JSON itself (default), 3 = the multilanguage protobuf State{aggregateId,
+   *  payload = the JSON} a multilanguage store hands the gateway; survives setStateWriter, reset by registerProgram */
+  @native def setStateWriterFraming(handle: Long, framing: Int): Int                // sgr_set_state_writer_framing
   /** getBatch with JSON values: value i = values[valueOffsets(i) until valueOffsets(i+1)] (u64 offsets), empty for None / unknown
    *  ids; returns the value bytes written, or -(bytes needed) when values is too small */
   @native def getBatchValues(handle: Long, keys: ByteBuffer, keyOffsets: ByteBuffer, n: Long, values: ByteBuffer, valueOffsets: ByteBuffer,
@@ -62,7 +65,11 @@ object Native {
   // raw record batches in, committed offsets out (include/sgr.h "ingest")
   @native def ingestCreate(): Long                                                 // sgr_ingest_create
   @native def ingestDestroy(ingest: Long): Int                                     // sgr_ingest_destroy
-  @native def ingestSetValueFraming(ingest: Long, framing: Int): Int               // sgr_ingest_set_value_framing (0 packed, 1 protobuf Event, 2 JSON)
+  @native def ingestSetValueFraming(ingest: Long, framing: Int): Int               // sgr_ingest_set_value_framing (0 packed, 1 protobuf Event, 2 JSON, 3 protobuf Event of JSON)
+  /** the JSON member table of framings 2 and 3, little endian: i32 unknownType, u32 length + discriminator, u32 nClasses, per class
+   *  u32 length + class name, u32 eventType, u32 nMembers (<= 8), per member u32 kind (SGR_JSON_*), u32 record offset, u32 PSTR
+   *  slot bytes, u32 length + member name */
+  @native def ingestSetJsonPacker(ingest: Long, table: ByteBuffer, tableBytes: Long): Int // sgr_ingest_set_json_packer
   @native def ingestSetNullValueType(ingest: Long, eventType: Int): Int            // sgr_ingest_set_null_value_type (state-topic tombstones)
   @native def ingestSetAborted(ingest: Long, partition: Int, producerIds: Array[Long], firstOffsets: Array[Long]): Int // sgr_ingest_set_aborted
   /** decodes one fetch response's bytes for `partition`; returns the number of packed records appended; throws on malformed input */
@@ -76,7 +83,9 @@ object Native {
   @native def dingestCreate(handle: Long, maxKeys: Long, maxIdBytes: Long): Long   // sgr_dingest_create (maxIdBytes 0 = 32 per id)
   @native def dingestDestroy(dingest: Long): Int                                   // sgr_dingest_destroy
   @native def dingestSetNullValueType(dingest: Long, eventType: Int): Int          // sgr_dingest_set_null_value_type
-  @native def dingestSetValueFraming(dingest: Long, framing: Int): Int             // sgr_dingest_set_value_framing (0 packed, 1 protobuf Event, 2 JSON)
+  @native def dingestSetValueFraming(dingest: Long, framing: Int): Int             // sgr_dingest_set_value_framing (0 packed, 1 protobuf Event, 2 JSON, 3 protobuf Event of JSON)
+  /** as ingestSetJsonPacker; in state-topic mode (set it first) the offsets are program byte offsets */
+  @native def dingestSetJsonPacker(dingest: Long, table: ByteBuffer, tableBytes: Long): Int // sgr_dingest_set_json_packer
   @native def dingestSetStateTopic(dingest: Long, on: Int): Int                    // sgr_dingest_set_state_topic (1: compacted state topic, before the first fold)
   @native def dingestSetAborted(dingest: Long, partition: Int, producerIds: Array[Long], firstOffsets: Array[Long]): Int // sgr_dingest_set_aborted
   /** queues one fetch response's bytes (a DIRECT buffer, untouched until dingestFold returns); returns the data batches queued */

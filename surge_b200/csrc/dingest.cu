@@ -17,9 +17,9 @@
 //          skip the holes in the atomic fold, the others group the live records first); only then do the partitions'
 //          positions advance. All or nothing.
 // The arena the batches decompress into is sized from the wire bytes (3x); if a poll compresses better than that the claims
-// overflow, the flag comes back with the verdicts and the poll is decoded again from an exact host-side layout. Protobuf and
-// JSON values (sgr_dingest_set_value_framing) are converted to packed events inside the parse kernel (value_framing.h); JSON
-// compresses better than packed values, so under those framings the claim multiple adapts (claim_mult).
+// overflow, the flag comes back with the verdicts and the poll is decoded again from an exact host-side layout. Protobuf, JSON
+// and protobuf-wrapped JSON values (sgr_dingest_set_value_framing) are converted to packed events inside the parse kernel
+// (value_framing.h); JSON compresses better than packed values, so under those framings the claim multiple adapts (claim_mult).
 // A compacted STATE topic (sgr_dingest_set_state_topic) takes the same chain; its parse writes rows of program bytes, and the
 // fold applies them last write wins with sgr_put_batch's kernels (put_decoded_poll) instead of folding events.
 #include <cuda_runtime.h>
@@ -51,7 +51,7 @@ struct sgr_dingest {
   std::map<int32_t, PartitionState> staged; // view after the submissions of the current poll
   int32_t null_value_type = -1;
   int32_t value_framing = SGR_VALUE_PACKED;
-  DevBuf json_table;                        // SGR_VALUE_JSON: member table (vf::Class[], vf::Field[], names) on the device
+  DevBuf json_table;                        // SGR_VALUE_JSON / SGR_VALUE_PROTOBUF_JSON: member table (vf::Class[], vf::Field[], names) on the device
   vf::Table json{};                         // ... its view; n_classes == 0 until a packer is registered
   // arena claim of an lz4 batch, in multiples of its compressed size: 3 for packed values; under protobuf / JSON framing raised
   // after a poll that needed the exact-layout repeat, to the power of two at or above the largest ratio it showed (at most 16)
@@ -344,9 +344,9 @@ int32_t sgr_dingest_set_null_value_type(sgr_dingest* g, int32_t event_type) {
 // Both settings are refused while a poll is pending: its groups were parsed at submit time, and the exact-layout repeat parses
 // again at fold time; one poll must not be decoded two ways.
 int32_t sgr_dingest_set_value_framing(sgr_dingest* g, int32_t framing) {
-  if (!g || (framing != SGR_VALUE_PACKED && framing != SGR_VALUE_PROTOBUF_EVENT && framing != SGR_VALUE_JSON)) return dfail(g, SGR_ERR_INVALID, "unknown value framing %d", framing);
+  if (!g || framing < SGR_VALUE_PACKED || framing > SGR_VALUE_PROTOBUF_JSON) return dfail(g, SGR_ERR_INVALID, "unknown value framing %d", framing);
   if (!g->subs.empty()) return dfail(g, SGR_ERR_STATE, "the value framing cannot change between a submit and its fold");
-  if (framing == SGR_VALUE_JSON && !g->json.n_classes) return dfail(g, SGR_ERR_INVALID, "register a JSON packer first (sgr_dingest_set_json_packer)");
+  if ((framing == SGR_VALUE_JSON || framing == SGR_VALUE_PROTOBUF_JSON) && !g->json.n_classes) return dfail(g, SGR_ERR_INVALID, "register a JSON packer first (sgr_dingest_set_json_packer)");
   g->value_framing = framing;
   return SGR_OK;
 }

@@ -319,7 +319,7 @@ __device__ __forceinline__ void state_row(const DgParse& p, DgBatch& bt, uint32_
       uint32_t n = 0;
       const uint32_t why = vf::convert<vf::STATE>(kFraming, p.json, val, (uint32_t)val_len, converted, &val, &n);
       if (why) { refuse_record(bt, r, (uint32_t)DG_VALUE_FRAMING | (why << 8)); return; }
-      val_len = kFraming == vf::JSON ? (int32_t)p.row_bytes : (int32_t)n;   // (the member table was checked against the row)
+      val_len = kFraming == vf::PROTOBUF_EVENT ? (int32_t)n : (int32_t)p.row_bytes;   // (the member table was checked against the row)
     }
   }
   if (val_len > (int32_t)p.row_bytes) { refuse_record(bt, r, (uint32_t)DG_STATE_LENGTH | ((uint32_t)min(val_len, 0xffffff) << 8)); return; }
@@ -466,13 +466,16 @@ cudaError_t dg_gather_keys(const DgDict& d, uint64_t from, uint32_t n, uint32_t*
 cudaError_t dg_launch_parse(const DgParse& p, cudaStream_t st) {
   if (p.n_records <= p.rec_begin) return cudaSuccess;
   const uint32_t blocks = (p.n_records - p.rec_begin + kThreads - 1) / kThreads;
-  switch (p.value_framing + (p.state_topic ? 3 : 0)) {
+  // (framing, topic mode) -> one instantiation: the framing in bits 0..1, the state-topic mode in bit 2
+  switch (p.value_framing | (p.state_topic ? 4 : 0)) {
     case vf::PACKED: dg_parse_kernel<vf::PACKED, false><<<blocks, kThreads, 0, st>>>(p); break;
     case vf::PROTOBUF_EVENT: dg_parse_kernel<vf::PROTOBUF_EVENT, false><<<blocks, kThreads, 0, st>>>(p); break;
     case vf::JSON: dg_parse_kernel<vf::JSON, false><<<blocks, kThreads, 0, st>>>(p); break;
-    case 3 + vf::PACKED: dg_parse_kernel<vf::PACKED, true><<<blocks, kThreads, 0, st>>>(p); break;
-    case 3 + vf::PROTOBUF_EVENT: dg_parse_kernel<vf::PROTOBUF_EVENT, true><<<blocks, kThreads, 0, st>>>(p); break;
-    case 3 + vf::JSON: dg_parse_kernel<vf::JSON, true><<<blocks, kThreads, 0, st>>>(p); break;
+    case vf::PROTOBUF_JSON: dg_parse_kernel<vf::PROTOBUF_JSON, false><<<blocks, kThreads, 0, st>>>(p); break;
+    case 4 | vf::PACKED: dg_parse_kernel<vf::PACKED, true><<<blocks, kThreads, 0, st>>>(p); break;
+    case 4 | vf::PROTOBUF_EVENT: dg_parse_kernel<vf::PROTOBUF_EVENT, true><<<blocks, kThreads, 0, st>>>(p); break;
+    case 4 | vf::JSON: dg_parse_kernel<vf::JSON, true><<<blocks, kThreads, 0, st>>>(p); break;
+    case 4 | vf::PROTOBUF_JSON: dg_parse_kernel<vf::PROTOBUF_JSON, true><<<blocks, kThreads, 0, st>>>(p); break;
     default: return cudaErrorInvalidValue;
   }
   return cudaGetLastError();

@@ -193,6 +193,7 @@ struct sgr_engine {
   // sgr_set_state_writer: the writer table (writer.n == 0: none; its literals in writer_lits) and the member names for refusal
   // messages; the scratch and the values of the value-returning reads (state_values.cuh)
   SwWriter writer{};
+  int32_t writer_framing = SGR_VALUE_JSON;  // sgr_set_state_writer_framing: SGR_VALUE_PROTOBUF_JSON wraps each value in a State
   DevBuf writer_lits;
   std::vector<std::string> writer_names;
   DevBuf sv_scratch, sv_values;
@@ -609,6 +610,7 @@ int32_t sgr_register_program(sgr_engine* e, const sgr_fold_program* prog) {
   e->plane_state = sgr_engine::kPlaneNone;
   e->states_valid = false; e->states_n = 0;
   e->writer.n = 0;   // its offsets belonged to the old program
+  e->writer_framing = SGR_VALUE_JSON;
   mark_dirty(e);
   return SGR_OK;
 }
@@ -1264,6 +1266,9 @@ int32_t sgr_get_batch(sgr_engine* e, const uint8_t* keys, const uint32_t* key_of
 // The message of a row the state writer refuses: `what` names the row's place, ctl holds state_values_measure's control words.
 static int32_t writer_refusal(sgr_engine* e, const char* api, const char* what, const unsigned long long* ctl) {
   const uint32_t member = (uint32_t)(ctl[kSvStatus] >> 8), why = (uint32_t)(ctl[kSvStatus] & 0xff);
+  if (member == sw::kWrapMember)
+    return fail(e, SGR_ERR_UNSUPPORTED, "%s: row %llu of the %s (aggregate %lld), the protobuf field State.aggregateId: %s", api, ctl[kSvRefused],
+                what, (long long)ctl[kSvIndex], sw::reason_text(why));
   return fail(e, SGR_ERR_UNSUPPORTED, "%s: row %llu of the %s (aggregate %lld), member %u \"%s\": %s", api, ctl[kSvRefused], what,
               (long long)ctl[kSvIndex], member, member < e->writer_names.size() ? e->writer_names[member].c_str() : "", sw::reason_text(why));
 }
@@ -1325,6 +1330,16 @@ int32_t sgr_set_state_writer(sgr_engine* e, const sgr_json_field* members, uint3
   return SGR_OK;
 }
 
+int32_t sgr_set_state_writer_framing(sgr_engine* e, int32_t framing) {
+  OpLock op_lock(e);
+  if (!e) return SGR_ERR_INVALID;
+  if (framing != SGR_VALUE_JSON && framing != SGR_VALUE_PROTOBUF_JSON)
+    return fail(e, SGR_ERR_INVALID, "state writer framing %d: SGR_VALUE_JSON or SGR_VALUE_PROTOBUF_JSON", framing);
+  if (!e->has_program) return fail(e, SGR_ERR_NO_PROGRAM, "register a fold program before the state writer's framing");
+  e->writer_framing = framing;
+  return SGR_OK;
+}
+
 int32_t sgr_get_batch_values(sgr_engine* e, const uint8_t* keys, const uint32_t* key_offsets, uint64_t n, uint8_t* values, uint64_t values_cap,
                              uint64_t* value_offsets, uint32_t* flags, int64_t* indices, uint64_t* values_len) {
   if (!e || !value_offsets || !flags || (!values && values_cap)) return fail(e, SGR_ERR_INVALID, "null argument");
@@ -1337,7 +1352,7 @@ int32_t sgr_get_batch_values(sgr_engine* e, const uint8_t* keys, const uint32_t*
                  (const uint32_t*)(dd + b.down), ~0ull, n};
   unsigned long long *d_offs = nullptr, *d_sv = nullptr;
   cudaError_t ce = e->sv_scratch.reserve(state_values_scratch_bytes(n));
-  if (ce == cudaSuccess) ce = state_values_measure(e->writer, r, ~0ull, e->sv_scratch.p, &d_offs, &d_sv, e->stream);
+  if (ce == cudaSuccess) ce = state_values_measure(e->writer, e->writer_framing == SGR_VALUE_PROTOBUF_JSON, r, ~0ull, e->sv_scratch.p, &d_offs, &d_sv, e->stream);
   if (ce != cudaSuccess) return fail(e, ce == cudaErrorMemoryAllocation ? SGR_ERR_OOM : SGR_ERR_CUDA, "get_batch_values launch: %s", cudaGetErrorString(ce));
   CUDA_TRY(e, cudaMemcpyAsync(b.hd, dd, 8 * kCtlCut, cudaMemcpyDeviceToHost, e->stream));
   CUDA_TRY(e, cudaMemcpyAsync(b.hd + b.down, d_sv, 8 * kSvCtlWords, cudaMemcpyDeviceToHost, e->stream));
@@ -1354,7 +1369,7 @@ int32_t sgr_get_batch_values(sgr_engine* e, const uint8_t* keys, const uint32_t*
     return fail(e, SGR_ERR_CAPACITY, "the batch's values need %llu bytes, values_cap is %llu", (unsigned long long)total, (unsigned long long)values_cap);
   }
   CUDA_TRY(e, e->sv_values.reserve(total));
-  ce = state_values_write(e->writer, r, n, d_offs, (uint8_t*)e->sv_values.p, e->stream);
+  ce = state_values_write(e->writer, e->writer_framing == SGR_VALUE_PROTOBUF_JSON, r, n, d_offs, (uint8_t*)e->sv_values.p, e->stream);
   if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "get_batch_values launch: %s", cudaGetErrorString(ce));
   // pinned, from its start (the stream is idle): results | value offsets | values
   const size_t h_offs = b.down, h_vals = h_offs + round16((n + 1) * 8);
@@ -1579,7 +1594,7 @@ static int32_t fetch_page(sgr_engine* e, const char* api, const uint32_t* map, u
       const SvRows r{dd + o_rows, user, (const uint32_t*)(dd + o_fl), (const long long*)dd, dd + o_ids, (const uint32_t*)(dd + o_off), x.n, page};
       CUDA_TRY(e, e->sv_scratch.reserve(state_values_scratch_bytes(page)));
       unsigned long long *offs = nullptr, *dctl = nullptr;
-      ce = state_values_measure(e->writer, r, out.values_cap, e->sv_scratch.p, &offs, &dctl, e->stream);
+      ce = state_values_measure(e->writer, e->writer_framing == SGR_VALUE_PROTOBUF_JSON, r, out.values_cap, e->sv_scratch.p, &offs, &dctl, e->stream);
       if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "%s launch: %s", api, cudaGetErrorString(ce));
       CUDA_TRY(e, cudaMemcpyAsync(e->gb_host.p, dctl, 8 * kSvCtlWords, cudaMemcpyDeviceToHost, e->stream));
       CUDA_TRY(e, cudaStreamSynchronize(e->stream));
@@ -1592,7 +1607,7 @@ static int32_t fetch_page(sgr_engine* e, const char* api, const uint32_t* map, u
       value_bytes = sv[kSvBytes];
       d_offs = offs;
       CUDA_TRY(e, e->sv_values.reserve(value_bytes));
-      ce = state_values_write(e->writer, r, rows_out, offs, (uint8_t*)e->sv_values.p, e->stream);
+      ce = state_values_write(e->writer, e->writer_framing == SGR_VALUE_PROTOBUF_JSON, r, rows_out, offs, (uint8_t*)e->sv_values.p, e->stream);
       if (ce != cudaSuccess) return fail(e, SGR_ERR_CUDA, "%s launch: %s", api, cudaGetErrorString(ce));
       rc = ensure_pinned(e, total + round16((rows_out + 1) * 8) + value_bytes); if (rc) return rc;
     }

@@ -657,7 +657,7 @@ struct sgr_ingest {
   sgr_ingest_stats total{};
   uint64_t keys_at_mark = 0;
   uint64_t max_ids = 1ull << 31, max_id_bytes = 1ull << 32;   // what the 32-bit dictionary fields can address
-  int32_t value_framing = 0;        // SGR_VALUE_PACKED | SGR_VALUE_PROTOBUF_EVENT | SGR_VALUE_JSON
+  int32_t value_framing = 0;        // SGR_VALUE_PACKED | SGR_VALUE_PROTOBUF_EVENT | SGR_VALUE_JSON | SGR_VALUE_PROTOBUF_JSON
   JsonPacker json;
   int32_t null_value_type = -1;     // >= 0: a keyed record with a null value becomes an event of this type (state-topic tombstones)
   std::vector<Staged> pool;         // staging buffers, reused across calls (a restore loop polls similar sizes)
@@ -723,8 +723,8 @@ int32_t sgr_ingest_set_json_packer(sgr_ingest* g, const char* discriminator, con
 }
 
 int32_t sgr_ingest_set_value_framing(sgr_ingest* g, int32_t framing) {
-  if (!g || (framing != SGR_VALUE_PACKED && framing != SGR_VALUE_PROTOBUF_EVENT && framing != SGR_VALUE_JSON)) return ifail(g, SGR_ERR_INVALID, "unknown value framing %d", framing);
-  if (framing == SGR_VALUE_JSON && g->json.events.empty()) return ifail(g, SGR_ERR_INVALID, "register a JSON packer first (sgr_ingest_set_json_packer)");
+  if (!g || framing < SGR_VALUE_PACKED || framing > SGR_VALUE_PROTOBUF_JSON) return ifail(g, SGR_ERR_INVALID, "unknown value framing %d", framing);
+  if ((framing == SGR_VALUE_JSON || framing == SGR_VALUE_PROTOBUF_JSON) && g->json.events.empty()) return ifail(g, SGR_ERR_INVALID, "register a JSON packer first (sgr_ingest_set_json_packer)");
   g->value_framing = framing;
   return SGR_OK;
 }
@@ -821,9 +821,10 @@ int32_t decode_fetch(int32_t partition, const uint8_t* buf, uint64_t nbytes, Sta
         if (key_len <= 0) { ++st.n_markers; continue; }                              // the producer's empty-key flush record
         if (wire_val_len < 0 && o->null_value_type < 0) { ++st.n_null_values; continue; }
         int32_t val_len = wire_val_len;
-        if (val_len >= 0 && o->value_framing == SGR_VALUE_PROTOBUF_EVENT) {
+        if (val_len >= 0 && (o->value_framing == SGR_VALUE_PROTOBUF_EVENT || o->value_framing == SGR_VALUE_PROTOBUF_JSON)) {
           // multilanguage topics: the value is protobuf Event { string aggregateId = 1; bytes payload = 2; }
-          // (multilanguage-protocol.proto:17-20, written by GenericSurgeCommandBusinessLogic.scala:30-33); the packed event is the payload
+          // (multilanguage-protocol.proto:17-20, written by GenericSurgeCommandBusinessLogic.scala:30-33); the payload is the packed
+          // event (SGR_VALUE_PROTOBUF_EVENT) or the business app's JSON (SGR_VALUE_PROTOBUF_JSON, packed next)
           Cursor pb(val, (uint64_t)val_len);
           const uint8_t* payload = nullptr; uint64_t payload_len = 0;
           while (pb.ok && pb.pos < pb.n) {
@@ -846,7 +847,7 @@ int32_t decode_fetch(int32_t partition, const uint8_t* buf, uint64_t nbytes, Sta
           val = payload; val_len = (int32_t)(payload_len > 0x7fffffff ? 0x7fffffff : payload_len);
         }
         uint8_t json_out[56];
-        if (val_len >= 0 && o->value_framing == SGR_VALUE_JSON) {
+        if (val_len >= 0 && (o->value_framing == SGR_VALUE_JSON || o->value_framing == SGR_VALUE_PROTOBUF_JSON)) {
           const char* why = json_pack(*o->json, val, (uint32_t)val_len, json_out, &o->json_tmp);
           if (why) return set_error(&o->err, SGR_ERR_INVALID, "partition %d offset %lld: JSON event: %s", partition, (long long)offset, why);
           val = json_out; val_len = 56;

@@ -1,4 +1,6 @@
 // state_values.cu — rows -> JSON state values (state_writer.h) on the device, for the value-returning reads of engine.cu.
+// Under the protobuf wrapping (kWrap: sgr_set_state_writer_framing) each value is the multilanguage State around the JSON value:
+// the length pass adds the wrapper to the JSON length, and the write pass recovers the JSON length from the value's span.
 //
 //   length   one thread per row: the value's bytes, or 0 for a None row and for a row that cannot be written (whose status it
 //            records, the lowest such row by atomicMin)
@@ -51,6 +53,7 @@ __device__ __forceinline__ void row_id(const SvRows& r, uint64_t i, const uint8_
   *len = *has ? r.id_offs[i + 1] - r.id_offs[i] : 0;
 }
 
+template <bool kWrap>
 __global__ void __launch_bounds__(kThreads) sv_len_kernel(const SwWriter w, const SvRows r, unsigned long long* lens, uint32_t* status,
                                                           unsigned long long* ctl) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i <= r.n; i += (uint64_t)gridDim.x * blockDim.x) {
@@ -65,6 +68,13 @@ __global__ void __launch_bounds__(kThreads) sv_len_kernel(const SwWriter w, cons
       for (; k < w.n; ++k) {
         len += sw::member_len(w.m[k], row, id, id_len, has_id, &why);
         if (why) break;
+      }
+      if constexpr (kWrap) {   // the State around it: the id must be one the ID member could write
+        if (!why) {
+          if (!has_id) { why = sw::NO_ID; k = sw::kWrapMember; }
+          else if (!sw::utf8_ok(id, id_len)) { why = sw::ID_UTF8; k = sw::kWrapMember; }
+          else len = sw::wrap_len(id_len, len);
+        }
       }
       if (why) {
         len = 0;
@@ -89,6 +99,7 @@ __global__ void sv_fit_kernel(const unsigned long long* offs, uint64_t n, unsign
   if (bad < lo) { ctl[kSvStatus] = status[bad]; ctl[kSvIndex] = (unsigned long long)idx[bad]; }
 }
 
+template <bool kWrap>
 __global__ void __launch_bounds__(kThreads) sv_write_kernel(const SwWriter w, const SvRows r, uint64_t n_rows, const unsigned long long* offs,
                                                             uint8_t* values) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_rows; i += (uint64_t)gridDim.x * blockDim.x) {
@@ -98,6 +109,7 @@ __global__ void __launch_bounds__(kThreads) sv_write_kernel(const SwWriter w, co
     row_id(r, i, &id, &id_len, &has_id);
     const uint8_t* row = r.rows + i * r.user;
     uint8_t* o = values + b;
+    if constexpr (kWrap) o = sw::wrap_head_write(o, id, id_len, sw::wrap_json_len(id_len, offs[i + 1] - b));
     for (uint32_t k = 0; k < w.n; ++k) o = sw::member_write(o, w.m[k], w.lits, row, id, id_len);
     *o = '}';
   }
@@ -107,23 +119,25 @@ __global__ void __launch_bounds__(kThreads) sv_write_kernel(const SwWriter w, co
 
 size_t state_values_scratch_bytes(uint64_t n) { return carve(nullptr, n).total; }
 
-cudaError_t state_values_measure(const SwWriter& w, const SvRows& r, uint64_t cap, void* scratch, unsigned long long** offs,
+cudaError_t state_values_measure(const SwWriter& w, bool wrap, const SvRows& r, uint64_t cap, void* scratch, unsigned long long** offs,
                                  unsigned long long** ctl, cudaStream_t st) {
   Carve c = carve(scratch, r.n);
   *offs = c.offs; *ctl = c.ctl;
   cudaError_t e;
   if ((e = cudaMemsetAsync(c.ctl, 0xff, 8 * kSvCtlWords, st)) != cudaSuccess) return e;
-  sv_len_kernel<<<blocks_for(r.n + 1), kThreads, 0, st>>>(w, r, c.lens, c.status, c.ctl);
+  if (wrap) sv_len_kernel<true><<<blocks_for(r.n + 1), kThreads, 0, st>>>(w, r, c.lens, c.status, c.ctl);
+  else sv_len_kernel<false><<<blocks_for(r.n + 1), kThreads, 0, st>>>(w, r, c.lens, c.status, c.ctl);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   if ((e = cub::DeviceScan::ExclusiveSum(c.tmp, c.tmp_bytes, c.lens, c.offs, (uint64_t)(r.n + 1), st)) != cudaSuccess) return e;
   sv_fit_kernel<<<1, 1, 0, st>>>(c.offs, r.n, cap, c.status, r.idx, c.ctl);
   return cudaGetLastError();
 }
 
-cudaError_t state_values_write(const SwWriter& w, const SvRows& r, uint64_t n_rows, const unsigned long long* offs, uint8_t* values,
+cudaError_t state_values_write(const SwWriter& w, bool wrap, const SvRows& r, uint64_t n_rows, const unsigned long long* offs, uint8_t* values,
                                cudaStream_t st) {
   if (!n_rows) return cudaSuccess;
-  sv_write_kernel<<<blocks_for(n_rows), kThreads, 0, st>>>(w, r, n_rows, offs, values);
+  if (wrap) sv_write_kernel<true><<<blocks_for(n_rows), kThreads, 0, st>>>(w, r, n_rows, offs, values);
+  else sv_write_kernel<false><<<blocks_for(n_rows), kThreads, 0, st>>>(w, r, n_rows, offs, values);
   return cudaGetLastError();
 }
 

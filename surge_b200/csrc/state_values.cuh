@@ -34,12 +34,13 @@ struct SvRows {
 size_t state_values_scratch_bytes(uint64_t n);
 
 // Enqueue the length pass, the exclusive scan of the lengths into offs[0 .. n] (u64, inside the scratch) and the fit step
-// against cap. *offs (out): where the offsets live; *ctl (out): the control words, kSvCtlWords u64.
-cudaError_t state_values_measure(const SwWriter& w, const SvRows& r, uint64_t cap, void* scratch, unsigned long long** offs,
+// against cap. wrap: each value is the protobuf State around the JSON value (SGR_VALUE_PROTOBUF_JSON; a refusal of the row's id
+// reports member sw::kWrapMember). *offs (out): where the offsets live; *ctl (out): the control words, kSvCtlWords u64.
+cudaError_t state_values_measure(const SwWriter& w, bool wrap, const SvRows& r, uint64_t cap, void* scratch, unsigned long long** offs,
                                  unsigned long long** ctl, cudaStream_t st);
 
-// Enqueue the write of rows [0, n_rows) at values + offs[i] (offs from state_values_measure over the same rows).
-cudaError_t state_values_write(const SwWriter& w, const SvRows& r, uint64_t n_rows, const unsigned long long* offs, uint8_t* values,
+// Enqueue the write of rows [0, n_rows) at values + offs[i] (offs from state_values_measure over the same rows and wrap).
+cudaError_t state_values_write(const SwWriter& w, bool wrap, const SvRows& r, uint64_t n_rows, const unsigned long long* offs, uint8_t* values,
                                cudaStream_t st);
 
 }  // namespace sgr

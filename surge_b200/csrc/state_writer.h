@@ -388,5 +388,42 @@ SW_HD uint8_t* member_write(uint8_t* o, const Member& m, const uint8_t* lits, co
   }
 }
 
+// --------------------------------------------------------------------------------------------- protobuf State wrapping
+// SGR_VALUE_PROTOBUF_JSON (sgr_set_state_writer_framing): the value is the multilanguage State { string aggregateId = 1; bytes
+// payload = 2; } around the JSON value, as ScalaPB's toByteArray writes it: field 1 (left out for an empty id, as proto3 leaves
+// out a default string), then field 2.
+constexpr uint32_t kWrapMember = kMaxMembers;   // the member index of a row refused for the wrapper's id (State.aggregateId)
+
+SW_HD uint32_t varint_len(uint64_t v) { uint32_t n = 1; while (v >= 0x80) { v >>= 7; ++n; } return n; }
+
+SW_HD uint8_t* varint_write(uint8_t* o, uint64_t v) {
+  while (v >= 0x80) { *o++ = (uint8_t)(v | 0x80); v >>= 7; }
+  *o++ = (uint8_t)v;
+  return o;
+}
+
+SW_HD uint64_t wrap_id_len(uint64_t id_len) { return id_len ? 1 + varint_len(id_len) + id_len : 0; }
+
+// the wrapped value of an id and a JSON value of json_len bytes
+SW_HD uint64_t wrap_len(uint64_t id_len, uint64_t json_len) { return wrap_id_len(id_len) + 1 + varint_len(json_len) + json_len; }
+
+// the JSON bytes inside a wrapped value of `total` bytes (json_len + varint_len(json_len) grows strictly: one answer)
+SW_HD uint64_t wrap_json_len(uint64_t id_len, uint64_t total) {
+  const uint64_t rest = total - wrap_id_len(id_len) - 1;
+  for (uint32_t k = 1; k < 10; ++k) if (varint_len(rest - k) == k) return rest - k;
+  return 0;
+}
+
+// the wrapper's bytes in front of the JSON value
+SW_HD uint8_t* wrap_head_write(uint8_t* o, const uint8_t* id, uint64_t id_len, uint64_t json_len) {
+  if (id_len) {
+    *o++ = 0x0A;
+    o = varint_write(o, id_len);
+    for (uint64_t k = 0; k < id_len; ++k) *o++ = id[k];
+  }
+  *o++ = 0x12;
+  return varint_write(o, json_len);
+}
+
 }  // namespace sw
 }  // namespace sgr

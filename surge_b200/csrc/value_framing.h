@@ -1,5 +1,5 @@
-// value_framing.h — record value -> the 56 bytes of a packed event (u32 type, u32 seq, payload[48]), for protobuf-wrapped and
-// play-json values. One source for the device ingest's parse kernel (dingest_kernels.cu) and the CPU tests.
+// value_framing.h — record value -> the 56 bytes of a packed event (u32 type, u32 seq, payload[48]), for protobuf-wrapped,
+// play-json and protobuf-wrapped play-json values. One source for the device ingest's parse kernel (dingest_kernels.cu) and the CPU tests.
 //
 // The host decoder (ingest.cpp: the protobuf unwrap of decode_fetch, JsonScan, json_unescape and json_pack) defines the
 // behaviour; this file gives the same result on every input, accepted or refused, with the same refusal text. What differs is
@@ -26,7 +26,7 @@ namespace sgr {
 namespace vf {
 
 // framings (include/sgr.h SGR_VALUE_*)
-enum : int32_t { PACKED = 0, PROTOBUF_EVENT = 1, JSON = 2 };
+enum : int32_t { PACKED = 0, PROTOBUF_EVENT = 1, JSON = 2, PROTOBUF_JSON = 3 };
 // member kinds (include/sgr.h SGR_JSON_*)
 enum : uint8_t { K_I32 = 0, K_I64 = 1, K_F64 = 2, K_UUID = 3, K_PSTR = 4 };
 
@@ -611,17 +611,21 @@ VF_HD uint32_t json_pack(const Table& t, const uint8_t* v, uint32_t n, uint8_t* 
   return OK;
 }
 
-// A non-null record value under `framing` (PROTOBUF_EVENT or JSON) -> the packed event value: on OK, *len bytes of it are at
-// *val (a part of the value itself, or out[56]). The caller applies the 8..56 length check, as the host decoder does next.
-// Under the STATE layout the value is a state-topic value (the protobuf State message has Event's field numbers) and a JSON
-// object fills out[kStateRowMax]; the caller checks the length against its program bytes.
+// A non-null record value under `framing` (PROTOBUF_EVENT, JSON or PROTOBUF_JSON) -> the packed event value: on OK, *len bytes
+// of it are at *val (a part of the value itself, or out[56]). The caller applies the 8..56 length check, as the host decoder
+// does next. Under the STATE layout the value is a state-topic value (the protobuf State message has Event's field numbers) and
+// a JSON object fills out[kStateRowMax]; the caller checks the length against its program bytes.
+// PROTOBUF_JSON is the multilanguage gateway's wrapping of a JSON business-app payload: the payload of the protobuf message (the
+// unwrap of PROTOBUF_EVENT; a message without field 2 has an empty payload) goes through json_pack. Field 1, the aggregate id,
+// is not read: the record key is the id, as under PROTOBUF_EVENT.
 template <int kLayout = RECORD>
 VF_HD uint32_t convert(int32_t framing, const Table& t, const uint8_t* v, uint32_t n, uint8_t* out, const uint8_t** val, uint32_t* len) {
-  if (framing == PROTOBUF_EVENT) {
+  if (framing == PROTOBUF_EVENT || framing == PROTOBUF_JSON) {
     uint32_t off;
     const uint32_t e = protobuf_payload(v, n, &off, len);
     *val = v + off;
-    return e;
+    if (e || framing == PROTOBUF_EVENT) return e;
+    v += off; n = *len;
   }
   *val = out; *len = kLayout == RECORD ? 56 : kStateRowMax;
   return json_pack<kLayout>(t, v, n, out);

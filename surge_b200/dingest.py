@@ -47,7 +47,9 @@ class DeviceIngest:
         self._check(self._lib.sgr_dingest_set_null_value_type(self._h, event_type))
 
     def set_value_framing(self, framing: int) -> None:
-        """N.VALUE_PACKED, N.VALUE_PROTOBUF_EVENT or N.VALUE_JSON (after set_json_packer), as Ingest.set_value_framing."""
+        """N.VALUE_PACKED, N.VALUE_PROTOBUF_EVENT, N.VALUE_JSON or N.VALUE_PROTOBUF_JSON (the last two after set_json_packer), as
+        Ingest.set_value_framing. In state-topic mode N.VALUE_PROTOBUF_JSON reads the multilanguage State, whose payload is the
+        app's JSON state, into the row through the member table."""
         self._check(self._lib.sgr_dingest_set_value_framing(self._h, framing))
 
     def set_json_packer(self, discriminator: str, events: Sequence[Tuple[str, int, Sequence[Tuple]]], unknown_type: int = -1) -> None:

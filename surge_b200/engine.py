@@ -386,6 +386,13 @@ class ReplayEngine:
                 arr[i].len = m[3] if len(m) > 3 else 0
         self._ck(self._lib.sgr_set_state_writer(self._h, arr, len(members)))
 
+    def set_state_writer_framing(self, framing: int) -> None:
+        """How the value-returning reads wrap the JSON value: N.VALUE_JSON (the default) returns it as it is;
+        N.VALUE_PROTOBUF_JSON returns the multilanguage protobuf State{aggregateId = the row's id, payload = the JSON value}, what a
+        multilanguage store hands the gateway and republishes. The setting survives set_state_writer; register_program resets it
+        to N.VALUE_JSON."""
+        self._ck(self._lib.sgr_set_state_writer_framing(self._h, framing))
+
     def get_many_values(self, keys: Sequence[str], values_cap: Optional[int] = None) -> List[Optional[bytes]]:
         """The JSON state value of each id (sgr_get_batch_values), None for a None state or an unknown id. values_cap: the byte
         budget of one call (None: sized from the first attempt)."""

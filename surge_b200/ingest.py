@@ -95,13 +95,17 @@ class Ingest:
         return self._h
 
     def set_value_framing(self, framing: int) -> None:
-        """0 = the value is the packed event; 1 = protobuf Event{aggregateId, payload} of the multilanguage module."""
+        """How a record value wraps its event (include/sgr.h SGR_VALUE_*): N.VALUE_PACKED, the value is the packed event;
+        N.VALUE_PROTOBUF_EVENT, the protobuf Event{aggregateId, payload} of the multilanguage module, whose payload is the packed
+        event; N.VALUE_JSON, a flat JSON object read through the member table of set_json_packer; N.VALUE_PROTOBUF_JSON, the
+        multilanguage Event whose payload is such a JSON object (what the gateway writes for an app that serializes its events as
+        JSON). The two JSON framings need set_json_packer first. Event.aggregateId is not read: the record key is the id."""
         self._check(self._lib.sgr_ingest_set_value_framing(self._h, framing))
 
     def set_json_packer(self, discriminator: str, events: Sequence[Tuple[str, int, Sequence[Tuple[str, int, int]]]], unknown_type: int = -1) -> None:
         """events = [(class name, event type index, [(member name, N.JSON_I32 | JSON_I64 | JSON_F64 | JSON_UUID, record byte offset) or
         (member name, N.JSON_PSTR, record byte offset, slot bytes)])].
-        Switches nothing by itself: follow with set_value_framing(N.VALUE_JSON)."""
+        Switches nothing by itself: follow with set_value_framing(N.VALUE_JSON) or set_value_framing(N.VALUE_PROTOBUF_JSON)."""
         self._check(self._lib.sgr_ingest_set_json_packer(self._h, discriminator.encode("utf-8"), json_events(events), len(events), unknown_type))
 
     def set_null_value_type(self, event_type: int) -> None:

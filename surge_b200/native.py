@@ -93,7 +93,7 @@ class sgr_json_event(C.Structure):
 
 JSON_I32, JSON_I64, JSON_F64, JSON_UUID, JSON_PSTR = 0, 1, 2, 3, 4
 JSON_ID = 5  # writer tables only (sgr_set_state_writer): the row's aggregate id
-VALUE_PACKED, VALUE_PROTOBUF_EVENT, VALUE_JSON = 0, 1, 2
+VALUE_PACKED, VALUE_PROTOBUF_EVENT, VALUE_JSON, VALUE_PROTOBUF_JSON = 0, 1, 2, 3
 
 # every symbol include/sgr.h declares: (name, restype, argtypes)
 _P = C.c_void_p
@@ -128,6 +128,7 @@ ABI = [
     ("sgr_scan", C.c_int32, [_P, _P, C.c_uint32, C.c_int32, _P, C.c_uint32, C.c_uint64, _P, _P, _P, _P, C.c_uint64, _P,
                              C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]),
     ("sgr_set_state_writer", C.c_int32, [_P, C.POINTER(sgr_json_field), C.c_uint32]),
+    ("sgr_set_state_writer_framing", C.c_int32, [_P, C.c_int32]),
     ("sgr_get_batch_values", C.c_int32, [_P, _P, _P, C.c_uint64, _P, C.c_uint64, _P, _P, _P, C.POINTER(C.c_uint64)]),
     ("sgr_export_changes_values", C.c_int32, [_P, C.c_uint32, C.POINTER(sgr_changes_cursor), C.c_uint64, _P, C.c_uint64, _P, _P, _P, _P, _P,
                                               C.c_uint64, _P, C.POINTER(C.c_uint64)]),

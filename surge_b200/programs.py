@@ -76,6 +76,24 @@ def int_balance_program() -> N.sgr_fold_program:
     return make_program(16, N.REC_FIXED64, [(N.MATERIALISE, [(N.OP_ADD_I32, 0, 16, 4)])])
 
 
+def csharp_bank_program() -> N.sgr_fold_program:
+    """multilanguage-csharp-sdk Sample/Program.cs:62-80
+        var balance = state.IsSome switch { true => state.ToList().Head().amount, _ => 0 };
+        return bankEvent switch {
+            MoneyWithdrawn m1 => Option<Account>.Some(new Account(balance - m1.Amount)),
+            MoneyDeposited m3 => Option<Account>.Some(new Account(balance + m3.Amount)),
+            _ => Option<Account>.None
+        };
+    = materialise 0 then subtract / add (C# int arithmetic wraps, as SUB_I32 / ADD_I32 do). Type 0 MoneyWithdrawn, type 1
+    MoneyDeposited, type 2 the `_ => None` arm: a JSON packer maps any other "Type" there with unknown_type = 2.
+    record: Amount @16; state: amount @0."""
+    return make_program(16, N.REC_FIXED64, [
+        (N.MATERIALISE, [(N.OP_SUB_I32, 0, 16, 4)]),
+        (N.MATERIALISE, [(N.OP_ADD_I32, 0, 16, 4)]),
+        (N.TOMBSTONE, []),
+    ])
+
+
 def counter_snapshot_restore_program() -> N.sgr_fold_program:
     """Today's recovery in the reference: Kafka Streams materialises the compacted STATE topic into a KTable — last
     write wins per key, a null value deletes (modules/common/src/main/scala/surge/kafka/streams/SurgeStateStoreConsumer.scala:57-76;

@@ -120,16 +120,20 @@ class StateCodec:
     a state-topic store, whose state records go to the table through sgr_put_batch (no extra rules, states of any width).
     writer: a JSON state writer table for ReplayEngine.set_state_writer, [(name, N.JSON_*, program offset[, slot bytes])] or
     (name, N.JSON_ID): the store's reads and on_changes then take the model's JSON value from the device (sgr_get_batch_values,
-    sgr_scan_values, sgr_export_changes_values) instead of calling from_packed, which becomes optional."""
+    sgr_scan_values, sgr_export_changes_values) instead of calling from_packed, which becomes optional.
+    writer_framing: how the device wraps those values, N.VALUE_JSON (the JSON value itself, the default) or N.VALUE_PROTOBUF_JSON
+    (the multilanguage protobuf State around it: what a multilanguage store holds, ReplayEngine.set_state_writer_framing)."""
 
     def __init__(self, to_packed: Callable[[str, bytes], bytes], from_packed: Optional[Callable[[str, bytes], bytes]] = None,
-                 snapshot_type: Optional[int] = None, tombstone_type: Optional[int] = None, writer: Optional[Sequence[Tuple]] = None):
+                 snapshot_type: Optional[int] = None, tombstone_type: Optional[int] = None, writer: Optional[Sequence[Tuple]] = None,
+                 writer_framing: int = N.VALUE_JSON):
         if (snapshot_type is None) != (tombstone_type is None):
             raise ValueError("a codec names both the snapshot and the tombstone type, or neither")
         if from_packed is None and writer is None:
             raise ValueError("a codec decodes rows with from_packed, or has the device write them with a writer table")
         self.to_packed, self.from_packed, self.snapshot_type, self.tombstone_type = to_packed, from_packed, snapshot_type, tombstone_type
         self.writer = None if writer is None else list(writer)
+        self.writer_framing = writer_framing
 
     @property
     def state_topic(self) -> bool:
@@ -175,6 +179,8 @@ class GpuReplayKeyValueStore:
         self._writer = codec is not None and codec.writer is not None
         if self._writer:
             self._engine.set_state_writer(codec.writer)
+            if codec.writer_framing != N.VALUE_JSON:
+                self._engine.set_state_writer_framing(codec.writer_framing)
         self._formatter = state_formatter
         self._keys: List[str] = []
         self._index: Dict[str, int] = {}
