@@ -1,5 +1,6 @@
 """TEST INFRASTRUCTURE — random fold programs and logs for the program tests (tests/test_gpu_program_fuzz.py,
 tests/test_gpu_program_scale.py, tests/test_gpu_var_limits.py, tests/test_gpu_fixed_alignment.py,
+tests/test_gpu_head_plane_matrix.py,
 tests/test_program_oracle_cpu.py).
 
 draw_program / draw_log / interleave / draw_var_program / draw_var_log are the small-case drawers of the fuzz test, moved
@@ -405,6 +406,69 @@ def row_program(rng, user_words, cls, n_src):
         rules.append((ex, ops))
     assert not todo
     return rules
+
+
+# Record words a head-only program reads: the head is record bytes 0..31, word 0 the event type, words 2..3 (the aggregate
+# index in fixed_log) included. A Double field is copied from one of the head's 8-byte pairs, record bytes 8, 16 or 24.
+HEAD_SOURCE_WORDS = list(range(1, 8))
+HEAD_F64_SOURCES = [8, 16, 24]
+
+
+def head_only_program(rng, user_words, cls, n_slots, f64=()):
+    """A program inside the transformer algebra that reads no record word past 7 (fold_rows.cu RowProgram::head_only), so
+    the runs fold may stage it from the head plane. Its ops read exactly n_slots - 1 distinct words of 1..7, so the kernel
+    sees n_slots slots (2..8). f64: state byte offsets of JVM Double fields; each is written by one 8-byte SET from its own
+    head pair (head_f64_sources), and rules without ops hand the instance back. cls 0: MATERIALISE / CREATE / TOMBSTONE /
+    THROW; cls 1: IF_EXISTS / CREATE / TOMBSTONE / THROW. Type 0 builds a state, type 1 carries the class."""
+    n_src = int(n_slots) - 1
+    f64 = [int(o) for o in f64]
+    assert 1 <= n_src <= len(HEAD_SOURCE_WORDS) and len(f64) <= len(HEAD_F64_SOURCES)
+    f64_words = [w for off in f64 for w in (off // 4, off // 4 + 1)]
+    assert all(off % 4 == 0 for off in f64) and len(set(f64_words)) == len(f64_words) and max(f64_words, default=0) < user_words
+    pairs = [int(s) for s in rng.permutation(HEAD_F64_SOURCES)[:len(f64)]]
+    pair_words = {w for s in pairs for w in (s // 4, s // 4 + 1)}
+    assert len(pair_words) <= n_src, "the Double sources are more words than n_slots allows"
+    rest = [w for w in HEAD_SOURCE_WORDS if w not in pair_words]
+    singles = [int(w) for w in rng.choice(rest, size=n_src - len(pair_words), replace=False)]
+    pool = sorted(pair_words | set(singles))
+    base = I.MATERIALISE if cls == 0 else I.IF_EXISTS
+    free = [w for w in range(user_words) if w not in f64_words]        # state words the 4-byte ops write
+    assert free or not singles
+    per_rule = max(1, min(len(free), 8 - len(f64)))                    # a rule holds at most 8 ops (SGR_MAX_OPS)
+    n_op_rules = 2 + (-(-len(singles) // per_rule))
+    n_types = min(16, n_op_rules + int(rng.integers(2, 6)))
+    exists = [I.MATERIALISE if cls == 0 else I.CREATE, base]
+    exists += [int(rng.choice([base, I.CREATE])) for _ in range(2, n_op_rules)]
+    exists += [int(rng.choice([base, base, I.CREATE, I.TOMBSTONE, I.THROW])) for _ in range(n_op_rules, n_types)]
+    todo = list(singles)
+    rng.shuffle(todo)
+    rules = []
+    for t, ex in enumerate(exists):
+        ops = []
+        if ex not in (I.TOMBSTONE, I.THROW):
+            if t == 0 or (f64 and rng.random() < 0.3):               # a Double copy, alone or beside 4-byte ops
+                ops += [(I.OP_SET, off, src, 8) for off, src in zip(f64, pairs)]
+            words = [int(w) for w in rng.permutation(free)][:8 - len(ops)]
+            if t < n_op_rules:
+                n_ops = len(words) if todo else int(rng.integers(0, len(words) + 1))
+            else:
+                n_ops = int(rng.integers(0, min(len(words), 4) + 1)) if rng.random() < 0.7 else 0
+            for w in words[:n_ops]:
+                src = todo.pop() if todo else int(rng.choice(pool))
+                ops.append((int(rng.choice([I.OP_SET, I.OP_ADD_I32, I.OP_SUB_I32])), 4 * w, 4 * src, 4))
+        rules.append((ex, ops))
+    assert not todo and row_slots(rules) == n_slots, (rules, n_slots)
+    return rules
+
+
+def head_f64_sources(rules, f64):
+    """Record byte offsets the Double fields f64 of a head_only_program are copied from."""
+    return sorted({src for _, ops in rules for opc, dst, src, ln in ops if ln == 8 and dst in f64})
+
+
+def reads_head_only(rules):
+    """fold_rows.cu RowProgram::head_only for a program build_row_program accepts: no op reads a record word past 7."""
+    return all(src + ln <= 32 for ex, ops in rules if ex not in (I.TOMBSTONE, I.THROW) for _, _, src, ln in ops)
 
 
 # ------------------------------------------------------------------ named programs the fixed-record GPU tests share

@@ -2193,7 +2193,8 @@ int32_t sgr_set_option(sgr_engine* e, const char* name, int64_t value) {
   if (!strcmp(name, "var_stage_bytes")) { e->opt_var_stage_bytes = value; return SGR_OK; }
   if (!strcmp(name, "var_stages")) { e->opt_var_stages = (value >= 1 && value <= 3) ? value : 2; return SGR_OK; }
   if (!strcmp(name, "run_variant")) {
-    if (value < 0 || value >= run_variant_count()) return fail(e, SGR_ERR_INVALID, "run_variant out of range");
+    // -1: automatic again (run variant 0, or the head plane), as on a fresh engine
+    if (value < -1 || value >= run_variant_count()) return fail(e, SGR_ERR_INVALID, "run_variant out of range");
     e->opt_run_variant = value; return SGR_OK;
   }
   // test aid: the look-back epoch the next record-parallel fold moves on from (a value near 2^32 makes a few folds wrap it)

@@ -48,10 +48,13 @@ def same(got, want, what):
         raise AssertionError(f"{what}: {len(bad)} of {len(want)} states differ; first {bad[:6]}\n got {got[bad[0]].tolist()}\nwant {want[bad[0]].tolist()}")
 
 
-def check(e, want, nev, nerr, what):
+def check(e, want, nev, nerr, what, plane=None):
+    """plane: the stats().head_plane the fold must report (1: it staged the record heads from the head plane)."""
     same(e.export_states(), want, what)
     st = e.stats()
     assert (st.n_events, st.n_errors) == (nev, nerr), f"{what}: stats (n_events, n_errors) = {(st.n_events, st.n_errors)}, oracle {(nev, nerr)}"
+    if plane is not None:
+        assert st.head_plane == plane, f"{what}: head_plane = {st.head_plane}, expected {plane}"
 
 
 def oracle(rules, sb, log, seg, prior=None, f64=()):
@@ -132,9 +135,17 @@ def test_record_parallel_kernels_at_an_unaligned_log_start(name, W, cls, n_src, 
         e.set_option("run_variant", 0)
         for kernel in ([3] if W == 2 else []) + [0, 1]:
             fold(e, kernel)
-            check(e, want, nev, nerr, f"{what}: kernel {kernel}")
+            check(e, want, nev, nerr, f"{what}: kernel {kernel}", plane=0)
             fold(e, kernel, prior=want)
-            check(e, want2, nev2, nerr2, f"{what}: kernel {kernel} on prior states")
+            check(e, want2, nev2, nerr2, f"{what}: kernel {kernel} on prior states", plane=0)
+        # automatic selection: a program that reads only record words 0..7 folds from the head plane
+        plane = int(PC.reads_head_only(rules))
+        for hp in (1, 0):
+            fold(e, 0, run_variant=-1, head_plane=hp)
+            check(e, want, nev, nerr, f"{what}: automatic selection, head_plane option {hp}", plane=plane * hp)
+            fold(e, 0, prior=want)
+            check(e, want2, nev2, nerr2, f"{what}: automatic selection, head_plane option {hp}, on prior states", plane=plane * hp)
+        e.set_option("run_variant", 0)
         # back-to-back folds of the same log, no wait in between: each overlaps the one before it
         e.set_option("kernel", 2)
         for _ in range(4):
@@ -204,9 +215,9 @@ def test_w14_double_program_at_an_unaligned_log_start(start):
             e.load_events(log, seg)
             for kernel in (0, 2, 1):
                 fold(e, kernel)
-                check(e, want, nev, nerr, f"{what}: kernel {kernel}")
+                check(e, want, nev, nerr, f"{what}: kernel {kernel}", plane=0)      # it reads record words 12..15
                 fold(e, kernel, prior=prior)
-                check(e, want2, nev2, nerr2, f"{what}: kernel {kernel} on a mixed prior table")
+                check(e, want2, nev2, nerr2, f"{what}: kernel {kernel} on a mixed prior table", plane=0)
 
 
 # ------------------------------------------------------------------ b. every 16-byte address class of a device log
@@ -215,6 +226,7 @@ def test_device_log_at_every_16_byte_address_class():
 
     rng = np.random.default_rng(74000)
     row_rules = PC.row_program(rng, 2, 0, 3)
+    row_plane = int(PC.reads_head_only(row_rules))
     sb32, lane_rules = OUTSIDE["materialise_and_if_exists_32B"]
     with ReplayEngine(0) as er, ReplayEngine(0) as el:
         er.register_program(P.make_program(16, N.REC_FIXED64, row_rules))
@@ -234,7 +246,10 @@ def test_device_log_at_every_16_byte_address_class():
                 er.load_events(dev, offs)
                 for kernel in (0, 3, 1):
                     fold(er, kernel)
-                    check(er, want, nev, nerr, f"{what}: kernel {kernel}")
+                    check(er, want, nev, nerr, f"{what}: kernel {kernel}", plane=row_plane if kernel == 0 else 0)
+                fold(er, 0, head_plane=0)
+                check(er, want, nev, nerr, f"{what}: kernel 0, head_plane option 0", plane=0)
+                er.set_option("head_plane", 1)
                 el.load_events(dev, offs)
                 fold(el, 0)
                 check(el, want_l, nev_l, nerr_l, f"{what}: lane-sequential program")
@@ -273,7 +288,12 @@ def test_at_scale_one_start_class_per_kernel_family(family, start):
                 check(e, want2, nev2, nerr2, f"{what}: run_variant {v} on prior states")
             e.set_option("run_variant", 0)
             fold(e, 0)
-            check(e, want, nev, nerr, f"{what}: automatic selection")
+            check(e, want, nev, nerr, f"{what}: kernel 0, run_variant 0", plane=0)
+            plane = int(PC.reads_head_only(rules))
+            fold(e, 0, run_variant=-1)
+            check(e, want, nev, nerr, f"{what}: automatic selection", plane=plane)
+            fold(e, 0, prior=want)
+            check(e, want2, nev2, nerr2, f"{what}: automatic selection on prior states", plane=plane)
         elif family == "rows":
             fold(e, 3)
             check(e, want, nev, nerr, f"{what}: rows kernel")

@@ -30,27 +30,40 @@ def assert_same(got, want, what=""):
 
 
 def pipelined(prog, rec, off, k, *, chunk=None, init=None, from_none=True, kernel=0):
-    """k fold_async calls with no wait in between; returns the table, the stats and one synchronous fold's table."""
-    with ReplayEngine(0) as e:
-        e.register_program(prog)
-        e.set_option("kernel", kernel)
-        if chunk is not None:
-            e.set_option("run_chunk_bytes", chunk)
-        if init is not None:
-            e.set_initial_states(init)
-        e.load_events(rec, off)
-        for _ in range(k):
-            if from_none:
+    """k fold_async calls with no wait in between; returns the table, the stats and one synchronous fold's table.
+    Under automatic selection ("kernel" 0) the Counter folds from the head plane (stats().head_plane 1); the same pipeline
+    is then run again with "head_plane" 0, on the log, and must give the same tables and counts."""
+    arms = []
+    for head_plane in ([1, 0] if kernel == 0 else [1]):
+        with ReplayEngine(0) as e:
+            e.register_program(prog)
+            e.set_option("kernel", kernel)
+            e.set_option("head_plane", head_plane)
+            if chunk is not None:
+                e.set_option("run_chunk_bytes", chunk)
+            if init is not None:
+                e.set_initial_states(init)
+            e.load_events(rec, off)
+            for _ in range(k):
+                if from_none:
+                    e.set_initial_states(None)
+                e.fold_async()
+            e.wait()
+            got, st = e.export_states(), e.stats()
+            if init is not None:
+                e.set_initial_states(init)
+            else:
                 e.set_initial_states(None)
-            e.fold_async()
-        e.wait()
-        got, st = e.export_states(), e.stats()
-        if init is not None:
-            e.set_initial_states(init)
-        else:
-            e.set_initial_states(None)
-        e.fold()
-        one = e.export_states()
+            e.fold()
+            one = e.export_states()
+            want_plane = int(kernel == 0 and head_plane == 1)
+            assert st.head_plane == want_plane and e.stats().head_plane == want_plane, f"head_plane {st.head_plane}, expected {want_plane}"
+        arms.append((got, st, one))
+    got, st, one = arms[0]
+    for got_log, st_log, one_log in arms[1:]:
+        assert_same(got_log, got, "pipelined, head_plane 0 against the plane")
+        assert_same(one_log, one, "synchronous, head_plane 0 against the plane")
+        assert (st_log.n_events, st_log.n_errors) == (st.n_events, st.n_errors)
     return got, st, one
 
 

@@ -18,7 +18,7 @@ import pytest
 
 from oracle import program_corpus as PC
 from oracle import program_interp as I
-from surge_b200 import ReplayEngine
+from surge_b200 import ReplayEngine, SgrError
 from surge_b200 import native as N
 from surge_b200 import programs as P
 
@@ -176,6 +176,12 @@ def test_forced_kernel_options_fold_the_log():
         e.set_option("run_variant", 0)
         fold(e)
         check(e, want, nev, nerr, 0, "run_variant 0")
+        e.set_option("run_variant", -1)   # automatic selection again, as on a fresh engine
+        fold(e)
+        check(e, want, nev, nerr, 1, "run_variant -1 after run_variant 0")
+        with pytest.raises(SgrError) as ei:
+            e.set_option("run_variant", -2)
+        assert ei.value.code == N.SGR_ERR_INVALID
 
 
 # ------------------------------------------------------------------ d. the plane's lifetime

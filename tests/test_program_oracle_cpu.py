@@ -312,6 +312,73 @@ def test_the_wide_draws_cover_what_the_pin_claims():
         assert {cap - 1, cap, cap + 1} <= set(lens.tolist()) and lens.max() > 2064, cap
 
 
+def draw_head_only_case(seed):
+    """One head-only program per seed (oracle/program_corpus.py head_only_program): state widths 16 / 32 / 64, class 0 and
+    1, every slot count 2..8 in turn, and on every other round a 64-byte program with a Double at +8 copied from a head
+    pair; a log that starts past byte 0, with special Doubles where the program reads one."""
+    rng = np.random.default_rng(39000 + seed)
+    W, cls, n_slots = [2, 6, 14][seed % 3], (seed // 3) % 2, 2 + (seed // 6) % 7
+    f64 = [8] if W == 14 and (seed // 42) % 2 and n_slots >= 3 else []
+    rules = PC.head_only_program(rng, W, cls, n_slots, f64)
+    counts = rng.geometric(1 / 6, size=120) - 1
+    counts[int(rng.integers(0, 120))] = 150
+    rec, off, _ = PC.fixed_log(rng, rules, counts, f64_offsets=PC.head_f64_sources(rules, f64), pad_records=int(rng.integers(0, 3)),
+                               p_throw=0.01)
+    return W, cls, n_slots, f64, rules, rec.reshape(-1), off, counts
+
+
+@pytest.mark.parametrize("seed", range(336))
+def test_head_only_programs_match_the_interpreter(seed):
+    """The compiled oracle equals the interpreter on the head-only draws, from None and on top of the first table."""
+    W, cls, n_slots, f64, rules, log, seg, counts = draw_head_only_case(seed)
+    sb = 4 * W + 8
+    what = f"seed {seed} W {W} class {cls} n_slots {n_slots} rules {rules} f64 {f64}"
+    recs = log[int(seg[0]):]
+    want = I.fold(rules, sb, recs, seg, f64_fields=f64)
+    got, nev, nerr = I.c_fold(rules, sb, recs, seg, f64_fields=f64)
+    same(got, want, what)
+    assert (nev, nerr) == implied_stats(want, sb, counts), what
+    want2 = I.fold(rules, sb, recs, seg, initial=want, f64_fields=f64)
+    got2, nev2, nerr2 = I.c_fold(rules, sb, recs, seg, initial=want, f64_fields=f64)
+    same(got2, want2, what + " with prior states")
+    assert (nev2, nerr2) == implied_stats(want2, sb, counts), what
+
+
+def test_the_head_only_draws_cover_what_the_pin_claims():
+    """Every (state width, class, slot count 2..8) and the 64-byte Double at every slot count it fits; every draw stays
+    inside the transformer algebra (32-bit ops or 8-byte Double copies, no state word written twice by one rule, never
+    MATERIALISE beside IF_EXISTS) and reads only record words 1..7, words 2..3 among them; a Double is copied alone by
+    some rule, and a rule without ops hands the instance back."""
+    seen = set()
+    for seed in range(336):
+        W, cls, n_slots, f64, rules, log, _, _ = draw_head_only_case(seed)
+        seen.add((W, cls, n_slots, bool(f64)))
+        kinds = {ex for ex, _ in rules}
+        assert not {I.MATERIALISE, I.IF_EXISTS} <= kinds and len(rules) <= 16, seed
+        assert PC.reads_head_only(rules) and PC.row_slots(rules) == n_slots, seed
+        for ex, ops in rules:
+            assert len(ops) <= 8, seed
+            written = [w for opc, dst, _, ln in ops for w in range(dst // 4, (dst + ln) // 4)]
+            assert len(written) == len(set(written)) and max(written, default=0) < W, seed
+            for opc, dst, src, ln in ops:
+                assert 4 <= src and src + ln <= 32, seed
+                assert (opc in (I.OP_SET, I.OP_ADD_I32, I.OP_SUB_I32) and ln == 4) or (opc == I.OP_SET and ln == 8 and dst in f64), seed
+                if 8 <= src < 16:
+                    seen.add("reads words 2..3")
+            if ex not in (I.TOMBSTONE, I.THROW) and not ops:
+                seen.add("hands the instance back")
+            if f64 and ops and all(ln == 8 for _, _, _, ln in ops):
+                seen.add("copies the Double alone")
+        for src in PC.head_f64_sources(rules, f64):
+            vals = log.reshape(-1, 64)[:, src:src + 8].copy().view(np.float64).ravel()
+            if np.isnan(vals).any() and (vals == 0).any():
+                seen.add("special Doubles in the log")
+    want = {(W, cls, s, False) for W in (2, 6, 14) for cls in (0, 1) for s in range(2, 9)}
+    want |= {(14, cls, s, True) for cls in (0, 1) for s in range(3, 9)}
+    assert want <= seen, sorted(want - seen)
+    assert {"reads words 2..3", "hands the instance back", "copies the Double alone", "special Doubles in the log"} <= seen, seen
+
+
 SAMPLE_MODELS = [("counter", O.MODEL_COUNTER, P.counter_program), ("ml_counter", O.MODEL_ML_COUNTER, P.ml_counter_program),
                  ("int_balance", O.MODEL_INT_BALANCE, P.int_balance_program), ("bank_account", O.MODEL_BANK_ACCOUNT, P.bank_account_program)]
 
