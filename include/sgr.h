@@ -188,8 +188,9 @@ typedef struct sgr_stats {
                                to its last warp's exit by %globaltimer, every other fold by CUDA events around it */
   float    ms_d2h;          /* device->host copy of the last export */
   uint32_t fold_launches;   /* kernels launched by the last fold */
-  uint32_t head_plane;      /* 1: the last fold read each record's 32-byte head from the head plane, not the log */
-  uint32_t reserved[6];
+  uint32_t head_plane;      /* 1: the last fold read its records from a plane (plane_bytes), not the log */
+  uint32_t plane_bytes;     /* record bytes of that plane: 16 (slot plane), 32 (head plane), 0 (the fold read the log) */
+  uint32_t reserved[5];
 } sgr_stats;
 
 int32_t sgr_abi_version(void);
@@ -213,11 +214,14 @@ int32_t sgr_load_events(sgr_engine* e, const void* events, uint64_t nbytes,
 /* The device log and offsets are borrowed: they must stay allocated and unmodified while they are loaded (until the next
  * load or sgr_destroy). The engine may keep derived copies of them, such as the head plane below, that a change would
  * leave stale; to fold changed records, load them again.
- * Head plane: for a fixed-record log whose segments are 64-byte aligned and a program that reads no record word past
- * word 7, the engine keeps bytes 0..31 of every record in a dense plane of half the log's size, and the record-parallel
- * fold reads that instead of the log. A host load builds it behind the copy; a borrowed log gets it from the first fold
- * that uses it. Every load and sgr_register_program drops it; if it cannot be allocated the fold reads the log.
- * sgr_set_option("head_plane", 0) keeps every fold on the log. */
+ * Planes: for a fixed-record log whose segments are 64-byte aligned and a program that reads no record word past word 7,
+ * the engine keeps a dense plane of the records and the record-parallel fold reads that instead of the log. A class-0
+ * program with a 16-byte state and at most 4 slots (the record words it reads, the type word included) gets the slot
+ * plane: those words of every record, 16 bytes per record, a quarter of the log's size. Any other such program gets the
+ * head plane: bytes 0..31 of every record, half the log's size. A host load builds the plane behind the copy; a
+ * borrowed log gets it from the first fold that uses it. Every load and sgr_register_program drops it; if it cannot be
+ * allocated the fold reads the log. sgr_set_option("head_plane", 0) keeps every fold on the log; ("head_variant", v >= 0)
+ * keeps a slot-plane program on the head plane; ("proj_variant", v) picks the slot-plane kernel configuration. */
 int32_t sgr_load_events_device(sgr_engine* e, const void* d_events, uint64_t nbytes,
                                const uint64_t* d_seg_offsets, uint64_t n_agg);
 

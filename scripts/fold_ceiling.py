@@ -8,11 +8,15 @@ On the log bench.py folds (synth.counter_csr_device(2^20, 32, seed=2): 2^20 aggr
   (d) the read probe over a dense buffer of half the log's bytes: the head plane the Counter fold stages instead of the
       log (32 bytes per record), and the fold from the head plane under each --head-variants entry, against (c) on the log
       ("head_plane" 0);
-  (e) a load of the borrowed log followed by one fold, which builds the head plane, against the same with "head_plane" 0;
-and reports each as GB/s over the log's bytes and the fold as a share of (a) (the head-plane folds: of (d)). Prints one JSON document and writes it to
+  (e) a load of the borrowed log followed by one fold, which builds its plane, against the same with "head_plane" 0;
+  (f) the read probe over a dense buffer of a quarter of the log's bytes: the slot plane the Counter fold stages by default
+      (its slot words 0, 4, 1 and a zero word, 16 bytes per record, gathered here with torch), and the fold from the slot
+      plane under each --proj-variants entry;
+and reports each as GB/s over the log's bytes and the fold as a share of (a) (the head-plane folds: of (d), the slot-plane
+folds: of (f)). Prints one JSON document and writes it to
 OUT/fold_ceiling.json. The card's name and power limit are part of the numbers and are recorded with them.
 
-    python scripts/fold_ceiling.py --out DIR [--reps 30] [--steps 200] [--head-variants 0,1,2,3,4]
+    python scripts/fold_ceiling.py --out DIR [--reps 30] [--steps 200] [--head-variants 0,1,2,3,4] [--proj-variants 0,1,2,3]
 """
 from __future__ import annotations
 
@@ -51,6 +55,8 @@ def main() -> None:
                     help="comma list of the fold's run_chunk_bytes to measure (0: the engine's default)")
     ap.add_argument("--head-variants", type=lambda s: [int(x) for x in s.split(",")], default=[0],
                     help="comma list of head_variant values of the head-plane fold to measure")
+    ap.add_argument("--proj-variants", type=lambda s: [int(x) for x in s.split(",")], default=[0],
+                    help="comma list of proj_variant values of the slot-plane fold to measure")
     args = ap.parse_args()
 
     import torch
@@ -95,6 +101,16 @@ def main() -> None:
     del plane
     for hv in args.head_variants:
         out.update(measure_fold(log, off, dev, 0, args.reps, args.steps, f"_head_variant{hv}", {"head_variant": hv}))
+    # the Counter's slot words (RowProgram::slot_word: the type, `by`, `seq`) in slot order, zero-padded to 16 bytes
+    words = log.view(torch.int32).view(-1, 16)
+    slots = torch.zeros(words.shape[0], 4, dtype=torch.int32, device=dev)
+    slots[:, :3] = words[:, [0, 4, 1]]
+    slots = slots.view(torch.uint8).reshape(-1)
+    out["f_read_probe_slot_plane_fixed_spans"] = summary(probe(0, slots), nbytes)
+    out["f_read_probe_slot_plane_ticketed"] = summary(probe(1, slots), nbytes)
+    del slots, words
+    for pv in args.proj_variants:
+        out.update(measure_fold(log, off, dev, 0, args.reps, args.steps, f"_proj_variant{pv}", {"proj_variant": pv}))
     out.update(measure_load_then_fold(log, off, dev, args.reps))
 
     a = out["a_read_probe_fixed_spans"]["ms_min"]
@@ -103,6 +119,9 @@ def main() -> None:
     d = out["d_read_probe_dense_plane_fixed_spans"]["ms_min"]
     out["head_fold_share_of_dense_probe"] = {k: d / v["ms_min"] for k, v in out.items()
                                              if k.startswith(("c_fold_alone_events", "c_fold_back")) and "head_variant" in k}
+    f = out["f_read_probe_slot_plane_fixed_spans"]["ms_min"]
+    out["slot_fold_share_of_slot_probe"] = {k: f / v["ms_min"] for k, v in out.items()
+                                            if k.startswith(("c_fold_alone_events", "c_fold_back")) and "proj_variant" in k}
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, "fold_ceiling.json"), "w") as f:
         json.dump(out, f, indent=1)
@@ -156,7 +175,8 @@ def measure_fold(log, off, dev: str, chunk_bytes: int, reps: int, steps: int, su
         e1.record(s)
         eng.wait()
         runs.append(e0.elapsed_time(e1) / steps)
-    out["c_fold_back_to_back" + suffix] = dict(summary(runs, nbytes), steps=steps, head_plane=int(eng.stats().head_plane))
+    st = eng.stats()
+    out["c_fold_back_to_back" + suffix] = dict(summary(runs, nbytes), steps=steps, head_plane=int(st.head_plane), plane_bytes=int(st.plane_bytes))
     eng.close()
     return out
 
@@ -186,7 +206,7 @@ def measure_load_then_fold(log, off, dev: str, reps: int) -> dict:
             ms.append((time.perf_counter() - t0) * 1e3)
             fold_ms.append(float(eng.stats().ms_fold))
         out[f"e_load_then_fold_head_plane{plane}"] = dict(summary(ms[2:], log.numel()), fold_ms_min=min(fold_ms[2:]),
-                                                          head_plane=int(eng.stats().head_plane))
+                                                          head_plane=int(eng.stats().head_plane), plane_bytes=int(eng.stats().plane_bytes))
         eng.close()
     return out
 

@@ -77,7 +77,7 @@ struct PendingFold {
   uint64_t n_seg = 0, event_bytes = 0;
   const uint8_t* events = nullptr; const uint64_t* offsets = nullptr; const uint32_t* ids = nullptr;
   const void* counters = nullptr;
-  bool heads = false;     // the runs fold staged the head plane
+  uint32_t plane = 0;     // record bytes of the plane the runs fold staged: 16 (slot plane), 32 (head plane), 0 (the log)
 };
 }  // namespace
 
@@ -117,7 +117,7 @@ struct sgr_engine {
   bool row_ok = false;            // program is inside the transformer algebra
   RowProgram row_prog{};
   int row_max_grid = 0;
-  int run_max_grid = 0, run_max_grid_variant = -2, run_max_grid_head = -2;  // -2: not yet sized
+  int run_max_grid = 0, run_max_grid_variant = -2, run_max_grid_plane = -2;  // -2: not yet sized
   int64_t opt_run_variant = -1;   // -1: automatic (run variant 0, or the head plane); >= 0 forces that variant on the log
   DevBuf part_flags, part_data, redo_ids;
   DevBuf run_counters;            // 2 x 16 u64, ping-pong; the runs kernel zeroes the other block itself
@@ -128,14 +128,17 @@ struct sgr_engine {
   size_t part_flags_cap_seen = 0;
   bool offsets_aligned64 = false; // every segment offset == log_begin (mod 64)
   uint64_t log_begin = 0, log_end = 0, max_seg_bytes = 0;
-  // The head plane (fold_runs.cu): bytes 0..31 of every record of the loaded log, 32 bytes apart, for programs that read no
-  // record word past 7 (RowProgram::head_only). A derived copy: every load and program registration drops it, the first runs
-  // fold that can read it builds it from the log (a host load builds it behind its copy), and a borrowed log must not change
-  // while it is loaded. If its memory cannot be had, the fold reads the log.
+  // The plane (fold_runs.cu), for programs that read no record word past 7 (RowProgram::head_only): the slot plane, each
+  // record's slot words 16 bytes apart (slot_plane_fits), or else the head plane, bytes 0..31 of every record 32 bytes
+  // apart. A derived copy: every load and program registration drops it, the first runs fold that can read it builds it
+  // from the log (a host load builds it behind its copy), and a borrowed log must not change while it is loaded. If its
+  // memory cannot be had, the fold reads the log.
   DevBuf head_plane;
   enum PlaneState { kPlaneNone, kPlaneValid, kPlaneNoMemory } plane_state = kPlaneNone;
+  uint32_t plane_bytes = 0;       // record bytes of the plane plane_state describes (16 or 32)
   int64_t opt_head_plane = 1;     // 0: the runs fold always reads the log
-  int64_t opt_head_variant = 0;
+  int64_t opt_head_variant = -1;  // -1: automatic (the slot plane where the program fits it); >= 0: the head plane, that variant
+  int64_t opt_proj_variant = 0;   // the slot plane's kernel configuration
   Stream side_stream;             // a host load builds the plane here, chunk by chunk behind the copy
   Event ev_copied, ev_split;
   bool fold_pending = false;      // a fold was enqueued and not yet finished (it is `pending`)
@@ -352,21 +355,39 @@ bool plane_wanted(const sgr_engine* e) {
          e->program.record_kind == SGR_REC_FIXED64 && e->offsets_aligned64 && e->log_end > e->log_begin;
 }
 
-// Build the head plane of the loaded log on the stream unless it is there. *ok: the plane is (or will be, in stream order)
-// valid; false when its memory cannot be had, once per load.
-int32_t ensure_plane(sgr_engine* e, bool* ok, bool* built) {
-  *ok = e->plane_state == sgr_engine::kPlaneValid; *built = false;
+// Record bytes of the plane a head-only program folds from: the slot plane (16) when the program fits it and no head
+// variant is forced, else the head plane (32). An explicit head_variant keeps the 32-byte plane, as an explicit
+// run_variant keeps the fold on the log.
+uint32_t plane_record_bytes(const sgr_engine* e) { return slot_plane_fits(e->row_prog) && e->opt_head_variant < 0 ? 16u : 32u; }
+
+// Write the plane of `rec` bytes per record for records [r0, r1) of the log at `log` on `st`.
+cudaError_t build_plane(sgr_engine* e, const uint8_t* log, uint32_t rec, uint64_t r0, uint64_t r1, cudaStream_t st) {
+  uint8_t* p = (uint8_t*)e->head_plane.p;
+  return rec == 16 ? launch_build_slots(log, p, r0, r1, e->row_prog, e->num_sms, st) : launch_build_heads(log, p, r0, r1, e->num_sms, st);
+}
+
+// Build the plane of the loaded log on the stream unless it is there in the layout the fold wants (a plane of the other
+// layout is rebuilt). *plane: the record bytes of the plane that is (or will be, in stream order) valid; 0 when its memory
+// cannot be had, once per load and layout.
+int32_t ensure_plane(sgr_engine* e, uint32_t* plane, bool* built) {
+  const uint32_t rec = plane_record_bytes(e);
+  *plane = 0; *built = false;
+  if (e->plane_bytes != rec) e->plane_state = sgr_engine::kPlaneNone;
+  if (e->plane_state == sgr_engine::kPlaneValid) *plane = rec;
   if (e->plane_state != sgr_engine::kPlaneNone) return SGR_OK;
+  e->plane_bytes = rec;
   const uint64_t n_rec = (e->log_end - e->log_begin) / 64;
-  if (e->head_plane.reserve(n_rec * 32) != cudaSuccess) {
+  // a plane of the other layout may be growing under a fold still queued: the old block is freed only once it is done
+  if (e->fold_pending && e->head_plane.cap < n_rec * rec) CUDA_TRY(e, cudaStreamSynchronize(e->stream));
+  if (e->head_plane.reserve(n_rec * rec) != cudaSuccess) {
     (void)cudaGetLastError();   // a failed allocation is not sticky; the fold reads the log instead
     e->plane_state = sgr_engine::kPlaneNoMemory;
     return SGR_OK;
   }
-  cudaError_t le = launch_build_heads(e->d_events + e->log_begin, (uint8_t*)e->head_plane.p, 0, n_rec, e->num_sms, e->stream);
-  if (le != cudaSuccess) return fail(e, SGR_ERR_CUDA, "head plane build: %s", cudaGetErrorString(le));
+  cudaError_t le = build_plane(e, e->d_events + e->log_begin, rec, 0, n_rec, e->stream);
+  if (le != cudaSuccess) return fail(e, SGR_ERR_CUDA, "plane build: %s", cudaGetErrorString(le));
   e->plane_state = sgr_engine::kPlaneValid;
-  *ok = *built = true;
+  *plane = rec; *built = true;
   return SGR_OK;
 }
 
@@ -384,9 +405,10 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
   if (use_rows && e->opt_kernel == 3 && (e->row_prog.user_words != 2 || e->row_prog.cls != 0 || e->row_prog.n_slots > 6 || e->row_prog.f64_mask))
     return fail(e, SGR_ERR_UNSUPPORTED, "the record-per-lane kernel takes 16-byte class-0 programs only");
   const bool runs = use_rows && e->opt_kernel != 3;
-  bool heads = false, plane_built = false;
+  uint32_t plane = 0;
+  bool plane_built = false;
   if (runs && plane_wanted(e) && d_events == e->d_events && d_offsets == e->d_offsets && !d_ids) {
-    int32_t rc = ensure_plane(e, &heads, &plane_built); if (rc) return rc;
+    int32_t rc = ensure_plane(e, &plane, &plane_built); if (rc) return rc;
   }
   unsigned long long* counters = (unsigned long long*)e->counters.p;
   if (runs) {
@@ -399,11 +421,11 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
     CUDA_TRY(e, cudaMemsetAsync(e->counters.p, 0, 64, e->stream));
   }
   // A runs fold queued right behind a runs fold of the same log overlaps it (programmatic dependent launch): before its
-  // griddepcontrol.wait it reads only the log (or its head plane), the offsets and the program, which the fold before it does
-  // not write. Behind anything else (a group-by or decode kernel that writes the log, a plane build, a copy) it is launched
-  // plainly.
+  // griddepcontrol.wait it reads only the log (or its plane), the offsets and the program, which the fold before it does
+  // not write. Behind anything else (a group-by or decode kernel that writes the log, a plane build, a copy, a fold from
+  // the other layout, whose plane buffer this one may have rebuilt) it is launched plainly.
   const bool overlap = runs && !plane_built && e->fold_pending && e->pending.kernel == PendingFold::kRuns && e->pending.events == d_events &&
-                       e->pending.offsets == d_offsets && e->pending.ids == d_ids && e->pending.heads == heads;
+                       e->pending.offsets == d_offsets && e->pending.ids == d_ids && e->pending.plane == plane;
   // an overlapping fold stamps its own start and end (counters[8], [9]): an event between two folds would keep the next
   // one from starting while this one drains. Every other fold is timed by CUDA events around its launch.
   if (!overlap) CUDA_TRY(e, cudaEventRecord(e->ev0, e->stream));
@@ -435,24 +457,26 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
   if (n_seg && kernel != PendingFold::kVarRuns) {
     if (use_rows) {
       const bool v1 = e->opt_kernel == 3;
-      const int rv = (int)e->opt_run_variant;
-      const int hv = heads ? (int)e->opt_head_variant : -1;
+      // the variant within the staged layout's table: run variant (the log), head variant, projected variant
+      const int rv = plane == 16 ? (int)e->opt_proj_variant : plane == 32 ? (e->opt_head_variant < 0 ? 0 : (int)e->opt_head_variant)
+                                                                          : (int)e->opt_run_variant;
+      const int pl = (int)plane;
       if (v1 && !e->row_max_grid) e->row_max_grid = row_kernel_max_grid(e->num_sms, e->row_prog);
-      if (!v1 && (e->run_max_grid_variant != rv || e->run_max_grid_head != hv)) {
-        e->run_max_grid = run_kernel_max_grid(e->num_sms, rv, hv, e->row_prog); e->run_max_grid_variant = rv; e->run_max_grid_head = hv;
+      if (!v1 && (e->run_max_grid_variant != rv || e->run_max_grid_plane != pl)) {
+        e->run_max_grid = run_kernel_max_grid(e->num_sms, rv, pl, e->row_prog); e->run_max_grid_variant = rv; e->run_max_grid_plane = pl;
       }
       const int max_grid = v1 ? e->row_max_grid : e->run_max_grid;
       const int wpc = v1 ? kRowThreads / 32 : run_warps_per_cta();
-      const uint64_t step_bytes = v1 ? 2048 : (uint64_t)run_variant_step_bytes(rv, hv, e->row_prog);
+      const uint64_t step_bytes = v1 ? 2048 : (uint64_t)run_variant_step_bytes(rv, pl, e->row_prog);
       const uint64_t steps = (log_end - log_begin + step_bytes - 1) / step_bytes;
       // the runs kernel publishes a look-back partial per chunk of chunk_steps steps, the rows kernel one per warp; a
       // small log is cut into smaller chunks, so that every resident warp gets one
-      const uint64_t chunk_steps = v1 ? 1 : run_variant_chunk_steps(rv, hv, e->row_prog, (uint64_t)e->opt_run_chunk_bytes, steps, (uint64_t)max_grid * wpc);
+      const uint64_t chunk_steps = v1 ? 1 : run_variant_chunk_steps(rv, pl, e->row_prog, (uint64_t)e->opt_run_chunk_bytes, steps, (uint64_t)max_grid * wpc);
       const uint64_t n_chunks = (steps + chunk_steps - 1) / chunk_steps;
       const uint64_t n_parts = v1 ? (uint64_t)max_grid * wpc : n_chunks;
       int32_t rc = begin_lookback(e, n_parts, e->row_prog.user_words + 2); if (rc) return rc;
       RowArgs r{};
-      r.events = d_events; r.heads = heads ? (const uint8_t*)e->head_plane.p : nullptr; r.seg_offsets = d_offsets; r.seg_ids = d_ids; r.n_seg = n_seg;
+      r.events = d_events; r.heads = plane ? (const uint8_t*)e->head_plane.p : nullptr; r.seg_offsets = d_offsets; r.seg_ids = d_ids; r.n_seg = n_seg;
       r.log_begin = log_begin; r.log_end = log_end;
       r.states_in = states_in; r.states_out = (uint8_t*)e->states.p;
       r.counters = counters;
@@ -463,7 +487,7 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
       uint64_t want = (n_chunks + wpc - 1) / wpc;
       if (want == 0) want = 1;  // all segments empty: one CTA still writes every (None) state
       const int grid = (int)(want < (uint64_t)max_grid ? want : (uint64_t)max_grid);
-      cudaError_t le = v1 ? launch_fold_rows(r, e->row_prog, grid, e->stream) : launch_fold_runs(r, e->row_prog, rv, hv, grid, overlap, e->stream);
+      cudaError_t le = v1 ? launch_fold_rows(r, e->row_prog, grid, e->stream) : launch_fold_runs(r, e->row_prog, rv, pl, grid, overlap, e->stream);
       if (le != cudaSuccess) return fail(e, SGR_ERR_CUDA, "fold launch: %s", cudaGetErrorString(le));
       if (runs) {
         e->run_counter_idx ^= 1;  // the kernel replays throwing segments itself and cleans the other block
@@ -489,9 +513,10 @@ int32_t enqueue_fold(sgr_engine* e, const uint8_t* d_events, const uint64_t* d_o
   }
   if (!overlap) CUDA_TRY(e, cudaEventRecord(e->ev1, e->stream));
   e->fold_pending = true;
-  e->pending = PendingFold{kernel, overlap, use_prior, n_seg, event_bytes, d_events, d_offsets, d_ids, counters, heads};
+  e->pending = PendingFold{kernel, overlap, use_prior, n_seg, event_bytes, d_events, d_offsets, d_ids, counters, plane};
   e->stats.fold_launches = launches;
-  e->stats.head_plane = heads ? 1u : 0u;
+  e->stats.head_plane = plane ? 1u : 0u;
+  e->stats.plane_bytes = plane;
   return SGR_OK;
 }
 
@@ -668,7 +693,8 @@ int32_t sgr_load_events(sgr_engine* e, const void* events, uint64_t nbytes, cons
   // (the copy is PCIe-bound, the split an HBM pass over the chunk)
   bool split = e->row_ok && e->row_prog.head_only && e->opt_head_plane && e->opt_kernel == 0 && e->opt_run_variant < 0 &&
                e->program.record_kind == SGR_REC_FIXED64 && e->row_prog.user_words != 14 && aligned64 && end > begin;
-  if (split && e->head_plane.reserve((end - begin) / 2) != cudaSuccess) { (void)cudaGetLastError(); split = false; }
+  const uint32_t plane_rec = plane_record_bytes(e);
+  if (split && e->head_plane.reserve((end - begin) / 64 * plane_rec) != cudaSuccess) { (void)cudaGetLastError(); split = false; }
   if (!split) {
     rc = upload_timed(e, e->ev0, e->ev1, {{e->own_events.p, events, nbytes}, {e->own_offsets.p, seg_offsets, (n_agg + 1) * 8}});
     if (rc) return rc;
@@ -688,8 +714,8 @@ int32_t sgr_load_events(sgr_engine* e, const void* events, uint64_t nbytes, cons
       CUDA_TRY(e, cudaMemcpyAsync(dst + begin + r0 * 64, src + begin + r0 * 64, (r1 - r0) * 64, cudaMemcpyHostToDevice, e->stream));
       CUDA_TRY(e, cudaEventRecord(e->ev_copied, e->stream));
       CUDA_TRY(e, cudaStreamWaitEvent(e->side_stream, e->ev_copied, 0));   // waits for this record of the event
-      cudaError_t le = launch_build_heads(dst + begin, (uint8_t*)e->head_plane.p, r0, r1, e->num_sms, e->side_stream);
-      if (le != cudaSuccess) return fail(e, SGR_ERR_CUDA, "head plane build: %s", cudaGetErrorString(le));
+      cudaError_t le = build_plane(e, dst + begin, plane_rec, r0, r1, e->side_stream);
+      if (le != cudaSuccess) return fail(e, SGR_ERR_CUDA, "plane build: %s", cudaGetErrorString(le));
     }
     if (nbytes > end) CUDA_TRY(e, cudaMemcpyAsync(dst + end, src + end, nbytes - end, cudaMemcpyHostToDevice, e->stream));
     CUDA_TRY(e, cudaEventRecord(e->ev_split, e->side_stream));
@@ -700,7 +726,9 @@ int32_t sgr_load_events(sgr_engine* e, const void* events, uint64_t nbytes, cons
   }
   e->stats.ms_group = 0;
   rc = after_load(e, (const uint8_t*)e->own_events.p, (const uint64_t*)e->own_offsets.p, nbytes, n_agg);
-  if (rc == SGR_OK && split && e->offsets_aligned64 && e->log_begin == begin && e->log_end == end) e->plane_state = sgr_engine::kPlaneValid;
+  if (rc == SGR_OK && split && e->offsets_aligned64 && e->log_begin == begin && e->log_end == end) {
+    e->plane_state = sgr_engine::kPlaneValid; e->plane_bytes = plane_rec;
+  }
   return rc;
 }
 
@@ -2201,8 +2229,13 @@ int32_t sgr_set_option(sgr_engine* e, const char* name, int64_t value) {
   if (!strcmp(name, "lookback_epoch")) { e->epoch = (uint32_t)value; return SGR_OK; }
   if (!strcmp(name, "head_plane")) { e->opt_head_plane = value ? 1 : 0; return SGR_OK; }
   if (!strcmp(name, "head_variant")) {
-    if (value < 0 || value >= head_variant_count()) return fail(e, SGR_ERR_INVALID, "head_variant out of range");
+    // -1: automatic (the slot plane where the program fits it, else head variant 0); >= 0 keeps the 32-byte head plane
+    if (value < -1 || value >= head_variant_count()) return fail(e, SGR_ERR_INVALID, "head_variant out of range");
     e->opt_head_variant = value; return SGR_OK;
+  }
+  if (!strcmp(name, "proj_variant")) {
+    if (value < 0 || value >= proj_variant_count()) return fail(e, SGR_ERR_INVALID, "proj_variant out of range");
+    e->opt_proj_variant = value; return SGR_OK;
   }
   if (!strcmp(name, "run_chunk_bytes")) {
     if (value < 2048 || value > (1ll << 30)) return fail(e, SGR_ERR_INVALID, "run_chunk_bytes must be in [2048, 2^30]");

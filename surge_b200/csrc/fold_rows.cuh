@@ -56,7 +56,8 @@ struct RowProgram {
 
 struct RowArgs {
   const uint8_t* events;        // device log; records at log_begin + 64*i
-  const uint8_t* heads;         // fold_runs head plane (or null): bytes 0..31 of record i at heads + 32*i
+  const uint8_t* heads;         // fold_runs plane (or null): bytes 0..31 of record i at heads + 32*i (head plane), or
+                                // its slot words at heads + 16*i (slot plane)
   const uint64_t* seg_offsets;  // n_seg+1 byte offsets, all == log_begin (mod 64)
   const uint32_t* seg_ids;      // optional state slot per segment
   uint64_t n_seg;
@@ -140,17 +141,24 @@ cudaError_t launch_fold_vruns(const VarArgs& args, const RowProgram& prog, int n
 int run_variant_count();
 const char* run_variant_name(int v);
 int head_variant_count();
-// head < 0: the kernel stages the log (run variant `variant`); head >= 0: it stages RowArgs::heads (head variant `head`)
-int run_kernel_max_grid(int num_sms, int variant, int head, const RowProgram& prog);
-int run_variant_step_bytes(int variant, int head, const RowProgram& prog);  // log bytes per step
+int proj_variant_count();
+// the program may fold from the slot plane: head-only, 16-byte state, class 0, at most 4 slots
+bool slot_plane_fits(const RowProgram& prog);
+// plane 0: the kernel stages the log (run variant `variant`); plane 32: the head plane RowArgs::heads (head variant
+// `variant`); plane 16: the slot plane RowArgs::heads (projected variant `variant`)
+int run_kernel_max_grid(int num_sms, int variant, int plane, const RowProgram& prog);
+int run_variant_step_bytes(int variant, int plane, const RowProgram& prog);  // log bytes per step
 int run_warps_per_cta();
 // steps per chunk of a log of `steps` steps folded by up to n_warps warps: at most chunk_bytes, small enough that every warp
 // gets a chunk, and at least the steps the variant stages ahead
-uint64_t run_variant_chunk_steps(int variant, int head, const RowProgram& prog, uint64_t chunk_bytes, uint64_t steps, uint64_t n_warps);
+uint64_t run_variant_chunk_steps(int variant, int plane, const RowProgram& prog, uint64_t chunk_bytes, uint64_t steps, uint64_t n_warps);
 // one launch, replay included; overlap: it may start while the runs fold before it on the stream drains (programmatic
 // dependent launch), for a fold of the same log right behind another
-cudaError_t launch_fold_runs(const RowArgs& args, const RowProgram& prog, int variant, int head, int grid, bool overlap, cudaStream_t stream);
+cudaError_t launch_fold_runs(const RowArgs& args, const RowProgram& prog, int variant, int plane, int grid, bool overlap, cudaStream_t stream);
 // copy bytes 0..31 of records [rec0, rec1) of `log` (64-byte records from its first byte) to heads + 32*i
 cudaError_t launch_build_heads(const uint8_t* log, uint8_t* heads, uint64_t rec0, uint64_t rec1, int num_sms, cudaStream_t stream);
+// write the slot words of records [rec0, rec1) of `log` to slots + 16*i, slot s at word s, zero-padded (slot_plane_fits)
+cudaError_t launch_build_slots(const uint8_t* log, uint8_t* slots, uint64_t rec0, uint64_t rec1, const RowProgram& prog, int num_sms,
+                               cudaStream_t stream);
 
 }  // namespace sgr

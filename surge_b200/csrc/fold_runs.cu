@@ -174,7 +174,8 @@ __device__ __forceinline__ void finish_empty(const RowArgs& a, uint32_t seg) {
   }
 }
 
-// REC: bytes staged per record, 64 (the log itself) or 32 (the head plane: each record's bytes 0..31)
+// REC: bytes staged per record, 64 (the log itself), 32 (the head plane: each record's bytes 0..31) or 16 (the slot plane:
+// the program's slot words, slot s at word s)
 template <int R, int NSTAGE, int REC = 64>
 __host__ __device__ constexpr int warp_smem_bytes() {
   return NSTAGE * 32 * REC * R  // staged steps
@@ -211,10 +212,14 @@ __device__ __forceinline__ Xf<W> look_back_chunks(const RowArgs& a, uint64_t c) 
 // DIRECT: programs with many source words read each state word's source straight from the staged record instead of
 // pre-fetching NS slots and selecting (NS is then unused)
 // REC == 32: the records are staged from the head plane (RowArgs::heads) rather than the log; offsets still count log bytes.
+// REC == 16: from the slot plane (RowArgs::heads): a lane reads a whole record with one 16-byte load, its slot words in slot
+// order (NS == 4: all four words are read, whatever the program's slot count).
 template <int W, int R, int NSTAGE, int NS, int MINB, bool DIRECT, int CLS, int REC = 64>
 __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __grid_constant__ RowArgs a, const __grid_constant__ RowProgram pg) {
   static_assert(R % 2 == 0 && 8 % R == 0, "R in {2,4,8}");
-  static_assert(REC == 64 || (REC == 32 && R >= 4), "a lane's run starts on a 128-byte line: R >= 128 / REC");
+  static_assert(REC == 64 || REC == 32 || REC == 16, "the log, the head plane or the slot plane");
+  static_assert(R * REC >= 128, "a lane's run starts on a 128-byte line: R >= 128 / REC");
+  static_assert(REC != 16 || (!DIRECT && NS == 4), "the slot plane holds four slot words, not record words");
   constexpr int STEP_BYTES = 2048 * R;          // log bytes per step
   constexpr int STEP_RECS = 32 * R;
   constexpr int STAGE_BYTES = STEP_RECS * REC;  // staged bytes per step
@@ -329,14 +334,18 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
   uint64_t kc = (chunk != kNone && chunk != 0) ? first_boundary(base + chunk * cs * STEP_BYTES) : 0;
 
   // where lane i finds word (c,k) of the record at place rl of its line: byte (((CPR*rl + c) ^ (i&7)) << 4) + 4k of the line
-  // (rl == t % RPL for the t-th record of the run: a run starts on a line)
+  // (rl == t % RPL for the t-th record of the run: a run starts on a line). The slot plane needs no table: record rl of
+  // the line is the chunk rl ^ (i&7).
   constexpr int NSOFF = DIRECT ? 1 : NS;
-  uint32_t soff[RPL][NSOFF];
+  constexpr int SOFF_RPL = REC == 16 ? 1 : RPL;
+  uint32_t soff[SOFF_RPL][NSOFF];
+  if constexpr (REC != 16) {
 #pragma unroll
-  for (int s = 0; s < NSOFF; ++s) {
-    const uint32_t c = pg.slot_word[s] >> 2, k = pg.slot_word[s] & 3u;
+    for (int s = 0; s < NSOFF; ++s) {
+      const uint32_t c = pg.slot_word[s] >> 2, k = pg.slot_word[s] & 3u;
 #pragma unroll
-    for (int rl = 0; rl < RPL; ++rl) soff[rl][s] = ((((uint32_t)(CPR * rl) + c) ^ (uint32_t)(lane & 7)) << 4) + (k << 2);
+      for (int rl = 0; rl < RPL; ++rl) soff[rl][s] = ((((uint32_t)(CPR * rl) + c) ^ (uint32_t)(lane & 7)) << 4) + (k << 2);
+    }
   }
   // boundary window: lane j holds off[kc+j] and off[kc+j+1]; reloaded right after boundaries are consumed,
   // so the values a step needs were requested one step earlier
@@ -441,7 +450,10 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
           const uint32_t rec = sbase + (uint32_t)(p / RPL) * 128u;
           const uint32_t lane7 = (uint32_t)(lane & 7), parc = (uint32_t)(t % RPL) * CPR;  // p%RPL == t%RPL: RPL divides R
           uint32_t sv[DIRECT ? 1 : NS];
-          if (DIRECT) {
+          if constexpr (REC == 16) {
+            const uint4 r4 = lds128(rec + ((((uint32_t)(t % RPL)) ^ lane7) << 4));
+            sv[0] = r4.x; sv[1] = r4.y; sv[2] = r4.z; sv[3] = r4.w;
+          } else if (DIRECT) {
             sv[0] = lds32(rec + soff[t % RPL][0]);
           } else {
 #pragma unroll
@@ -669,7 +681,7 @@ __device__ __noinline__ void replay_segments(const RowArgs& a, const RowProgram&
 }
 
 typedef void (*RunKernel)(const RowArgs, const RowProgram);
-struct RunVariant { RunKernel k[3]; int r, nstage; const char* name; };  // 16-byte states; k[i]: NS = 2, 3, 6
+struct RunVariant { RunKernel k[3]; int r, nstage; const char* name; };  // 16-byte states; k[i]: NS = 2, 3, 6 (slot plane: k[0])
 #define RUN_VARIANT(R, ST, MINB) {{fold_runs_kernel<2, R, ST, 2, MINB, false, 0>, fold_runs_kernel<2, R, ST, 3, MINB, false, 0>, fold_runs_kernel<2, R, ST, 6, MINB, false, 0>}, R, ST, "runs W2 R" #R " st" #ST}
 const RunVariant kRunVariants[] = {
     RUN_VARIANT(4, 2, 3), RUN_VARIANT(4, 1, 5), RUN_VARIANT(2, 2, 5), RUN_VARIANT(2, 1, 5), RUN_VARIANT(4, 3, 2), RUN_VARIANT(8, 1, 3), RUN_VARIANT(2, 3, 4),
@@ -682,23 +694,33 @@ const RunVariant kHeadVariants[] = {
     HEAD_VARIANT(8, 2, 3), HEAD_VARIANT(4, 3, 4), HEAD_VARIANT(4, 2, 4), HEAD_VARIANT(4, 4, 3), HEAD_VARIANT(8, 3, 2),
 };
 constexpr int kNumHeadVariants = sizeof(kHeadVariants) / sizeof(kHeadVariants[0]);
+// the slot plane (16 bytes per record, slot s at word s): a 128-byte line holds 8 records, so a run is R = 8 records, one
+// line, and one kernel serves every slot count. The first is the default (scripts/fold_ceiling.py --proj-variants,
+// DESIGN.md section 4)
+#define PROJ_VARIANT(ST, MINB) {{fold_runs_kernel<2, 8, ST, 4, MINB, false, 0, 16>, nullptr, nullptr}, 8, ST, "slots W2 R8 st" #ST}
+const RunVariant kProjVariants[] = {
+    PROJ_VARIANT(2, 5), PROJ_VARIANT(3, 3), PROJ_VARIANT(4, 2), PROJ_VARIANT(6, 2),
+};
+constexpr int kNumProjVariants = sizeof(kProjVariants) / sizeof(kProjVariants[0]);
 // wider states / many source words: one configuration each (R = 4, 2 stages, direct word reads)
 constexpr int kWideR = 4, kWideStages = 2;
 
 bool is_wide(const RowProgram& prog) { return prog.user_words != 2 || prog.n_slots > 6 || prog.cls != 0; }
-// head < 0: the row layout, run variant v; head >= 0: the head plane, head variant `head`
-const RunVariant& pick_variant(int v, int head) {
-  if (head >= 0) return kHeadVariants[head < kNumHeadVariants ? head : 0];
+// plane 0: the log, run variant v; 32: the head plane, head variant v; 16: the slot plane, projected variant v
+const RunVariant& pick_variant(int v, int plane) {
+  if (plane == 16) return kProjVariants[(v >= 0 && v < kNumProjVariants) ? v : 0];
+  if (plane == 32) return kHeadVariants[(v >= 0 && v < kNumHeadVariants) ? v : 0];
   return kRunVariants[(v >= 0 && v < kNumRunVariants) ? v : 0];
 }
-int variant_r(int v, int head, const RowProgram& prog) { return is_wide(prog) ? kWideR : pick_variant(v, head).r; }
-int variant_nstage(int v, int head, const RowProgram& prog) { return is_wide(prog) ? kWideStages : pick_variant(v, head).nstage; }
-size_t variant_smem(int v, int head, const RowProgram& prog) {
-  const size_t r = (size_t)variant_r(v, head, prog), ns = (size_t)variant_nstage(v, head, prog), rec = head >= 0 ? 32 : 64;
+int variant_r(int v, int plane, const RowProgram& prog) { return plane != 16 && is_wide(prog) ? kWideR : pick_variant(v, plane).r; }
+int variant_nstage(int v, int plane, const RowProgram& prog) { return plane != 16 && is_wide(prog) ? kWideStages : pick_variant(v, plane).nstage; }
+size_t variant_smem(int v, int plane, const RowProgram& prog) {
+  const size_t r = (size_t)variant_r(v, plane, prog), ns = (size_t)variant_nstage(v, plane, prog), rec = plane ? (size_t)plane : 64;
   return (size_t)kRunWarps * (ns * 32 * rec * r + 2 * 32 * r * 4 + 32 * 4);
 }
-RunKernel variant_kernel(int v, int head, const RowProgram& prog) {
-  if (head >= 0) {
+RunKernel variant_kernel(int v, int plane, const RowProgram& prog) {
+  if (plane == 16) return pick_variant(v, plane).k[0];
+  if (plane == 32) {
     if (prog.user_words == 14) return fold_runs_kernel<14, kWideR, kWideStages, 1, 1, true, 1, 32>;
     if (prog.user_words == 6) return fold_runs_kernel<6, kWideR, kWideStages, 1, 2, true, 1, 32>;
     if (is_wide(prog)) return fold_runs_kernel<2, kWideR, kWideStages, 1, 3, true, 1, 32>;
@@ -707,7 +729,7 @@ RunKernel variant_kernel(int v, int head, const RowProgram& prog) {
     if (prog.user_words == 6) return fold_runs_kernel<6, kWideR, kWideStages, 1, 2, true, 1>;
     if (is_wide(prog)) return fold_runs_kernel<2, kWideR, kWideStages, 1, 3, true, 1>;
   }
-  return pick_variant(v, head).k[prog.n_slots <= 2 ? 0 : (prog.n_slots <= 3 ? 1 : 2)];
+  return pick_variant(v, plane).k[prog.n_slots <= 2 ? 0 : (prog.n_slots <= 3 ? 1 : 2)];
 }
 
 }  // namespace
@@ -715,31 +737,35 @@ RunKernel variant_kernel(int v, int head, const RowProgram& prog) {
 int run_variant_count() { return kNumRunVariants; }
 const char* run_variant_name(int v) { return (v >= 0 && v < kNumRunVariants) ? kRunVariants[v].name : "?"; }
 int head_variant_count() { return kNumHeadVariants; }
+int proj_variant_count() { return kNumProjVariants; }
+bool slot_plane_fits(const RowProgram& prog) {
+  return prog.head_only && prog.user_words == 2 && prog.cls == 0 && prog.n_slots <= 4;
+}
 
-int run_kernel_max_grid(int num_sms, int variant, int head, const RowProgram& prog) {
-  const size_t smem = variant_smem(variant, head, prog);
-  RunKernel k = variant_kernel(variant, head, prog);
+int run_kernel_max_grid(int num_sms, int variant, int plane, const RowProgram& prog) {
+  const size_t smem = variant_smem(variant, plane, prog);
+  RunKernel k = variant_kernel(variant, plane, prog);
   cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   int per_sm = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kRunThreads, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
   return per_sm * num_sms;
 }
 
-int run_variant_step_bytes(int variant, int head, const RowProgram& prog) { return 2048 * variant_r(variant, head, prog); }
+int run_variant_step_bytes(int variant, int plane, const RowProgram& prog) { return 2048 * variant_r(variant, plane, prog); }
 int run_warps_per_cta() { return kRunWarps; }
 
-uint64_t run_variant_chunk_steps(int variant, int head, const RowProgram& prog, uint64_t chunk_bytes, uint64_t steps, uint64_t n_warps) {
-  const uint64_t ns = (uint64_t)variant_nstage(variant, head, prog);
+uint64_t run_variant_chunk_steps(int variant, int plane, const RowProgram& prog, uint64_t chunk_bytes, uint64_t steps, uint64_t n_warps) {
+  const uint64_t ns = (uint64_t)variant_nstage(variant, plane, prog);
   const uint64_t lo = ns > 1 ? ns - 1 : 1;  // what is staged ahead stays inside the next chunk
-  uint64_t hi = chunk_bytes / (uint64_t)run_variant_step_bytes(variant, head, prog);
+  uint64_t hi = chunk_bytes / (uint64_t)run_variant_step_bytes(variant, plane, prog);
   if (hi < lo) hi = lo;
   const uint64_t fair = n_warps ? steps / n_warps : hi;  // a chunk for every warp on a small log
   return fair < lo ? lo : (fair > hi ? hi : fair);
 }
 
-cudaError_t launch_fold_runs(const RowArgs& args, const RowProgram& prog, int variant, int head, int grid, bool overlap, cudaStream_t stream) {
-  const size_t smem = variant_smem(variant, head, prog);
-  RunKernel k = variant_kernel(variant, head, prog);  // its smem attribute was set by run_kernel_max_grid
+cudaError_t launch_fold_runs(const RowArgs& args, const RowProgram& prog, int variant, int plane, int grid, bool overlap, cudaStream_t stream) {
+  const size_t smem = variant_smem(variant, plane, prog);
+  RunKernel k = variant_kernel(variant, plane, prog);  // its smem attribute was set by run_kernel_max_grid
   // overlap: the launch may begin while the fold before it drains (programmatic dependent launch); the kernel waits on the
   // device for its predecessor before it touches anything that predecessor writes
   cudaLaunchAttribute attr[1];
@@ -768,6 +794,41 @@ cudaError_t launch_build_heads(const uint8_t* log, uint8_t* heads, uint64_t rec0
   const uint64_t want = ((rec1 - rec0) * 2 + 255) / 256;
   const uint64_t cap = (uint64_t)num_sms * 16;
   build_heads_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, stream>>>(log, heads, rec0, rec1);
+  return cudaGetLastError();
+}
+
+// ---- the slot plane: the program's slot words of every record, 16 bytes per record, slot s at word s --------------------
+// One thread per record: it reads the record's head (the second 16 bytes only when a slot word lies there) and keeps the
+// slot words, so a warp writes 32 records' slots as one contiguous 512-byte block. sel: slot word s in bits [4s, 4s+4).
+__global__ void __launch_bounds__(256) build_slots_kernel(const uint8_t* log, uint8_t* slots, uint64_t rec0, uint64_t rec1, uint32_t sel,
+                                                          uint32_t n_slots, bool upper) {
+  for (uint64_t r = rec0 + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < rec1; r += (uint64_t)gridDim.x * blockDim.x) {
+    const uint4* rp = reinterpret_cast<const uint4*>(log + r * 64);
+    const uint4 lo = __ldcs(rp), hi = upper ? __ldcs(rp + 1) : make_uint4(0, 0, 0, 0);
+    const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+    uint32_t o[4];
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const uint32_t sw = (sel >> (4 * s)) & 7u;
+      uint32_t v = 0;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) v = sw == (uint32_t)k ? w[k] : v;  // a select chain: no local-memory indexing
+      o[s] = (uint32_t)s < n_slots ? v : 0u;
+    }
+    reinterpret_cast<uint4*>(slots)[r] = make_uint4(o[0], o[1], o[2], o[3]);
+  }
+}
+
+cudaError_t launch_build_slots(const uint8_t* log, uint8_t* slots, uint64_t rec0, uint64_t rec1, const RowProgram& prog, int num_sms,
+                               cudaStream_t stream) {
+  if (rec1 <= rec0) return cudaSuccess;
+  if (!slot_plane_fits(prog)) return cudaErrorInvalidValue;
+  uint32_t sel = 0;
+  bool upper = false;
+  for (uint32_t s = 0; s < prog.n_slots; ++s) { sel |= prog.slot_word[s] << (4 * s); upper |= prog.slot_word[s] >= 4; }
+  const uint64_t want = (rec1 - rec0 + 255) / 256;
+  const uint64_t cap = (uint64_t)num_sms * 16;
+  build_slots_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, stream>>>(log, slots, rec0, rec1, sel, prog.n_slots, upper);
   return cudaGetLastError();
 }
 

@@ -141,7 +141,8 @@ class ReplayEngine:
     # -- loads
     def load_events(self, events, seg_offsets) -> None:
         """CSR event log. numpy -> copied to HBM; CUDA tensors -> borrowed, and must not be modified while loaded: the engine
-        may fold from a copy of their record heads (include/sgr.h, head plane). Load again to fold changed records."""
+        may fold from a copy of the record words its program reads (include/sgr.h, planes). Load again to fold changed
+        records."""
         if _is_cuda_tensor(events):
             assert _is_cuda_tensor(seg_offsets)
             ev, nbytes = self._lend(events, seg_offsets)
@@ -501,6 +502,9 @@ class ReplayEngine:
         return s
 
     def set_option(self, name: str, value: int) -> None:
+        """Engine options (include/sgr.h). Fold-source options: "head_plane" 0 keeps every fold on the log; "head_variant"
+        -1 (the default) picks the slot plane where the program fits it, 0..4 keeps the 32-byte head plane with that kernel
+        configuration; "proj_variant" picks the slot plane's kernel configuration."""
         self._ck(self._lib.sgr_set_option(self._h, name.encode(), int(value)))
 
     def stream_ptr(self) -> int:
