@@ -190,7 +190,8 @@ typedef struct sgr_stats {
   uint32_t fold_launches;   /* kernels launched by the last fold */
   uint32_t head_plane;      /* 1: the last fold read its records from a plane (plane_bytes), not the log */
   uint32_t plane_bytes;     /* record bytes of that plane: 16 (slot plane), 32 (head plane), 0 (the fold read the log) */
-  uint32_t reserved[5];
+  uint32_t chunk_table;     /* 1: the last fold started each chunk from the slot plane's chunk table, not a search */
+  uint32_t reserved[4];
 } sgr_stats;
 
 int32_t sgr_abi_version(void);
@@ -221,7 +222,9 @@ int32_t sgr_load_events(sgr_engine* e, const void* events, uint64_t nbytes,
  * head plane: bytes 0..31 of every record, half the log's size. A host load builds the plane behind the copy; a
  * borrowed log gets it from the first fold that uses it. Every load and sgr_register_program drops it; if it cannot be
  * allocated the fold reads the log. sgr_set_option("head_plane", 0) keeps every fold on the log; ("head_variant", v >= 0)
- * keeps a slot-plane program on the head plane; ("proj_variant", v) picks the slot-plane kernel configuration. */
+ * keeps a slot-plane program on the head plane; ("proj_variant", v) picks the slot-plane kernel configuration. A fold from
+ * the slot plane also keeps a table of each ticketed chunk's first segment boundary (8 bytes per "run_chunk_bytes" of log),
+ * dropped with the plane and rebuilt when the chunk size changes; without its memory the fold searches the offsets. */
 int32_t sgr_load_events_device(sgr_engine* e, const void* d_events, uint64_t nbytes,
                                const uint64_t* d_seg_offsets, uint64_t n_agg);
 

@@ -11,12 +11,15 @@ On the log bench.py folds (synth.counter_csr_device(2^20, 32, seed=2): 2^20 aggr
   (e) a load of the borrowed log followed by one fold, which builds its plane, against the same with "head_plane" 0;
   (f) the read probe over a dense buffer of a quarter of the log's bytes: the slot plane the Counter fold stages by default
       (its slot words 0, 4, 1 and a zero word, 16 bytes per record, gathered here with torch), and the fold from the slot
-      plane under each --proj-variants entry;
+      plane under each --proj-variants entry, the ticketed probe of that plane at each --slot-probe-chunk-bytes entry (the
+      slot-plane fold's default 128 KiB of log is 32 KiB of plane), and the slot-plane fold at each --slot-chunk-bytes
+      entry of run_chunk_bytes (log bytes per chunk);
 and reports each as GB/s over the log's bytes and the fold as a share of (a) (the head-plane folds: of (d), the slot-plane
 folds: of (f)). Prints one JSON document and writes it to
 OUT/fold_ceiling.json. The card's name and power limit are part of the numbers and are recorded with them.
 
     python scripts/fold_ceiling.py --out DIR [--reps 30] [--steps 200] [--head-variants 0,1,2,3,4] [--proj-variants 0,1,2,3]
+        [--slot-chunk-bytes 65536,131072,262144,524288,1048576] [--slot-probe-chunk-bytes 32768,131072]
 """
 from __future__ import annotations
 
@@ -57,6 +60,10 @@ def main() -> None:
                     help="comma list of head_variant values of the head-plane fold to measure")
     ap.add_argument("--proj-variants", type=lambda s: [int(x) for x in s.split(",")], default=[0],
                     help="comma list of proj_variant values of the slot-plane fold to measure")
+    ap.add_argument("--slot-chunk-bytes", type=lambda s: [int(x) for x in s.split(",")], default=[],
+                    help="comma list of run_chunk_bytes (log bytes) of the slot-plane fold to measure")
+    ap.add_argument("--slot-probe-chunk-bytes", type=lambda s: [int(x) for x in s.split(",")], default=[32768, 131072],
+                    help="comma list of chunks (plane bytes) of the ticketed slot-plane read probe")
     args = ap.parse_args()
 
     import torch
@@ -73,13 +80,13 @@ def main() -> None:
     ctl = torch.zeros(2, dtype=torch.int64, device=dev)
     stream = torch.cuda.current_stream()
 
-    def probe(ticketed: int, buf=log) -> list:
+    def probe(ticketed: int, buf=log, chunk_bytes: int = args.chunk_bytes) -> list:
         ms = []
         for _ in range(args.reps + 2):
             ctl.zero_()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record(stream)
-            rc = lib.sgr_probe_read(C.c_void_p(buf.data_ptr()), buf.numel(), ticketed, args.chunk_bytes, C.c_void_p(ctl.data_ptr()),
+            rc = lib.sgr_probe_read(C.c_void_p(buf.data_ptr()), buf.numel(), ticketed, chunk_bytes, C.c_void_p(ctl.data_ptr()),
                                     C.c_void_p(stream.cuda_stream))
             e1.record(stream)
             if rc != 0:
@@ -108,9 +115,13 @@ def main() -> None:
     slots = slots.view(torch.uint8).reshape(-1)
     out["f_read_probe_slot_plane_fixed_spans"] = summary(probe(0, slots), nbytes)
     out["f_read_probe_slot_plane_ticketed"] = summary(probe(1, slots), nbytes)
+    for cb in args.slot_probe_chunk_bytes:
+        out[f"f_read_probe_slot_plane_ticketed_chunk{cb}"] = summary(probe(1, slots, cb), nbytes)
     del slots, words
     for pv in args.proj_variants:
         out.update(measure_fold(log, off, dev, 0, args.reps, args.steps, f"_proj_variant{pv}", {"proj_variant": pv}))
+    for cb in args.slot_chunk_bytes:
+        out.update(measure_fold(log, off, dev, cb, args.reps, args.steps, f"_proj_variant0_chunk{cb}", {"proj_variant": 0}))
     out.update(measure_load_then_fold(log, off, dev, args.reps))
 
     a = out["a_read_probe_fixed_spans"]["ms_min"]

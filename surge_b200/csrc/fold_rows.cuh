@@ -76,6 +76,7 @@ struct RowArgs {
   uint32_t* part_data;          // per warp (fold_runs: per chunk): m, v[W], ex | has_head<<2
   uint32_t epoch;
   uint64_t chunk_steps;         // fold_runs: steps per chunk of the ticketed work order (run_variant_chunk_steps)
+  const uint64_t* chunk_kc;     // fold_runs from the slot plane (or null): per chunk, its first boundary (launch_build_chunk_table)
 };
 
 // false if the program is outside the transformer algebra (IF_EXISTS rules, 64-bit adds, f64 fields,
@@ -155,6 +156,10 @@ uint64_t run_variant_chunk_steps(int variant, int plane, const RowProgram& prog,
 // one launch, replay included; overlap: it may start while the runs fold before it on the stream drains (programmatic
 // dependent launch), for a fold of the same log right behind another
 cudaError_t launch_fold_runs(const RowArgs& args, const RowProgram& prog, int variant, int plane, int grid, bool overlap, cudaStream_t stream);
+// the chunk table of a runs fold: table[c] = the first k in [0, n_seg] with off[k] >= log_begin + c * chunk_steps * step_bytes,
+// for c in [0, n_chunks)
+cudaError_t launch_build_chunk_table(const uint64_t* off, uint64_t n_seg, uint64_t log_begin, uint64_t step_bytes, uint64_t chunk_steps,
+                                     uint64_t n_chunks, uint64_t* table, cudaStream_t stream);
 // copy bytes 0..31 of records [rec0, rec1) of `log` (64-byte records from its first byte) to heads + 32*i
 cudaError_t launch_build_heads(const uint8_t* log, uint8_t* heads, uint64_t rec0, uint64_t rec1, int num_sms, cudaStream_t stream);
 // write the slot words of records [rec0, rec1) of `log` to slots + 16*i, slot s at word s, zero-padded (slot_plane_fits)

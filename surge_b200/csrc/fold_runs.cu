@@ -36,7 +36,9 @@
 // in flight), which the fold before it only reads too, so it overlaps that fold's tail; states, look-back buffers,
 // counters, the replay list and the ticket come after the wait. Behind any other work (a kernel that writes the log, a
 // copy) it is launched plainly and the wait is a no-op. The chunk size shrinks on small logs so that every resident warp
-// gets a chunk (run_variant_chunk_steps).
+// gets a chunk (run_variant_chunk_steps). From the slot plane a chunk's first boundary comes from the engine's chunk table
+// (RowArgs::chunk_kc) instead of the search, and the next chunk's entry and boundary window are loaded a step or two
+// before the switch.
 #include <stdio.h>
 
 #include "../../include/sgr.h"
@@ -186,13 +188,38 @@ __host__ __device__ constexpr int warp_smem_bytes() {
 template <int W>
 __device__ __noinline__ void replay_segments(const RowArgs& a, const RowProgram& pg, const uint32_t* tab, int lane, unsigned long long n_redo);
 
+// The slot-plane fold publishes a chunk's open transformer as one 16-byte row of part_flags: m | ex << 4 | has_head << 6,
+// v[0], v[1], epoch. One aligned 16-byte access carries the row and its flag together, so neither side needs a fence
+// between them. Word 3 of a row lies where every other fold writes only epochs (a u32 flag per part), so a stale row never
+// shows the current epoch.
+__device__ __forceinline__ uint4 ld_volatile_v4(const uint32_t* p) {
+  uint4 v;
+  asm volatile("ld.volatile.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ void st_volatile_v4(uint32_t* p, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
+  asm volatile("st.volatile.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
+}
+constexpr uint32_t kRowEx = 4, kRowHead = 64u, kRowFields = 0x70u;  // fields of a packed row's word 0 (m bits 4..29 are free at W = 2)
+
 // Decoupled look-back (lane 0): compose the open transformers of the chunks before chunk c until one that contains a head.
 // They were all handed out before c, to warps that are running, and a chunk publishes without waiting on anyone.
-template <int W, int CLS>
+// PACKED: the rows of the slot-plane fold (above).
+template <int W, int CLS, bool PACKED = false>
 __device__ __forceinline__ Xf<W> look_back_chunks(const RowArgs& a, uint64_t c) {
   Xf<W> pre = identity<W>();
   while (c > 0) {
     --c;
+    if constexpr (PACKED) {
+      static_assert(W == 2, "a packed row holds two state words");
+      uint4 r = ld_volatile_v4(a.part_flags + 4 * c);
+      while (r.w != a.epoch) { __nanosleep(64); r = ld_volatile_v4(a.part_flags + 4 * c); }
+      Xf<W> e;
+      e.m = r.x & ~kRowFields; e.ex = (r.x >> kRowEx) & 3u; e.v[0] = r.y; e.v[1] = r.z;
+      pre = compose<W, CLS>(e, pre);
+      if (r.x & kRowHead) break;
+      continue;
+    }
     const uint32_t* pf = a.part_flags + c;
     while (ld_volatile_u32(pf) != a.epoch) { __nanosleep(64); }
     __threadfence();
@@ -331,7 +358,11 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
     issue_next();
     cp_async_commit();
   }
-  uint64_t kc = (chunk != kNone && chunk != 0) ? first_boundary(base + chunk * cs * STEP_BYTES) : 0;
+  uint64_t kc = 0;
+  if (chunk != kNone && chunk != 0) {
+    if constexpr (REC == 16) kc = a.chunk_kc ? a.chunk_kc[chunk] : first_boundary(base + chunk * cs * STEP_BYTES);
+    else kc = first_boundary(base + chunk * cs * STEP_BYTES);
+  }
 
   // where lane i finds word (c,k) of the record at place rl of its line: byte (((CPR*rl + c) ^ (i&7)) << 4) + 4k of the line
   // (rl == t % RPL for the t-th record of the run: a run starts on a line). The slot plane needs no table: record rl of
@@ -356,12 +387,18 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
     win_bn = k < n_seg ? a.seg_offsets[k + 1] : ~0ull;
   };
   if (chunk != kNone) load_window();
+  // the slot plane with a chunk table: the next chunk's first boundary (pf_kc, ~0u until loaded; n_seg < 2^32) and its
+  // boundary window (pf_b, pf_bn once pf_win) are loaded while this chunk is folded, so the switch only swaps registers
+  // instead of a search and a window load that no step hid
+  uint32_t pf_kc = ~0u;
+  uint64_t pf_b = ~0ull, pf_bn = ~0ull;
+  bool pf_win = false;
 
   // ---- after the wait: the previous fold (and its replay) has completed; its states, counters and buffers are free
   grid_dep_wait();
   if (threadIdx.x == 0) atomicMax(a.counters + 8, ~t_entry);  // the earliest CTA entry, complemented (stats ms_fold)
   if (gw == 0 && lane < 16) a.counters_next[lane] = 0ull;    // the next fold starts from clean counters without a memset
-  auto look_back = [&](uint64_t c) -> Xf<W> { return look_back_chunks<W, CLS>(a, c); };
+  auto look_back = [&](uint64_t c) -> Xf<W> { return look_back_chunks<W, CLS, REC == 16>(a, c); };
   // lane 0: a chunk's first segment, begun in an earlier chunk, is finished after the warp's next chunk (or at its exit),
   // so the warp does not wait on a predecessor that is still being folded
   bool dfr = false;
@@ -381,9 +418,17 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
     nxt_pending = true;
     if (prev_chunk != kNone && chunk != prev_chunk + 1) {
       // a chunk right after the previous one starts at the boundary where that one stopped
-      kc = chunk != 0 ? first_boundary(wb) : 0;
-      load_window();
+      bool have_win = false;
+      if constexpr (REC == 16) {
+        if (!a.chunk_kc) kc = first_boundary(wb);
+        else if (pf_win) { kc = pf_kc; win_b = pf_b; win_bn = pf_bn; have_win = true; }
+        else kc = pf_kc != ~0u ? pf_kc : a.chunk_kc[chunk];
+      } else {
+        kc = chunk != 0 ? first_boundary(wb) : 0;
+      }
+      if (!have_win) load_window();
     }
+    pf_kc = ~0u; pf_win = false;
 
     bool span_has_head = false;          // a segment head was seen in this chunk
     bool inh_pending = false;            // the segment flowing into the chunk awaits the look-back (held by lane 0)
@@ -531,6 +576,19 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
         span_has_head = true;
       }
       __syncwarp();
+      if constexpr (REC == 16) {
+        // one load per step, so each has a step's time to arrive: the ticket drawn at the chunk's start, then its table entry,
+        // then its window
+        if (a.chunk_kc && pf_kc == ~0u) {
+          resolve_next();
+          if (nxt != kNone && nxt != chunk + 1) pf_kc = (uint32_t)a.chunk_kc[nxt];
+        } else if (a.chunk_kc && !pf_win) {
+          const uint64_t k = (uint64_t)pf_kc + lane;
+          pf_b = k <= n_seg ? a.seg_offsets[k] : ~0ull;
+          pf_bn = k < n_seg ? a.seg_offsets[k + 1] : ~0ull;
+          pf_win = true;
+        }
+      }
       if (++stage == NSTAGE) stage = 0;
     }
 
@@ -548,8 +606,12 @@ __global__ void __launch_bounds__(kRunThreads, MINB) fold_runs_kernel(const __gr
 
     // ---- publish this chunk's open transformer, then finish what needs the preceding chunks -----------------
     {
-      uint32_t* part_data = a.part_data + chunk * (W + 2);
-      if (lane == 0) {
+      if constexpr (REC == 16) {
+        if (lane == 0)
+          st_volatile_v4(a.part_flags + 4 * chunk, carry.m | (carry.ex << kRowEx) | (span_has_head ? kRowHead : 0u), carry.v[0], carry.v[1],
+                         a.epoch);
+      } else if (lane == 0) {
+        uint32_t* part_data = a.part_data + chunk * (W + 2);
         part_data[0] = carry.m;
 #pragma unroll
         for (int w = 0; w < W; ++w) part_data[1 + w] = carry.v[w];
@@ -829,6 +891,26 @@ cudaError_t launch_build_slots(const uint8_t* log, uint8_t* slots, uint64_t rec0
   const uint64_t want = (rec1 - rec0 + 255) / 256;
   const uint64_t cap = (uint64_t)num_sms * 16;
   build_slots_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, stream>>>(log, slots, rec0, rec1, sel, prog.n_slots, upper);
+  return cudaGetLastError();
+}
+
+__global__ void __launch_bounds__(256) build_chunk_table_kernel(const uint64_t* off, uint64_t n_seg, uint64_t log_begin, uint64_t chunk_bytes,
+                                                               uint64_t n_chunks, uint64_t* table) {
+  const uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_chunks) return;
+  const uint64_t wb = log_begin + c * chunk_bytes;
+  uint64_t lo = 0, hi = n_seg + 1;  // the first k in [0, n_seg] with off[k] >= wb, as fold_runs_kernel's first_boundary
+  while (lo < hi) {
+    const uint64_t mid = lo + (hi - lo) / 2;
+    if (off[mid] >= wb) hi = mid; else lo = mid + 1;
+  }
+  table[c] = lo;
+}
+
+cudaError_t launch_build_chunk_table(const uint64_t* off, uint64_t n_seg, uint64_t log_begin, uint64_t step_bytes, uint64_t chunk_steps,
+                                     uint64_t n_chunks, uint64_t* table, cudaStream_t stream) {
+  if (!n_chunks) return cudaSuccess;
+  build_chunk_table_kernel<<<(unsigned)((n_chunks + 255) / 256), 256, 0, stream>>>(off, n_seg, log_begin, step_bytes * chunk_steps, n_chunks, table);
   return cudaGetLastError();
 }
 

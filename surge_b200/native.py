@@ -70,7 +70,7 @@ class sgr_stats(C.Structure):
                 ("algorithmic_bytes", C.c_uint64), ("n_errors", C.c_uint64), ("n_long_segments", C.c_uint64),
                 ("ms_h2d", C.c_float), ("ms_group", C.c_float), ("ms_fold", C.c_float), ("ms_d2h", C.c_float),
                 ("fold_launches", C.c_uint32), ("head_plane", C.c_uint32), ("plane_bytes", C.c_uint32),
-                ("reserved", C.c_uint32 * 5)]
+                ("chunk_table", C.c_uint32), ("reserved", C.c_uint32 * 4)]
 
 
 class sgr_changes_cursor(C.Structure):
